@@ -35,11 +35,11 @@ def load_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"], "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -307,6 +307,30 @@ def c5_problems(cabi, indices):
     return probs
 
 
+DUMP_BUDGET = 63 << 20  # bytes of array data --dump-outputs may write (64 MB in all with the .npy headers)
+
+
+def dump_outputs(out_dir, results):
+    """The arrays a caller of the headline batch receives, one row per image pair: models (q, t) float64, the stats
+    fields float64, inlier masks float32.  If the masks would overflow DUMP_BUDGET, a fixed seeded sample of the pairs is
+    written instead (indices in pair_index.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    count, n = len(results), max(len(r["inliers"]) for r in results)
+    stats_fields = list(results[0]["stats"])
+    row_bytes = 4 * n + 8 * (7 + len(stats_fields) + 1)
+    idx = np.arange(count)
+    if count * row_bytes > DUMP_BUDGET:
+        idx = np.sort(np.random.default_rng(0).choice(count, DUMP_BUDGET // row_bytes, replace=False))
+    masks = np.zeros((len(idx), n), dtype=np.float32)
+    for j, i in enumerate(idx):
+        masks[j, :len(results[i]["inliers"])] = results[i]["inliers"]
+    np.save(os.path.join(out_dir, "pair_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "models.npy"), np.stack([np.asarray(results[i]["model"], dtype=np.float64) for i in idx]))
+    np.save(os.path.join(out_dir, "inliers.npy"), masks)
+    for f in stats_fields:
+        np.save(os.path.join(out_dir, f"stats_{f}.npy"), np.array([float(results[i]["stats"][f]) for i in idx]))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -322,6 +346,8 @@ def main():
                     help="headline only: skip the configs 1/3/4 batches, the single calls and the config-5 strong-scaling pass")
     ap.add_argument("--c5", type=int, default=4096, help="problems of the config-5 batch (sharded over the ranks)")
     ap.add_argument("--quick", action="store_true", help="small extras (smoke test of the bench itself)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step of the headline batch computed "
+                    "(models, inlier masks, stats) to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     rank = int(os.environ.get("RANK", "0"))
@@ -356,7 +382,7 @@ def main():
     handles = [cabi.resident_create("relpose", a, b) for a, b in batch]
     res_probs = [dict(kind="relpose", resident=h, n=n, ransac=cabi.RansacOpt(**ropt), max_error=1.0 / G.FOCAL)
                  for h in handles]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -540,28 +566,6 @@ def main():
         k_sec = c_roof["gpu_seconds_score"]
         k_sec_all = c_roof["gpu_seconds"]
         ach = alg_bytes / k_sec / 1e9 if k_sec > 0 else 0.0
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "traffic_scoring_kernel.json")
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get(args.mode, {}).get("dram_bytes_per_launch")
-        # The §8d yardstick is an HBM-read roofline, but the kernel does not stream from HBM: operands are staged once per
-        # CTA into shared memory by TMA and reused by every model.  What actually binds it is the instruction issue rate:
-        # thread-instructions per (model, correspondence) pair from the committed ncu capture x pairs/s vs the SM issue
-        # peak at the measured clock.
-        binding = None
-        try:
-            prof = json.load(open(os.path.join(ROOT, "profiles", "issue_model.json")))[args.mode]
-            pairs_per_s = c_roof["models_evaluated"] * n / k_sec if k_sec > 0 else 0.0
-            clk = (sampler.summary().get("sm_mhz") or 1965.0) * 1e6
-            peak_issue = 148 * 4 * 32 * clk  # thread-instructions/s: 4 warp-instructions per clock per SM
-            binding = {"resource": "instruction issue (fp32 FMA + compare/record per pair), not HBM",
-                       "thread_instr_per_pair": prof["thread_instr_per_pair"], "source": prof["source"],
-                       "pairs_per_s": pairs_per_s, "achieved_thread_instr_per_s": pairs_per_s * prof["thread_instr_per_pair"],
-                       "peak_thread_instr_per_s": peak_issue,
-                       "frac_of_issue_peak": pairs_per_s * prof["thread_instr_per_pair"] / peak_issue,
-                       "whole_step_hbm_frac": (c_res["models_evaluated"] * n * bpc / T_res / 1e9) / peak}
-        except Exception as e:  # noqa: BLE001
-            binding = {"resource": "instruction issue, not HBM", "unavailable": str(e)}
         line = {
             "metric": "RANSAC hypotheses/sec (5pt E, 10k corrs)", "value": hyp / T_res, "unit": "hypotheses/s",
             "scored_corrs_per_s": cor / T_res, "samples_per_s": smp / T_res,
@@ -582,9 +586,10 @@ def main():
                            "ms_per_step": (1e3 * T_other / steps_other) if T_other < 1e29 else None,
                            "results_identical_to_headline_mode": bool(same_o == world),
                            "note": "same resident batch; stats, model bits and inlier masks compared problem by problem"},
-            "roofline": {"bound": "hbm", "binding": binding, "kernel": "k_screen<relpose> (fp32 MSAC screening, TMA-staged SMEM)" if args.mode == "fast"
+            "roofline": {"bound": "hbm", "kernel": "k_screen<relpose> (fp32 MSAC screening, TMA-staged SMEM)" if args.mode == "fast"
                          else "k_score_tiled<relpose> (fp64 MSAC scoring)", "achieved": ach,
-                         "peak": peak, "peak_kind": peak_kind, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+                         "peak": peak, "peak_kind": peak_kind, "unit": "GB/s", "frac": ach / peak,
+                         "whole_step_frac": (c_res["models_evaluated"] * n * bpc / T_res / 1e9) / peak,
                          "bytes_per_scored_corr": bpc,
                          "algorithmic_bytes_per_step": alg_bytes / roof_steps, "kernel_seconds_per_step": k_sec / roof_steps,
                          "solver_kernels_seconds_per_step": (k_sec_all - k_sec - c_roof["gpu_seconds_select"]) / roof_steps,
@@ -596,8 +601,7 @@ def main():
                          "note": "correspondences are SMEM/L2-resident and reused across thousands of models: DRAM "
                                  "traffic << algorithmic bytes by design (SURVEY H7); frac is the SURVEY §8d figure and "
                                  "can exceed 1 for the fp32 screening kernel: its operand stream is served from shared "
-                                 "memory after one TMA stage per CTA, the binding resource is fp32 issue (60 % of the "
-                                 "slots, profiles/r01_v7_summary.md)"},
+                                 "memory after one TMA stage per CTA, so HBM does not bind it"},
             "clocks": sampler.summary(),
         }
         line.update(extras)
@@ -616,6 +620,8 @@ def main():
         except Exception as e:  # the baseline is a reported number, never part of the product path
             line["cpu_baseline"] = {"value": None, "unit": "hypotheses/s", "cores": 0, "kind": "port", "sample": f"failed: {e}"}
         print(json.dumps(line))
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_value)
     for h in handles:
         cabi.resident_free(h)
     if dist is not None:

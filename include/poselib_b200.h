@@ -1,4 +1,4 @@
-/* poselib_b200 — C-ABI of the B200-native LO-RANSAC / minimal-solver engine.
+/* poselib_b200 — C-ABI of the H100-native LO-RANSAC / minimal-solver engine.
  *
  * Drop-in boundary for ONE hot path of PoseLib (reference @ a69263d, paths below are relative to the
  * reference checkout): the LO-RANSAC hypothesis pipeline behind PoseLib/robust.h and PoseLib/solvers/.

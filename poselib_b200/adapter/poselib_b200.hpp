@@ -43,7 +43,7 @@ template <typename RansacOptions> inline plb_ransac_opt to_c(const RansacOptions
     return c;
 }
 // PoseLib/types.h:60-95 -> plb_bundle_opt.  Only NIELSEN/LEVENBERG and the TRIVIAL/TRUNCATED/HUBER/CAUCHY losses are
-// on the B200 path; everything else is rejected loudly instead of being silently approximated.
+// on the CUDA path; everything else is rejected loudly instead of being silently approximated.
 template <typename BundleOptions> inline plb_bundle_opt bundle_to_c(const BundleOptions &o) {
     plb_bundle_opt c;
     c.max_iterations = o.max_iterations;

@@ -1,4 +1,4 @@
-// poselib_dropin.cc — the translation unit a PoseLib maintainer adds to route the ONE hot path to the B200 library.
+// poselib_dropin.cc — the translation unit a PoseLib maintainer adds to route the ONE hot path to the CUDA library.
 //
 // It DEFINES, with exactly the signatures PoseLib's own headers DECLARE, the functions of that path, in namespace poselib:
 //   PoseLib/robust.h          estimate_absolute_pose :45-46, estimate_relative_pose :68-70, estimate_fundamental :112-113,

@@ -1,4 +1,4 @@
-// poselib_b200 — device-side control of a LO-RANSAC round (sm_100a).
+// poselib_b200 — device-side control of a LO-RANSAC round (sm_90a).
 //
 // The serial loop of the reference (robust/ransac_impl.h:157-201) draws a sample, scores its models and compares each
 // with the running best-minimal state.  Here a whole round of iterations is evaluated at once, and these kernels keep

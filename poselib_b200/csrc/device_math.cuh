@@ -1,4 +1,4 @@
-// poselib_b200 — small fp64 vector / quaternion helpers for the device kernels (sm_100a).
+// poselib_b200 — small fp64 vector / quaternion helpers for the device kernels (sm_90a).
 //
 // The whole translation unit is compiled with -fmad=false: fp64 products and sums are rounded separately, like a
 // baseline x86-64 build of the reference (CMakeLists.txt:18,23-27: no -march=native, no fast-math), so that the

@@ -1532,7 +1532,7 @@ static int camera_dev(const plb_camera *c, CamDev *out) {
     case PLB_CAMERA_SIMPLE_RADIAL: np = 4; break;
     case PLB_CAMERA_RADIAL: np = 5; break;
     case PLB_CAMERA_OPENCV: np = 8; break;
-    default: g_err = "NYI: camera model not supported by the B200 path (undistort on the host first)"; return PLB_ERR_NYI;
+    default: g_err = "NYI: camera model not supported by the CUDA path (undistort on the host first)"; return PLB_ERR_NYI;
     }
     out->model = c->model_id;
     for (int i = 0; i < np; ++i) out->p[i] = c->params[i];

@@ -1,4 +1,4 @@
-// poselib_b200 — CUDA kernels of the LO-RANSAC hot path for sm_100a (B200).
+// poselib_b200 — CUDA kernels of the LO-RANSAC hot path for sm_90a (H100).
 //
 //   k_transpose        caller AoS doubles -> SoA fp64 (+ fp32 copy) in HBM, coalesced both ways
 //   k_hyp<KIND>        persistent, one warp = one minimal sample: gather -> minimal solve -> MSAC score of every
@@ -536,8 +536,7 @@ __global__ void __launch_bounds__(HYP_WARPS * 32, 3) k_solve(const RoundDesc R, 
 // p3p and homography_4pt are closed forms without any use for a warp (solvers.cuh: in k_solve all 32 lanes evaluate the
 // same scalar program): here every THREAD solves its own minimal sample — 32 samples per warp instead of one.  Same
 // scalar code, hence the same model bits; the lanes of a warp diverge where their samples take different branches
-// (number of real roots, Newton iterations), which still leaves an order of magnitude over the warp-per-sample kernel
-// (BASELINE config 1: solve kernels 6.1 -> see profiles/r02_summary.md).
+// (number of real roots, Newton iterations).
 template <int KIND>
 __global__ void __launch_bounds__(128) k_solve_lane(const RoundDesc R, HypOut out) {
     static_assert(KIND == KIND_PNP || KIND == KIND_HOMOG, "closed-form solvers only");
@@ -793,8 +792,8 @@ __global__ void __launch_bounds__(K7L_THREADS) k7_solve_lane(const RoundDesc R, 
 }
 
 // ---- relpose_5pt as three phase kernels -------------------------------------------------------------------------
-// The fused warp-per-sample 5-point solver is 181 KB of SASS and runs its Sturm root isolation on one lane; 16 warps
-// per SM at different places of that code starve on instruction fetch (profiles/r01_v2_batch64_summary.md).  The
+// The fused warp-per-sample 5-point solver is a large body of code and runs its Sturm root isolation on one lane; 16
+// warps per SM at different places of that code starve on instruction fetch.  The
 // arithmetic is unchanged, only regrouped so that each kernel's code is small and every phase uses the lanes it can:
 //   k5_prep  : warp  = sample   gather, pivoted-QR nullspace, trace constraints, LU, determinant polynomial
 //   k5_roots : lane  = sample   Sturm bracketing + Ridders/Newton (scalar, data dependent)
@@ -1280,10 +1279,6 @@ PLB_DEV void mbar_wait(uint64_t *bar, uint32_t phase) {
 PLB_DEV void lds_v4(const float *p, float *o) {
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]) : "r"(smem_u32(p)));
 }
-// the same from a 32-bit shared-memory address computed once (base + compile-time offset folds into the instruction)
-PLB_DEV void lds_v4_at(uint32_t addr, float *o) {
-    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]) : "r"(addr));
-}
 PLB_DEV float2 lds_f2(const float2 *p) {
     float2 v;
     asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)));
@@ -1298,7 +1293,7 @@ PLB_DEV float warp_sum_f(float v) {
 // NTHR: threads per CTA.  512 (one CTA per SM next to a 160 KB staging buffer) for the large problems the kernel was
 // shaped for; 128 (four CTAs per SM) for small ones (BASELINE config 1: 200 correspondences), where a 512-thread CTA
 // leaves most threads without a correspondence and the per-tile setup / reduction is what costs.
-template <int KIND, bool PACKED, int NTHR>
+template <int KIND, int NTHR>
 __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const RoundDesc R, HypOut out, int use_smem) {
     constexpr int SCR_THREADS = NTHR, SCR_WARPS = NTHR / 32; // shadow the file-scope defaults
     constexpr int MSZ = kind_model_size(KIND);
@@ -1312,10 +1307,6 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     __shared__ uint32_t red_c[SCR_WARPS][SCR_TM];
     __shared__ uint32_t s_border[SCR_TM];
     __shared__ uint16_t rq[SCR_WARPS][32 * SCR_RQ_TAKE]; // per-warp queue of recorded cases: lane << 8 | bit << 3 | model
-    // packed-fp32 streaming loop (Sampson kinds): the 9 model constants and the two constants of the streaming test,
-    // duplicated (m, m) so that one 64-bit broadcast load feeds both halves of an FFMA2
-    constexpr bool PK = PACKED && (KIND == KIND_RELPOSE || KIND == KIND_FUND);
-    __shared__ __align__(16) float2 ctx2[PK ? SCR_TM : 1][12];
     // ---- static, cost-balanced partition of the round's (problem, tile) list over the CTAs of the grid ------------
     // cost of a tile = correspondences of its problem; CTA c owns the tiles whose start cost lies in
     // [W c / G, W (c+1) / G).  The grid is ONE wave (resident CTAs x SMs), so there is no tail wave; a CTA touches a
@@ -1452,12 +1443,6 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             else if (KIND == KIND_HOMOG) scr::transfer_setup<2>(cp, cm, cm + 2, P.sq_thr, ctx[tid]);
             else scr::sampson_setup(cp, cm, P.sq_thr, ctx[tid]);
             if (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, ctx[tid]);
-            if (PK) {
-#pragma unroll
-                for (int k = 0; k < 9; ++k) ctx2[tid][k] = make_float2(ctx[tid][k], ctx[tid][k]);
-                ctx2[tid][9] = make_float2(ctx[tid][scr::S_THR_X], ctx[tid][scr::S_THR_X]);
-                ctx2[tid][10] = make_float2(ctx[tid][scr::S_BETA_X], ctx[tid][scr::S_BETA_X]);
-            }
         }
         __syncthreads();
         uint32_t cnt[SCR_TM];
@@ -1488,76 +1473,6 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                 uint32_t hit[SCR_TM];
 #pragma unroll
                 for (int i = 0; i < SCR_TM; ++i) hit[i] = 0u;
-                if constexpr (PK) {
-                    // Blackwell packed fp32 (FFMA2): lane-adjacent correspondences (2p, 2p+1) ride in the two halves of
-                    // 64-bit registers; every instruction of the residual evaluates both.  Bit 2j+h of a hit mask is
-                    // correspondence base + 2 (tid + j SCR_THREADS) + h.  The test is scr::sampson_maybe_x.
-                    auto pair_hits = [&](const float2 *M2, float2 a0, float2 a1, float2 b0, float2 b1, uint32_t bx, uint32_t by, uint32_t &h) {
-                        const float2 e0 = __ffma2_rn(M2[0], a0, __ffma2_rn(M2[1], a1, M2[2]));
-                        const float2 e1 = __ffma2_rn(M2[3], a0, __ffma2_rn(M2[4], a1, M2[5]));
-                        const float2 e2 = __ffma2_rn(M2[6], a0, __ffma2_rn(M2[7], a1, M2[8]));
-                        const float2 f0 = __ffma2_rn(M2[0], b0, __ffma2_rn(M2[3], b1, M2[6]));
-                        const float2 f1 = __ffma2_rn(M2[1], b0, __ffma2_rn(M2[4], b1, M2[7]));
-                        const float2 Cn = __ffma2_rn(b0, e0, __ffma2_rn(b1, e1, e2));
-                        const float2 D = __ffma2_rn(e0, e0, __ffma2_rn(e1, e1, __ffma2_rn(f0, f0, __fmul2_rn(f1, f1))));
-                        const float2 q = __fmul2_rn(Cn, Cn);
-                        const float2 rhs = __ffma2_rn(M2[9], D, M2[10]);
-                        if (q.x <= rhs.x) h |= bx; // predicated ORs
-                        if (q.y <= rhs.y) h |= by;
-                    };
-                    // the 11 duplicated constants of a model: six 128-bit loads (ctx2 rows are 16-byte aligned, 12 float2)
-                    const uint32_t ctx2_addr = smem_u32(&ctx2[0][0]);
-                    auto load_m2 = [&](int i, float2 *M2) {
-                        float t[24];
-#pragma unroll
-                        for (int k = 0; k < 6; ++k) lds_v4_at(ctx2_addr + (uint32_t)(i * 96 + k * 16), t + 4 * k);
-#pragma unroll
-                        for (int k = 0; k < 11; ++k) M2[k] = make_float2(t[2 * k], t[2 * k + 1]);
-                    };
-                    // FULL: the tile holds SCR_TM models (all but the last tile of a problem) -> no per-model bound checks
-                    auto stream = [&](auto full_c) {
-                    constexpr bool FULL = decltype(full_c)::value;
-                    int p0 = tid; // pair index inside the chunk
-                    uint32_t sh = 0;
-                    const int npairs = (lim - base + 1) >> 1;
-                    for (; p0 + SCR_THREADS < npairs; p0 += 2 * SCR_THREADS, sh += 4) {
-                        float2 pa[2][4];
-#pragma unroll
-                        for (int j = 0; j < 2; ++j) {
-                            const int k = base + 2 * (p0 + j * SCR_THREADS);
-#pragma unroll
-                            for (int c = 0; c < 4; ++c) pa[j][c] = *reinterpret_cast<const float2 *>(arr[c] + k);
-                        }
-                        const uint32_t q0 = 1u << sh, q1 = 2u << sh, q2 = 4u << sh, q3 = 8u << sh;
-#pragma unroll
-                        for (int i = 0; i < SCR_TM; ++i) {
-                            if (FULL || i < tm) {
-                                float2 M2[11];
-                                load_m2(i, M2);
-                                pair_hits(M2, pa[0][0], pa[0][1], pa[0][2], pa[0][3], q0, q1, hit[i]);
-                                pair_hits(M2, pa[1][0], pa[1][1], pa[1][2], pa[1][3], q2, q3, hit[i]);
-                            }
-                        }
-                    }
-                    for (; p0 < npairs; p0 += SCR_THREADS, sh += 2) { // remainder
-                        const int k = base + 2 * p0;
-                        float2 pa[4];
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) pa[c] = *reinterpret_cast<const float2 *>(arr[c] + k);
-                        const uint32_t q0 = 1u << sh, q1 = 2u << sh;
-#pragma unroll
-                        for (int i = 0; i < SCR_TM; ++i) {
-                            if (FULL || i < tm) {
-                                float2 M2[11];
-                                load_m2(i, M2);
-                                pair_hits(M2, pa[0], pa[1], pa[2], pa[3], q0, q1, hit[i]);
-                            }
-                        }
-                    }
-                    };
-                    if (tm == SCR_TM) stream(std::true_type{});
-                    else stream(std::false_type{});
-                } else {
                 int k0 = base + tid;
                 uint32_t qbit = 1u;
                 for (; k0 + (SCR_PB - 1) * SCR_THREADS < lim; k0 += SCR_THREADS * SCR_PB, qbit <<= SCR_PB) {
@@ -1592,7 +1507,6 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                             if (maybe(ctx[i], p)) hit[i] |= qbit;
                         }
                     }
-                }
                 }
                 // Handling of the recorded cases, compacted across the WARP: the lanes list their cases (model, bit, lane)
                 // in a per-warp queue in shared memory — at most SCR_RQ_TAKE per lane and pass, so the queue cannot
@@ -1634,15 +1548,14 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                     for (int eidx = lane; eidx < total; eidx += 32) {
                         const uint32_t ent = rq[warp][eidx];
                         const int mi = (int)(ent & 7u), q = (int)((ent >> 3) & 31u), otid = warp * 32 + (int)(ent >> 8);
-                        const int k = PK ? base + 2 * (otid + (q >> 1) * SCR_THREADS) + (q & 1) : base + otid + q * SCR_THREADS;
+                        const int k = base + otid + q * SCR_THREADS;
                         float p[NARR];
 #pragma unroll
                         for (int c = 0; c < NARR; ++c) p[c] = arr[c][k];
                         const float *M = ctx[mi];
                         bool plain = false, border = false;
                         float v = 0.f, e = 0.f;
-                        if (PK && k >= n) { // second half of the last pair of an odd-sized problem: padding, not data
-                        } else if (KIND == KIND_PNP) {
+                        if (KIND == KIND_PNP) {
                             scr::transfer_point<true>(M, scr::pnp_terms(M, p[0], p[1], p[2], p[3], p[4]), plain, border, v, e);
                         } else if (KIND == KIND_HOMOG) {
                             scr::transfer_point<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]), plain, border, v, e);
@@ -1779,7 +1692,7 @@ static int sm_count() {
     if (cached[dev] == 0) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        cached[dev] = n > 0 ? n : 148;
+        cached[dev] = n > 0 ? n : 132;
     }
     return cached[dev];
 }
@@ -1933,17 +1846,11 @@ static void launch_hyp_t(const RoundDesc &R, int *work, const HypOut &out, int m
         const int use_smem = bytes <= 200 * 1024 ? 1 : 0;
         static bool attr_done_dev[MAX_DEVICES] = {false};
         bool &attr_done = attr_done_dev[cur_dev()];
-        static const bool packed = [] { // Blackwell FFMA2 streaming loop for the Sampson kinds (PLB_SCREEN_PACKED=0/1)
-            const char *e = std::getenv("PLB_SCREEN_PACKED");
-            return e ? std::atoi(e) != 0 : true;
-        }();
         const bool small = max_n_pad <= 2048; // few correspondences per problem: 128-thread CTAs, four per SM
-        auto kern = small ? (packed ? k_screen<KIND, true, 128> : k_screen<KIND, false, 128>)
-                          : (packed ? k_screen<KIND, true, 512> : k_screen<KIND, false, 512>);
+        auto kern = small ? k_screen<KIND, 128> : k_screen<KIND, 512>;
         const int nthr = small ? 128 : 512;
         if (!attr_done) {
-            cudaFuncSetAttribute(k_screen<KIND, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-            cudaFuncSetAttribute(k_screen<KIND, false, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            cudaFuncSetAttribute(k_screen<KIND, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
             attr_done = true;
         }
         // one wave: resident CTAs per SM (occupancy API for this shared-memory size) x SMs; the kernel partitions the
@@ -2887,8 +2794,7 @@ __global__ void __launch_bounds__(LM_THREADS / MINB, MINB)
 // CTAs of k_lm per SM.  k_lm needs ~255 registers per thread.  1: 256 threads, one CTA (one job, or one slice of a job's
 // cluster) per SM.  2 (PLB_LM_MINB=2): 128 threads per CTA, still 255 registers, two CTAs per SM — every job gets half the
 // threads but twice as many jobs are in flight; the LM passes are latency bound (few correspondences per thread, a
-// cluster-wide reduction and a scalar solve per iteration).  (A 256-thread build capped at 128 registers was measured
-// and rejected: its spills cost more than the second resident CTA gained, profiles/r02_summary.md.)
+// cluster-wide reduction and a scalar solve per iteration).
 static int lm_minb() {
     static const int minb = [] {
         const char *e = std::getenv("PLB_LM_MINB");

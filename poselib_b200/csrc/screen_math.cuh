@@ -63,7 +63,6 @@ SCR_HD float fast_rsqrt(float x) {
 
 // ---- layout of one model's constants in shared memory (floats) -----------------------------------------------
 constexpr int CTX_FLOATS = 28;
-constexpr double SAMPSON_XI = 1.0 / 256.0; // slack of the |C|-free streaming test: residuals up to 0.2 % over the threshold
 // [0..15]  the model: 3x3 row-major (E / F / H) [+ q(4), t(3) for relpose]  |  3x4 row-major [R t] for pnp
 enum {
     // Sampson kinds (relpose, fundamental)
@@ -76,8 +75,6 @@ enum {
     S_ERR_K = 22,   // 4 beta + 2 thr beta_D   (constant part of the per-point score error numerator)
     S_DMIN = 23,    // 4 beta_D: below this denominator nothing can be said about the residual
     S_EH = 24,      // relpose: bound of the fp32 error of lambda - min_depth (cheirality test)
-    S_THR_X = 25,   // packed streaming test: thr^ (1 + 24u) / (1 - 24u - xi) (1 + 4u)
-    S_BETA_X = 26,  //                        (beta + alpha^2 / (4 xi)) / (1 - 24u - xi) (1 + 4u)
     // transfer kinds (homography, pnp): | d | < thr_s * w
     T_THRS_P = 16,  // prefilter: sqrt(thr) rounded up (1 + 8u)
     T_C_P = 17,     //            c (1 + 8u),  c = e_d + thr_s e_w
@@ -126,12 +123,6 @@ SCR_HD void sampson_setup(const double *M, const float *cmax, double sq_thr, flo
     ctx[S_BETA_P] = f_up(beta * (1.0 + 64.0 * Ud));
     ctx[S_ERR_K] = f_up((4.0 * beta + 2.0 * thr_hi * betaD) * (1.0 + 8.0 * Ud));
     ctx[S_DMIN] = f_up(4.0 * betaD);
-    // Variant of the streaming test without |C| (used by the packed-fp32 loop, which has no abs modifier):
-    // alpha |C| <= xi C^2 + alpha^2 / (4 xi), so  num (1 - kappa - xi) - beta - alpha^2/(4 xi) <= t (1 + kappa)  holds
-    // for every correspondence that is not provably an outlier; evaluated as  C C <= fma(thr_x, D, beta_x).
-    const double xi = SAMPSON_XI, den = 1.0 - 24.0 * Ud - xi;
-    ctx[S_THR_X] = f_up((double)thr * (1.0 + 24.0 * Ud) / den * (1.0 + 4.0 * Ud));
-    ctx[S_BETA_X] = f_up((beta + alpha * alpha / (4.0 * xi)) / den * (1.0 + 4.0 * Ud));
 }
 struct SampsonTerms {
     float C, D;
@@ -154,11 +145,6 @@ SCR_HD bool sampson_maybe(const float *ctx, float a0, float a1, float b0, float 
     const SampsonTerms T = sampson_terms(ctx, a0, a1, b0, b1);
     const float g = fmaf(-ctx[S_ALPHA_P], fabsf(T.C), fmaf(T.C, T.C, -ctx[S_BETA_P]));
     return g <= ctx[S_THR_P] * T.D;
-}
-// The same without |C| (see sampson_setup): what the packed-fp32 loop of k_screen evaluates two correspondences at a time.
-SCR_HD bool sampson_maybe_x(const float *ctx, float a0, float a1, float b0, float b1) {
-    const SampsonTerms T = sampson_terms(ctx, a0, a1, b0, b1);
-    return T.C * T.C <= fmaf(ctx[S_THR_X], T.D, ctx[S_BETA_X]);
 }
 // Full evaluation of one correspondence the streaming pass could not rule out.
 //   plain  : the fp32 decision num < t (what count32 / score32 use)

@@ -1,9 +1,9 @@
 // relpose_5pt, first half (nullspace, trace / determinant constraints, elimination, determinant polynomial) with ONE
 // THREAD PER MINIMAL SAMPLE.
 //
-// The group-of-8 version (solve_5pt_poly_grp8, solvers.cuh) spends ~56 k thread-instructions per sample: most steps are
+// The group-of-8 version (solve_5pt_poly_grp8, solvers.cuh) spends most of its instructions on narrow steps: most are
 // 5..20 wide, the lanes of a group repeat the index arithmetic, and every value travels through shared memory
-// (k5_prep: 74 % of the LSU wavefront peak, profiles/r02_summary.md).  Here a thread owns a sample: the monomial tables
+// (k5_prep is bound by shared-memory traffic).  Here a thread owns a sample: the monomial tables
 // are compile-time constants, so the nullspace basis and the quadratic blocks live in registers with static indices and
 // only the 10 x 20 elimination matrix (dynamic pivot rows) sits in the thread's slice of shared memory.  Every value is
 // produced by the same sequence of IEEE operations as in solve_5pt_poly / the CPU restatement (the file is compiled

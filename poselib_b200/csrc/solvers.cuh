@@ -764,8 +764,8 @@ PLB_DEV int sturm_bisect10(const double *coeffs, double *roots, SturmWork *w) {
 }
 
 // ---- warp-cooperative variant used by k5_roots: lane = sample, 32 samples per warp ------------------------------------
-// sturm_bisect10 run by 32 lanes on 32 different polynomials diverges badly (3.8 active lanes per instruction,
-// profiles/r01_v7_summary.md): every lane is at a different point of the interval walk or inside a Ridders/Newton
+// sturm_bisect10 run by 32 lanes on 32 different polynomials diverges badly: every lane is at a different point of the
+// interval walk or inside a Ridders/Newton
 // refinement.  The same computation is regrouped into phases that keep the warp converged:
 //   A  Sturm sequence of every lane's polynomial (uniform);
 //   B  interval walk: cheap transitions (pop / split bookkeeping / emit) advance until the lane needs ONE
@@ -1194,8 +1194,8 @@ PLB_DEV void solve_5pt_poly(const double *x1s, const double *x2s, Scratch5 *S, c
 }
 
 // ---- the same first half, FOUR samples per warp (k5_prep) ------------------------------------------------------------
-// Most steps of solve_5pt_poly have 4..20-way parallelism, so a whole warp per sample leaves most lanes idle (7.7 k
-// warp-instructions per sample, profiles/r01_v4_summary.md).  Here lanes [8s, 8s+8) own sample s: the serial steps
+// Most steps of solve_5pt_poly have 4..20-way parallelism, so a whole warp per sample leaves most lanes idle.  Here
+// lanes [8s, 8s+8) own sample s: the serial steps
 // (pivoted QR, LU pivots, back substitution) advance four samples per instruction, and the table-driven steps map a
 // lane to a MONOMIAL (its factor tables live in registers) instead of to a matrix entry.  Every element is computed
 // by the same sequence of operations as in solve_5pt_poly / the reference, so the outputs are bit-identical.

@@ -1,4 +1,4 @@
-"""`poselib`-compatible Python call surface for the B200 path (SURVEY.md §8f row N4).
+"""`poselib`-compatible Python call surface for the CUDA path (SURVEY.md §8f row N4).
 
 Mirrors the signatures, option dictionaries and `(model, info)` returns of the reference's pybind module
 (/root/reference/pybind/bindings/estimators/{absolute_pose.cc:317-330, relative_pose.cc:405-463, homography.cc:75-77},
@@ -58,7 +58,7 @@ def _camera(cam):
     name = str(cam["model"]).upper()
     if name not in _CAMERA_IDS:
         # unknown ids raise inside the library exactly like Camera::unproject's "NYI" (camera_models.cc:184-185)
-        raise cabi.PoseLibB200Error(cabi.PLB_ERR_NYI, f"NYI: camera model {name} is not on the B200 path")
+        raise cabi.PoseLibB200Error(cabi.PLB_ERR_NYI, f"NYI: camera model {name} is not on the CUDA path")
     return cabi.Camera(name, tuple(cam["params"]), int(cam.get("width", 0)), int(cam.get("height", 0)))
 
 
@@ -81,7 +81,7 @@ def _ransac(d):
 
 
 def _bundle(d):
-    """update_bundle_options (helpers.h:42-95); options the B200 path does not implement are rejected loudly."""
+    """update_bundle_options (helpers.h:42-95); options the CUDA path does not implement are rejected loudly."""
     kw = {}
     if "max_iterations" in d:
         kw["max_iterations"] = int(d["max_iterations"])
@@ -95,7 +95,7 @@ def _bundle(d):
             raise cabi.PoseLibB200Error(cabi.PLB_ERR_NYI, f"NYI: loss_type {lt}")
         kw["loss_type"] = lt
     if str(d.get("lambda_update", "NIELSEN")).upper() != "NIELSEN" or str(d.get("damping", "LEVENBERG")).upper() != "LEVENBERG":
-        raise cabi.PoseLibB200Error(cabi.PLB_ERR_NYI, "NYI: only NIELSEN / LEVENBERG are on the B200 path")
+        raise cabi.PoseLibB200Error(cabi.PLB_ERR_NYI, "NYI: only NIELSEN / LEVENBERG are on the CUDA path")
     return kw
 
 
@@ -110,7 +110,7 @@ def RansacOptions(opt=None):
 
 def BundleOptions(opt=None):
     """poselib.BundleOptions(opt={}) (types.cc:22-28,169): defaults of PoseLib/types.h:60-95, keys of helpers.h:185-235.
-    Values the B200 path does not implement (FIXED_FACTOR, MARQUARDT, TRUNCATED_CAUCHY / TRUNCATED_LE_ZACH) raise NYI."""
+    Values the CUDA path does not implement (FIXED_FACTOR, MARQUARDT, TRUNCATED_CAUCHY / TRUNCATED_LE_ZACH) raise NYI."""
     opt = dict(opt or {})
     out = {"max_iterations": 100, "loss_scale": 1.0, "loss_type": "CAUCHY", "gradient_tol": 1e-12, "step_tol": 1e-8,
            "relative_cost_tol": 1e-10, "initial_lambda": 1e-3, "min_lambda": 1e-10, "max_lambda": 1e10,

@@ -15,7 +15,7 @@ NEEDS_LIB = {"test_a_device_control.py", "test_cabi_exports.py", "test_gpu_parit
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     # Several test modules import the C-ABI binding at collection time; it refuses to load without the in-tree library.
     # A fresh checkout that runs pytest before __graft_entry__.build() would otherwise fail to collect.
     if not (os.path.exists(LIB) and os.path.exists(os.path.join(ROOT, "oracle", "_build", "libplo.so"))):

@@ -2,8 +2,8 @@
 // poselib_b200/adapter/poselib_dropin.cc + libposelib_b200.so instead of PoseLib's CPU sources for the hot path
 // (tests/test_dropin_reference_headers.py; Eigen is replaced by the test stand-in oracle/ref/mini at compile time because
 // this image has no Eigen3).  Linking succeeds only if the drop-in defines every function below with exactly the
-// signature PoseLib's headers declare.   ./_dropin_client       -> link check only
-//                                         ./_dropin_client run   -> one call of every entry point on cuda:0
+// signature PoseLib's headers declare.   oracle/_ref/dropin_client       -> link check only
+//                                         oracle/_ref/dropin_client run   -> one call of every entry point on cuda:0
 #include <PoseLib/robust.h>
 #include <PoseLib/robust/bundle.h>
 #include <PoseLib/robust/ransac.h>
@@ -100,7 +100,7 @@ int main(int argc, char **argv) {
         return 0;
     }
 
-    // ---- run: PoseLib call sites, B200 implementation ------------------------------------------------------------
+    // ---- run: PoseLib call sites, CUDA implementation ------------------------------------------------------------
     const double f = 1000.0;
     Camera cam(1 /* PINHOLE */, std::vector<double>{f, f, 0.0, 0.0});
     Scene sc = make_scene(2000, 0.5, 1, false);

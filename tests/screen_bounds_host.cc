@@ -110,9 +110,8 @@ void scr_check_sampson(int kind, int n, const double *pts, const double *M, cons
             T.s64 += r2;
         }
         const float fa0 = f[k], fa1 = f[(size_t)n + k], fb0 = f[2 * (size_t)n + k], fb1 = f[3 * (size_t)n + k];
-        const bool mb = sampson_maybe(ctx, fa0, fa1, fb0, fb1), mbx = sampson_maybe_x(ctx, fa0, fa1, fb0, fb1);
-        if ((!mb || !mbx) && r2 < sq_thr) ++T.viol_point; // ruled out although the fp64 residual is under the threshold
-        if (mb && !mbx) ++T.viol_point;                    // the |C|-free test must be the wider one
+        const bool mb = sampson_maybe(ctx, fa0, fa1, fb0, fb1);
+        if (!mb && r2 < sq_thr) ++T.viol_point; // ruled out although the fp64 residual is under the threshold
         if (!mb) continue;
         ++T.maybe;
         bool plain, border;

@@ -26,7 +26,7 @@ CAMERAS = [
 def exe():
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
-    subprocess.check_call(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-ffp-contract=off", "-o", EXE,
+    subprocess.check_call(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-ffp-contract=off", "-o", EXE,
                            os.path.join(HERE, "camera_host_test.cu")])
     return EXE
 

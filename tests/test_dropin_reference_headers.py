@@ -10,14 +10,14 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = "/root/reference"
-EXE = os.path.join(ROOT, "tests", "_dropin_client")
+EXE = os.path.join(ROOT, "oracle", "_ref", "dropin_client")
 
 pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "PoseLib")), reason="needs the reference's headers")
 
 
 def test_dropin_defines_poselibs_own_declarations():
     import __graft_entry__ as ge
-    ge.build()  # builds the library and, where the reference is mounted, tests/_dropin_client (build_dropin_client)
+    ge.build()  # builds the library and, where the reference is mounted, oracle/_ref/dropin_client (build_dropin_client)
     out = subprocess.run([EXE], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and "dropin link ok: 19 PoseLib entry points resolved" in out.stdout, out.stdout + out.stderr
 
@@ -26,7 +26,7 @@ def test_the_same_client_passes_on_poselibs_own_cpu_implementation():
     """The client's `run` mode (one PoseLib-style call of every estimate_*, ransac_relpose, refine_relpose, relpose_5pt on
     synthetic scenes with ground truth, with accuracy / inlier-count checks) is first held to PoseLib ITSELF: linked with the
     reference's own sources (the mini-Eigen build, `make -C oracle ref2`) instead of the drop-in, it must pass.  The GPU
-    test (tests/test_zz_golden_reference_gpu.py) then runs the identical client on the B200 backend."""
+    test (tests/test_zz_golden_reference_gpu.py) then runs the identical client on the CUDA backend."""
     import glob
     subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "ref2"], stdout=subprocess.DEVNULL,
                           stderr=subprocess.DEVNULL)

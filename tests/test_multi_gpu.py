@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def cabi():
     from poselib_b200 import cabi as c
     if c.device_count() == 0:
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device: the GPU tests need a CUDA device")
     c.set_device(0)
     return c
 

@@ -17,7 +17,7 @@ EXE = os.path.join(HERE, "_solver5_lane_host_test")
 def exe():
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
-    subprocess.check_call(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.check_call(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_90a,code=sm_90a",
                            "-Xcompiler", "-ffp-contract=off", "-o", EXE, os.path.join(HERE, "solver5_lane_host_test.cu")])
     return EXE
 

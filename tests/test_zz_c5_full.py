@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_all_4096_config5_problems_match_the_oracle():
     from poselib_b200 import cabi
     if cabi.device_count() == 0:
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device: the GPU tests need a CUDA device")
     cabi.set_device(0)
     gold = np.load(os.path.join(ROOT, "tests", "golden", "c5_oracle.npz"))
     count = len(gold["iterations"])

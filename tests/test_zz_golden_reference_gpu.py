@@ -22,7 +22,7 @@ GOLD = json.load(open(os.path.join(HERE, "golden", "reference_sources.json")))["
 def test_cuda_path_reproduces_the_reference_sources_fixtures(name):
     from poselib_b200 import cabi
     if cabi.device_count() == 0:
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device: the GPU tests need a CUDA device")
     cabi.set_device(0)
     case, gold = RC.CASES[name](), GOLD[name]
     RC.check(RC.run(cabi, case), gold, case["kind"], model_tol=2e-6, score_rtol=2e-9)
@@ -39,7 +39,7 @@ def test_cuda_refiners_reproduce_the_reference_sources_refinements(kind, loss):
     the oracle reproduces these fixtures bit for bit on the CPU)."""
     from poselib_b200 import cabi
     if cabi.device_count() == 0:
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device: the GPU tests need a CUDA device")
     cabi.set_device(0)
     for (m0, a, b, kw), gold in zip(RC.refine_cases(kind, loss), REFINE[f"{kind}/{loss}"]):
         m, bs = cabi.refine(kind, m0, a, b, cabi.BundleOpt(**kw))
@@ -58,7 +58,7 @@ def test_cuda_solvers_reproduce_the_reference_sources_solver_outputs(name):
     import numpy as np
     from poselib_b200 import cabi
     if cabi.device_count() == 0:
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device: the GPU tests need a CUDA device")
     cabi.set_device(0)
     a, b = RC.solver_instances(name)
     fn = {"p3p": cabi.p3p_batch, "p3p_lambdatwist": cabi.p3p_lambdatwist_batch, "relpose_7pt": cabi.relpose_7pt_batch, "homography_4pt": cabi.homography_4pt_batch}[name]
@@ -83,9 +83,9 @@ def test_poselib_client_runs_on_the_b200_backend():
     libposelib_b200.so instead: every estimate_*, ransac_relpose, refine_relpose and relpose_5pt call goes through PoseLib's
     declared signatures into the CUDA path.  The binary is built in the CPU container (it needs the reference's headers)."""
     import subprocess
-    exe = os.path.join(HERE, "_dropin_client")
+    exe = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "dropin_client")
     if not os.path.exists(exe):
-        pytest.skip("tests/_dropin_client was not built (needs /root/reference; run the CPU test-suite or build() first)")
+        pytest.skip("oracle/_ref/dropin_client was not built (build() builds it where the reference's headers are)")
     out = subprocess.run([exe, "run"], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "dropin run ok" in out.stdout, out.stdout + out.stderr
 

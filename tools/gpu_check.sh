@@ -1,6 +1,6 @@
 #!/bin/bash
-# One gpurun call that validates a tree on the B200 box and brings the evidence back in gpurun_out/:
-#   /usr/local/graft/bin/gpurun --timeout 1500 -- 'bash tools/gpu_check.sh'
+# Validates a built tree on an H100 and collects the evidence in the output directory it creates:
+#   bash tools/gpu_check.sh        (from the repository root)
 # 1. the whole GPU test-suite (oracle parity first, then the reference-sources fixtures), 2. bench fast + exact,
 # 3. the ncu launch list of one fast-mode bench step.  Every stage has its own timeout so a hang cannot eat the box.
 mkdir -p gpurun_out
