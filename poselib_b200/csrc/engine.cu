@@ -3,7 +3,7 @@
 // The reference runs one serial loop per problem (robust/ransac_impl.h:157-201).  Its sample sequence is a pure
 // function of (seed, N, sample size, PROSAC options) and neither scoring nor refinement touch the RNG, so the engine
 //   1. generates the sample table for a whole round of iterations on the host (robust/sampling.cc restated below),
-//   2. lets the GPU solve + score every sample of the round (one warp per sample, kernels.cu),
+//   2. lets the GPU solve + score every sample of the round (one thread per minimal solve, kernels.cu),
 //   3. finds, from the per-model (inlier count, MSAC score) records, every model that improves the best-minimal
 //      state — that sub-sequence does not depend on LO results — and refines all of them in one batched LM launch,
 //   4. replays score_models() (ransac_impl.h:106-154) in iteration order over those records, which reproduces the
@@ -1127,9 +1127,9 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         launch_sample(E.rp.p, na, E.smp.p + (size_t)smp_cur * NP, E.smp.p + (size_t)(smp_cur ^ 1) * NP, E.samples.p, st);
         E.launches++;
         mark(PH_SAMPLE);
-        launch_hypotheses(kind, R, E.work.p, out, mode, max_n_pad, st, E.ev2);
+        launch_hypotheses(kind, R, out, mode, max_n_pad, st, E.ev2);
         PLB_CUDA(cudaEventRecord(E.ev1, st));
-        E.launches += kind_is_relpose(kind) ? 5 : 2; // k_solve (or k5_gather + k5_prep_lane + k5_roots + k5_back) + scoring
+        E.launches += kind_is_relpose(kind) ? 5 : 2; // one solve kernel (5pt: k5_gather, k5_prep_lane, k5_roots, k5_back) + scoring
         SelectArgs SA;
         SA.rp = E.rp.p;
         SA.na = na;
@@ -1945,15 +1945,25 @@ static int solver_batch(int kind, int variant, size_t count, const double *a, si
     Engine &E = *engine();
     int rc = E.init();
     if (rc != PLB_OK) return rc;
-    DevBuf<double> da, db, dout;
-    DevBuf<int> dn;
+    DevBuf<double> da, db, dout, s5_blk, s5_park, s5_cpoly, s5_roots;
+    DevBuf<int> dn, s5_nroots;
     if ((rc = da.ensure(count * a_sz)) || (rc = db.ensure(count * b_sz)) || (rc = dout.ensure(count * out_sz)) ||
         (rc = dn.ensure(count)))
         return rc;
+    HypOut s5{};
+    if (kind == KIND_RELPOSE) { // phase buffers of the 5-point solver, laid out as in a round of `count` samples
+        if ((rc = s5_blk.ensure(count * 105)) || (rc = s5_park.ensure(count * 100)) || (rc = s5_cpoly.ensure(count * 11)) ||
+            (rc = s5_roots.ensure(count * 10)) || (rc = s5_nroots.ensure(count)))
+            return rc;
+        s5.s5_blk = s5_blk.p;
+        s5.s5_park = s5_park.p;
+        s5.s5_cpoly = s5_cpoly.p;
+        s5.s5_roots = s5_roots.p;
+        s5.s5_nroots = s5_nroots.p;
+    }
     PLB_CUDA(cudaMemcpyAsync(da.p, a, sizeof(double) * count * a_sz, cudaMemcpyHostToDevice, E.stream));
     PLB_CUDA(cudaMemcpyAsync(db.p, b, sizeof(double) * count * b_sz, cudaMemcpyHostToDevice, E.stream));
-    launch_solver_batch(kind, variant, count, da.p, db.p, dout.p, dn.p, flags, E.stream);
-    E.launches++;
+    E.launches += launch_solver_batch(kind, variant, count, da.p, db.p, dout.p, dn.p, flags, s5, E.stream);
     PLB_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * count * out_sz, cudaMemcpyDeviceToHost, E.stream));
     PLB_CUDA(cudaMemcpyAsync(n_out, dn.p, sizeof(int) * count, cudaMemcpyDeviceToHost, E.stream));
     PLB_CUDA(cudaStreamSynchronize(E.stream));

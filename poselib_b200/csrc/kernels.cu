@@ -1,13 +1,16 @@
 // poselib_b200 — CUDA kernels of the LO-RANSAC hot path for sm_90a (H100).
 //
 //   k_transpose        caller AoS doubles -> SoA fp64 (+ fp32 copy) in HBM, coalesced both ways
-//   k_hyp<KIND>        persistent, one warp = one minimal sample: gather -> minimal solve -> MSAC score of every
-//                      model over all correspondences (lanes stride the SoA arrays, warp-shuffle reduction)
+//   k_solve_lane<KIND> / k7_solve_lane / k5_gather -> k5_prep_lane -> k5_roots -> k5_back
+//                      minimal solvers of a round, one thread per minimal sample (the 5-point solver in phases)
+//   k_score_tiled / k_screen
+//                      MSAC scoring of every model of a round over all correspondences (exact fp64 / fp32 screening)
 //   k_score_models     exact rescoring of explicit models (initial model, fast-mode confirmation)
 //   k_lm<KIND>         Levenberg-Marquardt refit (LO step + final polish): one CTA per job, block-wide reductions of
 //                      the normal equations, scalar LM logic on thread 0
 //   k_inlier_mask      final inlier masks
-//   k_solver_batch     the solvers/*.h surface: one warp per instance
+//   k_solver_batch     the solvers/*.h surface: one thread per instance (relpose_5pt: k5_load -> k5_prep_lane ->
+//                      k5_roots -> k5_solver_out)
 //
 // Compiled with -fmad=false (see device_math.cuh).  Reference citations are relative to /root/reference.
 #include "kernels.cuh"
@@ -383,95 +386,8 @@ PLB_DEV void cta_score(const ProblemDev &P, const double *model, double sq_thr, 
 }
 
 // ============================================================================================================
-// fused hypothesis kernel
+// hypothesis kernels: one minimal solve per thread
 // ============================================================================================================
-constexpr int HYP_WARPS = 8;
-
-template <int KIND> struct HypScratch;
-template <> struct HypScratch<KIND_PNP> {
-    double models[4 * 7];
-};
-template <> struct HypScratch<KIND_RELPOSE> {
-    Scratch5 s5;
-    double xs[30]; // x1s[15], x2s[15]
-    double models[40 * 7];
-};
-template <> struct HypScratch<KIND_FUND> {
-    Scratch7 s7;
-    double xs[42];
-    double models[3 * 9];
-};
-template <> struct HypScratch<KIND_HOMOG> {
-    double models[9];
-};
-
-// Gathers the sample and runs the minimal solver; models land in W->models.  Returns the number of models.
-template <int KIND>
-PLB_DEV int warp_generate_models(const ProblemDev &P, const uint32_t *sample, HypScratch<KIND> *W,
-                                 const MonoTables *T, int lane) {
-    if (KIND == KIND_PNP) {
-        d3 xs[3], Xs[3];
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            const uint32_t id = sample[i];
-            xs[i] = bearing(P.p[0][id], P.p[1][id]);
-            Xs[i] = mk(P.p[2][id], P.p[3][id], P.p[4][id]);
-        }
-        return solve_p3p(xs, Xs, reinterpret_cast<double *>(W), lane);
-    } else if (KIND == KIND_HOMOG) {
-        d3 a[4], b[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const uint32_t id = sample[i];
-            a[i] = bearing(P.p[0][id], P.p[1][id]);
-            b[i] = bearing(P.p[2][id], P.p[3][id]);
-        }
-        return solve_h4(a, b, reinterpret_cast<double *>(W), lane, true);
-    } else if (KIND == KIND_RELPOSE) {
-        HypScratch<KIND_RELPOSE> *S = reinterpret_cast<HypScratch<KIND_RELPOSE> *>(W);
-        if (lane < 10) {
-            const int i = lane % 5, side = lane / 5;
-            const uint32_t id = sample[i];
-            const d3 v = bearing(P.p[2 * side][id], P.p[2 * side + 1][id]);
-            double *o = S->xs + 15 * side + 3 * i;
-            o[0] = v.x; o[1] = v.y; o[2] = v.z;
-        }
-        __syncwarp();
-        return solve_5pt_poses(S->xs, S->xs + 15, &S->s5, T, S->models, lane);
-    } else {
-        HypScratch<KIND_FUND> *S = reinterpret_cast<HypScratch<KIND_FUND> *>(W);
-        if (lane < 14) {
-            const int i = lane % 7, side = lane / 7;
-            const uint32_t id = sample[i];
-            const d3 v = bearing(P.p[2 * side][id], P.p[2 * side + 1][id]);
-            double *o = S->xs + 21 * side + 3 * i;
-            o[0] = v.x; o[1] = v.y; o[2] = v.z;
-        }
-        __syncwarp();
-        int nm = solve_7pt(S->xs, S->xs + 21, &S->s7, S->models, lane);
-        if (P.rfc) {
-            // estimators/relative_pose.cc:393-398: drop models failing the real-focal check, order preserved
-            bool keep = false;
-            double f[9];
-            if (lane < nm) {
-#pragma unroll
-                for (int k = 0; k < 9; ++k) f[k] = S->models[9 * lane + k];
-                keep = rfc_ok(f);
-            }
-            const unsigned km = __ballot_sync(0xffffffffu, keep);
-            __syncwarp();
-            if (keep) {
-                const int pos = __popc(km & ((1u << lane) - 1u));
-#pragma unroll
-                for (int k = 0; k < 9; ++k) S->models[9 * pos + k] = f[k];
-            }
-            __syncwarp();
-            nm = __popc(km);
-        }
-        return nm;
-    }
-}
-
 PLB_DEV int sample_problem_slot(const RoundDesc &R, int g) {
     int lo = 0, hi = R.n_active - 1;
     while (lo < hi) {
@@ -482,61 +398,10 @@ PLB_DEV int sample_problem_slot(const RoundDesc &R, int g) {
     return lo;
 }
 
-// Solve kernel: persistent, one warp = one minimal sample of one problem of the group.  Models are appended to a
-// compact list (slot range reserved with one atomicAdd per sample); n_models[g] / first_slot[g] let the host walk them
-// in (sample, model) order per problem.
-template <int KIND>
-__global__ void __launch_bounds__(HYP_WARPS * 32, 3) k_solve(const RoundDesc R, int *work_counter, HypOut out) {
-    constexpr int K = (KIND == KIND_PNP) ? 3 : (KIND == KIND_RELPOSE) ? 5 : (KIND == KIND_FUND) ? 7 : 4;
-    constexpr int MSZ = kind_model_size(KIND);
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MonoTables *T = reinterpret_cast<MonoTables *>(smem_raw);
-    HypScratch<KIND> *Wall = reinterpret_cast<HypScratch<KIND> *>(smem_raw + 256);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    HypScratch<KIND> *W = Wall + warp;
-    if (KIND == KIND_RELPOSE) {
-        fill_tables(T);
-        __syncthreads();
-    }
-    for (;;) {
-        int g = 0;
-        if (lane == 0) g = atomicAdd(work_counter, 1);
-        g = __shfl_sync(0xffffffffu, g, 0);
-        if (g >= R.n_total) break;
-        const int aslot = sample_problem_slot(R, g);
-        const int pidx = __ldg(R.active + aslot);
-        const ProblemDev &P = R.probs[pidx];
-        uint32_t sample[K];
-#pragma unroll
-        for (int i = 0; i < K; ++i) sample[i] = R.samples[(size_t)g * K + i];
-        int nm = warp_generate_models<KIND>(P, sample, W, T, lane);
-        int base = 0;
-        if (lane == 0) {
-            if (nm) {
-                const int loc = atomicAdd(out.prob_count + aslot, nm);
-                if (loc + nm > __ldg(out.seg_cap + aslot)) { // cannot happen with the worst-case capacity; the engine
-                    atomicExch(out.overflow, 1);             // redoes the round with it when the optimistic one fails
-                    nm = 0;
-                }
-                base = __ldg(out.seg_base + aslot) + loc;
-            }
-            out.n_models[g] = nm;
-            out.first_slot[g] = base;
-        }
-        base = __shfl_sync(0xffffffffu, base, 0);
-        nm = __shfl_sync(0xffffffffu, nm, 0);
-        const double *models = W->models;
-        for (int e = lane; e < nm * MSZ; e += 32) out.models[(size_t)base * MSZ + e] = models[e];
-        if (lane < nm) out.model_prob[base + lane] = pidx;
-        for (int m = 32 + lane; m < nm; m += 32) out.model_prob[base + m] = pidx;
-        __syncwarp();
-    }
-}
-
-// p3p and homography_4pt are closed forms without any use for a warp (solvers.cuh: in k_solve all 32 lanes evaluate the
-// same scalar program): here every THREAD solves its own minimal sample — 32 samples per warp instead of one.  Same
-// scalar code, hence the same model bits; the lanes of a warp diverge where their samples take different branches
-// (number of real roots, Newton iterations).
+// p3p and homography_4pt: every thread solves its own minimal sample with the scalar closed form; the lanes of a warp
+// diverge where their samples take different branches (number of real roots, Newton iterations).  Models are appended
+// to the problem's segment (slot range reserved with one atomicAdd per sample); n_models[g] / first_slot[g] let the
+// ordered scans walk them in (sample, model) order per problem.
 template <int KIND>
 __global__ void __launch_bounds__(128) k_solve_lane(const RoundDesc R, HypOut out) {
     static_assert(KIND == KIND_PNP || KIND == KIND_HOMOG, "closed-form solvers only");
@@ -557,7 +422,7 @@ __global__ void __launch_bounds__(128) k_solve_lane(const RoundDesc R, HypOut ou
             xs[i] = bearing(P.p[0][id], P.p[1][id]);
             Xs[i] = mk(P.p[2][id], P.p[3][id], P.p[4][id]);
         }
-        nm = solve_p3p(xs, Xs, models, 0, false);
+        nm = solve_p3p(xs, Xs, models);
     } else {
         d3 a[4], b[4];
 #pragma unroll
@@ -566,7 +431,7 @@ __global__ void __launch_bounds__(128) k_solve_lane(const RoundDesc R, HypOut ou
             a[i] = bearing(P.p[0][id], P.p[1][id]);
             b[i] = bearing(P.p[2][id], P.p[3][id]);
         }
-        nm = solve_h4(a, b, models, 0, true, false);
+        nm = solve_h4(a, b, models, true);
     }
     if (!live) return;
     int base = 0;
@@ -587,111 +452,8 @@ __global__ void __launch_bounds__(128) k_solve_lane(const RoundDesc R, HypOut ou
     }
 }
 
-// relpose_7pt with FOUR minimal samples per warp (8 lanes each), like k5_prep: the pivoted-QR nullspace of the 9 x 7
-// system is the group-of-8 routine of the 5-point solver (one lane per column), the cubic in the pencil of the two
-// nullspace vectors and its roots are scalar (every lane of the group evaluates them, lanes 0..2 build one F each), the
-// real-focal check keeps the surviving models in order (estimators/relative_pose.cc:393-398).  Same arithmetic as the
-// warp-per-sample solve_7pt (solvers.cuh), a quarter of the warps.
-constexpr int P7_M = 0, P7_N = 63, P7_XS = 81, P7_OUT = 123, P7_STRIDE = 152; // 152 = 8 (mod 16): see P5_STRIDE
-constexpr size_t K7_SMEM = sizeof(double) * P7_STRIDE * 4 * HYP_WARPS;
-__global__ void __launch_bounds__(HYP_WARPS * 32) k7_solve(const RoundDesc R, int *work_counter, HypOut out) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int lane = threadIdx.x & 31, sl = lane & 7, grp = lane >> 3;
-    double *W = reinterpret_cast<double *>(smem_raw) + (size_t)((threadIdx.x >> 5) * 4 + grp) * P7_STRIDE;
-    const unsigned gmask = 0xffu << (8 * grp);
-    for (;;) {
-        int g0 = 0;
-        if (lane == 0) g0 = atomicAdd(work_counter, 4);
-        g0 = __shfl_sync(0xffffffffu, g0, 0);
-        if (g0 >= R.n_total) break;
-        int g = g0 + grp;
-        const bool live = g < R.n_total;
-        if (!live) g = R.n_total - 1; // idle groups redo the last sample (uniform control flow), nothing is stored
-        const int aslot = sample_problem_slot(R, g);
-        const int pidx = __ldg(R.active + aslot);
-        const ProblemDev &P = R.probs[pidx];
-        double *x1s = W + P7_XS, *x2s = W + P7_XS + 21;
-        for (int idx = sl; idx < 14; idx += 8) {
-            const int i = idx % 7, side = idx / 7;
-            const uint32_t id = R.samples[(size_t)g * 7 + i];
-            const d3 v = bearing(P.p[2 * side][id], P.p[2 * side + 1][id]);
-            double *o = W + P7_XS + 21 * side + 3 * i;
-            o[0] = v.x; o[1] = v.y; o[2] = v.z;
-        }
-        __syncwarp();
-        for (int e = sl; e < 63; e += 8) {
-            const int i = e / 9, k = e % 9;
-            W[P7_M + e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
-        }
-        __syncwarp();
-        grp8_nullspace_9xC<7>(W + P7_M, W + P7_N, sl);
-        const double *n0 = W + P7_N, *n1 = W + P7_N + 9;
-        // mixed determinants: column j of the 3x3 (col-major 9-vector) taken from a, b, c respectively
-        auto detc = [](const double *a, const double *b, const double *c) -> double {
-            const double *c0 = a, *c1 = b + 3, *c2 = c + 6;
-            return c0[0] * (c1[1] * c2[2] - c1[2] * c2[1]) - c1[0] * (c0[1] * c2[2] - c0[2] * c2[1]) +
-                   c2[0] * (c0[1] * c1[2] - c0[2] * c1[1]);
-        };
-        const double c3 = detc(n0, n0, n0);
-        const double c2 = detc(n1, n0, n0) + detc(n0, n1, n0) + detc(n0, n0, n1);
-        const double c1 = detc(n0, n1, n1) + detc(n1, n0, n1) + detc(n1, n1, n0);
-        const double c0 = detc(n1, n1, n1);
-        double roots[3];
-        int n_roots;
-        if (fabs(c3) < 1e-14) {
-            n_roots = quadratic_real(c2, c1, c0, roots);
-        } else {
-            const double inv_c3 = 1.0 / c3;
-            n_roots = cubic_real(c2 * inv_c3, c1 * inv_c3, c0 * inv_c3, roots);
-        }
-        bool keep = false;
-        double f[9];
-        if (sl < n_roots) {
-            double r = roots[0];
-            if (sl == 1) r = roots[1];
-            if (sl == 2) r = roots[2];
-            double n2 = 0.0;
-#pragma unroll
-            for (int k = 0; k < 9; ++k) {
-                f[k] = n0[k] * r + n1[k];
-                n2 += f[k] * f[k];
-            }
-            if (n2 > 0) {
-                const double nn = sqrt(n2);
-#pragma unroll
-                for (int k = 0; k < 9; ++k) f[k] /= nn;
-            }
-            keep = P.rfc ? rfc_ok(f) : true;
-        }
-        const unsigned km = __ballot_sync(0xffffffffu, keep) & gmask;
-        const int nm_all = __popc(km);
-        int nm = nm_all, base = 0;
-        if (sl == 0 && live) {
-            if (nm) {
-                const int loc = atomicAdd(out.prob_count + aslot, nm);
-                if (loc + nm > __ldg(out.seg_cap + aslot)) { // cannot happen: this kind uses the worst-case capacity
-                    atomicExch(out.overflow, 1);
-                    nm = 0;
-                }
-                base = __ldg(out.seg_base + aslot) + loc;
-            }
-            out.n_models[g] = nm;
-            out.first_slot[g] = base;
-        }
-        base = __shfl_sync(0xffffffffu, base, 8 * grp);
-        nm = __shfl_sync(0xffffffffu, nm, 8 * grp);
-        if (keep && live && nm) {
-            const int pos = base + __popc(km & ((1u << lane) - 1u));
-#pragma unroll
-            for (int k = 0; k < 9; ++k) out.models[(size_t)pos * 9 + k] = f[k];
-            out.model_prob[pos] = pidx;
-        }
-        __syncwarp();
-    }
-}
-
-// relpose_7pt with ONE THREAD PER SAMPLE: the scalar nullspace routine of solver5_lane.cuh on a 63-double slice of shared
-// memory (odd stride: conflict-free), the rest is the scalar code of k7_solve.  Same arithmetic, same model bits.
+// relpose_7pt with ONE THREAD PER SAMPLE: fundamental_7pt on a 63-double slice of shared memory per thread (odd stride:
+// conflict-free).
 constexpr int K7L_THREADS = 256;
 constexpr int K7L_STRIDE = 63;
 constexpr size_t K7L_SMEM = sizeof(double) * K7L_STRIDE * K7L_THREADS;
@@ -704,73 +466,18 @@ __global__ void __launch_bounds__(K7L_THREADS) k7_solve_lane(const RoundDesc R, 
     const int aslot = sample_problem_slot(R, g);
     const int pidx = __ldg(R.active + aslot);
     const ProblemDev &P = R.probs[pidx];
-    {
-        double x1s[21], x2s[21];
+    double x1s[21], x2s[21];
 #pragma unroll
-        for (int i = 0; i < 7; ++i) {
-            const uint32_t id = R.samples[(size_t)g * 7 + i];
-            const d3 a = bearing(P.p[0][id], P.p[1][id]), b = bearing(P.p[2][id], P.p[3][id]);
-            x1s[3 * i] = a.x; x1s[3 * i + 1] = a.y; x1s[3 * i + 2] = a.z;
-            x2s[3 * i] = b.x; x2s[3 * i + 1] = b.y; x2s[3 * i + 2] = b.z;
-        }
-#pragma unroll
-        for (int e = 0; e < 63; ++e) {
-            const int i = e / 9, k = e % 9;
-            W[e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
-        }
+    for (int i = 0; i < 7; ++i) {
+        const uint32_t id = R.samples[(size_t)g * 7 + i];
+        const d3 a = bearing(P.p[0][id], P.p[1][id]), b = bearing(P.p[2][id], P.p[3][id]);
+        x1s[3 * i] = a.x; x1s[3 * i + 1] = a.y; x1s[3 * i + 2] = a.z;
+        x2s[3 * i] = b.x; x2s[3 * i + 1] = b.y; x2s[3 * i + 2] = b.z;
     }
-    double nn[18];
-    lane5::nullspace_9xC<7>(W, nn);
-    const double *n0 = nn, *n1 = nn + 9;
-    // mixed determinants: column j of the 3x3 (col-major 9-vector) taken from a, b, c respectively
-    auto detc = [](const double *a, const double *b, const double *c) -> double {
-        const double *c0 = a, *c1 = b + 3, *c2 = c + 6;
-        return c0[0] * (c1[1] * c2[2] - c1[2] * c2[1]) - c1[0] * (c0[1] * c2[2] - c0[2] * c2[1]) +
-               c2[0] * (c0[1] * c1[2] - c0[2] * c1[1]);
-    };
-    const double c3 = detc(n0, n0, n0);
-    const double c2 = detc(n1, n0, n0) + detc(n0, n1, n0) + detc(n0, n0, n1);
-    const double c1 = detc(n0, n1, n1) + detc(n1, n0, n1) + detc(n1, n1, n0);
-    const double c0 = detc(n1, n1, n1);
-    double roots[3];
-    int n_roots;
-    if (fabs(c3) < 1e-14) {
-        n_roots = quadratic_real(c2, c1, c0, roots);
-    } else {
-        const double inv_c3 = 1.0 / c3;
-        n_roots = cubic_real(c2 * inv_c3, c1 * inv_c3, c0 * inv_c3, roots);
-    }
-    if (!live) return;
     double F[3][9];
-    int nm = 0;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        if (j < n_roots) {
-            const double r = roots[j];
-            double f[9];
-            double n2 = 0.0;
-#pragma unroll
-            for (int k = 0; k < 9; ++k) {
-                f[k] = n0[k] * r + n1[k];
-                n2 += f[k] * f[k];
-            }
-            if (n2 > 0) {
-                const double nrm = sqrt(n2);
-#pragma unroll
-                for (int k = 0; k < 9; ++k) f[k] /= nrm;
-            }
-            if (P.rfc ? rfc_ok(f) : true) {
-                // nm is 0, 1 or 2 here: predicated copies keep F in registers
-#pragma unroll
-                for (int m = 0; m < 3; ++m)
-                    if (m == nm) {
-#pragma unroll
-                        for (int k = 0; k < 9; ++k) F[m][k] = f[k];
-                    }
-                ++nm;
-            }
-        }
-    }
+    // P.rfc is read after the solve (loaded up front, it would stay live across the nullspace routine)
+    int nm = fundamental_7pt(x1s, x2s, W, [&](const double *f) { return P.rfc ? rfc_ok(f) : true; }, F);
+    if (!live) return;
     int base = 0;
     if (nm) {
         const int loc = atomicAdd(out.prob_count + aslot, nm);
@@ -791,61 +498,15 @@ __global__ void __launch_bounds__(K7L_THREADS) k7_solve_lane(const RoundDesc R, 
         }
 }
 
-// ---- relpose_5pt as three phase kernels -------------------------------------------------------------------------
-// The fused warp-per-sample 5-point solver is a large body of code and runs its Sturm root isolation on one lane; 16
-// warps per SM at different places of that code starve on instruction fetch.  The
-// arithmetic is unchanged, only regrouped so that each kernel's code is small and every phase uses the lanes it can:
-//   k5_prep  : warp  = sample   gather, pivoted-QR nullspace, trace constraints, LU, determinant polynomial
-//   k5_roots : lane  = sample   Sturm bracketing + Ridders/Newton (scalar, data dependent)
-//   k5_back  : lane  = (sample, root)  back-substitution, motion decomposition, cheirality; 3 samples per warp
+// ---- relpose_5pt as phase kernels ----------------------------------------------------------------------------------
+// The 5-point solver is a large body of code; as one kernel, warps at different places of it starve on instruction
+// fetch.  Split into phases, each kernel's code is small and every phase maps its threads to the work it has:
+//   k5_gather    : thread = sample          the sample's bearings
+//   k5_prep_lane : thread = sample          pivoted-QR nullspace, trace constraints, LU, determinant polynomial
+//   k5_roots     : lane   = sample          Sturm bracketing + Ridders/Newton, warp-cooperative
+//   k5_back      : lane   = (sample, root)  back-substitution, motion decomposition, cheirality
+// The solver surface (k5_load, k5_solver_out) runs k5_prep_lane and k5_roots on the caller's instances.
 constexpr int S5_BLK = 105;
-
-constexpr int PREP_SAMPLES_PER_WARP = 4;
-constexpr size_t PREP_SMEM = 256 + sizeof(double) * P5_STRIDE * PREP_SAMPLES_PER_WARP * HYP_WARPS;
-__global__ void __launch_bounds__(HYP_WARPS * 32) k5_prep(const RoundDesc R, int *work_counter, HypOut out) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MonoTables *T = reinterpret_cast<MonoTables *>(smem_raw);
-    const int lane = threadIdx.x & 31, sl = lane & 7, grp = lane >> 3;
-    double *W = reinterpret_cast<double *>(smem_raw + 256) +
-                (size_t)((threadIdx.x >> 5) * PREP_SAMPLES_PER_WARP + grp) * P5_STRIDE;
-    fill_tables(T);
-    __syncthreads();
-    for (;;) {
-        int g0 = 0;
-        if (lane == 0) g0 = atomicAdd(work_counter, PREP_SAMPLES_PER_WARP);
-        g0 = __shfl_sync(0xffffffffu, g0, 0);
-        if (g0 >= R.n_total) break;
-        int g = g0 + grp;
-        const bool live = g < R.n_total;
-        if (!live) g = R.n_total - 1; // idle groups redo the last sample (uniform control flow), nothing is stored
-        const ProblemDev &P = R.probs[__ldg(R.active + sample_problem_slot(R, g))];
-        // bearings of the 5 sampled correspondences (estimators/relative_pose.cc:51-54,90-94)
-        for (int idx = sl; idx < 10; idx += 8) {
-            const int i = idx % 5, side = idx / 5;
-            const uint32_t id = R.samples[(size_t)g * 5 + i];
-            d3 v;
-            if (P.kind == KIND_RELPOSE_TS) {
-                const double *t = P.ts + (size_t)(3 * side) * P.n_pad + id;
-                v = mk(t[0], t[P.n_pad], t[2 * (size_t)P.n_pad]);
-            } else {
-                v = bearing(P.p[2 * side][id], P.p[2 * side + 1][id]);
-            }
-            double *o = W + P5_XS + 15 * side + 3 * i;
-            o[0] = v.x; o[1] = v.y; o[2] = v.z;
-        }
-        __syncwarp();
-        solve_5pt_poly_grp8(W, T, sl);
-        if (live) {
-            double *blk = out.s5_blk + g; // entry-major: blk[e * n_total]
-            const size_t nt = (size_t)R.n_total;
-            for (int e = sl; e < 39; e += 8) blk[e * nt] = W[P5_A + e];
-            for (int e = sl; e < 36; e += 8) blk[(39 + e) * nt] = W[P5_NB + e];
-            for (int e = sl; e < 30; e += 8) blk[(75 + e) * nt] = W[P5_XS + e];
-            for (int k = sl; k < 11; k += 8) out.s5_cpoly[(size_t)k * R.n_total + g] = W[P5_CPOLY + k];
-        }
-        __syncwarp();
-    }
-}
 
 // Bearings of the 5 sampled correspondences of every sample (estimators/relative_pose.cc:51-54,90-94) into the
 // entry-major per-sample block (entries 75..104).  Its chain of dependent global loads (problem slot -> problem ->
@@ -878,7 +539,7 @@ __global__ void __launch_bounds__(256) k5_gather(const RoundDesc R, HypOut out) 
     }
 }
 
-// The same phase with ONE THREAD PER SAMPLE (solver5_lane.cuh): the nullspace basis and the quadratic blocks live in
+// First half with ONE THREAD PER SAMPLE (solver5_lane.cuh): the nullspace basis and the quadratic blocks live in
 // registers (compile-time monomial tables); shared memory holds only the LEFT 10 x 10 block of the elimination matrix
 // (dynamic pivot rows) plus 10 doubles of scratch per thread, the right-hand sides are parked in global memory (L2)
 // while the block is factored and come back column by column.  111 doubles per thread (odd: the 32 lanes of a warp
@@ -886,7 +547,7 @@ __global__ void __launch_bounds__(256) k5_gather(const RoundDesc R, HypOut out) 
 constexpr int PREPL_THREADS = 256;
 constexpr int PREPL_STRIDE = 111;
 constexpr size_t PREPL_SMEM = sizeof(double) * PREPL_STRIDE * PREPL_THREADS;
-template <int UNR>
+// Of R, only n_total is read.  (With an int parameter in its place the compiler schedules this kernel differently.)
 __global__ void __launch_bounds__(PREPL_THREADS, 1) k5_prep_lane(const RoundDesc R, HypOut out) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *W = reinterpret_cast<double *>(smem_raw) + (size_t)threadIdx.x * PREPL_STRIDE;
@@ -926,7 +587,7 @@ __global__ void __launch_bounds__(PREPL_THREADS, 1) k5_prep_lane(const RoundDesc
     }
     int idx[10];
     lane5::lu_left(CL, S, idx);
-    lane5::solve_rhs<UNR>(CL, S, idx, [&](int r, int c) { return park[(size_t)(r * 10 + c) * nt]; }, CL);
+    lane5::solve_rhs(CL, S, idx, [&](int r, int c) { return park[(size_t)(r * 10 + c) * nt]; }, CL);
     double A[39], cp[11];
     lane5::poly_matrix(CL, A);
 #pragma unroll
@@ -1676,8 +1337,6 @@ __global__ void __launch_bounds__(SCORE_THREADS, 4)
     }
 }
 
-template <int KIND> static size_t hyp_smem_bytes() { return 256 + sizeof(HypScratch<KIND>) * HYP_WARPS; }
-
 // Occupancy figures and opt-in attributes are per device: the caches below are indexed by the current device so that a
 // process driving several GPUs (plb_set_device from different threads) configures each of them.
 constexpr int MAX_DEVICES = 64;
@@ -1697,18 +1356,6 @@ static int sm_count() {
     return cached[dev];
 }
 
-template <int KIND> static int solve_blocks_per_sm() {
-    static int cached_dev[MAX_DEVICES] = {0};
-    int &cached = cached_dev[cur_dev()];
-    if (cached <= 0) {
-        const size_t smem = hyp_smem_bytes<KIND>();
-        cudaFuncSetAttribute(k_solve<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int nb = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_solve<KIND>, HYP_WARPS * 32, smem);
-        cached = nb > 0 ? nb : 1;
-    }
-    return cached;
-}
 template <int KIND> static int score_blocks_per_sm() {
     static int cached_dev[MAX_DEVICES] = {0};
     int &cached = cached_dev[cur_dev()];
@@ -1721,115 +1368,37 @@ template <int KIND> static int score_blocks_per_sm() {
 }
 int device_sm_count() { return sm_count(); }
 
-static int prep_blocks_per_sm() {
-    static int cached_dev[MAX_DEVICES] = {0};
-    int &cached = cached_dev[cur_dev()];
-    if (cached <= 0) {
-        const size_t smem = PREP_SMEM;
-        cudaFuncSetAttribute(k5_prep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int nb = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k5_prep, HYP_WARPS * 32, smem);
-        cached = nb > 0 ? nb : 1;
+// relpose_5pt first half and root isolation of the R.n_total samples whose bearings are in out.s5_blk (entries
+// 75..104): the round chain and the solver surface both run them through here.
+static void launch_5pt_prep_roots(const RoundDesc &R, const HypOut &out, cudaStream_t stream) {
+    static bool attr_set[MAX_DEVICES] = {false};
+    if (!attr_set[cur_dev()]) {
+        cudaFuncSetAttribute(k5_prep_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PREPL_SMEM);
+        attr_set[cur_dev()] = true;
     }
-    return cached;
+    const int n = R.n_total;
+    k5_prep_lane<<<(unsigned)((n + PREPL_THREADS - 1) / PREPL_THREADS), PREPL_THREADS, PREPL_SMEM, stream>>>(R, out);
+    k5_roots<<<(n + ROOTS_THREADS - 1) / ROOTS_THREADS, ROOTS_THREADS, 0, stream>>>(n, out);
 }
 
 template <int KIND>
-static void launch_hyp_t(const RoundDesc &R, int *work, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
+static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
                          cudaEvent_t ev_between) {
-    // persistent grids: a multiple of the SM count (resident CTAs per SM from the occupancy API), never more CTAs
-    // than there is work for
     if constexpr (KIND == KIND_RELPOSE_TS) mode = 0; // no fp32 screening copy of the 18-array layout: exact scoring
-    if (kind_is_relpose(KIND) && (KIND == KIND_RELPOSE_TS || out.s5_blk != nullptr)) {
-        // first half: one thread per sample (PLB_PREP_LANE=0: four samples per warp, k5_prep)
-        static const bool lane_prep = [] {
-            const char *e = std::getenv("PLB_PREP_LANE");
-            return e ? std::atoi(e) != 0 : true;
-        }();
-        if (lane_prep) {
-            static const int unr = [] {
-                const char *e = std::getenv("PLB_PREP_UNR"); // columns of the right-hand side solved per loop pass
-                return e ? std::atoi(e) : 1;
-            }();
-            static bool attr_set[MAX_DEVICES] = {false};
-            if (!attr_set[cur_dev()]) {
-                cudaFuncSetAttribute(k5_prep_lane<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PREPL_SMEM);
-                cudaFuncSetAttribute(k5_prep_lane<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PREPL_SMEM);
-                attr_set[cur_dev()] = true;
-            }
-            k5_gather<<<(R.n_total + 255) / 256, 256, 0, stream>>>(R, out);
-            const unsigned grid = (unsigned)((R.n_total + PREPL_THREADS - 1) / PREPL_THREADS);
-            if (unr == 1) k5_prep_lane<1><<<grid, PREPL_THREADS, PREPL_SMEM, stream>>>(R, out);
-            else k5_prep_lane<2><<<grid, PREPL_THREADS, PREPL_SMEM, stream>>>(R, out);
-        } else {
-            int blocks = prep_blocks_per_sm() * sm_count();
-            const int per_cta = HYP_WARPS * PREP_SAMPLES_PER_WARP;
-            const int need = (R.n_total + per_cta - 1) / per_cta;
-            if (blocks > need) blocks = need;
-            if (blocks < 1) blocks = 1;
-            k5_prep<<<blocks, HYP_WARPS * 32, PREP_SMEM, stream>>>(R, work, out);
-        }
-        k5_roots<<<(R.n_total + ROOTS_THREADS - 1) / ROOTS_THREADS, ROOTS_THREADS, 0, stream>>>(R.n_total, out);
+    if constexpr (kind_is_relpose(KIND)) {
+        k5_gather<<<(R.n_total + 255) / 256, 256, 0, stream>>>(R, out);
+        launch_5pt_prep_roots(R, out, stream);
         const int warps = (R.n_total + 31) / 32;
         k5_back<<<(warps * 32 + 127) / 128, 128, 0, stream>>>(R, out);
-    } else if constexpr (KIND == KIND_PNP || KIND == KIND_HOMOG) {
-        // closed-form solvers: one thread per minimal sample (PLB_SOLVE_LANE=0: the warp-per-sample kernel)
-        static const bool lane_solve = [] {
-            const char *e = std::getenv("PLB_SOLVE_LANE");
-            return e ? std::atoi(e) != 0 : true;
-        }();
-        if (lane_solve) {
-            k_solve_lane<KIND><<<(R.n_total + 127) / 128, 128, 0, stream>>>(R, out);
-        } else {
-            int blocks = solve_blocks_per_sm<KIND>() * sm_count();
-            const int need = (R.n_total + HYP_WARPS - 1) / HYP_WARPS;
-            if (blocks > need) blocks = need;
-            if (blocks < 1) blocks = 1;
-            k_solve<KIND><<<blocks, HYP_WARPS * 32, hyp_smem_bytes<KIND>(), stream>>>(R, work, out);
-        }
     } else if constexpr (KIND == KIND_FUND) {
-        // relpose_7pt: one thread per sample (PLB_SOLVE7_LANE=0: four samples per warp; PLB_SOLVE7_GRP=0: the
-        // warp-per-sample kernel)
-        static const bool lane7 = [] {
-            const char *e = std::getenv("PLB_SOLVE7_LANE");
-            return e ? std::atoi(e) != 0 : true;
-        }();
-        static const bool grp7 = [] {
-            const char *e = std::getenv("PLB_SOLVE7_GRP");
-            return e ? std::atoi(e) != 0 : true;
-        }();
-        if (lane7) {
-            static bool attr_set[MAX_DEVICES] = {false};
-            if (!attr_set[cur_dev()]) {
-                cudaFuncSetAttribute(k7_solve_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K7L_SMEM);
-                attr_set[cur_dev()] = true;
-            }
-            k7_solve_lane<<<(R.n_total + K7L_THREADS - 1) / K7L_THREADS, K7L_THREADS, K7L_SMEM, stream>>>(R, out);
-        } else if (grp7) {
-            static int per_sm_dev[MAX_DEVICES] = {0};
-            int &per_sm = per_sm_dev[cur_dev()];
-            if (per_sm <= 0) {
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k7_solve, HYP_WARPS * 32, K7_SMEM);
-                if (per_sm < 1) per_sm = 1;
-            }
-            int blocks = per_sm * sm_count();
-            const int need = (R.n_total + 4 * HYP_WARPS - 1) / (4 * HYP_WARPS);
-            if (blocks > need) blocks = need;
-            if (blocks < 1) blocks = 1;
-            k7_solve<<<blocks, HYP_WARPS * 32, K7_SMEM, stream>>>(R, work, out);
-        } else {
-            int blocks = solve_blocks_per_sm<KIND>() * sm_count();
-            const int need = (R.n_total + HYP_WARPS - 1) / HYP_WARPS;
-            if (blocks > need) blocks = need;
-            if (blocks < 1) blocks = 1;
-            k_solve<KIND><<<blocks, HYP_WARPS * 32, hyp_smem_bytes<KIND>(), stream>>>(R, work, out);
+        static bool attr_set[MAX_DEVICES] = {false};
+        if (!attr_set[cur_dev()]) {
+            cudaFuncSetAttribute(k7_solve_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K7L_SMEM);
+            attr_set[cur_dev()] = true;
         }
-    } else if constexpr (KIND != KIND_RELPOSE_TS) {
-        int blocks = solve_blocks_per_sm<KIND>() * sm_count();
-        const int need = (R.n_total + HYP_WARPS - 1) / HYP_WARPS;
-        if (blocks > need) blocks = need;
-        if (blocks < 1) blocks = 1;
-        k_solve<KIND><<<blocks, HYP_WARPS * 32, hyp_smem_bytes<KIND>(), stream>>>(R, work, out);
+        k7_solve_lane<<<(R.n_total + K7L_THREADS - 1) / K7L_THREADS, K7L_THREADS, K7L_SMEM, stream>>>(R, out);
+    } else {
+        k_solve_lane<KIND><<<(R.n_total + 127) / 128, 128, 0, stream>>>(R, out);
     }
     if (ev_between) cudaEventRecord(ev_between, stream); // solve | score boundary for the per-kernel timing
     if (mode == 0) {
@@ -1865,16 +1434,15 @@ static void launch_hyp_t(const RoundDesc &R, int *work, const HypOut &out, int m
         kern<<<gx, nthr, use_smem ? bytes : 0, stream>>>(R, out, use_smem);
     }
 }
-void launch_hypotheses(int kind, const RoundDesc &R, int *work, const HypOut &out, int mode, int max_n_pad,
-                       cudaStream_t stream, cudaEvent_t ev_between) {
-    cudaMemsetAsync(work, 0, 3 * sizeof(int), stream); // [0] sample queue, [2] overflow flag
+void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
+                       cudaEvent_t ev_between) {
     cudaMemsetAsync(out.prob_count, 0, sizeof(int) * R.n_active, stream);
     switch (kind) {
-    case KIND_PNP: launch_hyp_t<KIND_PNP>(R, work, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_RELPOSE: launch_hyp_t<KIND_RELPOSE>(R, work, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_FUND: launch_hyp_t<KIND_FUND>(R, work, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_RELPOSE_TS: launch_hyp_t<KIND_RELPOSE_TS>(R, work, out, mode, max_n_pad, stream, ev_between); break;
-    default: launch_hyp_t<KIND_HOMOG>(R, work, out, mode, max_n_pad, stream, ev_between); break;
+    case KIND_PNP: launch_hyp_t<KIND_PNP>(R, out, mode, max_n_pad, stream, ev_between); break;
+    case KIND_RELPOSE: launch_hyp_t<KIND_RELPOSE>(R, out, mode, max_n_pad, stream, ev_between); break;
+    case KIND_FUND: launch_hyp_t<KIND_FUND>(R, out, mode, max_n_pad, stream, ev_between); break;
+    case KIND_RELPOSE_TS: launch_hyp_t<KIND_RELPOSE_TS>(R, out, mode, max_n_pad, stream, ev_between); break;
+    default: launch_hyp_t<KIND_HOMOG>(R, out, mode, max_n_pad, stream, ev_between); break;
     }
 }
 void launch_score_list(int kind, const ProblemDev *probs, const double *models, const int *model_prob, const int *slots,
@@ -3061,98 +2629,149 @@ void launch_eightpt(size_t count, int n, const double *x1, const double *x2, int
 }
 
 // ============================================================================================================
-// direct solver surface: one warp per instance
+// direct solver surface (solvers/*.h): one thread per instance, the solver code of the round kernels
 // ============================================================================================================
-// variant: 0 = native output (p3p poses / 5pt E / 7pt F / H), 1 = 5pt poses / p3p_lambdatwist
+// p3p (variant 0) / p3p_lambdatwist (variant 1), homography_4pt and relpose_7pt; every output slot is written, unused
+// ones with zeros.  relpose_7pt runs without the real-focal check.
 template <int KIND, int VARIANT>
-__global__ void __launch_bounds__(HYP_WARPS * 32)
+__global__ void __launch_bounds__(K7L_THREADS)
     k_solver_batch(size_t count, const double *__restrict__ a, const double *__restrict__ b, double *out, int *n_out,
                    int flags) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MonoTables *T = reinterpret_cast<MonoTables *>(smem_raw);
-    HypScratch<KIND> *W = reinterpret_cast<HypScratch<KIND> *>(smem_raw + 256) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (KIND == KIND_RELPOSE) {
-        fill_tables(T);
-        __syncthreads();
-    }
-    const size_t gw = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((size_t)gridDim.x * blockDim.x) >> 5;
-    for (size_t i = gw; i < count; i += nw) {
-        if (KIND == KIND_PNP) {
-            d3 xs[3], Xs[3];
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    if constexpr (KIND == KIND_PNP) {
+        d3 xs[3], Xs[3];
 #pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                xs[k] = mk(a[9 * i + 3 * k], a[9 * i + 3 * k + 1], a[9 * i + 3 * k + 2]);
-                Xs[k] = mk(b[9 * i + 3 * k], b[9 * i + 3 * k + 1], b[9 * i + 3 * k + 2]);
-            }
-            double *models = reinterpret_cast<double *>(W);
-            const int n = (VARIANT == 1) ? solve_p3p_lambdatwist(xs, Xs, models, lane) : solve_p3p(xs, Xs, models, lane);
-            if (lane < 28) out[28 * i + lane] = (lane < 7 * n) ? models[lane] : 0.0;
-            if (lane == 0) n_out[i] = n;
-        } else if (KIND == KIND_HOMOG) {
-            d3 xa[4], xb[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                xa[k] = mk(a[12 * i + 3 * k], a[12 * i + 3 * k + 1], a[12 * i + 3 * k + 2]);
-                xb[k] = mk(b[12 * i + 3 * k], b[12 * i + 3 * k + 1], b[12 * i + 3 * k + 2]);
-            }
-            double *models = reinterpret_cast<double *>(W);
-            const int n = solve_h4(xa, xb, models, lane, flags != 0);
-            if (lane < 9) out[9 * i + lane] = n ? models[lane] : 0.0;
-            if (lane == 0) n_out[i] = n;
-        } else if (KIND == KIND_RELPOSE) {
-            HypScratch<KIND_RELPOSE> *S = reinterpret_cast<HypScratch<KIND_RELPOSE> *>(W);
-            if (lane < 30) S->xs[lane] = (lane < 15) ? a[15 * i + lane] : b[15 * i + lane - 15];
-            __syncwarp();
-            if (VARIANT == 0) {
-                const int n = solve_5pt_E(S->xs, S->xs + 15, &S->s5, T, lane);
-                for (int e = lane; e < 90; e += 32) {
-                    const int m = e / 9, k = e % 9; // output column-major
-                    out[90 * i + e] = (m < n) ? S->s5.Es[9 * m + 3 * (k % 3) + k / 3] : 0.0;
-                }
-                if (lane == 0) n_out[i] = n;
-            } else {
-                const int n = solve_5pt_poses(S->xs, S->xs + 15, &S->s5, T, S->models, lane);
-                for (int e = lane; e < 280; e += 32) out[280 * i + e] = (e < 7 * n) ? S->models[e] : 0.0;
-                if (lane == 0) n_out[i] = n;
-            }
-        } else {
-            HypScratch<KIND_FUND> *S = reinterpret_cast<HypScratch<KIND_FUND> *>(W);
-            for (int e = lane; e < 42; e += 32) S->xs[e] = (e < 21) ? a[21 * i + e] : b[21 * i + e - 21];
-            __syncwarp();
-            const int n = solve_7pt(S->xs, S->xs + 21, &S->s7, S->models, lane);
-            if (lane < 27) out[27 * i + lane] = (lane < 9 * n) ? S->models[lane] : 0.0;
-            if (lane == 0) n_out[i] = n;
+        for (int k = 0; k < 3; ++k) {
+            xs[k] = mk(a[9 * i + 3 * k], a[9 * i + 3 * k + 1], a[9 * i + 3 * k + 2]);
+            Xs[k] = mk(b[9 * i + 3 * k], b[9 * i + 3 * k + 1], b[9 * i + 3 * k + 2]);
         }
-        __syncwarp();
+        double models[28];
+        const int n = (VARIANT == 1) ? solve_p3p_lambdatwist(xs, Xs, models) : solve_p3p(xs, Xs, models);
+#pragma unroll
+        for (int e = 0; e < 28; ++e) out[28 * i + e] = (e < 7 * n) ? models[e] : 0.0;
+        n_out[i] = n;
+    } else if constexpr (KIND == KIND_HOMOG) {
+        d3 xa[4], xb[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            xa[k] = mk(a[12 * i + 3 * k], a[12 * i + 3 * k + 1], a[12 * i + 3 * k + 2]);
+            xb[k] = mk(b[12 * i + 3 * k], b[12 * i + 3 * k + 1], b[12 * i + 3 * k + 2]);
+        }
+        double H[9];
+        const int n = solve_h4(xa, xb, H, flags != 0);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) out[9 * i + k] = n ? H[k] : 0.0;
+        n_out[i] = n;
+    } else {
+        static_assert(KIND == KIND_FUND, "relpose_5pt runs on the phase kernels");
+        extern __shared__ __align__(16) unsigned char smem_raw[];
+        double *W = reinterpret_cast<double *>(smem_raw) + (size_t)threadIdx.x * K7L_STRIDE;
+        double x1s[21], x2s[21];
+#pragma unroll
+        for (int e = 0; e < 21; ++e) {
+            x1s[e] = a[21 * i + e];
+            x2s[e] = b[21 * i + e];
+        }
+        double F[3][9];
+        const int n = fundamental_7pt(x1s, x2s, W, [](const double *) { return true; }, F);
+#pragma unroll
+        for (int m = 0; m < 3; ++m)
+#pragma unroll
+            for (int k = 0; k < 9; ++k) out[27 * i + 9 * m + k] = (m < n) ? F[m][k] : 0.0;
+        n_out[i] = n;
+    }
+}
+
+// relpose_5pt: the caller's bearings (5 x 3 doubles per side and instance) into entries 75..104 of the entry-major
+// per-instance block, where k5_prep_lane and k5_back expect the sample's bearings.
+__global__ void __launch_bounds__(256) k5_load(int n, const double *__restrict__ a, const double *__restrict__ b,
+                                               HypOut s5) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n) return;
+    double *blk = s5.s5_blk + g;
+#pragma unroll
+    for (int e = 0; e < 15; ++e) {
+        blk[(size_t)(75 + e) * n] = a[(size_t)g * 15 + e];
+        blk[(size_t)(90 + e) * n] = b[(size_t)g * 15 + e];
+    }
+}
+
+// relpose_5pt output, one thread per instance: per root, the back-substitution of k5_back.  Variant 0: up to 10 E
+// (column-major, 90 doubles); variant 1: the poses of motions_from_E in the reference's order (E-major, then the four
+// candidates; 280 doubles).  Unused slots are zeroed.
+template <int VARIANT>
+__global__ void __launch_bounds__(128) k5_solver_out(int n, HypOut s5, double *out, int *n_out) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n) return;
+    const StridedD blk{s5.s5_blk + g, (size_t)n};
+    const int nr = s5.s5_nroots[g];
+    const double *roots = s5.s5_roots + (size_t)g * 10;
+    if constexpr (VARIANT == 0) {
+        double *o = out + (size_t)g * 90;
+        for (int m = 0; m < 10; ++m) {
+            double E[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+            if (m < nr) backsub_5pt(blk, blk + 39, roots[m], E);
+#pragma unroll
+            for (int k = 0; k < 9; ++k) o[9 * m + k] = E[3 * (k % 3) + k / 3];
+        }
+        n_out[g] = nr;
+    } else {
+        double *o = out + (size_t)g * 280;
+        int pos = 0;
+        for (int r = 0; r < nr; ++r) {
+            double E[9], cand[4][7];
+            backsub_5pt(blk, blk + 39, roots[r], E);
+            const unsigned mask = motions_from_E(E, blk + 75, blk + 90, 5, cand);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                if (mask & (1u << c)) {
+#pragma unroll
+                    for (int k = 0; k < 7; ++k) o[7 * pos + k] = cand[c][k];
+                    ++pos;
+                }
+            }
+        }
+        for (int e = 7 * pos; e < 280; ++e) o[e] = 0.0;
+        n_out[g] = pos;
     }
 }
 
 template <int KIND, int VARIANT>
 static void launch_solver_t(size_t count, const double *a, const double *b, double *out, int *n_out, int flags,
                             cudaStream_t stream) {
-    const size_t smem = hyp_smem_bytes<KIND>();
-    cudaFuncSetAttribute(k_solver_batch<KIND, VARIANT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    size_t blocks = (count + HYP_WARPS - 1) / HYP_WARPS;
-    const size_t cap = (size_t)sm_count() * 4;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    k_solver_batch<KIND, VARIANT><<<(unsigned)blocks, HYP_WARPS * 32, smem, stream>>>(count, a, b, out, n_out, flags);
+    size_t smem = 0;
+    if constexpr (KIND == KIND_FUND) {
+        smem = K7L_SMEM;
+        static bool attr_set[MAX_DEVICES] = {false};
+        if (!attr_set[cur_dev()]) {
+            cudaFuncSetAttribute(k_solver_batch<KIND, VARIANT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            attr_set[cur_dev()] = true;
+        }
+    }
+    k_solver_batch<KIND, VARIANT><<<(unsigned)((count + K7L_THREADS - 1) / K7L_THREADS), K7L_THREADS, smem, stream>>>(
+        count, a, b, out, n_out, flags);
 }
-void launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out,
-                         int *n_out, int flags, cudaStream_t stream) {
-    if (count == 0) return;
+int launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out, int *n_out,
+                        int flags, const HypOut &s5, cudaStream_t stream) {
+    if (count == 0) return 0;
     switch (kind) {
     case KIND_PNP:
         if (variant == 0) launch_solver_t<KIND_PNP, 0>(count, a, b, out, n_out, flags, stream);
         else launch_solver_t<KIND_PNP, 1>(count, a, b, out, n_out, flags, stream);
-        break;
-    case KIND_RELPOSE:
-        if (variant == 0) launch_solver_t<KIND_RELPOSE, 0>(count, a, b, out, n_out, flags, stream);
-        else launch_solver_t<KIND_RELPOSE, 1>(count, a, b, out, n_out, flags, stream);
-        break;
-    case KIND_FUND: launch_solver_t<KIND_FUND, 0>(count, a, b, out, n_out, flags, stream); break;
-    default: launch_solver_t<KIND_HOMOG, 0>(count, a, b, out, n_out, flags, stream); break;
+        return 1;
+    case KIND_RELPOSE: {
+        const int n = (int)count; // the s5 buffers of `count` instances bound it far below INT_MAX
+        RoundDesc R{};
+        R.n_total = n;
+        k5_load<<<(n + 255) / 256, 256, 0, stream>>>(n, a, b, s5);
+        launch_5pt_prep_roots(R, s5, stream);
+        if (variant == 0) k5_solver_out<0><<<(n + 127) / 128, 128, 0, stream>>>(n, s5, out, n_out);
+        else k5_solver_out<1><<<(n + 127) / 128, 128, 0, stream>>>(n, s5, out, n_out);
+        return 4;
+    }
+    case KIND_FUND: launch_solver_t<KIND_FUND, 0>(count, a, b, out, n_out, flags, stream); return 1;
+    default: launch_solver_t<KIND_HOMOG, 0>(count, a, b, out, n_out, flags, stream); return 1;
     }
 }
 

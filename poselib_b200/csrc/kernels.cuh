@@ -113,7 +113,7 @@ struct LoJobSrc {
     int slot;  // model slot in the round's model list
 };
 // round control words in device memory (ints)
-enum { CTL_QUEUE = 0, CTL_OVERFLOW = 2, CTL_NW = 4, CTL_IMP_TOTAL = 5, CTL_JOB_TOTAL = 6, CTL_FLAGS = 7, CTL_WORDS = 8 };
+enum { CTL_OVERFLOW = 2, CTL_NW = 4, CTL_IMP_TOTAL = 5, CTL_JOB_TOTAL = 6, CTL_FLAGS = 7, CTL_WORDS = 8 };
 enum { FLAG_IMP_OVERFLOW = 1, FLAG_JOB_OVERFLOW = 2 };
 
 struct SelectArgs {
@@ -212,11 +212,11 @@ struct MaskDesc {
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream);
 // AoS (caller layout) -> SoA fp64 + fp32 for n_desc problems (descriptors in device memory), camera pre-step fused.
 void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream);
-// Solve + score kernels of one round (kind = kind of every problem of the group).  work: 3 ints of device scratch.
+// Solve + score kernels of one round (kind = kind of every problem of the group); *out.overflow must be zeroed.
 // mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (exact rescoring of the candidates
 // is launched separately with launch_score_list once the host has selected them).
-void launch_hypotheses(int kind, const RoundDesc &R, int *work, const HypOut &out, int mode, int max_n_pad,
-                       cudaStream_t stream, cudaEvent_t ev_between = nullptr);
+void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
+                       cudaEvent_t ev_between = nullptr);
 void launch_score_list(int kind, const ProblemDev *probs, const double *models, const int *model_prob, const int *slots,
                        int n_slots, uint32_t *counts, double *scores, cudaStream_t stream);
 // Exact fp64 scoring of an explicit list of models (9 doubles stride MSZ) with problem indices; *n_models_dev = count.
@@ -249,9 +249,10 @@ void launch_inlier_masks(int kind, const ProblemDev *probs, const MaskDesc *desc
                          char *mask_base, cudaStream_t stream);
 // Inlier masks as bits (bit k & 31 of word k >> 5) for the device -> host copy; n_bytes is a multiple of 32.
 void launch_pack_mask(const char *mask, uint32_t *bits, size_t n_bytes, cudaStream_t stream);
-// Batched direct solver calls (solvers/*.h surface): one warp per instance.
-void launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out,
-                         int *n_out, int flags, cudaStream_t stream);
+// Batched direct solver calls (solvers/*.h surface): one thread per instance.  kind KIND_RELPOSE also needs the s5_*
+// phase buffers of s5 for `count` instances (the other fields are unused).  Returns the number of kernels launched.
+int launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out, int *n_out,
+                        int flags, const HypOut &s5, cudaStream_t stream);
 // relpose_8pt / essential_matrix_8pt (solvers/relpose_8pt.cc:52-95): count instances of n >= 8 unit bearing pairs each.
 void launch_eightpt(size_t count, int n, const double *x1, const double *x2, int want_poses, double *E_out, double *poses_out,
                     int *n_out, cudaStream_t stream);

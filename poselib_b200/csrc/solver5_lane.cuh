@@ -1,17 +1,15 @@
 // relpose_5pt, first half (nullspace, trace / determinant constraints, elimination, determinant polynomial) with ONE
 // THREAD PER MINIMAL SAMPLE.
 //
-// The group-of-8 version (solve_5pt_poly_grp8, solvers.cuh) spends most of its instructions on narrow steps: most are
-// 5..20 wide, the lanes of a group repeat the index arithmetic, and every value travels through shared memory
-// (k5_prep is bound by shared-memory traffic).  Here a thread owns a sample: the monomial tables
-// are compile-time constants, so the nullspace basis and the quadratic blocks live in registers with static indices and
-// only the 10 x 20 elimination matrix (dynamic pivot rows) sits in the thread's slice of shared memory.  Every value is
-// produced by the same sequence of IEEE operations as in solve_5pt_poly / the CPU restatement (the file is compiled
-// with -fmad=false), so the outputs are bit-identical; tests/test_solver5_lane_host.py checks that on the host build of
-// this very source.
+// Most steps of this half are only 5..20 wide, so a thread owns a sample.  The monomial tables are compile-time
+// constants: the nullspace basis and the quadratic blocks live in registers with static indices, and only the left
+// 10 x 10 block of the elimination matrix (dynamic pivot rows) sits in the thread's slice of shared memory while the
+// right-hand sides are parked elsewhere.  Every value is produced by the same sequence of IEEE operations as in the CPU
+// restatement (the file is compiled with -fmad=false), so the outputs are bit-identical;
+// tests/test_solver5_lane_host.py checks that on the host build of this very source.
 //
 // Reference: PoseLib/solvers/relpose_5pt.cc:101-157 (constraints), :159-189 (nullspace, elimination), :191-352
-// (determinant polynomial).  Eigen's FullPivHouseholderQR / PartialPivLU are restated as in solvers.cuh.
+// (determinant polynomial).  Eigen's FullPivHouseholderQR / PartialPivLU are restated below.
 #pragma once
 #include <cmath>
 #include <type_traits>
@@ -69,9 +67,9 @@ constexpr Tables TB = make_tables();
 
 // ---- nullspace of the 9 x C epipolar matrix (C = 5: relpose_5pt, C = 7: relpose_7pt) --------------------------------------------------------------------------
 // a: 9 C doubles, column-major (a[c * 9 + r]), overwritten; qn: 9 (9 - C) doubles, qn[9 * s + r] = entry r of the s-th
-// basis vector = column C + s of the Householder Q of the full-pivoting QR (relpose_5pt.cc:167-168).  The scalar form of
-// grp8_nullspace_9xC<5> (solvers.cuh): same pivot rule (largest |entry|, first in column-major order on ties), same
-// reflectors, same order of the row transpositions.
+// basis vector = column C + s of the Householder Q of the full-pivoting QR (relpose_5pt.cc:167-168, relpose_7pt.cc:18-19):
+// Eigen's pivot rule (largest |entry|, first in column-major order on ties), reflectors and order of the row
+// transpositions.
 template <int COLS> PLB_L5 void nullspace_9xC(double *a, double *qn) {
     constexpr int ROWS = 9;
     double tau_k[COLS];
@@ -395,7 +393,7 @@ PLB_L5 void lu_left(double *CL, double *S, int *idx) {
 // the unit-lower solve (per element the same products, subtracted in the same order, as the rank-1 updates of the fused
 // form) and the back substitution of rows 9..4.  X (60 doubles, may alias CL: the factors are in registers by then)
 // receives rows 4..9 of A^{-1} B, X[(r - 4) * 10 + column].
-template <int UNR = 1, class Get> PLB_L5 void solve_rhs(const double *CL, double *S, const int *idx, Get &&get, double *X) {
+template <class Get> PLB_L5 void solve_rhs(const double *CL, double *S, const int *idx, Get &&get, double *X) {
     double L[10][10], U[10][10], diag[10]; // static indices: 45 + 15 + 6 values in registers
 #pragma unroll
     for (int r = 0; r < 10; ++r)
@@ -406,7 +404,7 @@ template <int UNR = 1, class Get> PLB_L5 void solve_rhs(const double *CL, double
         }
 #pragma unroll
     for (int r = 4; r < 10; ++r) diag[r] = CL[r * 10 + r];
-#pragma unroll UNR
+#pragma unroll 1
     for (int c = 0; c < 10; ++c) {
         double b[10];
 #pragma unroll

@@ -1,17 +1,17 @@
-// poselib_b200 — minimal solvers as warp-level device functions (one warp = one minimal sample).
+// poselib_b200 — minimal solvers as scalar device functions (one thread = one minimal sample).
 //
-// p3p and homography_4pt are short closed forms: every lane evaluates the same scalar program (no divergence, no
-// shared memory) and lane 0 publishes the models.  relpose_5pt and relpose_7pt stage their matrices in per-warp
-// shared memory and spread the wide steps (pivoted QR, the 10x20 trace-constraint build, the 10x10 LU with 10
-// right-hand sides, the polynomial products, per-root back-substitution and the 4-way motion decomposition) over
-// the lanes.  Every individual dot product / accumulation keeps the left-to-right order of the reference so results
-// agree with the CPU path to the last bits wherever libm is not involved.
+// p3p, p3p_lambdatwist and homography_4pt are closed forms.  relpose_7pt runs the scalar nullspace routine of
+// solver5_lane.cuh on the calling thread's slice of shared memory.  relpose_5pt is split into phase kernels
+// (kernels.cu): its first half is solver5_lane.cuh, the Sturm root isolation, back-substitution and motion
+// decomposition are below.  Every individual dot product / accumulation keeps the left-to-right order of the
+// reference so results agree with the CPU path to the last bits wherever libm is not involved.
 //
 // Reference (relative to /root/reference): solvers/p3p.cc:39-202 + p3p_common.h; solvers/relpose_5pt.cc:101-409;
 // solvers/relpose_7pt.cc:10-60; solvers/homography_4pt.cc:36-128; misc/sturm.h:47-274; misc/univariate.cc:48-126;
 // misc/essential.cc:103-169.
 #pragma once
 #include "device_math.cuh"
+#include "solver5_lane.cuh"
 
 namespace plb {
 
@@ -119,10 +119,8 @@ PLB_DEV void p3p_refine_lambda(double &l1, double &l2, double &l3, double a12, d
 }
 
 // Solves one P3P instance.  xs: 3 unit bearings, Xs: 3 world points.  Writes up to 4 poses (7 doubles each) to
-// `out` (lane 0 writes) and returns the count (uniform across the warp).   p3p.cc:39-202
-// warp_uniform: all 32 lanes run the SAME instance (lane 0 publishes, warp barrier at the end); false: every lane runs
-// its own instance (call with lane = 0 and a per-lane `out`) — no barrier then, lanes leave at different times.
-PLB_DEV int solve_p3p(const d3 *xs, const d3 *Xs, double *out, int lane, bool warp_uniform = true) {
+// `out` and returns the count.   p3p.cc:39-202
+PLB_DEV int solve_p3p(const d3 *xs, const d3 *Xs, double *out) {
     d3 x0 = xs[0], x1 = xs[1], x2 = xs[2];
     d3 P0 = Xs[0], P1 = Xs[1], P2 = Xs[2];
     d3 X01 = P0 - P1, X02 = P0 - P2, X12 = P1 - P2;
@@ -234,17 +232,14 @@ PLB_DEV int solve_p3p(const d3 *xs, const d3 *Xs, double *out, int lane, bool wa
                 const d3 t = d0 * x0 - mvec(R, P0);
                 double q[4];
                 rot_to_quat(R, q);
-                if (lane == 0) {
-                    double *o = out + 7 * n_sols;
-                    o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3];
-                    o[4] = t.x; o[5] = t.y; o[6] = t.z;
-                }
+                double *o = out + 7 * n_sols;
+                o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3];
+                o[4] = t.x; o[5] = t.y; o[6] = t.z;
                 ++n_sols;
             }
         }
         if (n_sols > 0 && G) break;
     }
-    if (warp_uniform) __syncwarp();
     return n_sols;
 }
 
@@ -276,7 +271,7 @@ PLB_DEV double lt_array_prod_sum(const m3 &A, const m3 &B) {
             if (c + r > 0) s = s + A(r, c) * B(r, c);
     return s;
 }
-PLB_DEV int solve_p3p_lambdatwist(const d3 *xs, const d3 *Xs, double *out, int lane, bool warp_uniform = true) {
+PLB_DEV int solve_p3p_lambdatwist(const d3 *xs, const d3 *Xs, double *out) {
     const d3 x0 = xs[0], x1 = xs[1], x2 = xs[2];
     const d3 dX12 = Xs[0] - Xs[1], dX13 = Xs[0] - Xs[2], dX23 = Xs[1] - Xs[2];
     const double a12 = dot(dX12, dX12), b12 = dot(x0, x1);
@@ -392,23 +387,20 @@ PLB_DEV int solve_p3p_lambdatwist(const d3 *xs, const d3 *Xs, double *out, int l
                 const d3 t = l1 * x0 - mvec(R, Xs[0]);
                 double q[4];
                 rot_to_quat(R, q);
-                if (lane == 0) {
-                    double *o = out + 7 * n_sols;
-                    o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3];
-                    o[4] = t.x; o[5] = t.y; o[6] = t.z;
-                }
+                double *o = out + 7 * n_sols;
+                o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3];
+                o[4] = t.x; o[5] = t.y; o[6] = t.z;
                 ++n_sols;
             }
             if (b2m4ac < TOL_DOUBLE_ROOT) break;
         }
     }
-    if (warp_uniform) __syncwarp();
     return n_sols;
 }
 
 // ================================ homography_4pt (SKS / ACA closed form) ===================================
 // homography_4pt.cc:36-128.  Writes H (9 doubles COLUMN-major) to out; returns 0/1.
-PLB_DEV int solve_h4(const d3 *x1, const d3 *x2, double *out, int lane, bool check_cheirality, bool warp_uniform = true) {
+PLB_DEV int solve_h4(const d3 *x1, const d3 *x2, double *out, bool check_cheirality) {
     if (check_cheirality) {
         d3 p = cross(x1[0], x1[1]), q = cross(x2[0], x2[1]);
         if (dot(p, x1[2]) * dot(q, x2[2]) < 0) return 0;
@@ -465,142 +457,9 @@ PLB_DEV int solve_h4(const d3 *x1, const d3 *x2, double *out, int lane, bool che
         for (int k = 0; k < 9; ++k) H.a[k] /= n;
     }
     if (fabs(det3(H)) < 1e-8) return 0;
-    if (lane == 0) {
 #pragma unroll
-        for (int k = 0; k < 9; ++k) out[k] = H(k % 3, k / 3);
-    }
-    if (warp_uniform) __syncwarp();
+    for (int k = 0; k < 9; ++k) out[k] = H(k % 3, k / 3);
     return 1;
-}
-
-// ================================ pivoted Householder nullspace ============================================
-// Restates Eigen's FullPivHouseholderQR::matrixQ() for a 9 x COLS matrix and returns the last (9-COLS) columns of Q,
-// i.e. an orthonormal basis of the left nullspace (relpose_5pt.cc:167-168, relpose_7pt.cc:18-19).
-//   a   : shared, 9*COLS doubles, column-major, destroyed
-//   qn  : shared, (9-COLS)*9 doubles; column j of the basis at qn[9*j .. 9*j+8]
-template <int COLS> PLB_DEV void warp_nullspace_9xC(double *a, double *qn, int lane) {
-    constexpr int ROWS = 9;
-    double tau_k[COLS];
-    int rt_k[COLS];
-    const double precision = 2.220446049250313e-16 * double(COLS);
-    double biggest = 0.0;
-    bool stopped = false;
-#pragma unroll
-    for (int k = 0; k < COLS; ++k) {
-        if (stopped) {
-            tau_k[k] = 0.0;
-            rt_k[k] = k;
-            continue;
-        }
-        // ---- pivot: largest |a_rc| in the trailing block, first one in column-major order
-        const int nr = ROWS - k, cnt = nr * (COLS - k);
-        double best = -1.0;
-        int bord = 0x7fffffff;
-        for (int e = lane; e < cnt; e += 32) {
-            const int c = k + e / nr, r = k + e % nr;
-            const double v = fabs(a[c * ROWS + r]);
-            if (v > best) {
-                best = v;
-                bord = e;
-            }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oo = __shfl_xor_sync(0xffffffffu, bord, o);
-            if (ob > best || (ob == best && oo < bord)) {
-                best = ob;
-                bord = oo;
-            }
-        }
-        if (k == 0) biggest = best;
-        if (fabs(best) <= fabs(biggest) * precision) {
-            stopped = true;
-            tau_k[k] = 0.0;
-            rt_k[k] = k;
-            continue;
-        }
-        const int cb = k + bord / nr, rb = k + bord % nr;
-        rt_k[k] = rb;
-        if (rb != k && lane >= k && lane < COLS) {
-            const double t = a[lane * ROWS + k];
-            a[lane * ROWS + k] = a[lane * ROWS + rb];
-            a[lane * ROWS + rb] = t;
-        }
-        __syncwarp();
-        if (cb != k && lane < ROWS) {
-            const double t = a[k * ROWS + lane];
-            a[k * ROWS + lane] = a[cb * ROWS + lane];
-            a[cb * ROWS + lane] = t;
-        }
-        __syncwarp();
-        // ---- Householder vector of column k (every lane evaluates the same scalars)
-        double tail_sq = 0.0;
-        for (int r = k + 1; r < ROWS; ++r) tail_sq += a[k * ROWS + r] * a[k * ROWS + r];
-        const double c0 = a[k * ROWS + k];
-        double tau, beta;
-        __syncwarp();
-        if (tail_sq <= 2.2250738585072014e-308) {
-            tau = 0.0;
-            beta = c0;
-            if (lane > k && lane < ROWS) a[k * ROWS + lane] = 0.0;
-        } else {
-            beta = sqrt(c0 * c0 + tail_sq);
-            if (c0 >= 0) beta = -beta;
-            if (lane > k && lane < ROWS) a[k * ROWS + lane] = a[k * ROWS + lane] / (c0 - beta);
-            tau = (beta - c0) / beta;
-        }
-        if (lane == k) a[k * ROWS + k] = beta;
-        tau_k[k] = tau;
-        __syncwarp();
-        // ---- reflect the trailing columns: one lane per column
-        if (tau != 0.0 && lane > k && lane < COLS) {
-            double *col = a + lane * ROWS;
-            const double *v = a + k * ROWS;
-            double tmp = 0.0;
-            for (int r = k + 1; r < ROWS; ++r) tmp += v[r] * col[r];
-            tmp += col[k];
-            col[k] -= tau * tmp;
-            for (int r = k + 1; r < ROWS; ++r) col[r] -= tau * v[r] * tmp;
-        }
-        __syncwarp();
-    }
-    // ---- columns COLS..8 of Q = P_0 H_0 ... P_{COLS-1} H_{COLS-1} applied to unit vectors; one lane per column
-    if (lane < ROWS - COLS) {
-        double q[ROWS];
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) q[r] = (r == COLS + lane) ? 1.0 : 0.0;
-#pragma unroll
-        for (int k = COLS - 1; k >= 0; --k) {
-            const double tau = tau_k[k];
-            const double *v = a + k * ROWS;
-            if (tau != 0.0) {
-                double tmp = 0.0;
-#pragma unroll
-                for (int r = k + 1; r < ROWS; ++r) tmp += v[r] * q[r];
-                tmp += q[k];
-                q[k] -= tau * tmp;
-#pragma unroll
-                for (int r = k + 1; r < ROWS; ++r) q[r] -= tau * v[r] * tmp;
-            }
-            const int rt = rt_k[k];
-            if (rt != k) {
-                // swap q[k] <-> q[rt] with a register-resident select (rt is uniform but dynamic)
-                const double qk = q[k];
-                double qr = 0.0;
-#pragma unroll
-                for (int r = 0; r < ROWS; ++r)
-                    if (r == rt) qr = q[r];
-#pragma unroll
-                for (int r = 0; r < ROWS; ++r)
-                    if (r == rt) q[r] = qk;
-                q[k] = qr;
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) qn[lane * ROWS + r] = q[r];
-    }
-    __syncwarp();
 }
 
 // ================================ Sturm root isolation, degree 10 ==========================================
@@ -930,644 +789,6 @@ PLB_DEV int sturm_bisect10_warp(const double *c, bool has_poly, double *roots, R
 }
 
 // ================================ relpose_5pt (Nister) =====================================================
-// Monomial tables, filled once per CTA into shared memory (see fill_tables):
-//   quad_idx[i][j]      : index of lin_i*lin_j in [x^2,xy,xz,x,y^2,yz,y,z^2,z,1]       (relpose_5pt.cc:11-12)
-//   cub_n[ci], cub_q/l  : the (quadratic, linear) factor pairs, in (q,l) lexicographic order, whose product is the
-//                         cubic monomial ci of [x^3,y^3,x^2y,xy^2,x^2z,x^2,y^2z,y^2,xyz,xy,xz^2,xz,x,yz^2,yz,y,
-//                         z^3,z^2,z,1]                                                      (relpose_5pt.cc:54-55)
-struct MonoTables {
-    int8_t quad_i[10], quad_j[10]; // the (i<=j) pair of each quadratic monomial
-    int8_t cub_n[20];
-    int8_t cub_q[20][3], cub_l[20][3];
-};
-// The tables are built once at compile time (host constexpr) into constant memory; each CTA copies them to shared
-// memory (lane-varying indices would serialise constant-cache reads).
-constexpr MonoTables make_mono_tables() {
-    MonoTables T{};
-    const int qexp[10][3] = {{2, 0, 0}, {1, 1, 0}, {1, 0, 1}, {1, 0, 0}, {0, 2, 0},
-                             {0, 1, 1}, {0, 1, 0}, {0, 0, 2}, {0, 0, 1}, {0, 0, 0}};
-    const int cexp[20][3] = {{3, 0, 0}, {0, 3, 0}, {2, 1, 0}, {1, 2, 0}, {2, 0, 1}, {2, 0, 0}, {0, 2, 1},
-                             {0, 2, 0}, {1, 1, 1}, {1, 1, 0}, {1, 0, 2}, {1, 0, 1}, {1, 0, 0}, {0, 1, 2},
-                             {0, 1, 1}, {0, 1, 0}, {0, 0, 3}, {0, 0, 2}, {0, 0, 1}, {0, 0, 0}};
-    const int lexp[4][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}, {0, 0, 0}};
-    int qn = 0;
-    for (int i = 0; i < 4; ++i)
-        for (int j = i; j < 4; ++j) {
-            T.quad_i[qn] = (int8_t)i;
-            T.quad_j[qn] = (int8_t)j;
-            ++qn;
-        }
-    for (int ci = 0; ci < 20; ++ci) {
-        int n = 0;
-        for (int q = 0; q < 10; ++q)
-            for (int l = 0; l < 4; ++l)
-                if (qexp[q][0] + lexp[l][0] == cexp[ci][0] && qexp[q][1] + lexp[l][1] == cexp[ci][1] &&
-                    qexp[q][2] + lexp[l][2] == cexp[ci][2]) {
-                    T.cub_q[ci][n] = (int8_t)q;
-                    T.cub_l[ci][n] = (int8_t)l;
-                    ++n;
-                }
-        T.cub_n[ci] = (int8_t)n;
-    }
-    return T;
-}
-__constant__ MonoTables c_mono_tables = make_mono_tables();
-// cooperative copy constant -> shared (whole CTA), followed by a barrier at the call site
-__device__ __forceinline__ void fill_tables(MonoTables *T) {
-    const unsigned char *src = reinterpret_cast<const unsigned char *>(&c_mono_tables);
-    unsigned char *dst = reinterpret_cast<unsigned char *>(T);
-    for (int i = threadIdx.x; i < (int)sizeof(MonoTables); i += blockDim.x) dst[i] = src[i];
-}
-
-// per-warp shared scratch of the 5-point solver (doubles)
-struct Scratch5 {
-    double M[45];       // 9x5 epipolar matrix (col-major); reused
-    double Nb[36];      // Nb[4*k + r]: coefficient of basis r (x,y,z,1) in entry k (col-major) of E
-    double quad[9][10]; // 6 EE^T entries (+3 determinant minors) as quadratics
-    double coeffs[200]; // 10 x 20 (row-major, lda 20)
-    double A[39];       // 3 x 13
-    double cpoly[11];
-    double roots[10];
-    double minors[3][8];
-    SturmWork sturm;
-    double Es[90];      // up to 10 essential matrices, row-major 3x3 each
-    int nroots;
-};
-
-// One quadratic coefficient of  acc + sgn * (a*b)  with linear a,b in accumulation order of the reference.
-PLB_DEV double lin_mul_coef(double acc, const double *a, const double *b, int i, int j, double sgn) {
-    acc = acc + sgn * (a[i] * b[j]);
-    if (i != j) acc = acc + sgn * (a[j] * b[i]);
-    return acc;
-}
-
-// Essential matrices from 5 bearing pairs.  x1s/x2s: shared arrays of 5 unit bearings (3 doubles each).
-// On return S->Es holds nroots row-major E matrices (relpose_5pt.cc:159-395).  Returns nroots (uniform).
-// First half of the 5-point solver: nullspace basis S->Nb, polynomial matrix S->A (3x13) and the degree-10
-// determinant polynomial S->cpoly (ascending)   (relpose_5pt.cc:162-352).
-PLB_DEV void solve_5pt_poly(const double *x1s, const double *x2s, Scratch5 *S, const MonoTables *T, int lane) {
-    // ---- 9x5 epipolar constraints (:163-166): entry 3a+b of column i = x1[i][a]*x2[i][b]
-    for (int e = lane; e < 45; e += 32) {
-        const int i = e / 9, k = e % 9;
-        S->M[e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
-    }
-    __syncwarp();
-    // ---- nullspace basis (:167-168); qn column r -> Nb[4k+r]
-    warp_nullspace_9xC<5>(S->M, S->coeffs /*tmp: 36 doubles*/, lane);
-    for (int e = lane; e < 36; e += 32) {
-        const int r = e / 9, k = e % 9;
-        S->Nb[4 * k + r] = S->coeffs[9 * r + k];
-    }
-    __syncwarp();
-#define PLB_EE(i, j) (S->Nb + 4 * (3 * (j) + (i)))
-    // ---- quadratic building blocks (:113-123,129-144): 6 entries of EE^T and 3 minors of the last-row expansion
-    for (int e = lane; e < 90; e += 32) {
-        const int blk = e / 10, m = e % 10;
-        const int qi = T->quad_i[m], qj = T->quad_j[m];
-        double v = 0.0;
-        if (blk < 6) {
-            // (i,j) in (0,0),(0,1),(0,2),(1,1),(1,2),(2,2)
-            const int i = (blk < 3) ? 0 : (blk < 5 ? 1 : 2);
-            const int j = (blk < 3) ? blk : (blk < 5 ? blk - 2 : 2);
-#pragma unroll
-            for (int k = 0; k < 3; ++k) v = lin_mul_coef(v, PLB_EE(i, k), PLB_EE(j, k), qi, qj, 1.0);
-        } else {
-            // minors d_t of the cofactor expansion along row 2
-            const int t = blk - 6;
-            const int c1 = (t == 0) ? 1 : (t == 1 ? 2 : 0);
-            const int c2 = (t == 0) ? 2 : (t == 1 ? 0 : 1);
-            v = lin_mul_coef(v, PLB_EE(0, c1), PLB_EE(1, c2), qi, qj, 1.0);
-            v = lin_mul_coef(v, PLB_EE(0, c2), PLB_EE(1, c1), qi, qj, -1.0);
-        }
-        S->quad[blk][m] = v;
-    }
-    __syncwarp();
-    // trace subtraction (:139-144)
-    if (lane < 10) {
-        const double t = 0.5 * (S->quad[0][lane] + S->quad[3][lane] + S->quad[5][lane]);
-        S->quad[0][lane] -= t;
-        S->quad[3][lane] -= t;
-        S->quad[5][lane] -= t;
-    }
-    __syncwarp();
-    // ---- 10 x 20 coefficient matrix (:146-154 rows 0..8, :113-125 row 9)
-    for (int e = lane; e < 200; e += 32) {
-        const int row = e / 20, ci = e % 20;
-        const int np = T->cub_n[ci];
-        double v = 0.0;
-        if (row < 9) {
-            const int i = row / 3, j = row % 3;
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                // symmetric index of EET[i][k]
-                const int lo = i < k ? i : k, hi = i < k ? k : i;
-                const int blk = (lo == 0) ? hi : (lo == 1 ? 2 + hi : 5);
-                const double *Q = S->quad[blk];
-                const double *Lk = PLB_EE(k, j);
-                for (int p = 0; p < np; ++p) v += Q[T->cub_q[ci][p]] * Lk[T->cub_l[ci][p]];
-            }
-        } else {
-#pragma unroll
-            for (int t = 0; t < 3; ++t) {
-                const double *Q = S->quad[6 + t];
-                const double *Lk = PLB_EE(2, t);
-                for (int p = 0; p < np; ++p) v += Q[T->cub_q[ci][p]] * Lk[T->cub_l[ci][p]];
-            }
-        }
-        S->coeffs[e] = v;
-    }
-    __syncwarp();
-#undef PLB_EE
-    // ---- [A | B] -> A^{-1} B by partial-pivot LU, 10 right-hand sides (:173)
-    {
-        double *C = S->coeffs;
-        for (int k = 0; k < 10; ++k) {
-            int p = k;
-            double best = fabs(C[k * 20 + k]);
-            for (int r = k + 1; r < 10; ++r) {
-                const double v = fabs(C[r * 20 + k]);
-                if (v > best) {
-                    best = v;
-                    p = r;
-                }
-            }
-            __syncwarp();
-            if (best != 0.0) {
-                if (p != k && lane < 20) {
-                    const double t = C[k * 20 + lane];
-                    C[k * 20 + lane] = C[p * 20 + lane];
-                    C[p * 20 + lane] = t;
-                }
-                __syncwarp();
-                const double pv = C[k * 20 + k];
-                __syncwarp();
-                if (lane > k && lane < 10) C[lane * 20 + k] /= pv;
-                __syncwarp();
-            }
-            // rank-1 update of the trailing block, one lane per column c > k.  Columns 10..19 are the right-hand sides:
-            // updating them here IS the forward substitution (same operands, same order per element) of the
-            // reference's permute / unit-lower solve, so only the back substitution is left afterwards.
-            {
-                const int c = k + 1 + lane;
-                if (c < 20) {
-                    const double ckc = C[k * 20 + c];
-                    for (int r = k + 1; r < 10; ++r) C[r * 20 + c] -= C[r * 20 + k] * ckc;
-                }
-            }
-            __syncwarp();
-        }
-        if (lane < 10) {
-            const int c = 10 + lane;
-            for (int r = 9; r >= 0; --r) {
-                double s = C[r * 20 + c];
-                for (int k = r + 1; k < 10; ++k) s -= C[r * 20 + k] * C[k * 20 + c];
-                C[r * 20 + c] = s / C[r * 20 + r];
-            }
-        }
-        __syncwarp();
-    }
-    // ---- 3 x 13 polynomial matrix (:176-189)
-    for (int e = lane; e < 39; e += 32) {
-        const int i = e / 13, c = e % 13;
-        const double *top = S->coeffs + (4 + 2 * i) * 20 + 10, *bot = S->coeffs + (5 + 2 * i) * 20 + 10;
-        // block g: columns [0..3] <- cols 0..2 ; [4..7] <- cols 3..5 ; [8..12] <- cols 6..9
-        const int g0 = (c < 4) ? 0 : (c < 8 ? 4 : 8), src0 = (c < 4) ? 0 : (c < 8 ? 3 : 6);
-        const int w = (c < 8) ? 3 : 4, o = c - g0;
-        double v = 0.0;
-        if (o >= 1) v = top[src0 + o - 1];
-        if (o < w) v -= bot[src0 + o];
-        S->A[e] = v;
-    }
-    __syncwarp();
-    // ---- det(A(z)) as a degree-10 polynomial, ascending coefficients (:191-352)
-    // p_ij ascending: p_i0[k] = A[i][3-k], p_i1[k] = A[i][7-k], p_i2[k] = A[i][12-k]
-    {
-        const double *A = S->A;
-        auto P = [&](int i, int j, int k) -> double {
-            return (j == 0) ? A[13 * i + 3 - k] : (j == 1 ? A[13 * i + 7 - k] : A[13 * i + 12 - k]);
-        };
-        // minors of rows 1,2: m0 = p11*p22 - p12*p21 (deg 7), m1 = p10*p22 - p12*p20 (deg 7), m2 = p10*p21 - p11*p20 (6)
-        if (lane < 24) {
-            const int t = lane / 8, k = lane % 8;
-            const int ja = (t == 0) ? 1 : 0, jb = (t == 2) ? 1 : 2; // first product p1[ja]*p2[jb]
-            const int da = 3, db = (jb == 2) ? 4 : 3;
-            double v = 0.0;
-            if (k <= da + db) {
-                double s1 = 0.0, s2 = 0.0;
-                for (int i = 0; i <= da; ++i) {
-                    const int j = k - i;
-                    if (j >= 0 && j <= db) s1 += P(1, ja, i) * P(2, jb, j);
-                }
-                // second product p1[jb]*p2[ja]
-                for (int i = 0; i <= db; ++i) {
-                    const int j = k - i;
-                    if (j >= 0 && j <= da) s2 += P(1, jb, i) * P(2, ja, j);
-                }
-                v = s1 - s2;
-            }
-            S->minors[t][k] = v;
-        }
-        __syncwarp();
-        if (lane < 11) {
-            const int k = lane;
-            double t0 = 0.0, t1 = 0.0, t2 = 0.0;
-            for (int i = 0; i <= 3; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 7) t0 += P(0, 0, i) * S->minors[0][j];
-            }
-            for (int i = 0; i <= 3; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 7) t1 += P(0, 1, i) * S->minors[1][j];
-            }
-            for (int i = 0; i <= 4; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 6) t2 += P(0, 2, i) * S->minors[2][j];
-            }
-            double c = 0.0;
-            c += t0;
-            c -= t1;
-            c += t2;
-            S->cpoly[k] = c;
-        }
-        __syncwarp();
-    }
-}
-
-// ---- the same first half, FOUR samples per warp (k5_prep) ------------------------------------------------------------
-// Most steps of solve_5pt_poly have 4..20-way parallelism, so a whole warp per sample leaves most lanes idle.  Here
-// lanes [8s, 8s+8) own sample s: the serial steps
-// (pivoted QR, LU pivots, back substitution) advance four samples per instruction, and the table-driven steps map a
-// lane to a MONOMIAL (its factor tables live in registers) instead of to a matrix entry.  Every element is computed
-// by the same sequence of operations as in solve_5pt_poly / the reference, so the outputs are bit-identical.
-// Control flow is uniform across the warp (every __syncwarp is reached by all lanes; sample-dependent cases are
-// predicated), which is what allows four independent samples to share the barriers.
-// Per-sample shared scratch W (doubles):  C[200] coefficient matrix (first 36: nullspace tmp) | Q[90] quadratic blocks
-// (before: M[45]; after: A[39] @0, minors[24] @40, cpoly[11] @64) | Nb[36] | xs[30]
-// stride 360 = 8 (mod 16) doubles: the two groups of a half-warp sit 16 banks apart (conflict-free 64-bit accesses)
-constexpr int P5_C = 0, P5_Q = 200, P5_NB = 290, P5_XS = 326, P5_STRIDE = 360;
-constexpr int P5_A = P5_Q, P5_MIN = P5_Q + 40, P5_CPOLY = P5_Q + 64;
-
-// warp_nullspace_9xC for a group of 8 lanes (sl = lane & 7)
-template <int COLS> PLB_DEV void grp8_nullspace_9xC(double *a, double *qn, int sl) {
-    constexpr int ROWS = 9;
-    static_assert(COLS <= 8, "one lane per column");
-    double tau_k[COLS];
-    int rt_k[COLS];
-    const double precision = 2.220446049250313e-16 * double(COLS);
-    double biggest = 0.0;
-    bool stopped = false;
-#pragma unroll
-    for (int k = 0; k < COLS; ++k) {
-        const int nr = ROWS - k, cnt = nr * (COLS - k);
-        double best = -1.0;
-        int bord = 0x7fffffff;
-        for (int e = sl; e < cnt; e += 8) {
-            const int c = k + e / nr, r = k + e % nr;
-            const double v = fabs(a[c * ROWS + r]);
-            if (v > best) {
-                best = v;
-                bord = e;
-            }
-        }
-#pragma unroll
-        for (int o = 4; o > 0; o >>= 1) {
-            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oo = __shfl_xor_sync(0xffffffffu, bord, o);
-            if (ob > best || (ob == best && oo < bord)) {
-                best = ob;
-                bord = oo;
-            }
-        }
-        if (k == 0) biggest = best;
-        if (!stopped && fabs(best) <= fabs(biggest) * precision) stopped = true;
-        int cb = k, rb = k;
-        if (!stopped) {
-            cb = k + bord / nr;
-            rb = k + bord % nr;
-        }
-        rt_k[k] = rb;
-        if (rb != k && sl >= k && sl < COLS) {
-            const double t = a[sl * ROWS + k];
-            a[sl * ROWS + k] = a[sl * ROWS + rb];
-            a[sl * ROWS + rb] = t;
-        }
-        __syncwarp();
-        if (cb != k) {
-            for (int r = sl; r < ROWS; r += 8) {
-                const double t = a[k * ROWS + r];
-                a[k * ROWS + r] = a[cb * ROWS + r];
-                a[cb * ROWS + r] = t;
-            }
-        }
-        __syncwarp();
-        double tail_sq = 0.0;
-        for (int r = k + 1; r < ROWS; ++r) tail_sq += a[k * ROWS + r] * a[k * ROWS + r];
-        const double c0 = a[k * ROWS + k];
-        double tau = 0.0;
-        __syncwarp();
-        if (!stopped) {
-            double beta;
-            if (tail_sq <= 2.2250738585072014e-308) {
-                beta = c0;
-                for (int r = sl; r < ROWS; r += 8)
-                    if (r > k) a[k * ROWS + r] = 0.0;
-            } else {
-                beta = sqrt(c0 * c0 + tail_sq);
-                if (c0 >= 0) beta = -beta;
-                for (int r = sl; r < ROWS; r += 8)
-                    if (r > k) a[k * ROWS + r] = a[k * ROWS + r] / (c0 - beta);
-                tau = (beta - c0) / beta;
-            }
-            if (sl == k) a[k * ROWS + k] = beta;
-        }
-        tau_k[k] = tau;
-        __syncwarp();
-        if (tau != 0.0 && sl > k && sl < COLS) {
-            double *col = a + sl * ROWS;
-            const double *v = a + k * ROWS;
-            double tmp = 0.0;
-            for (int r = k + 1; r < ROWS; ++r) tmp += v[r] * col[r];
-            tmp += col[k];
-            col[k] -= tau * tmp;
-            for (int r = k + 1; r < ROWS; ++r) col[r] -= tau * v[r] * tmp;
-        }
-        __syncwarp();
-    }
-    if (sl < ROWS - COLS) {
-        double q[ROWS];
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) q[r] = (r == COLS + sl) ? 1.0 : 0.0;
-#pragma unroll
-        for (int k = COLS - 1; k >= 0; --k) {
-            const double tau = tau_k[k];
-            const double *v = a + k * ROWS;
-            if (tau != 0.0) {
-                double tmp = 0.0;
-#pragma unroll
-                for (int r = k + 1; r < ROWS; ++r) tmp += v[r] * q[r];
-                tmp += q[k];
-                q[k] -= tau * tmp;
-#pragma unroll
-                for (int r = k + 1; r < ROWS; ++r) q[r] -= tau * v[r] * tmp;
-            }
-            const int rt = rt_k[k];
-            if (rt != k) {
-                const double qk = q[k];
-                double qr = 0.0;
-#pragma unroll
-                for (int r = 0; r < ROWS; ++r)
-                    if (r == rt) qr = q[r];
-#pragma unroll
-                for (int r = 0; r < ROWS; ++r)
-                    if (r == rt) q[r] = qk;
-                q[k] = qr;
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) qn[sl * ROWS + r] = q[r];
-    }
-    __syncwarp();
-}
-
-// W: this sample's scratch (xs filled, see layout above); on return Nb, A (P5_A), cpoly (P5_CPOLY) are valid.
-PLB_DEV void solve_5pt_poly_grp8(double *W, const MonoTables *T, int sl) {
-    double *C = W + P5_C, *Q = W + P5_Q, *Nb = W + P5_NB;
-    const double *x1s = W + P5_XS, *x2s = W + P5_XS + 15;
-    // ---- 9x5 epipolar constraints (relpose_5pt.cc:163-166), M aliases Q
-    double *M = Q;
-    for (int e = sl; e < 45; e += 8) {
-        const int i = e / 9, k = e % 9;
-        M[e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
-    }
-    __syncwarp();
-    grp8_nullspace_9xC<5>(M, C /*tmp: 36 doubles*/, sl);
-    for (int e = sl; e < 36; e += 8) {
-        const int r = e / 9, k = e % 9;
-        Nb[4 * k + r] = C[9 * r + k];
-    }
-    __syncwarp();
-#define PLB_EE(i, j) (Nb + 4 * (3 * (j) + (i)))
-    // ---- quadratic building blocks (:113-123,129-144): lane <-> quadratic monomial m.  The 2 x 9 nullspace
-    // coefficients the monomial needs are read into registers once (the kernel is bound by shared-memory wavefronts).
-#pragma unroll 1
-    for (int m = sl; m < 10; m += 8) {
-        const int qi = T->quad_i[m], qj = T->quad_j[m];
-        const bool same = qi == qj;
-        double ei[3][3], ej[3][3]; // [row i][col j] of E: coefficient of basis qi / qj
-#pragma unroll
-        for (int i = 0; i < 3; ++i)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                ei[i][j] = PLB_EE(i, j)[qi];
-                ej[i][j] = PLB_EE(i, j)[qj];
-            }
-        // acc + sgn * (a*b) in the accumulation order of lin_mul_coef
-        auto lmc = [&](double acc, int ia, int ja, int ib, int jb, double sgn) -> double {
-            acc = acc + sgn * (ei[ia][ja] * ej[ib][jb]);
-            if (!same) acc = acc + sgn * (ej[ia][ja] * ei[ib][jb]);
-            return acc;
-        };
-        double qv[9];
-#pragma unroll
-        for (int blk = 0; blk < 9; ++blk) {
-            double v = 0.0;
-            if (blk < 6) {
-                const int i = (blk < 3) ? 0 : (blk < 5 ? 1 : 2);
-                const int j = (blk < 3) ? blk : (blk < 5 ? blk - 2 : 2);
-#pragma unroll
-                for (int k = 0; k < 3; ++k) v = lmc(v, i, k, j, k, 1.0);
-            } else {
-                const int t = blk - 6;
-                const int c1 = (t == 0) ? 1 : (t == 1 ? 2 : 0);
-                const int c2 = (t == 0) ? 2 : (t == 1 ? 0 : 1);
-                v = lmc(v, 0, c1, 1, c2, 1.0);
-                v = lmc(v, 0, c2, 1, c1, -1.0);
-            }
-            qv[blk] = v;
-        }
-        // trace subtraction (:139-144) touches only this lane's monomial
-        const double t = 0.5 * (qv[0] + qv[3] + qv[5]);
-        qv[0] -= t;
-        qv[3] -= t;
-        qv[5] -= t;
-#pragma unroll
-        for (int blk = 0; blk < 9; ++blk) Q[10 * blk + m] = qv[blk];
-    }
-    __syncwarp();
-    // ---- 10 x 20 coefficient matrix (:146-154 rows 0..8, :113-125 row 9): lane <-> cubic monomial ci; the linear
-    // factors (27 values) are read once per monomial, the quadratic ones once per row group
-#pragma unroll 1
-    for (int ci = sl; ci < 20; ci += 8) {
-        const int np = T->cub_n[ci];
-        const int q0 = T->cub_q[ci][0], q1 = T->cub_q[ci][1], q2 = T->cub_q[ci][2];
-        const int l0 = T->cub_l[ci][0], l1 = T->cub_l[ci][1], l2 = T->cub_l[ci][2];
-        double L0[3][3], L1[3][3], L2[3][3]; // [k][j]: PLB_EE(k, j)[l_p]
-#pragma unroll
-        for (int k = 0; k < 3; ++k)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                const double *Lk = PLB_EE(k, j);
-                L0[k][j] = Lk[l0];
-                L1[k][j] = Lk[l1];
-                L2[k][j] = Lk[l2];
-            }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { // i = 3: the determinant row
-            double Q0[3], Q1[3], Q2[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                int blk;
-                if (i < 3) {
-                    const int lo = i < k ? i : k, hi = i < k ? k : i;
-                    blk = (lo == 0) ? hi : (lo == 1 ? 2 + hi : 5);
-                } else {
-                    blk = 6 + k;
-                }
-                const double *Qb = Q + 10 * blk;
-                Q0[k] = Qb[q0];
-                Q1[k] = Qb[q1];
-                Q2[k] = Qb[q2];
-            }
-            if (i < 3) {
-#pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    double v = 0.0;
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        v += Q0[k] * L0[k][j];
-                        if (np > 1) v += Q1[k] * L1[k][j];
-                        if (np > 2) v += Q2[k] * L2[k][j];
-                    }
-                    C[(3 * i + j) * 20 + ci] = v;
-                }
-            } else {
-                double v = 0.0;
-#pragma unroll
-                for (int t = 0; t < 3; ++t) { // quad[6 + t] * PLB_EE(2, t)
-                    v += Q0[t] * L0[2][t];
-                    if (np > 1) v += Q1[t] * L1[2][t];
-                    if (np > 2) v += Q2[t] * L2[2][t];
-                }
-                C[9 * 20 + ci] = v;
-            }
-        }
-    }
-    __syncwarp();
-#undef PLB_EE
-    // ---- [A | B] -> A^{-1} B by partial-pivot LU with the forward substitution fused (:173)
-    for (int k = 0; k < 10; ++k) {
-        int p = k;
-        double best = fabs(C[k * 20 + k]);
-        for (int r = k + 1; r < 10; ++r) {
-            const double v = fabs(C[r * 20 + k]);
-            if (v > best) {
-                best = v;
-                p = r;
-            }
-        }
-        __syncwarp();
-        if (best != 0.0 && p != k) {
-            for (int c = sl; c < 20; c += 8) {
-                const double t = C[k * 20 + c];
-                C[k * 20 + c] = C[p * 20 + c];
-                C[p * 20 + c] = t;
-            }
-        }
-        __syncwarp();
-        const double pv = C[k * 20 + k];
-        __syncwarp();
-        if (best != 0.0) {
-            for (int r = sl; r < 10; r += 8)
-                if (r > k) C[r * 20 + k] /= pv;
-        }
-        __syncwarp();
-        // the multipliers of this step are read once into registers (every column of the lane reuses them); rows are
-        // walked bottom-up with static register indices, each element is updated exactly as before
-        double lmul[9];
-#pragma unroll
-        for (int j = 0; j < 9; ++j) lmul[j] = (9 - j > k) ? C[(9 - j) * 20 + k] : 0.0;
-        for (int c = k + 1 + sl; c < 20; c += 8) {
-            const double ckc = C[k * 20 + c];
-#pragma unroll
-            for (int j = 0; j < 9; ++j)
-                if (9 - j > k) C[(9 - j) * 20 + c] -= lmul[j] * ckc;
-        }
-        __syncwarp();
-    }
-    // back-substitution: only rows 4..9 of A^{-1} B enter the polynomial matrix below (:176-189), and row r depends on
-    // the rows below it only, so rows 0..3 (30 of the 45 inner-product terms per column) are never formed
-    for (int c = 10 + sl; c < 20; c += 8) {
-        for (int r = 9; r >= 4; --r) {
-            double s = C[r * 20 + c];
-            for (int k = r + 1; k < 10; ++k) s -= C[r * 20 + k] * C[k * 20 + c];
-            C[r * 20 + c] = s / C[r * 20 + r];
-        }
-    }
-    __syncwarp();
-    // ---- 3 x 13 polynomial matrix (:176-189); A aliases the dead quadratic blocks
-    double *A = W + P5_A;
-    for (int e = sl; e < 39; e += 8) {
-        const int i = e / 13, c = e % 13;
-        const double *top = C + (4 + 2 * i) * 20 + 10, *bot = C + (5 + 2 * i) * 20 + 10;
-        const int g0 = (c < 4) ? 0 : (c < 8 ? 4 : 8), src0 = (c < 4) ? 0 : (c < 8 ? 3 : 6);
-        const int w = (c < 8) ? 3 : 4, o = c - g0;
-        double v = 0.0;
-        if (o >= 1) v = top[src0 + o - 1];
-        if (o < w) v -= bot[src0 + o];
-        A[e] = v;
-    }
-    __syncwarp();
-    // ---- det(A(z)) as a degree-10 polynomial, ascending coefficients (:191-352)
-    {
-        auto P = [&](int i, int j, int k) -> double {
-            return (j == 0) ? A[13 * i + 3 - k] : (j == 1 ? A[13 * i + 7 - k] : A[13 * i + 12 - k]);
-        };
-        double *minors = W + P5_MIN;
-#pragma unroll
-        for (int t = 0; t < 3; ++t) { // minor t, coefficient k = sl
-            const int k = sl;
-            const int ja = (t == 0) ? 1 : 0, jb = (t == 2) ? 1 : 2;
-            const int da = 3, db = (jb == 2) ? 4 : 3;
-            double v = 0.0;
-            if (k <= da + db) {
-                double s1 = 0.0, s2 = 0.0;
-                for (int i = 0; i <= da; ++i) {
-                    const int j = k - i;
-                    if (j >= 0 && j <= db) s1 += P(1, ja, i) * P(2, jb, j);
-                }
-                for (int i = 0; i <= db; ++i) {
-                    const int j = k - i;
-                    if (j >= 0 && j <= da) s2 += P(1, jb, i) * P(2, ja, j);
-                }
-                v = s1 - s2;
-            }
-            minors[8 * t + k] = v;
-        }
-        __syncwarp();
-        for (int k = sl; k < 11; k += 8) {
-            double t0 = 0.0, t1 = 0.0, t2 = 0.0;
-            for (int i = 0; i <= 3; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 7) t0 += P(0, 0, i) * minors[j];
-            }
-            for (int i = 0; i <= 3; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 7) t1 += P(0, 1, i) * minors[8 + j];
-            }
-            for (int i = 0; i <= 4; ++i) {
-                const int j = k - i;
-                if (j >= 0 && j <= 6) t2 += P(0, 2, i) * minors[16 + j];
-            }
-            double c = 0.0;
-            c += t0;
-            c -= t1;
-            c += t2;
-            W[P5_CPOLY + k] = c;
-        }
-        __syncwarp();
-    }
-}
-
 // Back-substitution for one root z of the determinant polynomial: E (row-major 9) from the polynomial matrix A (3x13)
 // and the nullspace basis Nb (relpose_5pt.cc:359-392).
 // A / Nb: anything indexable (plain pointers, or StridedD views of the entry-major per-sample blocks).
@@ -1655,20 +876,6 @@ template <class VA, class VN> PLB_DEV void backsub_5pt(VA A, VN Nb, double z, do
     }
 }
 
-// Essential matrices from 5 bearing pairs.  x1s/x2s: shared arrays of 5 unit bearings (3 doubles each).
-// On return S->Es holds nroots row-major E matrices (relpose_5pt.cc:159-395).  Returns nroots (uniform).
-PLB_DEV int solve_5pt_E(const double *x1s, const double *x2s, Scratch5 *S, const MonoTables *T, int lane) {
-    solve_5pt_poly(x1s, x2s, S, T, lane);
-    // ---- real roots by Sturm bracketing (:356): scalar work on lane 0
-    if (lane == 0) S->nroots = sturm_bisect10(S->cpoly, S->roots, &S->sturm);
-    __syncwarp();
-    const int n = S->nroots;
-    // ---- back-substitution, one lane per root (:359-392)
-    if (lane < n) backsub_5pt(S->A, S->Nb, S->roots[lane], S->Es + 9 * lane);
-    __syncwarp();
-    return n;
-}
-
 // Four motion hypotheses of an essential matrix, filtered by cheirality on the sample (misc/essential.cc:103-169).
 // E: row-major; x1s/x2s: ns unit bearings each.  Returns a 4-bit mask of accepted candidates and writes all four
 // candidate poses to cand[4][7] (registers of the calling lane).
@@ -1751,91 +958,6 @@ template <class VX> PLB_DEV unsigned motions_from_E(const double *E9, VX x1s, VX
     return mask;
 }
 
-// Full relpose_5pt: poses (7 doubles each, up to 40) into `out` in the reference's order (E-major, then the four
-// candidates); returns the number of poses (uniform).   relpose_5pt.cc:397-409
-PLB_DEV int solve_5pt_poses(const double *x1s, const double *x2s, Scratch5 *S, const MonoTables *T, double *out,
-                            int lane) {
-    const int n = solve_5pt_E(x1s, x2s, S, T, lane);
-    double cand[4][7];
-    unsigned mask = 0;
-    if (lane < n) mask = motions_from_E(S->Es + 9 * lane, x1s, x2s, 5, cand);
-    const int mine = __popc(mask);
-    // exclusive prefix over lanes
-    int pre = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, pre, o);
-        if (lane >= o) pre += v;
-    }
-    const int total = __shfl_sync(0xffffffffu, pre, 31);
-    int pos = pre - mine;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        if (mask & (1u << c)) {
-            double *o = out + 7 * pos;
-#pragma unroll
-            for (int k = 0; k < 7; ++k) o[k] = cand[c][k];
-            ++pos;
-        }
-    }
-    __syncwarp();
-    return total;
-}
-
-// ================================ relpose_7pt ==============================================================
-struct Scratch7 {
-    double M[63];  // 9x7, col-major
-    double N[18];  // two basis vectors, N[9*j + k]
-};
-// F matrices (9 doubles COLUMN-major each, up to 3) into out; returns count (uniform).  relpose_7pt.cc:10-60
-PLB_DEV int solve_7pt(const double *x1s, const double *x2s, Scratch7 *S, double *out, int lane) {
-    for (int e = lane; e < 63; e += 32) {
-        const int i = e / 9, k = e % 9;
-        S->M[e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
-    }
-    __syncwarp();
-    warp_nullspace_9xC<7>(S->M, S->N, lane);
-    const double *n0 = S->N, *n1 = S->N + 9;
-    // mixed determinants: column j of the 3x3 (col-major 9-vector) taken from a, b, c respectively
-    auto detc = [](const double *a, const double *b, const double *c) -> double {
-        const double *c0 = a, *c1 = b + 3, *c2 = c + 6;
-        return c0[0] * (c1[1] * c2[2] - c1[2] * c2[1]) - c1[0] * (c0[1] * c2[2] - c0[2] * c2[1]) +
-               c2[0] * (c0[1] * c1[2] - c0[2] * c1[1]);
-    };
-    const double c3 = detc(n0, n0, n0);
-    const double c2 = detc(n1, n0, n0) + detc(n0, n1, n0) + detc(n0, n0, n1);
-    const double c1 = detc(n0, n1, n1) + detc(n1, n0, n1) + detc(n1, n1, n0);
-    const double c0 = detc(n1, n1, n1);
-    double roots[3];
-    int n_roots;
-    if (fabs(c3) < 1e-14) {
-        n_roots = quadratic_real(c2, c1, c0, roots);
-    } else {
-        const double inv_c3 = 1.0 / c3;
-        n_roots = cubic_real(c2 * inv_c3, c1 * inv_c3, c0 * inv_c3, roots);
-    }
-    if (lane < n_roots) {
-        double r = roots[0];
-        if (lane == 1) r = roots[1];
-        if (lane == 2) r = roots[2];
-        double f[9], n2 = 0.0;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) {
-            f[k] = n0[k] * r + n1[k];
-            n2 += f[k] * f[k];
-        }
-        if (n2 > 0) {
-            const double nn = sqrt(n2);
-#pragma unroll
-            for (int k = 0; k < 9; ++k) f[k] /= nn;
-        }
-#pragma unroll
-        for (int k = 0; k < 9; ++k) out[9 * lane + k] = f[k];
-    }
-    __syncwarp();
-    return n_roots;
-}
-
 // robust/utils.cc:646-672 — note the reference stores the products in `float`
 PLB_DEV bool rfc_ok(const double *Fc /*column-major*/) {
 #define F_(r, c) Fc[3 * (c) + (r)]
@@ -1856,6 +978,69 @@ PLB_DEV bool rfc_ok(const double *Fc /*column-major*/) {
     if (num * den < 0) return false;
     return true;
 #undef F_
+}
+
+// ================================ relpose_7pt ==============================================================
+// F matrices (column-major) of 7 bearing pairs into F[0..n), n returned; only those for which keep(f) holds are listed,
+// order preserved (the real-focal check of estimators/relative_pose.cc:393-398).  relpose_7pt.cc:10-60
+// W: the thread's 63-double scratch (the 9 x 7 system for lane5::nullspace_9xC).
+template <class Keep> PLB_DEV int fundamental_7pt(const double *x1s, const double *x2s, double *W, Keep &&keep, double F[3][9]) {
+#pragma unroll
+    for (int e = 0; e < 63; ++e) {
+        const int i = e / 9, k = e % 9;
+        W[e] = x1s[3 * i + k / 3] * x2s[3 * i + k % 3];
+    }
+    double nn[18];
+    lane5::nullspace_9xC<7>(W, nn);
+    const double *n0 = nn, *n1 = nn + 9;
+    // mixed determinants: column j of the 3x3 (col-major 9-vector) taken from a, b, c respectively
+    auto detc = [](const double *a, const double *b, const double *c) -> double {
+        const double *c0 = a, *c1 = b + 3, *c2 = c + 6;
+        return c0[0] * (c1[1] * c2[2] - c1[2] * c2[1]) - c1[0] * (c0[1] * c2[2] - c0[2] * c2[1]) +
+               c2[0] * (c0[1] * c1[2] - c0[2] * c1[1]);
+    };
+    const double c3 = detc(n0, n0, n0);
+    const double c2 = detc(n1, n0, n0) + detc(n0, n1, n0) + detc(n0, n0, n1);
+    const double c1 = detc(n0, n1, n1) + detc(n1, n0, n1) + detc(n1, n1, n0);
+    const double c0 = detc(n1, n1, n1);
+    double roots[3];
+    int n_roots;
+    if (fabs(c3) < 1e-14) {
+        n_roots = quadratic_real(c2, c1, c0, roots);
+    } else {
+        const double inv_c3 = 1.0 / c3;
+        n_roots = cubic_real(c2 * inv_c3, c1 * inv_c3, c0 * inv_c3, roots);
+    }
+    int nm = 0;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        if (j < n_roots) {
+            const double r = roots[j];
+            double f[9];
+            double n2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 9; ++k) {
+                f[k] = n0[k] * r + n1[k];
+                n2 += f[k] * f[k];
+            }
+            if (n2 > 0) {
+                const double nrm = sqrt(n2);
+#pragma unroll
+                for (int k = 0; k < 9; ++k) f[k] /= nrm;
+            }
+            if (keep(f)) {
+                // nm is 0, 1 or 2 here: predicated copies keep F in registers
+#pragma unroll
+                for (int m = 0; m < 3; ++m)
+                    if (m == nm) {
+#pragma unroll
+                        for (int k = 0; k < 9; ++k) F[m][k] = f[k];
+                    }
+                ++nm;
+            }
+        }
+    }
+    return nm;
 }
 
 } // namespace plb
