@@ -193,14 +193,6 @@ template <typename T> struct MapBuf {
     }
 };
 
-__global__ void k_gather_models(const double *__restrict__ models, const int *__restrict__ slots, int n, int msz,
-                                double *__restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * 9) return;
-    const int j = i / 9, k = i % 9;
-    out[i] = (k < msz) ? models[(size_t)slots[j] * msz + k] : 0.0;
-}
-
 struct Engine {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr;
@@ -553,7 +545,7 @@ struct Task {
 struct PState {
     Task *t = nullptr;
     int n = 0, n_pad = 0, pidx = 0;
-    bool enough = false, active = false, broke = false;
+    bool enough = false, active = false;
     bool hyp_pending = false; // hypotheses of the last (broken) round still to be added from Engine::h_hypfix
     size_t it = 0, chunk = 1024;
     size_t best_minimal_inlier_count = 0;
@@ -577,64 +569,85 @@ static void update_dynamic(PState &S, int K) { // ransac_impl.h:150-153
                                                   S.t->opt.max_iterations);
 }
 
-// Runs a group of problems of the same kind in lock-step rounds: one solve launch, one score launch and (when some
-// model improved) one gather + one LM launch per round for the WHOLE group.
-static int run_group(int kind, std::vector<Task *> &tasks) {
-    Engine &E = *engine();
-    const int K = kind_sample_size(kind), MAXM = kind_max_models(kind), MSZ = kind_model_size(kind);
+// One LM job staged by the host: its start model (MSZ doubles) and its description.
+struct LmTask {
+    const double *model;
+    LmJob job;
+};
+static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
+    LmJob J;
+    J.pidx = pidx;
+    J.reserved = 0;
+    J.mask_off = mask_off;
+    J.scratch_off = 0;
+    J.prm = prm;
+    return J;
+}
+
+static bool profiling() {
+    static const bool on = std::getenv("PLB_PROFILE") != nullptr;
+    return on;
+}
+
+// A group of problems of the same kind, run in lock-step rounds: one solve launch, one score launch and one LM launch
+// per round for the WHOLE group.  The member functions are the phases of run_group, in the order it calls them.
+struct Group {
+    Engine &E;
+    const int kind, K, MAXM, MSZ;
     // in_arr: doubles per correspondence in the caller layout; n_arr: SoA arrays resident per correspondence
-    const int b_dim = (kind == KIND_PNP) ? 3 : 2, in_arr = 2 + b_dim, n_arr = (kind == KIND_RELPOSE_TS) ? TS_ARRAYS : in_arr;
-    const int NP = (int)tasks.size();
-    std::vector<PState> PS(NP);
-    bool any_points = false;
-    for (int i = 0; i < NP; ++i) {
-        Task &t = *tasks[i];
-        PState &S = PS[i];
-        S.t = &t;
-        std::memset(&S.cnt, 0, sizeof(S.cnt));
-        S.stats.refinements = S.stats.iterations = S.stats.num_inliers = 0;
-        S.stats.inlier_ratio = 0;
-        S.stats.model_score = std::numeric_limits<double>::max();
-        if (!t.opt.score_initial_model) { // ransac.cc:47-50 etc.: identity unless an initial model is scored
-            std::fill(t.model, t.model + MSZ, 0.0);
-            if (MSZ == 7) t.model[0] = 1.0;
-            else t.model[0] = t.model[4] = t.model[8] = 1.0;
-        }
-        std::fill(S.best_model, S.best_model + 9, 0.0);
-        std::copy(t.model, t.model + MSZ, S.best_model);
-        if (t.n > (size_t)(1u << 26)) {
-            g_err = "too many correspondences";
-            return PLB_ERR_ARG;
-        }
-        S.n = (int)t.n;
-        S.n_pad = (S.n + 31) & ~31;
-        S.enough = t.n >= (size_t)K; // ransac_impl.h:161-163
-        S.dynamic_max_iter = t.opt.max_iterations;
-        S.log_prob_missing_model = std::log(1.0 - t.opt.success_prob);
-        any_points |= (t.n > 0);
-    }
-    auto finish = [&]() {
-        for (int i = 0; i < NP; ++i) {
-            PState &S = PS[i];
-            if (S.hyp_pending) S.cnt.hypotheses += (uint64_t)E.h_hypfix.p[S.pidx];
-            S.cnt.scored_corrs = S.cnt.hypotheses * S.t->n;
-            if (S.t->stats_out) *S.t->stats_out = S.stats;
-            if (S.t->cnt_out) *S.t->cnt_out = S.cnt;
-        }
-    };
-    if (!any_points) {
-        finish();
-        return PLB_OK;
-    }
-    int rc = E.init();
-    if (rc != PLB_OK) return rc;
-    lm_set_sm_share(t_batch_worker ? 50 : 100); // a lone call owns the GPU; batch groups share it
-    cudaStream_t st = E.stream;
-    const uint64_t launches0 = E.launches;
-    uint64_t h2d = 0, d2h = 0;
+    const int b_dim, in_arr, n_arr, NP;
+    std::vector<PState> PS;
+    cudaStream_t st = nullptr;
+    // device layout of the group (upload)
+    size_t in_doubles = 0, soa_elems = 0, mask_bytes = 0, px_elems = 0;
+    int max_n = 0, max_n_pad = 0, n_up = 0, n_probdev = 0;
+    // Round sizes.  A small group leaves the GPU mostly idle, so speculating further ahead costs little time while every
+    // round saved is a whole launch chain of latency: the first round and the per-round cap grow as the group shrinks
+    // (1 problem: 4096 doubling up to 65536 samples; >= 16 problems: 1024 doubling to 16384).  The first round stays
+    // moderate on purpose: a loop that stops right after min_iterations (high inlier ratio) would otherwise pay for
+    // thousands of speculative samples and their LO refits (measured: C4 single call 2.0 -> 3.3 ms with 16384).
+    const size_t few, CHUNK_MAX, ROUND_MAX;
+    static constexpr size_t S_TOT_MAX = 262144;
+    // 0 exact, 1 fast (fp32 screen + fp64 confirmation of candidates); the tangent-Sampson kind has no fp32 copy
+    const int mode;
+    int cap_factor;
+    bool big_caps = false;
+    int smp_cur = 0; // sampler states of the current round: E.smp[smp_cur * NP ..]; the advanced ones land in the other half
+    std::vector<int> act; // active problems of the current round
+    std::vector<uint8_t> first_round;
+    // counters of the group
+    uint64_t launches0 = 0, h2d = 0, d2h = 0;
+    int n_rounds = 0;
     double lo_wait = 0.0;
     float gpu_ms_total = 0.f, gpu_ms_score = 0.f, gpu_ms_confirm = 0.f, gpu_ms_lo = 0.f;
-    auto sync_timed = [&](double *acc) -> int {
+    // host-side phase timer (PLB_PROFILE=1 prints one line per group to stderr)
+    enum { PH_SETUP, PH_SAMPLE, PH_LAUNCH, PH_WAIT_HYP, PH_REPLAY, PH_FINAL, PH_N };
+    double ph[PH_N] = {0};
+    std::chrono::steady_clock::time_point ph_t = std::chrono::steady_clock::now();
+
+    Group(int kind_, std::vector<Task *> &tasks)
+        : E(*engine()), kind(kind_), K(kind_sample_size(kind_)), MAXM(kind_max_models(kind_)),
+          MSZ(kind_model_size(kind_)), b_dim(kind_ == KIND_PNP ? 3 : 2), in_arr(2 + b_dim),
+          n_arr(kind_ == KIND_RELPOSE_TS ? TS_ARRAYS : in_arr), NP((int)tasks.size()), PS(NP),
+          few((size_t)std::max(1, std::min(NP, 16))), CHUNK_MAX(std::max<size_t>(16384, 65536 / few)),
+          ROUND_MAX(std::max<size_t>(32768, 65536 / few)), mode(kind_ == KIND_RELPOSE_TS ? 0 : current_mode()),
+          cap_factor(kind_is_relpose(kind_) ? 8 : MAXM), first_round(NP, 1) {
+        for (int i = 0; i < NP; ++i) {
+            PState &S = PS[i];
+            S.t = tasks[i];
+            S.pidx = i;
+            S.n = (int)S.t->n;
+            S.n_pad = (S.n + 31) & ~31;
+        }
+    }
+
+    int init() {
+        int rc = E.init();
+        st = E.stream;
+        launches0 = E.launches;
+        return rc;
+    }
+    int sync(double *acc = nullptr) {
         auto t0 = std::chrono::steady_clock::now();
         if (t_blocking_sync) { // more waiting threads than cores: sleep on an event instead of spinning on the stream
             PLB_CUDA(cudaEventRecord(E.ev_block, st));
@@ -644,49 +657,68 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         }
         if (acc) *acc += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
         return PLB_OK;
-    };
-
-    // host-side phase timer (PLB_PROFILE=1 prints one line per group to stderr)
-    static const bool prof_on = std::getenv("PLB_PROFILE") != nullptr;
-    enum { PH_SETUP, PH_SAMPLE, PH_LAUNCH, PH_WAIT_HYP, PH_SELECT, PH_WAIT_CONF, PH_PASS1, PH_WAIT_LM, PH_PASS2, PH_FINAL, PH_N };
-    double ph[PH_N] = {0};
-    auto ph_t = std::chrono::steady_clock::now();
-    auto mark = [&](int which) {
-        if (!prof_on) return;
+    }
+    void mark(int which) {
+        if (!profiling()) return;
         const auto now = std::chrono::steady_clock::now();
         ph[which] += std::chrono::duration<double>(now - ph_t).count();
         ph_t = now;
-    };
-    int n_rounds = 0;
-
-    // ---- device layout of the group: SoA arrays of every non-resident problem, masks, ProblemDev table -----------
-    size_t in_doubles = 0, soa_elems = 0, mask_bytes = 0, px_elems = 0;
-    int max_n = 0, max_n_pad = 0, n_up = 0, n_polish_pnp = 0;
-    for (PState &S : PS) {
-        if (S.n == 0) continue;
-        if (!S.t->res) {
-            in_doubles += (size_t)in_arr * S.n;
-            soa_elems += (size_t)n_arr * S.n_pad;
-            ++n_up;
-        }
-        S.mask_off = (long long)mask_bytes;
-        mask_bytes += (size_t)S.n_pad;
-        max_n = std::max(max_n, S.n);
-        max_n_pad = std::max(max_n_pad, S.n_pad);
-        if (kind == KIND_PNP && S.t->polish.enabled && S.t->polish.px_scaled) {
-            px_elems += 2 * (size_t)S.n_pad;
-            ++n_polish_pnp;
-        }
     }
-    const int n_probdev = NP + n_polish_pnp;
-    if ((rc = E.h_in.ensure(in_doubles + px_elems)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
-        (rc = E.soa32.ensure(soa_elems)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
-        (rc = E.mask_bits.ensure(mask_bytes / 32 + 1)) || (rc = E.h_mask_bits.ensure(mask_bytes / 32 + 1)) ||
-        (rc = E.work.ensure(8)) || (rc = E.probs.ensure(n_probdev)) ||
-        (rc = E.h_probs.ensure(n_probdev)) || (rc = E.tdesc.ensure(std::max(n_up, 1))) ||
-        (rc = E.h_tdesc.ensure(std::max(n_up, 1))))
-        return rc;
-    {
+
+    // ---- state of the serial loop before its first iteration (ransac_impl.h:157-176) --------------------------------
+    int init_states() {
+        for (PState &S : PS) {
+            Task &t = *S.t;
+            std::memset(&S.cnt, 0, sizeof(S.cnt));
+            S.stats.refinements = S.stats.iterations = S.stats.num_inliers = 0;
+            S.stats.inlier_ratio = 0;
+            S.stats.model_score = std::numeric_limits<double>::max();
+            if (!t.opt.score_initial_model) { // ransac.cc:47-50 etc.: identity unless an initial model is scored
+                std::fill(t.model, t.model + MSZ, 0.0);
+                if (MSZ == 7) t.model[0] = 1.0;
+                else t.model[0] = t.model[4] = t.model[8] = 1.0;
+            }
+            std::fill(S.best_model, S.best_model + 9, 0.0);
+            std::copy(t.model, t.model + MSZ, S.best_model);
+            if (t.n > (size_t)(1u << 26)) {
+                g_err = "too many correspondences";
+                return PLB_ERR_ARG;
+            }
+            S.enough = t.n >= (size_t)K; // ransac_impl.h:161-163
+            S.dynamic_max_iter = t.opt.max_iterations;
+            S.log_prob_missing_model = std::log(1.0 - t.opt.success_prob);
+        }
+        return PLB_OK;
+    }
+
+    // ---- device layout of the group: SoA arrays of every non-resident problem, masks, ProblemDev table -------------
+    // Stages the caller's arrays and issues their host -> device copies; the layout kernel runs in transpose().
+    int upload() {
+        int rc, n_polish_pnp = 0;
+        for (PState &S : PS) {
+            if (S.n == 0) continue;
+            if (!S.t->res) {
+                in_doubles += (size_t)in_arr * S.n;
+                soa_elems += (size_t)n_arr * S.n_pad;
+                ++n_up;
+            }
+            S.mask_off = (long long)mask_bytes;
+            mask_bytes += (size_t)S.n_pad;
+            max_n = std::max(max_n, S.n);
+            max_n_pad = std::max(max_n_pad, S.n_pad);
+            if (kind == KIND_PNP && S.t->polish.enabled && S.t->polish.px_scaled) {
+                px_elems += 2 * (size_t)S.n_pad;
+                ++n_polish_pnp;
+            }
+        }
+        n_probdev = NP + n_polish_pnp;
+        if ((rc = E.h_in.ensure(in_doubles + px_elems)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
+            (rc = E.soa32.ensure(soa_elems)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
+            (rc = E.mask_bits.ensure(mask_bytes / 32 + 1)) || (rc = E.h_mask_bits.ensure(mask_bytes / 32 + 1)) ||
+            (rc = E.work.ensure(8)) || (rc = E.probs.ensure(n_probdev)) ||
+            (rc = E.h_probs.ensure(n_probdev)) || (rc = E.tdesc.ensure(std::max(n_up, 1))) ||
+            (rc = E.h_tdesc.ensure(std::max(n_up, 1))))
+            return rc;
         struct DirectCopy {
             double *dst;
             const double *src;
@@ -698,7 +730,6 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         int iu = 0, ipol = 0;
         for (int i = 0; i < NP; ++i) {
             PState &S = PS[i];
-            S.pidx = i;
             ProblemDev &P = E.h_probs.p[i];
             std::memset(&P, 0, sizeof(P));
             P.n = S.n;
@@ -787,50 +818,56 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             PLB_CUDA(cudaMemcpyAsync(E.px64.p, E.h_in.p + in_doubles, sizeof(double) * px_elems, cudaMemcpyHostToDevice, st));
             h2d += sizeof(double) * px_elems;
         }
-        if (upload_turn.owns_lock()) upload_turn.unlock();
-        // ---- normalize_points on the device (robust/utils.cc:584-644), then the thresholds that depend on its scale
-        {
-            std::vector<int> who;
-            for (int i = 0; i < NP; ++i)
-                if (PS[i].t->norm_mode != 0 && PS[i].in_off >= 0 && PS[i].n > 0) who.push_back(i);
-            const int nn = (int)who.size();
-            if (nn) {
-                if ((rc = E.ndesc.ensure(nn)) || (rc = E.h_ndesc.ensure(nn)) || (rc = E.h_norm.ensure(5 * (size_t)nn))) return rc;
-                for (int j = 0; j < nn; ++j) {
-                    const PState &S = PS[who[j]];
-                    NormDesc &D = E.h_ndesc.p[j];
-                    D.a = E.in.p + S.in_off;
-                    D.b = D.a + 2 * (size_t)S.n;
-                    D.out = E.h_norm.d + 5 * (size_t)j;
-                    D.n = S.n;
-                    D.centroid = S.t->norm_mode == 2 ? 1 : 0;
-                }
-                PLB_CUDA(cudaMemcpyAsync(E.ndesc.p, E.h_ndesc.p, sizeof(NormDesc) * nn, cudaMemcpyHostToDevice, st));
-                launch_normalize(E.ndesc.p, nn, st);
-                E.launches++;
-                if ((rc = sync_timed(nullptr))) return rc;
-                d2h += sizeof(double) * 5 * (size_t)nn;
-                for (int j = 0; j < nn; ++j) {
-                    Task &t = *PS[who[j]].t;
-                    std::copy(E.h_norm.p + 5 * (size_t)j, E.h_norm.p + 5 * (size_t)j + 5, t.norm_out);
-                    const double scale = t.norm_out[4];
-                    t.max_error = t.max_error / scale;                                 // robust.cc:562,725
-                    t.polish.bundle.loss_scale = t.polish.bundle.loss_scale / scale; // :563,726
-                    E.h_probs.p[who[j]].sq_thr = t.max_error * t.max_error;
-                    if (t.opt.score_initial_model) { // robust.cc:566-569 / 729-732: the start model in normalised coordinates
-                        HM3 T1, T2;
-                        norm_transforms(t.norm_out, T1, T2);
-                        HM3 M = (kind == KIND_FUND) ? hm_mul(hm_mul(hm_inv(hm_T(T2)), hm_from_cm(t.model)), hm_inv(T1))
-                                                    : hm_mul(hm_mul(T2, hm_from_cm(t.model)), hm_inv(T1));
-                        const double nm = hm_norm(M);
-                        for (int r = 0; r < 3; ++r)
-                            for (int c = 0; c < 3; ++c) M.m[r][c] /= nm;
-                        hm_to_cm(M, t.model);
-                        std::copy(t.model, t.model + 9, PS[who[j]].best_model);
-                    }
-                }
+        return PLB_OK;
+    }
+
+    // ---- normalize_points on the device (robust/utils.cc:584-644), then the thresholds that depend on its scale ------
+    int normalize() {
+        std::vector<int> who;
+        for (int i = 0; i < NP; ++i)
+            if (PS[i].t->norm_mode != 0 && PS[i].in_off >= 0 && PS[i].n > 0) who.push_back(i);
+        const int nn = (int)who.size();
+        if (!nn) return PLB_OK;
+        int rc;
+        if ((rc = E.ndesc.ensure(nn)) || (rc = E.h_ndesc.ensure(nn)) || (rc = E.h_norm.ensure(5 * (size_t)nn))) return rc;
+        for (int j = 0; j < nn; ++j) {
+            const PState &S = PS[who[j]];
+            NormDesc &D = E.h_ndesc.p[j];
+            D.a = E.in.p + S.in_off;
+            D.b = D.a + 2 * (size_t)S.n;
+            D.out = E.h_norm.d + 5 * (size_t)j;
+            D.n = S.n;
+            D.centroid = S.t->norm_mode == 2 ? 1 : 0;
+        }
+        PLB_CUDA(cudaMemcpyAsync(E.ndesc.p, E.h_ndesc.p, sizeof(NormDesc) * nn, cudaMemcpyHostToDevice, st));
+        launch_normalize(E.ndesc.p, nn, st);
+        E.launches++;
+        if ((rc = sync())) return rc;
+        d2h += sizeof(double) * 5 * (size_t)nn;
+        for (int j = 0; j < nn; ++j) {
+            Task &t = *PS[who[j]].t;
+            std::copy(E.h_norm.p + 5 * (size_t)j, E.h_norm.p + 5 * (size_t)j + 5, t.norm_out);
+            const double scale = t.norm_out[4];
+            t.max_error = t.max_error / scale;                                 // robust.cc:562,725
+            t.polish.bundle.loss_scale = t.polish.bundle.loss_scale / scale; // :563,726
+            E.h_probs.p[who[j]].sq_thr = t.max_error * t.max_error;
+            if (t.opt.score_initial_model) { // robust.cc:566-569 / 729-732: the start model in normalised coordinates
+                HM3 T1, T2;
+                norm_transforms(t.norm_out, T1, T2);
+                HM3 M = (kind == KIND_FUND) ? hm_mul(hm_mul(hm_inv(hm_T(T2)), hm_from_cm(t.model)), hm_inv(T1))
+                                            : hm_mul(hm_mul(T2, hm_from_cm(t.model)), hm_inv(T1));
+                const double nm = hm_norm(M);
+                for (int r = 0; r < 3; ++r)
+                    for (int c = 0; c < 3; ++c) M.m[r][c] /= nm;
+                hm_to_cm(M, t.model);
+                std::copy(t.model, t.model + 9, PS[who[j]].best_model);
             }
         }
+        return PLB_OK;
+    }
+
+    // ---- ProblemDev table (final thresholds) and the layout kernel: caller AoS -> resident SoA ------------------------
+    int transpose() {
         PLB_CUDA(cudaMemcpyAsync(E.probs.p, E.h_probs.p, sizeof(ProblemDev) * n_probdev, cudaMemcpyHostToDevice, st));
         if (n_up) {
             PLB_CUDA(cudaMemsetAsync(E.cmax.p, 0, sizeof(float) * 5 * (size_t)NP, st));
@@ -838,114 +875,103 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             launch_transpose(E.tdesc.p, n_up, max_n_pad, st);
             E.launches++;
         }
+        return PLB_OK;
     }
 
-    // LM launch helper: jobs[] + their input models already in E.h_lm_in[0 .. 9*njobs) (or on device, see gathered)
-    auto launch_lm_jobs = [&](int njobs, bool models_on_device, size_t dev_model_off) -> int {
-        int r;
-        if ((r = E.jobs.ensure(njobs)) || (r = E.h_lm_out.ensure(njobs)) || (r = E.lm_in.ensure(9 * (size_t)njobs + dev_model_off)))
-            return r;
-        PLB_CUDA(cudaMemcpyAsync(E.jobs.p, E.h_jobs.p, sizeof(LmJob) * njobs, cudaMemcpyHostToDevice, st));
-        h2d += sizeof(LmJob) * njobs;
-        if (!models_on_device) {
-            PLB_CUDA(cudaMemcpyAsync(E.lm_in.p + dev_model_off, E.h_lm_in.p, sizeof(double) * 9 * njobs, cudaMemcpyHostToDevice, st));
-            h2d += sizeof(double) * 9 * njobs;
+    // Stages a batch of LM jobs (job j: start model batch[j].model, results in E.h_lm_out[j]) and launches them in one
+    // k_lm launch.  The caller synchronises.
+    int lm_batch(const std::vector<LmTask> &batch) {
+        const int nj = (int)batch.size();
+        int rc;
+        if ((rc = E.h_lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_jobs.ensure(nj)) || (rc = E.jobs.ensure(nj)) ||
+            (rc = E.lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_lm_out.ensure(nj)) ||
+            (rc = E.subset.ensure((size_t)nj * max_n_pad)))
+            return rc;
+        for (int j = 0; j < nj; ++j) {
+            double *row = E.h_lm_in.p + 9 * (size_t)j;
+            std::fill(row, row + 9, 0.0);
+            std::copy(batch[j].model, batch[j].model + MSZ, row);
+            E.h_jobs.p[j] = batch[j].job;
+            E.h_jobs.p[j].scratch_off = (long long)j * max_n_pad;
         }
-        launch_lm(kind, E.probs.p, E.jobs.p, E.lm_in.p + dev_model_off, njobs, max_n, E.mask.p, E.subset.p, max_n_pad,
-                  E.h_lm_out.d, st);
+        PLB_CUDA(cudaMemcpyAsync(E.jobs.p, E.h_jobs.p, sizeof(LmJob) * nj, cudaMemcpyHostToDevice, st));
+        PLB_CUDA(cudaMemcpyAsync(E.lm_in.p, E.h_lm_in.p, sizeof(double) * 9 * nj, cudaMemcpyHostToDevice, st));
+        h2d += (sizeof(LmJob) + sizeof(double) * 9) * nj;
+        launch_lm(kind, E.probs.p, E.jobs.p, E.lm_in.p, nj, max_n, E.mask.p, E.subset.p, max_n_pad, E.h_lm_out.d, st);
         E.launches++;
-        d2h += sizeof(LmJobOut) * njobs;
+        d2h += sizeof(LmJobOut) * nj;
         return PLB_OK;
-    };
-    auto make_lo_job = [&](LmJob &J, const PState &S, long long scratch_off) {
-        J.pidx = S.pidx;
-        J.reserved = 0;
-        J.mask_off = -1;
-        J.scratch_off = scratch_off;
-        J.prm = lo_params(kind, S.t->max_error);
-    };
+    }
+    LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
+    // one LO call of the serial loop and its result (ransac_impl.h:135-153)
+    void apply_lo(PState &S, const LmJobOut &o) const {
+        S.stats.refinements++;
+        S.cnt.lo_calls++;
+        S.cnt.hypotheses++;
+        if (o.score < S.stats.model_score) {
+            S.stats.model_score = o.score;
+            S.stats.num_inliers = o.count;
+            std::copy(o.model, o.model + MSZ, S.best_model);
+        }
+        update_dynamic(S, K);
+    }
 
-    // ---- initial models (ransac_impl.h:173-176) ------------------------------------------------------------------
-    {
+    // ---- initial models (ransac_impl.h:173-176) ----------------------------------------------------------------------
+    int score_initial_models() {
         std::vector<int> who;
         for (int i = 0; i < NP; ++i)
             if (PS[i].enough && PS[i].t->opt.score_initial_model) who.push_back(i);
         const int nw = (int)who.size();
-        if (nw) {
-            if ((rc = E.h_lm_in.ensure(9 * (size_t)nw)) || (rc = E.lm_in.ensure(9 * (size_t)nw)) || (rc = E.h_slots.ensure(nw)) ||
-                (rc = E.slots.ensure(nw)) || (rc = E.h_counts.ensure(nw)) || (rc = E.h_scores.ensure(nw)) ||
-                (rc = E.h_jobs.ensure(nw)) || (rc = E.subset.ensure((size_t)nw * max_n_pad)))
-                return rc;
-            // the 9-double staging rows double as the MSZ-strided model list expected by k_score
-            std::vector<double> packed((size_t)nw * MSZ);
-            for (int j = 0; j < nw; ++j) {
-                std::fill(E.h_lm_in.p + 9 * j, E.h_lm_in.p + 9 * j + 9, 0.0);
-                std::copy(PS[who[j]].t->model, PS[who[j]].t->model + MSZ, E.h_lm_in.p + 9 * j);
-                std::copy(PS[who[j]].t->model, PS[who[j]].t->model + MSZ, packed.data() + (size_t)j * MSZ);
-                E.h_slots.p[j] = who[j];
-            }
-            if ((rc = E.models.ensure((size_t)nw * MSZ))) return rc;
-            PLB_CUDA(cudaMemcpyAsync(E.models.p, packed.data(), sizeof(double) * nw * MSZ, cudaMemcpyHostToDevice, st));
-            PLB_CUDA(cudaMemcpyAsync(E.slots.p, E.h_slots.p, sizeof(int) * nw, cudaMemcpyHostToDevice, st));
-            PLB_CUDA(cudaMemcpyAsync(E.work.p + 4, &nw, sizeof(int), cudaMemcpyHostToDevice, st));
-            launch_score_models(kind, E.probs.p, E.models.p, E.slots.p, nw, E.work.p + 4, E.h_counts.d, E.h_scores.d, st);
-            E.launches++;
-            if ((rc = sync_timed(nullptr))) return rc;
-            int nj = 0;
-            std::vector<int> jw;
-            for (int j = 0; j < nw; ++j) {
-                PState &S = PS[who[j]];
-                const size_t ic = E.h_counts.p[j];
-                const double sc = E.h_scores.p[j];
-                S.cnt.hypotheses++;
-                const bool more = ic > S.best_minimal_inlier_count, better = sc < S.best_minimal_msac_score;
-                if (more || better) {
-                    if (more) S.best_minimal_inlier_count = ic;
-                    if (better) S.best_minimal_msac_score = sc;
-                    if (sc < S.stats.model_score) {
-                        S.stats.model_score = sc;
-                        S.stats.num_inliers = ic;
-                    }
-                    make_lo_job(E.h_jobs.p[nj], S, (long long)nj * max_n_pad);
-                    if (nj != j) std::copy(E.h_lm_in.p + 9 * j, E.h_lm_in.p + 9 * j + 9, E.h_lm_in.p + 9 * nj);
-                    jw.push_back(who[j]);
-                    ++nj;
+        if (!nw) return PLB_OK;
+        int rc;
+        if ((rc = E.h_slots.ensure(nw)) || (rc = E.slots.ensure(nw)) || (rc = E.h_counts.ensure(nw)) ||
+            (rc = E.h_scores.ensure(nw)) || (rc = E.models.ensure((size_t)nw * MSZ)))
+            return rc;
+        std::vector<double> packed((size_t)nw * MSZ); // the MSZ-strided model list k_score reads
+        for (int j = 0; j < nw; ++j) {
+            std::copy(PS[who[j]].t->model, PS[who[j]].t->model + MSZ, packed.data() + (size_t)j * MSZ);
+            E.h_slots.p[j] = who[j];
+        }
+        PLB_CUDA(cudaMemcpyAsync(E.models.p, packed.data(), sizeof(double) * nw * MSZ, cudaMemcpyHostToDevice, st));
+        PLB_CUDA(cudaMemcpyAsync(E.slots.p, E.h_slots.p, sizeof(int) * nw, cudaMemcpyHostToDevice, st));
+        launch_score_models(kind, E.probs.p, E.models.p, E.slots.p, nw, E.h_counts.d, E.h_scores.d, st);
+        E.launches++;
+        if ((rc = sync())) return rc;
+        std::vector<LmTask> lo;
+        std::vector<PState *> lo_of;
+        for (int j = 0; j < nw; ++j) {
+            PState &S = PS[who[j]];
+            const size_t ic = E.h_counts.p[j];
+            const double sc = E.h_scores.p[j];
+            S.cnt.hypotheses++;
+            const bool more = ic > S.best_minimal_inlier_count, better = sc < S.best_minimal_msac_score;
+            if (more || better) {
+                if (more) S.best_minimal_inlier_count = ic;
+                if (better) S.best_minimal_msac_score = sc;
+                if (sc < S.stats.model_score) {
+                    S.stats.model_score = sc;
+                    S.stats.num_inliers = ic;
                 }
-            }
-            if (nj) {
-                if ((rc = launch_lm_jobs(nj, false, 0))) return rc;
-                if ((rc = sync_timed(&lo_wait))) return rc;
-                for (int j = 0; j < nj; ++j) {
-                    PState &S = PS[jw[j]];
-                    const LmJobOut &o = E.h_lm_out.p[j];
-                    S.stats.refinements++;
-                    S.cnt.lo_calls++;
-                    S.cnt.hypotheses++;
-                    if (o.score < S.stats.model_score) {
-                        S.stats.model_score = o.score;
-                        S.stats.num_inliers = o.count;
-                        std::copy(o.model, o.model + MSZ, S.best_model);
-                    }
-                    update_dynamic(S, K);
-                }
+                lo.push_back({S.t->model, lo_job(S)});
+                lo_of.push_back(&S);
             }
         }
+        if (lo.empty()) return PLB_OK;
+        if ((rc = lm_batch(lo)) || (rc = sync(&lo_wait))) return rc;
+        for (size_t j = 0; j < lo.size(); ++j) apply_lo(*lo_of[j], E.h_lm_out.p[j]);
+        return PLB_OK;
     }
 
-    mark(PH_SETUP);
-    // ---- main loop in lock-step rounds ------------------------------------------------------------------------------
-    // Every round is ONE chain of launches with ONE host synchronisation at its end:
-    //   k_sample -> solve kernels -> scoring (fp64 of every model, or fp32 screening) -> k_select -> [k_confirm] ->
-    //   k_pass1 -> k_lm over the LO triggers it listed.
-    // The sampler state, the per-model records and the candidate lists never leave the device; the host receives, per
-    // problem, one header, the few models that improved the best-minimal state and the LO results, and replays
-    // score_models() (ransac_impl.h:106-154) over those.
-    for (PState &S : PS) S.active = S.enough && S.t->opt.max_iterations > 0;
-    {
-        // device sampler states (robust/sampling.h:49-83) + PROSAC growth tables (sampling.cc:105-136)
+    // ---- device sampler states (robust/sampling.h:49-83), PROSAC growth tables (sampling.cc:105-136), LO templates --
+    int init_samplers() {
+        for (PState &S : PS) {
+            S.active = S.enough && S.t->opt.max_iterations > 0;
+            S.chunk = std::min<size_t>(4096, std::max<size_t>(1024, 16384 / few));
+        }
         size_t growth_total = 0;
         for (PState &S : PS)
             if (S.active && S.t->opt.progressive_sampling) growth_total += std::max<size_t>(S.t->n, (size_t)K);
+        int rc;
         if ((rc = E.h_smp.ensure(NP)) || (rc = E.smp.ensure(2 * (size_t)NP)) || (rc = E.h_growth.ensure(growth_total)) ||
             (rc = E.growth.ensure(growth_total)) || (rc = E.h_lo_tmpl.ensure(NP)) || (rc = E.lo_tmpl.ensure(NP)) ||
             (rc = E.h_hypfix.ensure(NP)))
@@ -955,7 +981,7 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             PState &S = PS[i];
             SamplerDev &D = E.h_smp.p[i];
             std::memset(&D, 0, sizeof(D));
-            make_lo_job(E.h_lo_tmpl.p[i], S, 0);
+            E.h_lo_tmpl.p[i] = lo_job(S);
             if (!S.active) continue;
             D.state = S.t->opt.seed;
             D.n = (uint32_t)S.t->n;
@@ -983,37 +1009,34 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             PLB_CUDA(cudaMemcpyAsync(E.growth.p, E.h_growth.p, sizeof(uint64_t) * growth_total, cudaMemcpyHostToDevice, st));
             h2d += sizeof(uint64_t) * growth_total;
         }
+        return PLB_OK;
     }
-    int smp_cur = 0; // sampler states of the current round: E.smp[smp_cur * NP ..]; the advanced ones land in the other half
-    // Round sizes.  A small group leaves the GPU mostly idle, so speculating further ahead costs little time while every
-    // round saved is a whole launch chain of latency: the first round and the per-round cap grow as the group shrinks
-    // (1 problem: 4096 doubling up to 65536 samples; >= 16 problems: 1024 doubling to 16384).  The first round stays
-    // moderate on purpose: a loop that stops right after min_iterations (high inlier ratio) would otherwise pay for
-    // thousands of speculative samples and their LO refits (measured: C4 single call 2.0 -> 3.3 ms with 16384).
-    const size_t few = (size_t)std::max(1, std::min(NP, 16));
-    const size_t CHUNK_MAX = std::max<size_t>(16384, 65536 / few), ROUND_MAX = std::max<size_t>(32768, 65536 / few),
-                 S_TOT_MAX = 262144;
-    for (PState &S : PS) S.chunk = std::min<size_t>(4096, std::max<size_t>(1024, 16384 / few));
-    // 0 exact, 1 fast (fp32 screen + fp64 confirmation of candidates); the tangent-Sampson kind has no fp32 copy
-    const int mode = (kind == KIND_RELPOSE_TS) ? 0 : current_mode();
-    int cap_factor = kind_is_relpose(kind) ? 8 : MAXM;
-    bool big_caps = false;
-    std::vector<int> act;
-    std::vector<uint8_t> first_round(NP, 1);
-    for (;;) {
+
+    // break test at the top of iteration `it` (ransac_impl.h:180-184); returns the number of problems still running
+    int select_active() {
         act.clear();
         for (int i = 0; i < NP; ++i) {
             PState &S = PS[i];
             if (!S.active) continue;
-            // break test at the top of iteration `it` (ransac_impl.h:180-184)
             if (S.it >= S.t->opt.max_iterations || (S.it > S.t->opt.min_iterations && S.it > S.dynamic_max_iter)) {
                 S.active = false;
                 continue;
             }
             act.push_back(i);
         }
+        return (int)act.size();
+    }
+
+    // ---- one lock-step round -----------------------------------------------------------------------------------------
+    // Every round is ONE chain of launches with ONE host synchronisation at its end:
+    //   k_sample -> solve kernels -> scoring (fp64 of every model, or fp32 screening) -> k_select -> [k_confirm] ->
+    //   k_pass1 -> k_lm over the LO triggers it listed.
+    // The sampler states, the per-model records and the candidate lists never leave the device; the host receives, per
+    // problem, one header, the few models that improved the best-minimal state and the LO results, and replays
+    // score_models() (ransac_impl.h:106-154) over those.  A round whose records overflow is redone with larger
+    // capacities: nothing was committed, the sampler states of the round are still current.
+    int round() {
         const int na = (int)act.size();
-        if (!na) break;
         // round sizes: up to the iteration at which the serial loop would stop for the current dynamic_max_iter
         size_t total = 0;
         const size_t per_cap = std::max<size_t>(256, S_TOT_MAX / (size_t)na);
@@ -1033,11 +1056,51 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             total += B;
             est_jobs += first_round[act[a]] ? 12 : 2; // LO triggers: a record chain at first, then the odd improvement
         }
+        for (;;) {
+            int rc;
+            if ((rc = launch_round(total, est_jobs)) || (rc = sync())) return rc;
+            mark(PH_WAIT_HYP);
+            d2h += CTL_WORDS * sizeof(int);
+            if (E.h_work.p[CTL_OVERFLOW] != 0) { // model list overflow: redo the round with the worst-case capacity
+                if (cap_factor >= MAXM) {
+                    g_err = "internal error: model capacity exceeded";
+                    return PLB_ERR_CUDA;
+                }
+                cap_factor = MAXM;
+                continue;
+            }
+            if (E.h_work.p[CTL_FLAGS] != 0) { // more improving models / LO triggers than the record buffers hold
+                if (big_caps) {
+                    g_err = "internal error: record capacity exceeded";
+                    return PLB_ERR_CUDA;
+                }
+                big_caps = true;
+                continue;
+            }
+            break;
+        }
+        smp_cur ^= 1;
+        float ms = 0.f, ms_sc = 0.f, ms_cf = 0.f, ms_lo = 0.f;
+        cudaEventElapsedTime(&ms, E.ev0, E.ev1);
+        cudaEventElapsedTime(&ms_sc, E.ev2, E.ev1);
+        cudaEventElapsedTime(&ms_cf, E.ev1, E.ev3);
+        cudaEventElapsedTime(&ms_lo, E.ev3, E.ev4);
+        gpu_ms_total += ms + ms_cf;
+        gpu_ms_score += ms_sc;
+        gpu_ms_confirm += ms_cf;
+        gpu_ms_lo += ms_lo;
+        return PLB_OK;
+    }
+
+    // the launch chain of one round over the `total` samples sized by round(), ending with the control words' copy
+    int launch_round(size_t total, int est_jobs) {
+        const int na = (int)act.size();
         const size_t cap_models = total * (size_t)cap_factor;
         // capacity of the host-visible records of the round; exceeded -> the round is redone with the worst case
         const size_t job_cap = big_caps ? total : std::min(total, std::max<size_t>(1024, total / 8));
         const size_t imp_cap = big_caps ? cap_models : std::min(cap_models, 2 * job_cap);
         const int lm_clusters = lm_round_max_clusters(kind, est_jobs, max_n);
+        int rc;
         if ((rc = E.samples.ensure(total * K)) || (rc = E.n_models.ensure(total)) || (rc = E.first_slot.ensure(total)) ||
             (rc = E.prefix.ensure(total)) || (rc = E.counts.ensure(cap_models)) || (rc = E.scores.ensure(cap_models)) ||
             (rc = E.models.ensure(cap_models * MSZ)) || (rc = E.model_prob.ensure(cap_models)) ||
@@ -1051,29 +1114,27 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         ++n_rounds;
         // h_act layout: active[na] | g_off[na+1] | seg_base[na] | seg_cap[na]
         int max_seg_cap = 0;
-        {
-            size_t seg = 0;
-            for (int a = 0; a < na; ++a) {
-                const PState &S = PS[act[a]];
-                E.h_act.p[a] = act[a];
-                E.h_act.p[na + a] = (int)S.g0;
-                E.h_act.p[2 * na + 1 + a] = (int)seg;
-                const int cap = (int)(S.B * (size_t)cap_factor);
-                E.h_act.p[3 * na + 1 + a] = cap;
-                max_seg_cap = std::max(max_seg_cap, cap);
-                RoundProb &Q = E.h_rp.p[a];
-                Q.pidx = act[a];
-                Q.g0 = (int)S.g0;
-                Q.B = (int)S.B;
-                Q.seg_base = (int)seg;
-                Q.seg_cap = cap;
-                Q.reserved = 0;
-                Q.lb0 = (double)S.best_minimal_inlier_count;
-                Q.ub0 = S.best_minimal_msac_score;
-                seg += (size_t)cap;
-            }
-            E.h_act.p[2 * na] = (int)total;
+        size_t seg = 0;
+        for (int a = 0; a < na; ++a) {
+            const PState &S = PS[act[a]];
+            E.h_act.p[a] = act[a];
+            E.h_act.p[na + a] = (int)S.g0;
+            E.h_act.p[2 * na + 1 + a] = (int)seg;
+            const int cap = (int)(S.B * (size_t)cap_factor);
+            E.h_act.p[3 * na + 1 + a] = cap;
+            max_seg_cap = std::max(max_seg_cap, cap);
+            RoundProb &Q = E.h_rp.p[a];
+            Q.pidx = act[a];
+            Q.g0 = (int)S.g0;
+            Q.B = (int)S.B;
+            Q.seg_base = (int)seg;
+            Q.seg_cap = cap;
+            Q.reserved = 0;
+            Q.lb0 = (double)S.best_minimal_inlier_count;
+            Q.ub0 = S.best_minimal_msac_score;
+            seg += (size_t)cap;
         }
+        E.h_act.p[2 * na] = (int)total;
         PLB_CUDA(cudaMemcpyAsync(E.act.p, E.h_act.p, sizeof(int) * (4 * na + 1), cudaMemcpyHostToDevice, st));
         PLB_CUDA(cudaMemcpyAsync(E.rp.p, E.h_rp.p, sizeof(RoundProb) * na, cudaMemcpyHostToDevice, st));
         h2d += sizeof(int) * (4 * na + 1) + sizeof(RoundProb) * na;
@@ -1085,7 +1146,7 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         R.n_active = na;
         R.samples = E.samples.p;
         R.n_total = (int)total;
-        HypOut out;
+        HypOut out{}; // fast-mode and 5-point buffers stay null unless set below
         out.n_models = E.n_models.p;
         out.first_slot = E.first_slot.p;
         out.seg_base = E.act.p + 2 * na + 1;
@@ -1097,10 +1158,6 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         out.scores = E.scores.p;
         out.models = E.models.p;
         out.model_prob = E.model_prob.p;
-        out.fcounts = nullptr;
-        out.fscores = nullptr;
-        out.fborder = nullptr;
-        out.ferr = nullptr;
         if (mode == 1) {
             if ((rc = E.fcounts.ensure(cap_models)) || (rc = E.fscores.ensure(cap_models)) ||
                 (rc = E.fborder.ensure(cap_models)) || (rc = E.ferr.ensure(cap_models)))
@@ -1110,8 +1167,6 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             out.fborder = E.fborder.p;
             out.ferr = E.ferr.p;
         }
-        out.s5_blk = out.s5_park = out.s5_cpoly = out.s5_roots = nullptr;
-        out.s5_nroots = nullptr;
         if (kind_is_relpose(kind)) { // phase buffers of the 3-kernel 5-point solver
             if ((rc = E.s5_blk.ensure(total * 105)) || (rc = E.s5_park.ensure(total * 100)) || (rc = E.s5_cpoly.ensure(total * 11)) ||
                 (rc = E.s5_roots.ensure(total * 10)) || (rc = E.s5_nroots.ensure(total)))
@@ -1178,42 +1233,14 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         PLB_CUDA(cudaEventRecord(E.ev4, st));
         PLB_CUDA(cudaMemcpyAsync(E.h_work.p, E.work.p, CTL_WORDS * sizeof(int), cudaMemcpyDeviceToHost, st));
         mark(PH_LAUNCH);
-        if ((rc = sync_timed(nullptr))) return rc;
-        mark(PH_WAIT_HYP);
-        d2h += CTL_WORDS * sizeof(int);
-        if (E.h_work.p[CTL_OVERFLOW] != 0) { // model list overflow: redo the round with the worst-case capacity
-            if (cap_factor >= MAXM) {        // (nothing was committed: the sampler states of this round are still current)
-                g_err = "internal error: model capacity exceeded";
-                return PLB_ERR_CUDA;
-            }
-            cap_factor = MAXM;
-            continue;
-        }
-        if (E.h_work.p[CTL_FLAGS] != 0) { // more improving models / LO triggers than the record buffers hold
-            if (big_caps) {
-                g_err = "internal error: record capacity exceeded";
-                return PLB_ERR_CUDA;
-            }
-            big_caps = true;
-            continue;
-        }
-        smp_cur ^= 1;
-        float ms = 0.f, ms_sc = 0.f, ms_cf = 0.f;
-        cudaEventElapsedTime(&ms, E.ev0, E.ev1);
-        cudaEventElapsedTime(&ms_sc, E.ev2, E.ev1);
-        cudaEventElapsedTime(&ms_cf, E.ev1, E.ev3);
-        gpu_ms_total += ms + ms_cf;
-        gpu_ms_score += ms_sc;
-        gpu_ms_confirm += ms_cf;
-        {
-            float ms_lo = 0.f;
-            cudaEventElapsedTime(&ms_lo, E.ev3, E.ev4);
-            gpu_ms_lo += ms_lo;
-        }
+        return PLB_OK;
+    }
 
-        // ---- replay of the serial loop over this round, problem by problem (ransac_impl.h:106-154,180-188) --------
-        // Only samples with an improving model change the state; between two of them the break test
-        // `it > min_iterations && it > dynamic_max_iter` (:182) first holds at max(min_iterations, dyn) + 1.
+    // ---- replay of the serial loop over the round, problem by problem (ransac_impl.h:106-154,180-188) ----------------
+    // Only samples with an improving model change the state; between two of them the break test
+    // `it > min_iterations && it > dynamic_max_iter` (:182) first holds at max(min_iterations, dyn) + 1.
+    int replay() {
+        const int na = (int)act.size();
         for (int a = 0; a < na; ++a) {
             PState &S = PS[act[a]];
             first_round[act[a]] = 0;
@@ -1256,22 +1283,12 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
                     }
                     ++ip;
                 }
-                const LmJobOut &o = lo[tp++];
-                S.stats.refinements++;
-                S.cnt.lo_calls++;
-                S.cnt.hypotheses++;
-                if (o.score < S.stats.model_score) {
-                    S.stats.model_score = o.score;
-                    S.stats.num_inliers = o.count;
-                    std::copy(o.model, o.model + MSZ, S.best_model);
-                }
-                update_dynamic(S, K);
+                apply_lo(S, lo[tp++]);
                 cur = next_trig + 1;
             }
             S.cnt.samples += cur - it0;
             S.it = cur;
             if (broke) {
-                S.broke = true;
                 S.active = false;
                 // hypotheses of the samples before the break: one prefix-sum word, fetched behind the round (read at
                 // the end of the call; stream order keeps it ahead of the next round's kernels)
@@ -1285,49 +1302,44 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
                 S.cnt.hypotheses += (uint64_t)H.n_models;
             }
         }
-        mark(PH_PASS2);
+        mark(PH_REPLAY);
+        return PLB_OK;
     }
-    for (PState &S : PS)
-        if (S.enough) S.stats.iterations = S.it;
 
     // ---- final refinement of every problem (ransac_impl.h:190-198), one launch ---------------------------------------
-    {
-        std::vector<int> who;
-        for (int i = 0; i < NP; ++i)
-            if (PS[i].enough) who.push_back(i);
-        const int nw = (int)who.size();
-        if (nw) {
-            if ((rc = E.h_lm_in.ensure(9 * (size_t)nw)) || (rc = E.h_jobs.ensure(nw)) ||
-                (rc = E.subset.ensure((size_t)nw * max_n_pad)))
-                return rc;
-            for (int j = 0; j < nw; ++j) {
-                PState &S = PS[who[j]];
-                std::fill(E.h_lm_in.p + 9 * j, E.h_lm_in.p + 9 * j + 9, 0.0);
-                std::copy(S.best_model, S.best_model + MSZ, E.h_lm_in.p + 9 * j);
-                make_lo_job(E.h_jobs.p[j], S, (long long)j * max_n_pad);
-            }
-            if ((rc = launch_lm_jobs(nw, false, 0))) return rc;
-            if ((rc = sync_timed(&lo_wait))) return rc;
-            for (int j = 0; j < nw; ++j) {
-                PState &S = PS[who[j]];
-                const LmJobOut &o = E.h_lm_out.p[j];
-                S.stats.refinements++;
-                S.cnt.lo_calls++;
-                S.cnt.hypotheses++;
-                if (o.score < S.stats.model_score) { // NB: model_score itself is not updated by the reference here
-                    std::copy(o.model, o.model + MSZ, S.best_model);
-                    S.stats.num_inliers = o.count;
-                }
+    int final_refine() {
+        std::vector<LmTask> jobs;
+        std::vector<PState *> of;
+        for (PState &S : PS) {
+            if (!S.enough) continue;
+            S.stats.iterations = S.it;
+            jobs.push_back({S.best_model, lo_job(S)});
+            of.push_back(&S);
+        }
+        if (jobs.empty()) return PLB_OK;
+        int rc;
+        if ((rc = lm_batch(jobs)) || (rc = sync(&lo_wait))) return rc;
+        for (size_t j = 0; j < jobs.size(); ++j) {
+            PState &S = *of[j];
+            const LmJobOut &o = E.h_lm_out.p[j];
+            S.stats.refinements++;
+            S.cnt.lo_calls++;
+            S.cnt.hypotheses++;
+            if (o.score < S.stats.model_score) { // NB: model_score itself is not updated by the reference here
+                std::copy(o.model, o.model + MSZ, S.best_model);
+                S.stats.num_inliers = o.count;
             }
         }
+        return PLB_OK;
     }
 
     // ---- final inlier masks (ransac.cc:54,151,259,311) + optional polish over the inliers (robust.cc) -----------------
-    {
+    int masks_and_polish() {
         std::vector<int> who;
         for (int i = 0; i < NP; ++i)
             if (PS[i].n > 0) who.push_back(i);
         const int nw = (int)who.size();
+        int rc;
         if ((rc = E.h_mdesc.ensure(nw)) || (rc = E.mdesc.ensure(nw))) return rc;
         for (int j = 0; j < nw; ++j) {
             PState &S = PS[who[j]];
@@ -1341,44 +1353,28 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
         h2d += sizeof(MaskDesc) * nw;
         launch_inlier_masks(kind, E.probs.p, E.mdesc.p, nw, max_n, E.mask.p, st);
         E.launches++;
-        std::vector<int> pol;
-        for (int i = 0; i < NP; ++i)
-            if (PS[i].n > 0 && PS[i].t->polish.enabled && PS[i].stats.num_inliers > PS[i].t->polish.min_inliers) pol.push_back(i);
-        const int npol = (int)pol.size();
-        if (npol) {
-            // robust.cc:103-123,296-311,573-588,736-751: LM over the inliers with the user's BundleOptions
-            if ((rc = E.h_lm_in.ensure(9 * (size_t)npol)) || (rc = E.h_jobs.ensure(npol)) ||
-                (rc = E.subset.ensure((size_t)npol * max_n_pad)))
-                return rc;
-            for (int j = 0; j < npol; ++j) {
-                PState &S = PS[pol[j]];
-                std::fill(E.h_lm_in.p + 9 * j, E.h_lm_in.p + 9 * j + 9, 0.0);
-                std::copy(S.best_model, S.best_model + MSZ, E.h_lm_in.p + 9 * j);
-                LmJob &J = E.h_jobs.p[j];
-                J.pidx = S.pidx;
-                J.reserved = 0;
-                J.mask_off = S.mask_off;
-                J.scratch_off = (long long)j * max_n_pad;
-                J.prm = bundle_params(S.t->polish.bundle);
-                if (S.polish_pidx >= 0) {
-                    J.pidx = S.polish_pidx;
-                    J.prm.use_camera = 1;
-                    J.prm.cam = S.t->polish.cam;
-                }
+        // robust.cc:103-123,296-311,573-588,736-751: LM over the inliers with the user's BundleOptions
+        std::vector<LmTask> pol;
+        std::vector<PState *> pol_of;
+        for (PState &S : PS) {
+            if (S.n == 0 || !S.t->polish.enabled || S.stats.num_inliers <= S.t->polish.min_inliers) continue;
+            LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(S.t->polish.bundle));
+            if (S.polish_pidx >= 0) {
+                J.pidx = S.polish_pidx;
+                J.prm.use_camera = 1;
+                J.prm.cam = S.t->polish.cam;
             }
-            if ((rc = launch_lm_jobs(npol, false, 0))) return rc;
+            pol.push_back({S.best_model, J});
+            pol_of.push_back(&S);
         }
+        if (!pol.empty() && (rc = lm_batch(pol))) return rc;
         // the masks cross PCIe as bits (1/8 of the bytes) and are expanded into the caller's char[n] below
         launch_pack_mask(E.mask.p, E.mask_bits.p, mask_bytes, st);
         E.launches++;
         PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
-        if ((rc = sync_timed(nullptr))) return rc;
-        for (int j = 0; j < npol; ++j) {
-            PState &S = PS[pol[j]];
-            std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, S.best_model);
-        }
-        for (int i = 0; i < NP; ++i) {
-            PState &S = PS[i];
+        if ((rc = sync())) return rc;
+        for (size_t j = 0; j < pol.size(); ++j) std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
+        for (PState &S : PS) {
             if (S.t->inliers && S.n > 0) {
                 const uint32_t *w = E.h_mask_bits.p + (S.mask_off >> 5); // mask_off is a multiple of 32
                 char *dst = S.t->inliers;
@@ -1387,29 +1383,63 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
             std::copy(S.best_model, S.best_model + MSZ, S.t->model);
             d2h += (size_t)S.n_pad / 8;
         }
+        PLB_CUDA(cudaGetLastError());
+        return PLB_OK;
     }
-    PLB_CUDA(cudaGetLastError());
-    mark(PH_FINAL);
-    if (prof_on) {
-        double tot = 0;
-        for (int i = 0; i < PH_N; ++i) tot += ph[i];
-        std::fprintf(stderr,
-                     "[plb profile] kind %d problems %d rounds %d total %.2f ms | setup %.2f sample %.2f launch %.2f wait_hyp %.2f "
-                     "select %.2f wait_conf %.2f pass1 %.2f wait_lm %.2f pass2 %.2f final %.2f\n",
-                     kind, NP, n_rounds, 1e3 * tot, 1e3 * ph[0], 1e3 * ph[1], 1e3 * ph[2], 1e3 * ph[3], 1e3 * ph[4], 1e3 * ph[5],
-                     1e3 * ph[6], 1e3 * ph[7], 1e3 * ph[8], 1e3 * ph[9]);
+
+    // ---- the profile line and the counters; group-level counters are attributed to the first problem ----------------
+    void report() {
+        mark(PH_FINAL);
+        if (profiling()) {
+            double tot = 0;
+            for (int i = 0; i < PH_N; ++i) tot += ph[i];
+            std::fprintf(stderr,
+                         "[plb profile] kind %d problems %d rounds %d total %.2f ms | setup %.2f sample %.2f launch %.2f "
+                         "wait_hyp %.2f replay %.2f final %.2f\n",
+                         kind, NP, n_rounds, 1e3 * tot, 1e3 * ph[PH_SETUP], 1e3 * ph[PH_SAMPLE], 1e3 * ph[PH_LAUNCH],
+                         1e3 * ph[PH_WAIT_HYP], 1e3 * ph[PH_REPLAY], 1e3 * ph[PH_FINAL]);
+        }
+        PS[0].cnt.lo_seconds = lo_wait;
+        PS[0].cnt.gpu_launches = E.launches - launches0;
+        PS[0].cnt.gpu_seconds = gpu_ms_total * 1e-3;
+        PS[0].cnt.gpu_seconds_score = gpu_ms_score * 1e-3;
+        PS[0].cnt.gpu_seconds_select = gpu_ms_confirm * 1e-3;
+        PS[0].cnt.gpu_seconds_lo = gpu_ms_lo * 1e-3;
+        PS[0].cnt.rounds = (uint64_t)n_rounds;
+        PS[0].cnt.h2d_bytes = h2d;
+        PS[0].cnt.d2h_bytes = d2h;
+        finish();
     }
-    // group-level counters are attributed to the first problem; per-problem ones are exact
-    PS[0].cnt.lo_seconds = lo_wait;
-    PS[0].cnt.gpu_launches = E.launches - launches0;
-    PS[0].cnt.gpu_seconds = gpu_ms_total * 1e-3;
-    PS[0].cnt.gpu_seconds_score = gpu_ms_score * 1e-3;
-    PS[0].cnt.gpu_seconds_select = gpu_ms_confirm * 1e-3;
-    PS[0].cnt.gpu_seconds_lo = gpu_ms_lo * 1e-3;
-    PS[0].cnt.rounds = (uint64_t)n_rounds;
-    PS[0].cnt.h2d_bytes = h2d;
-    PS[0].cnt.d2h_bytes = d2h;
-    finish();
+    // per-problem outputs: stats and counters
+    void finish() {
+        for (PState &S : PS) {
+            if (S.hyp_pending) S.cnt.hypotheses += (uint64_t)E.h_hypfix.p[S.pidx];
+            S.cnt.scored_corrs = S.cnt.hypotheses * S.t->n;
+            if (S.t->stats_out) *S.t->stats_out = S.stats;
+            if (S.t->cnt_out) *S.t->cnt_out = S.cnt;
+        }
+    }
+};
+
+// Runs a group of problems of the same kind in lock-step rounds (see Group).
+static int run_group(int kind, std::vector<Task *> &tasks) {
+    Group G(kind, tasks);
+    int rc = G.init_states();
+    if (rc != PLB_OK) return rc;
+    if (std::none_of(G.PS.begin(), G.PS.end(), [](const PState &S) { return S.n > 0; })) {
+        G.finish();
+        return PLB_OK;
+    }
+    if ((rc = G.init())) return rc;
+    lm_set_sm_share(t_batch_worker ? 50 : 100); // a lone call owns the GPU; batch groups share it
+    if ((rc = G.upload()) || (rc = G.normalize()) || (rc = G.transpose()) || (rc = G.score_initial_models()) ||
+        (rc = G.init_samplers()))
+        return rc;
+    G.mark(Group::PH_SETUP);
+    while (G.select_active())
+        if ((rc = G.round()) || (rc = G.replay())) return rc;
+    if ((rc = G.final_refine()) || (rc = G.masks_and_polish())) return rc;
+    G.report();
     return PLB_OK;
 }
 
@@ -1441,79 +1471,34 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
     return run_group(kind, v);
 }
 
-// One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411)
+// One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
+// group (sq_thr 0, no normalisation, no pre-step beyond the cameras), then one LM job over every point.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cam_a = nullptr,
                       const CamDev *cam_b = nullptr) {
     if (n_pts == 0) return PLB_OK;
-    Engine &E = *engine();
-    int rc = E.init();
-    if (rc != PLB_OK) return rc;
-    cudaStream_t st = E.stream;
-    const int n = (int)n_pts, n_pad = (n + 31) & ~31;
-    const int b_dim = (kind == KIND_PNP) ? 3 : 2, in_arr = 2 + b_dim, MSZ = kind_model_size(kind);
-    const int n_arr = (kind == KIND_RELPOSE_TS) ? TS_ARRAYS : in_arr;
-    if ((rc = E.h_in.ensure((size_t)in_arr * n)) || (rc = E.in.ensure((size_t)in_arr * n)) ||
-        (rc = E.soa64.ensure((size_t)n_arr * n_pad)) || (rc = E.soa32.ensure((size_t)n_arr * n_pad)) ||
-        (rc = E.lm_in.ensure(9)) || (rc = E.h_lm_in.ensure(9)) || (rc = E.h_lm_out.ensure(1)) ||
-        (rc = E.probs.ensure(1)) || (rc = E.h_probs.ensure(1)) || (rc = E.tdesc.ensure(1)) || (rc = E.h_tdesc.ensure(1)) ||
-        (rc = E.jobs.ensure(1)) || (rc = E.h_jobs.ensure(1)))
-        return rc;
-    std::memcpy(E.h_in.p, a, sizeof(double) * 2 * n);
-    std::memcpy(E.h_in.p + 2 * (size_t)n, b, sizeof(double) * b_dim * n);
-    PLB_CUDA(cudaMemcpyAsync(E.in.p, E.h_in.p, sizeof(double) * (size_t)in_arr * n, cudaMemcpyHostToDevice, st));
-    TransposeDesc &D = E.h_tdesc.p[0];
-    D.a = E.in.p;
-    D.b = E.in.p + 2 * (size_t)n;
-    D.s64 = E.soa64.p;
-    D.s32 = E.soa32.p;
-    D.cmax = nullptr;
-    D.n = n;
-    D.n_pad = n_pad;
-    D.b_dim = b_dim;
-    D.mode = (kind == KIND_RELPOSE_TS) ? 2 : 0;
-    D.scale = 1.0;
-    D.cam_a.model = D.cam_b.model = CAMM_NULL;
-    if (cam_a) D.cam_a = *cam_a;
-    if (cam_b) D.cam_b = *cam_b;
-    ProblemDev &P = E.h_probs.p[0];
-    std::memset(&P, 0, sizeof(P));
-    if (kind == KIND_RELPOSE_TS) {
-        P.ts = E.soa64.p;
-    } else {
-        for (int c = 0; c < n_arr; ++c) {
-            P.p[c] = E.soa64.p + (size_t)c * n_pad;
-            P.f[c] = E.soa32.p + (size_t)c * n_pad;
-        }
-    }
-    P.n_pad = n_pad;
-    P.n = n;
-    P.kind = kind;
-    P.sq_thr = 0.0;
-    LmJob &J = E.h_jobs.p[0];
-    J.pidx = 0;
-    J.reserved = 0;
-    J.mask_off = -1;
-    J.scratch_off = 0;
-    J.prm = bundle_params(bopt);
-    J.prm.subset_mode = 0;
-    std::fill(E.h_lm_in.p, E.h_lm_in.p + 9, 0.0);
-    std::copy(model, model + MSZ, E.h_lm_in.p);
-    PLB_CUDA(cudaMemcpyAsync(E.tdesc.p, E.h_tdesc.p, sizeof(TransposeDesc), cudaMemcpyHostToDevice, st));
-    PLB_CUDA(cudaMemcpyAsync(E.probs.p, E.h_probs.p, sizeof(ProblemDev), cudaMemcpyHostToDevice, st));
-    PLB_CUDA(cudaMemcpyAsync(E.jobs.p, E.h_jobs.p, sizeof(LmJob), cudaMemcpyHostToDevice, st));
-    PLB_CUDA(cudaMemcpyAsync(E.lm_in.p, E.h_lm_in.p, sizeof(double) * 9, cudaMemcpyHostToDevice, st));
-    launch_transpose(E.tdesc.p, 1, n_pad, st);
+    Task t;
+    t.kind = kind;
+    t.a = a;
+    t.b = b;
+    t.n = n_pts;
+    if (cam_a) t.cam_a = *cam_a;
+    if (cam_b) t.cam_b = *cam_b;
+    std::vector<Task *> v{&t};
+    Group G(kind, v);
+    int rc;
+    if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose())) return rc;
+    LmParams prm = bundle_params(bopt);
+    prm.subset_mode = 0;
     lm_set_sm_share(100);
-    launch_lm(kind, E.probs.p, E.jobs.p, E.lm_in.p, 1, n, nullptr, nullptr, 0, E.h_lm_out.d, st);
-    E.launches += 2;
-    PLB_CUDA(cudaStreamSynchronize(st));
+    if ((rc = G.lm_batch({{model, lm_job(0, -1, prm)}})) || (rc = G.sync())) return rc;
     PLB_CUDA(cudaGetLastError());
-    std::copy(E.h_lm_out.p[0].model, E.h_lm_out.p[0].model + MSZ, model);
+    const LmJobOut &o = G.E.h_lm_out.p[0];
+    std::copy(o.model, o.model + G.MSZ, model);
     if (bstats) {
-        bstats[0] = E.h_lm_out.p[0].iterations;
-        bstats[1] = E.h_lm_out.p[0].initial_cost;
-        bstats[2] = E.h_lm_out.p[0].cost;
+        bstats[0] = o.iterations;
+        bstats[1] = o.initial_cost;
+        bstats[2] = o.cost;
     }
     return PLB_OK;
 }

@@ -5,7 +5,8 @@
 //                      minimal solvers of a round, one thread per minimal sample (the 5-point solver in phases)
 //   k_score_tiled / k_screen
 //                      MSAC scoring of every model of a round over all correspondences (exact fp64 / fp32 screening)
-//   k_score_models     exact rescoring of explicit models (initial model, fast-mode confirmation)
+//   k_score            exact scoring of explicit models (initial models)
+//   k_confirm          exact rescoring of the fast-mode candidates of a round
 //   k_lm<KIND>         Levenberg-Marquardt refit (LO step + final polish): one CTA per job, block-wide reductions of
 //                      the normal equations, scalar LM logic on thread 0
 //   k_inlier_mask      final inlier masks
@@ -289,82 +290,73 @@ struct ScoreRed {
     double s[SCORE_WARPS];
     uint32_t c[SCORE_WARPS];
 };
-template <int KIND, int NT = SCORE_THREADS>
+template <int KIND>
 PLB_DEV void cta_score(const ProblemDev &P, const double *model, double sq_thr, ScoreRed *red, uint32_t &count_out,
                        double &score_out) {
-    // NT physical threads (256, or 128 in the two-jobs-per-SM LM build) stand for the SCORE_THREADS = 256 threads of the
-    // fixed summation order: thread tid accumulates the partial sums of the "virtual" threads tid, tid + NT, ... in
-    // separate registers and reduces them as the virtual warps they belong to — same bits for any NT.
-    static_assert(SCORE_THREADS % NT == 0 && NT % 32 == 0, "NT must divide the virtual thread count");
-    constexpr int VPT = SCORE_THREADS / NT;
     const int tid = threadIdx.x, lane = tid & 31;
     const int n = P.n;
-    if (tid < NT) {
+    if (tid < SCORE_THREADS) {
         ModelCtx<KIND> C;
         C.init(model);
-#pragma unroll
-        for (int v = 0; v < VPT; ++v) {
-            const int vt = tid + v * NT;
-            uint32_t cnt = 0;
-            double score = 0.0;
-            if (KIND == KIND_PNP) {
-                const double *__restrict__ xx = P.p[0], *__restrict__ xy = P.p[1];
-                const double *__restrict__ Xx = P.p[2], *__restrict__ Xy = P.p[3], *__restrict__ Xz = P.p[4];
-                const double *Pm = reinterpret_cast<const double *>(&C);
-                for (int k = vt; k < n; k += SCORE_THREADS) {
-                    const double X0 = Xx[k], X1 = Xy[k], X2 = Xz[k];
-                    const double x0 = xx[k], x1 = xy[k];
-                    const double z0 = Pm[0] * X0 + Pm[1] * X1 + Pm[2] * X2 + Pm[3];
-                    const double z1 = Pm[4] * X0 + Pm[5] * X1 + Pm[6] * X2 + Pm[7];
-                    const double z2 = Pm[8] * X0 + Pm[9] * X1 + Pm[10] * X2 + Pm[11];
-                    if (z2 <= 0.0) continue;
-                    const double inv_z2 = 1.0 / z2;
-                    const double r_0 = z0 * inv_z2 - x0;
-                    const double r_1 = z1 * inv_z2 - x1;
-                    const double r_sq = r_0 * r_0 + r_1 * r_1;
-                    if (r_sq < sq_thr) {
-                        ++cnt;
-                        score += r_sq;
-                    }
-                }
-            } else if (KIND == KIND_RELPOSE_TS) {
-                const double *M = reinterpret_cast<const double *>(&C);
-                for (int k = vt; k < n; k += SCORE_THREADS) {
-                    double vv[TS_ARRAYS];
-                    load_ts(P, k, vv);
-                    const double r2 = tangent_r2(M, vv);
-                    bool inl = r2 < sq_thr;
-                    if (inl) inl = cheirality_ok(M + 9, M + 13, mk(vv[0], vv[1], vv[2]), mk(vv[3], vv[4], vv[5]), 0.01);
-                    if (inl) {
-                        ++cnt;
-                        score += r2;
-                    }
-                }
-            } else {
-                const double *__restrict__ ax = P.p[0], *__restrict__ ay = P.p[1];
-                const double *__restrict__ bx = P.p[2], *__restrict__ by = P.p[3];
-                const double *M = reinterpret_cast<const double *>(&C); // first 9 doubles: E / F / H row-major
-                for (int k = vt; k < n; k += SCORE_THREADS) {
-                    const double x1_0 = ax[k], x1_1 = ay[k], x2_0 = bx[k], x2_1 = by[k];
-                    double r2;
-                    if (KIND == KIND_HOMOG) r2 = homography_r2(M, x1_0, x1_1, x2_0, x2_1);
-                    else r2 = sampson_r2(M, x1_0, x1_1, x2_0, x2_1);
-                    bool inl = r2 < sq_thr;
-                    if (KIND == KIND_RELPOSE) {
-                        if (inl) inl = cheirality_ok(M + 9, M + 13, bearing(x1_0, x1_1), bearing(x2_0, x2_1), 0.01);
-                    }
-                    if (inl) {
-                        ++cnt;
-                        score += r2;
-                    }
+        uint32_t cnt = 0;
+        double score = 0.0;
+        if (KIND == KIND_PNP) {
+            const double *__restrict__ xx = P.p[0], *__restrict__ xy = P.p[1];
+            const double *__restrict__ Xx = P.p[2], *__restrict__ Xy = P.p[3], *__restrict__ Xz = P.p[4];
+            const double *Pm = reinterpret_cast<const double *>(&C);
+            for (int k = tid; k < n; k += SCORE_THREADS) {
+                const double X0 = Xx[k], X1 = Xy[k], X2 = Xz[k];
+                const double x0 = xx[k], x1 = xy[k];
+                const double z0 = Pm[0] * X0 + Pm[1] * X1 + Pm[2] * X2 + Pm[3];
+                const double z1 = Pm[4] * X0 + Pm[5] * X1 + Pm[6] * X2 + Pm[7];
+                const double z2 = Pm[8] * X0 + Pm[9] * X1 + Pm[10] * X2 + Pm[11];
+                if (z2 <= 0.0) continue;
+                const double inv_z2 = 1.0 / z2;
+                const double r_0 = z0 * inv_z2 - x0;
+                const double r_1 = z1 * inv_z2 - x1;
+                const double r_sq = r_0 * r_0 + r_1 * r_1;
+                if (r_sq < sq_thr) {
+                    ++cnt;
+                    score += r_sq;
                 }
             }
-            cnt = warp_sum_u(cnt);
-            score = warp_sum(score);
-            if (lane == 0) {
-                red->c[vt >> 5] = cnt;
-                red->s[vt >> 5] = score;
+        } else if (KIND == KIND_RELPOSE_TS) {
+            const double *M = reinterpret_cast<const double *>(&C);
+            for (int k = tid; k < n; k += SCORE_THREADS) {
+                double vv[TS_ARRAYS];
+                load_ts(P, k, vv);
+                const double r2 = tangent_r2(M, vv);
+                bool inl = r2 < sq_thr;
+                if (inl) inl = cheirality_ok(M + 9, M + 13, mk(vv[0], vv[1], vv[2]), mk(vv[3], vv[4], vv[5]), 0.01);
+                if (inl) {
+                    ++cnt;
+                    score += r2;
+                }
             }
+        } else {
+            const double *__restrict__ ax = P.p[0], *__restrict__ ay = P.p[1];
+            const double *__restrict__ bx = P.p[2], *__restrict__ by = P.p[3];
+            const double *M = reinterpret_cast<const double *>(&C); // first 9 doubles: E / F / H row-major
+            for (int k = tid; k < n; k += SCORE_THREADS) {
+                const double x1_0 = ax[k], x1_1 = ay[k], x2_0 = bx[k], x2_1 = by[k];
+                double r2;
+                if (KIND == KIND_HOMOG) r2 = homography_r2(M, x1_0, x1_1, x2_0, x2_1);
+                else r2 = sampson_r2(M, x1_0, x1_1, x2_0, x2_1);
+                bool inl = r2 < sq_thr;
+                if (KIND == KIND_RELPOSE) {
+                    if (inl) inl = cheirality_ok(M + 9, M + 13, bearing(x1_0, x1_1), bearing(x2_0, x2_1), 0.01);
+                }
+                if (inl) {
+                    ++cnt;
+                    score += r2;
+                }
+            }
+        }
+        cnt = warp_sum_u(cnt);
+        score = warp_sum(score);
+        if (lane == 0) {
+            red->c[tid >> 5] = cnt;
+            red->s[tid >> 5] = score;
         }
     }
     __syncthreads();
@@ -725,12 +717,10 @@ __global__ void __launch_bounds__(128) k5_back(const RoundDesc R, HypOut out) {
 template <int KIND>
 __global__ void __launch_bounds__(SCORE_THREADS, 4)
     k_score(const ProblemDev *__restrict__ probs, const double *__restrict__ models, const int *__restrict__ model_prob,
-            const int *__restrict__ model_count, int cap, uint32_t *counts, double *scores) {
+            int n_models, uint32_t *counts, double *scores) {
     constexpr int MSZ = kind_model_size(KIND);
     __shared__ ScoreRed red;
-    int nmod = *model_count;
-    if (nmod > cap) nmod = cap;
-    for (int m = blockIdx.x; m < nmod; m += gridDim.x) {
+    for (int m = blockIdx.x; m < n_models; m += gridDim.x) {
         const ProblemDev P = probs[model_prob[m]];
         double mdl[MSZ];
 #pragma unroll
@@ -902,7 +892,7 @@ __global__ void __launch_bounds__(SCORE_THREADS, 2)
 // 2D-3D corr).  The CTA stages its problem's arrays into shared memory with TMA bulk copies (cp.async.bulk, one
 // mbarrier) and then walks that problem's model tiles; every thread evaluates SCR_TM models per correspondence read
 // from shared memory.  The records (count32, score32) only decide which models COULD change the RANSAC state; those
-// candidates are rescored in fp64 (k_score_list) before the serial replay, so results are those of the exact mode.
+// candidates are rescored in fp64 (k_confirm) before the serial replay, so results are those of the exact mode.
 constexpr int SCR_THREADS = 512;
 constexpr int SCR_WARPS = SCR_THREADS / 32;
 constexpr int SCR_TM = 8;
@@ -1286,30 +1276,6 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     } // problems of this CTA
 }
 
-// Exact fp64 rescoring of a list of model slots (fast mode confirmation): one CTA per listed slot.
-template <int KIND>
-__global__ void __launch_bounds__(SCORE_THREADS, 4)
-    k_score_list(const ProblemDev *__restrict__ probs, const double *__restrict__ models,
-                 const int *__restrict__ model_prob, const int *__restrict__ slots, int n_slots, uint32_t *counts,
-                 double *scores) {
-    constexpr int MSZ = kind_model_size(KIND);
-    __shared__ ScoreRed red;
-    for (int j = blockIdx.x; j < n_slots; j += gridDim.x) {
-        const int m = slots[j];
-        const ProblemDev P = probs[model_prob[m]];
-        double mdl[MSZ];
-#pragma unroll
-        for (int k = 0; k < MSZ; ++k) mdl[k] = models[(size_t)m * MSZ + k];
-        uint32_t cnt;
-        double score;
-        cta_score<KIND>(P, mdl, P.sq_thr, &red, cnt, score);
-        if (threadIdx.x == 0) {
-            counts[m] = cnt;
-            scores[m] = score;
-        }
-    }
-}
-
 // fast mode confirmation driven by the device-side candidate lists of k_select: CTA (x, a) rescores the candidates
 // x, x + gridDim.x, ... of active problem a in fp64 (same cta_score routine, hence the same bits, as everywhere else).
 template <int KIND>
@@ -1355,18 +1321,6 @@ static int sm_count() {
     }
     return cached[dev];
 }
-
-template <int KIND> static int score_blocks_per_sm() {
-    static int cached_dev[MAX_DEVICES] = {0};
-    int &cached = cached_dev[cur_dev()];
-    if (cached <= 0) {
-        int nb = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_score<KIND>, SCORE_THREADS, 0);
-        cached = nb > 0 ? nb : 1;
-    }
-    return cached;
-}
-int device_sm_count() { return sm_count(); }
 
 // relpose_5pt first half and root isolation of the R.n_total samples whose bearings are in out.s5_blk (entries
 // 75..104): the round chain and the solver surface both run them through here.
@@ -1445,20 +1399,6 @@ void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode
     default: launch_hyp_t<KIND_HOMOG>(R, out, mode, max_n_pad, stream, ev_between); break;
     }
 }
-void launch_score_list(int kind, const ProblemDev *probs, const double *models, const int *model_prob, const int *slots,
-                       int n_slots, uint32_t *counts, double *scores, cudaStream_t stream) {
-    if (n_slots <= 0) return;
-    int blocks = n_slots;
-    if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
-    switch (kind) {
-    case KIND_PNP: k_score_list<KIND_PNP><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, slots, n_slots, counts, scores); break;
-    case KIND_RELPOSE: k_score_list<KIND_RELPOSE><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, slots, n_slots, counts, scores); break;
-    case KIND_FUND: k_score_list<KIND_FUND><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, slots, n_slots, counts, scores); break;
-    case KIND_RELPOSE_TS: k_score_list<KIND_RELPOSE_TS><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, slots, n_slots, counts, scores); break;
-    default: k_score_list<KIND_HOMOG><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, slots, n_slots, counts, scores); break;
-    }
-}
-
 void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, const double *models, cudaStream_t stream) {
     if (A.na <= 0) return;
     int gx = (8 * sm_count() + A.na - 1) / A.na;
@@ -1478,16 +1418,16 @@ void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, cons
 // explicit model scoring
 // ============================================================================================================
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
-                         const int *n_models_dev, uint32_t *counts, double *scores, cudaStream_t stream) {
+                         uint32_t *counts, double *scores, cudaStream_t stream) {
     if (n_models <= 0) return;
     int blocks = n_models;
     if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
     switch (kind) {
-    case KIND_PNP: k_score<KIND_PNP><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models_dev, n_models, counts, scores); break;
-    case KIND_RELPOSE: k_score<KIND_RELPOSE><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models_dev, n_models, counts, scores); break;
-    case KIND_FUND: k_score<KIND_FUND><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models_dev, n_models, counts, scores); break;
-    case KIND_RELPOSE_TS: k_score<KIND_RELPOSE_TS><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models_dev, n_models, counts, scores); break;
-    default: k_score<KIND_HOMOG><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models_dev, n_models, counts, scores); break;
+    case KIND_PNP: k_score<KIND_PNP><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
+    case KIND_RELPOSE: k_score<KIND_RELPOSE><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
+    case KIND_FUND: k_score<KIND_FUND><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
+    case KIND_RELPOSE_TS: k_score<KIND_RELPOSE_TS><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
+    default: k_score<KIND_HOMOG><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
     }
 }
 
@@ -2128,8 +2068,8 @@ template <int NP> PLB_DEV void llt_solve(const double *A, const double *rhs, dou
 // [r*chunk, (r+1)*chunk).  Every CTA runs the scalar LM logic (optim/lm_impl.h:56-140) redundantly on identical
 // cluster totals, so no broadcast between CTAs is needed.  The reference evaluates the residual of a trial step and,
 // if accepted, the Jacobian at the same parameters in a second pass; here both come from one pass.
-template <int KIND, int MINB>
-__global__ void __launch_bounds__(LM_THREADS / MINB, MINB)
+template <int KIND>
+__global__ void __launch_bounds__(LM_THREADS, 1)
     k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
          const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
          int *idx_scratch, int scratch_stride, LmJobOut *outs) {
@@ -2349,7 +2289,7 @@ __global__ void __launch_bounds__(LM_THREADS / MINB, MINB)
         double mdl[9];
 #pragma unroll
         for (int k = 0; k < 9; ++k) mdl[k] = S.par_new[k];
-        cta_score<KIND, LM_THREADS / MINB>(P, mdl, P.sq_thr, &S.sred, cnt, score);
+        cta_score<KIND>(P, mdl, P.sq_thr, &S.sred, cnt, score);
         if (threadIdx.x == 0) {
             out->count = cnt;
             out->score = score;
@@ -2359,17 +2299,7 @@ __global__ void __launch_bounds__(LM_THREADS / MINB, MINB)
     } // jobs of this cluster
 }
 
-// CTAs of k_lm per SM.  k_lm needs ~255 registers per thread.  1: 256 threads, one CTA (one job, or one slice of a job's
-// cluster) per SM.  2 (PLB_LM_MINB=2): 128 threads per CTA, still 255 registers, two CTAs per SM — every job gets half the
-// threads but twice as many jobs are in flight; the LM passes are latency bound (few correspondences per thread, a
-// cluster-wide reduction and a scalar solve per iteration).
-static int lm_minb() {
-    static const int minb = [] {
-        const char *e = std::getenv("PLB_LM_MINB");
-        return (e && std::atoi(e) == 2) ? 2 : 1;
-    }();
-    return minb;
-}
+// k_lm needs ~255 registers per thread: one 256-thread CTA (one job, or one slice of a job's cluster) per SM.
 static thread_local int t_lm_sm_share = 50;
 void lm_set_sm_share(int pct) { t_lm_sm_share = (pct > 0 && pct <= 100) ? pct : 50; }
 static int lm_cluster_size(int n_jobs, int max_n) {
@@ -2404,7 +2334,7 @@ static void launch_lm_t(const ProblemDev *probs, const LmJob *jobs, const LoJobS
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
-    cfg.blockDim = dim3((unsigned)(LM_THREADS / lm_minb()), 1, 1);
+    cfg.blockDim = dim3((unsigned)LM_THREADS, 1, 1);
     cfg.dynamicSmemBytes = 0;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
@@ -2414,12 +2344,8 @@ static void launch_lm_t(const ProblemDev *probs, const LmJob *jobs, const LoJobS
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    if (lm_minb() == 2)
-        cudaLaunchKernelEx(&cfg, k_lm<KIND, 2>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
-                           scratch_stride, out);
-    else
-        cudaLaunchKernelEx(&cfg, k_lm<KIND, 1>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
-                           scratch_stride, out);
+    cudaLaunchKernelEx(&cfg, k_lm<KIND>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
+                       scratch_stride, out);
 }
 static void launch_lm_any(int kind, const ProblemDev *probs, const LmJob *jobs, const LoJobSrc *job_src,
                           const double *models_in, const int *n_jobs_dev, int n_jobs, int n_clusters, int csize,
@@ -2444,7 +2370,7 @@ int lm_round_max_clusters(int kind, int est_jobs, int max_n) {
     (void)kind;
     if (est_jobs < 1) est_jobs = 1;
     const int csize = lm_cluster_size(est_jobs, max_n);
-    int nc = lm_minb() * sm_count() / csize;
+    int nc = sm_count() / csize;
     if (nc > est_jobs) nc = est_jobs;
     return nc < 1 ? 1 : nc;
 }

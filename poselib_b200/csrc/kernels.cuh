@@ -113,7 +113,7 @@ struct LoJobSrc {
     int slot;  // model slot in the round's model list
 };
 // round control words in device memory (ints)
-enum { CTL_OVERFLOW = 2, CTL_NW = 4, CTL_IMP_TOTAL = 5, CTL_JOB_TOTAL = 6, CTL_FLAGS = 7, CTL_WORDS = 8 };
+enum { CTL_OVERFLOW = 2, CTL_IMP_TOTAL = 5, CTL_JOB_TOTAL = 6, CTL_FLAGS = 7, CTL_WORDS = 8 };
 enum { FLAG_IMP_OVERFLOW = 1, FLAG_JOB_OVERFLOW = 2 };
 
 struct SelectArgs {
@@ -213,15 +213,13 @@ void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream
 // AoS (caller layout) -> SoA fp64 + fp32 for n_desc problems (descriptors in device memory), camera pre-step fused.
 void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream);
 // Solve + score kernels of one round (kind = kind of every problem of the group); *out.overflow must be zeroed.
-// mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (exact rescoring of the candidates
-// is launched separately with launch_score_list once the host has selected them).
+// mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (the candidates k_select lists are
+// rescored exactly by launch_confirm).
 void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
                        cudaEvent_t ev_between = nullptr);
-void launch_score_list(int kind, const ProblemDev *probs, const double *models, const int *model_prob, const int *slots,
-                       int n_slots, uint32_t *counts, double *scores, cudaStream_t stream);
-// Exact fp64 scoring of an explicit list of models (9 doubles stride MSZ) with problem indices; *n_models_dev = count.
+// Exact fp64 scoring of an explicit list of n_models models (stride MSZ) with problem indices.
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
-                         const int *n_models_dev, uint32_t *counts, double *scores, cudaStream_t stream);
+                         uint32_t *counts, double *scores, cudaStream_t stream);
 // LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.
 void launch_lm(int kind, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in, int n_jobs,
                int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream);
@@ -256,6 +254,5 @@ int launch_solver_batch(int kind, int variant, size_t count, const double *a, co
 // relpose_8pt / essential_matrix_8pt (solvers/relpose_8pt.cc:52-95): count instances of n >= 8 unit bearing pairs each.
 void launch_eightpt(size_t count, int n, const double *x1, const double *x2, int want_poses, double *E_out, double *poses_out,
                     int *n_out, cudaStream_t stream);
-int device_sm_count();
 
 } // namespace plb
