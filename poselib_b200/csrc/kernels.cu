@@ -10,6 +10,9 @@
 //   k_lm<KIND>         Levenberg-Marquardt refit (LO step + final polish): one CTA per job, block-wide reductions of
 //                      the normal equations, scalar LM logic on thread 0
 //   k_inlier_mask      final inlier masks
+//   Every exact score (k_score_tiled, k_score, k_confirm, the rescoring in k_lm) comes from one routine, msac_score,
+//   and every fp64 inlier decision (those, k_inlier_mask, the LO subset in k_lm) from one test per kind, under_thr
+//   (+ cheirality for the relpose kinds); the PnP mask alone keeps the reference's own formula.
 //   k_solver_batch     the solvers/*.h surface: one thread per instance (relpose_5pt: k5_load -> k5_prep_lane ->
 //                      k5_roots -> k5_solver_out)
 //
@@ -180,53 +183,32 @@ void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad,
 }
 
 // ============================================================================================================
-// exact fp64 MSAC scoring of one model by one warp
+// exact fp64 inlier test and MSAC scoring
 // ============================================================================================================
-template <int KIND> struct ModelCtx;
-
-// reprojection error with z2 <= 0 skip (robust/utils.cc:36-63)
-template <> struct ModelCtx<KIND_PNP> {
-    double P[12];
-    PLB_DEV void init(const double *m) {
+// The model context: the per-model constants of the inlier test, row-major doubles.
+//   PnP              [R | t] as a 3x4 matrix
+//   relpose kinds    E = [t]x R, then q at 9..12 and t at 13..15 (cheirality)
+//   F / H            the column-major model transposed
+constexpr __host__ __device__ int kind_ctx_size(int kind) { return kind == KIND_PNP ? 12 : kind_is_relpose(kind) ? 16 : 9; }
+constexpr int CTX_MAX = 16;
+template <int KIND> PLB_DEV void model_ctx(const double *m, double *ctx) {
+    if constexpr (KIND == KIND_PNP) {
         const m3 R = quat_to_rot(m);
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
-            P[4 * r + 0] = R(r, 0); P[4 * r + 1] = R(r, 1); P[4 * r + 2] = R(r, 2); P[4 * r + 3] = m[4 + r];
+            ctx[4 * r + 0] = R(r, 0); ctx[4 * r + 1] = R(r, 1); ctx[4 * r + 2] = R(r, 2); ctx[4 * r + 3] = m[4 + r];
         }
+    } else if constexpr (kind_is_relpose(KIND)) {
+        const m3 E = essential_from_pose(m, m + 4);
+#pragma unroll
+        for (int i = 0; i < 9; ++i) ctx[i] = E.a[i];
+#pragma unroll
+        for (int i = 0; i < 7; ++i) ctx[9 + i] = m[i];
+    } else {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) ctx[3 * (k % 3) + k / 3] = m[k];
     }
-};
-// Sampson error + cheirality on candidates under threshold (robust/utils.cc:158-201)
-template <> struct ModelCtx<KIND_RELPOSE> {
-    double E[9];
-    double q[4], t[3];
-    PLB_DEV void init(const double *m) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) q[i] = m[i];
-#pragma unroll
-        for (int i = 0; i < 3; ++i) t[i] = m[4 + i];
-        const m3 Em = essential_from_pose(q, t);
-#pragma unroll
-        for (int i = 0; i < 9; ++i) E[i] = Em.a[i];
-    }
-};
-// tangent Sampson error + cheirality (robust/utils.cc:269-298): same model constants as KIND_RELPOSE
-template <> struct ModelCtx<KIND_RELPOSE_TS> : ModelCtx<KIND_RELPOSE> {};
-// Sampson error (robust/utils.cc:204-239); model is column-major
-template <> struct ModelCtx<KIND_FUND> {
-    double E[9];
-    PLB_DEV void init(const double *m) {
-#pragma unroll
-        for (int k = 0; k < 9; ++k) E[3 * (k % 3) + k / 3] = m[k];
-    }
-};
-// one-way transfer error (robust/utils.cc:300-329); model is column-major
-template <> struct ModelCtx<KIND_HOMOG> {
-    double H[9];
-    PLB_DEV void init(const double *m) {
-#pragma unroll
-        for (int k = 0; k < 9; ++k) H[3 * (k % 3) + k / 3] = m[k];
-    }
-};
+}
 
 PLB_DEV double sampson_r2(const double *E, double x1_0, double x1_1, double x2_0, double x2_1) {
     const double Ex1_0 = E[0] * x1_0 + E[1] * x1_1 + E[2];
@@ -279,102 +261,164 @@ PLB_DEV double homography_r2(const double *H, double x1_0, double x1_1, double x
     return r0 * r0 + r1 * r1;
 }
 
-// Scores `model` over all correspondences with the first SCORE_THREADS (=256) threads of the CTA; every thread of
-// the CTA must call it (it contains CTA barriers) and receives the same (count, score).
-// The summation order is fixed — thread-strided partial sums, xor-butterfly inside each warp, the 8 warp partials
-// added left to right — so the same model gets the same score bits wherever it is scored (hypothesis scoring,
-// LO rescoring, explicit rescoring): the equalities the serial loop relies on (ransac_impl.h:127,143) are preserved.
+// One correspondence as the inlier test reads it: x.x x.y X.x X.y X.z (PnP), x1.x x1.y x2.x x2.y (relpose, F, H) or
+// the 18 tangent-Sampson values.
+constexpr __host__ __device__ int kind_corr_size(int kind) { return kind == KIND_PNP ? 5 : kind == KIND_RELPOSE_TS ? TS_ARRAYS : 4; }
+template <int KIND> PLB_DEV void load_corr(const ProblemDev &P, int k, double *v) {
+    if constexpr (KIND == KIND_RELPOSE_TS) {
+        load_ts(P, k, v);
+    } else {
+#pragma unroll
+        for (int j = 0; j < kind_corr_size(KIND); ++j) v[j] = P.p[j][k];
+    }
+}
+// The fp64 inlier test, split so that a tile of models can share one load of the correspondence and one computation
+// of its bearings.  under_thr: r2 of correspondence v under model context C, and r2 < sq_thr.
+//   PnP              reprojection error, points with z2 <= 0 skipped (robust/utils.cc:36-63)
+//   relpose, F       Sampson error (robust/utils.cc:158-201, 204-239)
+//   tangent Sampson  robust/utils.cc:269-298
+//   H                one-way transfer error (robust/utils.cc:300-329)
+template <int KIND> PLB_DEV bool under_thr(const double *C, const double *v, double sq_thr, double &r2) {
+    if constexpr (KIND == KIND_PNP) {
+        const double z0 = C[0] * v[2] + C[1] * v[3] + C[2] * v[4] + C[3];
+        const double z1 = C[4] * v[2] + C[5] * v[3] + C[6] * v[4] + C[7];
+        const double z2 = C[8] * v[2] + C[9] * v[3] + C[10] * v[4] + C[11];
+        if (z2 <= 0.0) return false;
+        const double inv_z2 = 1.0 / z2;
+        const double r_0 = z0 * inv_z2 - v[0];
+        const double r_1 = z1 * inv_z2 - v[1];
+        r2 = r_0 * r_0 + r_1 * r_1;
+    } else if constexpr (KIND == KIND_RELPOSE_TS) {
+        r2 = tangent_r2(C, v);
+    } else if constexpr (KIND == KIND_HOMOG) {
+        r2 = homography_r2(C, v[0], v[1], v[2], v[3]);
+    } else {
+        r2 = sampson_r2(C, v[0], v[1], v[2], v[3]);
+    }
+    return r2 < sq_thr;
+}
+// Relpose kinds: cheirality, tested only for correspondences under the threshold (robust/utils.cc:187-197), on the unit
+// bearings of the correspondence.
+template <int KIND> PLB_DEV void corr_bearings(const double *v, d3 &b1, d3 &b2) {
+    if constexpr (KIND == KIND_RELPOSE_TS) {
+        b1 = mk(v[0], v[1], v[2]);
+        b2 = mk(v[3], v[4], v[5]);
+    } else {
+        b1 = bearing(v[0], v[1]);
+        b2 = bearing(v[2], v[3]);
+    }
+}
+PLB_DEV bool cheirality_ctx(const double *C, d3 b1, d3 b2) { return cheirality_ok(C + 9, C + 13, b1, b2, 0.01); }
+template <int KIND> PLB_DEV bool is_inlier(const double *C, const double *v, double sq_thr) {
+    double r2;
+    if (!under_thr<KIND>(C, v, sq_thr, r2)) return false;
+    if constexpr (kind_is_relpose(KIND)) {
+        d3 b1, b2;
+        corr_bearings<KIND>(v, b1, b2);
+        return cheirality_ctx(C, b1, b2);
+    }
+    return true;
+}
+
+// Exact MSAC scoring of a tile of models (contexts ctx[0..tm), tm <= TM) over all correspondences of P, by the CTA's
+// SCORE_THREADS (=256) threads, all of which must call it (it contains CTA barriers and warp reductions).
+// Model i's record goes to counts[i], scores[i].  Every correspondence is loaded once for the whole tile.
+// A model's summation order depends neither on TM nor on its place in the tile — thread-strided partial sums,
+// xor-butterfly inside each warp, the 8 warp partials added left to right — so the same model gets the same score bits
+// wherever it is scored (round tiles, initial models, LO rescoring, fast-mode confirmation): the equalities the serial
+// loop relies on (ransac_impl.h:127,143) are preserved.
 constexpr int SCORE_THREADS = 256;
 constexpr int SCORE_WARPS = SCORE_THREADS / 32;
-struct ScoreRed {
-    double s[SCORE_WARPS];
-    uint32_t c[SCORE_WARPS];
+template <int TM> struct ScoreRed {
+    double s[SCORE_WARPS][TM];
+    uint32_t c[SCORE_WARPS][TM];
 };
-template <int KIND>
-PLB_DEV void cta_score(const ProblemDev &P, const double *model, double sq_thr, ScoreRed *red, uint32_t &count_out,
-                       double &score_out) {
+template <int KIND, int TM>
+PLB_DEV void msac_score(const ProblemDev &P, const double (&ctx)[TM][CTX_MAX], int tm, ScoreRed<TM> &red,
+                        uint32_t *counts, double *scores) {
     const int tid = threadIdx.x, lane = tid & 31;
     const int n = P.n;
-    if (tid < SCORE_THREADS) {
-        ModelCtx<KIND> C;
-        C.init(model);
-        uint32_t cnt = 0;
-        double score = 0.0;
-        if (KIND == KIND_PNP) {
-            const double *__restrict__ xx = P.p[0], *__restrict__ xy = P.p[1];
-            const double *__restrict__ Xx = P.p[2], *__restrict__ Xy = P.p[3], *__restrict__ Xz = P.p[4];
-            const double *Pm = reinterpret_cast<const double *>(&C);
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                const double X0 = Xx[k], X1 = Xy[k], X2 = Xz[k];
-                const double x0 = xx[k], x1 = xy[k];
-                const double z0 = Pm[0] * X0 + Pm[1] * X1 + Pm[2] * X2 + Pm[3];
-                const double z1 = Pm[4] * X0 + Pm[5] * X1 + Pm[6] * X2 + Pm[7];
-                const double z2 = Pm[8] * X0 + Pm[9] * X1 + Pm[10] * X2 + Pm[11];
-                if (z2 <= 0.0) continue;
-                const double inv_z2 = 1.0 / z2;
-                const double r_0 = z0 * inv_z2 - x0;
-                const double r_1 = z1 * inv_z2 - x1;
-                const double r_sq = r_0 * r_0 + r_1 * r_1;
-                if (r_sq < sq_thr) {
-                    ++cnt;
-                    score += r_sq;
-                }
-            }
-        } else if (KIND == KIND_RELPOSE_TS) {
-            const double *M = reinterpret_cast<const double *>(&C);
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                double vv[TS_ARRAYS];
-                load_ts(P, k, vv);
-                const double r2 = tangent_r2(M, vv);
-                bool inl = r2 < sq_thr;
-                if (inl) inl = cheirality_ok(M + 9, M + 13, mk(vv[0], vv[1], vv[2]), mk(vv[3], vv[4], vv[5]), 0.01);
-                if (inl) {
-                    ++cnt;
-                    score += r2;
-                }
-            }
-        } else {
-            const double *__restrict__ ax = P.p[0], *__restrict__ ay = P.p[1];
-            const double *__restrict__ bx = P.p[2], *__restrict__ by = P.p[3];
-            const double *M = reinterpret_cast<const double *>(&C); // first 9 doubles: E / F / H row-major
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                const double x1_0 = ax[k], x1_1 = ay[k], x2_0 = bx[k], x2_1 = by[k];
-                double r2;
-                if (KIND == KIND_HOMOG) r2 = homography_r2(M, x1_0, x1_1, x2_0, x2_1);
-                else r2 = sampson_r2(M, x1_0, x1_1, x2_0, x2_1);
-                bool inl = r2 < sq_thr;
-                if (KIND == KIND_RELPOSE) {
-                    if (inl) inl = cheirality_ok(M + 9, M + 13, bearing(x1_0, x1_1), bearing(x2_0, x2_1), 0.01);
-                }
-                if (inl) {
-                    ++cnt;
-                    score += r2;
-                }
-            }
-        }
-        cnt = warp_sum_u(cnt);
-        score = warp_sum(score);
-        if (lane == 0) {
-            red->c[tid >> 5] = cnt;
-            red->s[tid >> 5] = score;
-        }
-    }
-    __syncthreads();
-    uint32_t ct = 0;
-    double st = 0.0;
+    const double sq_thr = P.sq_thr;
+    uint32_t cnt[TM];
+    double sc[TM];
 #pragma unroll
-    for (int w = 0; w < SCORE_WARPS; ++w) {
-        ct += red->c[w];
-        st += red->s[w];
+    for (int i = 0; i < TM; ++i) {
+        cnt[i] = 0;
+        sc[i] = 0.0;
     }
-    // Outliers contribute (n - count) * thr in ONE product for every kind (the reference does so for reprojection
-    // scores, robust/utils.cc:62, and adds thr per outlier for the others).  Position-independent on purpose: models
-    // supported only by their own minimal sample all score (n - K) thr to the last bit, as in the CPU's sequential
-    // sum where the K negligible residuals are absorbed — so such ties are not "better scores" (ransac_impl.h:116).
-    st += (double)(n - (int)ct) * sq_thr;
+    // One correspondence per iteration: unrolled, the loop keeps the problem's array pointers of several iterations
+    // live, and the 64-register one-model kernels (k_score, k_confirm) spill them.
+#pragma unroll 1
+    for (int k = tid; k < n; k += SCORE_THREADS) {
+        double v[kind_corr_size(KIND)];
+        load_corr<KIND>(P, k, v);
+        // Without cheirality a model under the threshold is an inlier and is accumulated at once; the relpose kinds
+        // collect the models under the threshold first, so that the bearings are computed once for the tile.
+        double r2u[TM];
+        unsigned under = 0;
+#pragma unroll
+        for (int i = 0; i < TM; ++i) {
+            double r2;
+            if (i < tm && under_thr<KIND>(ctx[i], v, sq_thr, r2)) {
+                if constexpr (kind_is_relpose(KIND)) {
+                    r2u[i] = r2;
+                    under |= 1u << i;
+                } else {
+                    ++cnt[i];
+                    sc[i] += r2;
+                }
+            }
+        }
+        if (kind_is_relpose(KIND) && under) {
+            d3 b1, b2;
+            corr_bearings<KIND>(v, b1, b2);
+#pragma unroll 1
+            for (int i = 0; i < TM; ++i)
+                if (((under >> i) & 1u) && !cheirality_ctx(ctx[i], b1, b2)) under &= ~(1u << i);
+#pragma unroll
+            for (int i = 0; i < TM; ++i) {
+                if ((under >> i) & 1u) {
+                    ++cnt[i];
+                    sc[i] += r2u[i];
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < TM; ++i) {
+        const uint32_t c = warp_sum_u(cnt[i]);
+        const double s = warp_sum(sc[i]);
+        if (lane == 0) {
+            red.c[tid >> 5][i] = c;
+            red.s[tid >> 5][i] = s;
+        }
+    }
     __syncthreads();
-    count_out = ct;
-    score_out = st;
+    if (tid < tm) {
+        uint32_t ct = 0;
+        double st = 0.0;
+#pragma unroll
+        for (int w = 0; w < SCORE_WARPS; ++w) {
+            ct += red.c[w][tid];
+            st += red.s[w][tid];
+        }
+        // Outliers contribute (n - count) * thr in ONE product for every kind (the reference does so for reprojection
+        // scores, robust/utils.cc:62, and adds thr per outlier for the others).  Position-independent on purpose:
+        // models supported only by their own minimal sample all score (n - K) thr to the last bit, as in the CPU's
+        // sequential sum where the K negligible residuals are absorbed — so such ties are not "better scores"
+        // (ransac_impl.h:116).
+        st += (double)(n - (int)ct) * sq_thr;
+        counts[tid] = ct;
+        scores[tid] = st;
+    }
+    __syncthreads(); // red and ctx may be rewritten after this
+}
+// One model, its context built by every thread in registers.
+template <int KIND>
+PLB_DEV void cta_score(const ProblemDev &P, const double *model, ScoreRed<1> &red, uint32_t *count, double *score) {
+    double ctx[1][CTX_MAX];
+    model_ctx<KIND>(model, ctx[0]);
+    msac_score<KIND, 1>(P, ctx, 1, red, count, score);
 }
 
 // ============================================================================================================
@@ -719,26 +763,18 @@ __global__ void __launch_bounds__(SCORE_THREADS, 4)
     k_score(const ProblemDev *__restrict__ probs, const double *__restrict__ models, const int *__restrict__ model_prob,
             int n_models, uint32_t *counts, double *scores) {
     constexpr int MSZ = kind_model_size(KIND);
-    __shared__ ScoreRed red;
+    __shared__ ScoreRed<1> red;
     for (int m = blockIdx.x; m < n_models; m += gridDim.x) {
         const ProblemDev P = probs[model_prob[m]];
         double mdl[MSZ];
 #pragma unroll
         for (int k = 0; k < MSZ; ++k) mdl[k] = models[(size_t)m * MSZ + k];
-        uint32_t cnt;
-        double score;
-        cta_score<KIND>(P, mdl, P.sq_thr, &red, cnt, score);
-        if (threadIdx.x == 0) {
-            counts[m] = cnt;
-            scores[m] = score;
-        }
+        cta_score<KIND>(P, mdl, red, counts + m, scores + m);
     }
 }
 
-// Tiled score kernel of the round path: CTA (x, a) scores tiles of SCORE_TM models of active problem a.  Every thread
-// loads a correspondence ONCE and evaluates all models of the tile against it (model constants are broadcast reads from
-// shared memory), which divides the L2 -> SM traffic of the one-CTA-per-model kernel by the tile size; the per-model
-// summation order is exactly that of cta_score, so both kernels produce the same bits for the same model.
+// Tiled score kernel of the round path: CTA (x, a) scores tiles of SCORE_TM models of active problem a (model constants
+// are broadcast reads from shared memory), which divides the L2 -> SM traffic of one CTA per model by the tile size.
 constexpr int SCORE_TM = 4;
 // the tangent-Sampson kind carries 18 values per correspondence: two models per tile keep it inside 128 registers
 template <int KIND> constexpr __host__ __device__ int score_tm() { return KIND == KIND_RELPOSE_TS ? 2 : SCORE_TM; }
@@ -746,142 +782,25 @@ template <int KIND>
 __global__ void __launch_bounds__(SCORE_THREADS, 2)
     k_score_tiled(const RoundDesc R, HypOut out) {
     constexpr int MSZ = kind_model_size(KIND);
-    constexpr int CTX = (KIND == KIND_PNP) ? 12 : kind_is_relpose(KIND) ? 16 : 9;
     constexpr int TM = score_tm<KIND>();
-    __shared__ double ctx[TM][16];
-    __shared__ double red_s[SCORE_WARPS][TM];
-    __shared__ uint32_t red_c[SCORE_WARPS][TM];
+    __shared__ double ctx[TM][CTX_MAX];
+    __shared__ ScoreRed<TM> red;
     const int a = blockIdx.y;
     const int count = out.prob_count[a];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     if (blockIdx.x * TM >= count) return;
     const ProblemDev P = R.probs[R.active[a]];
-    const int n = P.n;
-    const double sq_thr = P.sq_thr;
     const int seg = out.seg_base[a];
     for (int m0 = blockIdx.x * TM; m0 < count; m0 += gridDim.x * TM) {
         const int tm = (count - m0 < TM) ? (count - m0) : TM;
-        __syncthreads();
         if (tid < tm) {
             double mdl[MSZ];
 #pragma unroll
             for (int k = 0; k < MSZ; ++k) mdl[k] = out.models[(size_t)(seg + m0 + tid) * MSZ + k];
-            ModelCtx<KIND> C;
-            C.init(mdl);
-            const double *cp = reinterpret_cast<const double *>(&C);
-#pragma unroll
-            for (int k = 0; k < CTX; ++k) ctx[tid][k] = cp[k];
+            model_ctx<KIND>(mdl, ctx[tid]);
         }
         __syncthreads();
-        uint32_t cnt[TM];
-        double sc[TM];
-#pragma unroll
-        for (int i = 0; i < TM; ++i) {
-            cnt[i] = 0;
-            sc[i] = 0.0;
-        }
-        if (KIND == KIND_PNP) {
-            const double *__restrict__ xx = P.p[0], *__restrict__ xy = P.p[1];
-            const double *__restrict__ Xx = P.p[2], *__restrict__ Xy = P.p[3], *__restrict__ Xz = P.p[4];
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                const double X0 = Xx[k], X1 = Xy[k], X2 = Xz[k];
-                const double x0 = xx[k], x1 = xy[k];
-#pragma unroll
-                for (int i = 0; i < TM; ++i) {
-                    if (i < tm) {
-                        const double *Pm = ctx[i];
-                        const double z0 = Pm[0] * X0 + Pm[1] * X1 + Pm[2] * X2 + Pm[3];
-                        const double z1 = Pm[4] * X0 + Pm[5] * X1 + Pm[6] * X2 + Pm[7];
-                        const double z2 = Pm[8] * X0 + Pm[9] * X1 + Pm[10] * X2 + Pm[11];
-                        if (z2 > 0.0) {
-                            const double inv_z2 = 1.0 / z2;
-                            const double r_0 = z0 * inv_z2 - x0;
-                            const double r_1 = z1 * inv_z2 - x1;
-                            const double r_sq = r_0 * r_0 + r_1 * r_1;
-                            if (r_sq < sq_thr) {
-                                ++cnt[i];
-                                sc[i] += r_sq;
-                            }
-                        }
-                    }
-                }
-            }
-        } else if (KIND == KIND_RELPOSE_TS) {
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                double v[TS_ARRAYS];
-                load_ts(P, k, v);
-#pragma unroll
-                for (int i = 0; i < TM; ++i) {
-                    if (i < tm) {
-                        const double r2 = tangent_r2(ctx[i], v);
-                        bool inl = r2 < sq_thr;
-                        if (inl)
-                            inl = cheirality_ok(ctx[i] + 9, ctx[i] + 13, mk(v[0], v[1], v[2]), mk(v[3], v[4], v[5]), 0.01);
-                        if (inl) {
-                            ++cnt[i];
-                            sc[i] += r2;
-                        }
-                    }
-                }
-            }
-        } else {
-            const double *__restrict__ ax = P.p[0], *__restrict__ ay = P.p[1];
-            const double *__restrict__ bx = P.p[2], *__restrict__ by = P.p[3];
-            for (int k = tid; k < n; k += SCORE_THREADS) {
-                const double x1_0 = ax[k], x1_1 = ay[k], x2_0 = bx[k], x2_1 = by[k];
-                double r2v[TM];
-                unsigned under = 0; // models whose residual is under the threshold at this correspondence
-#pragma unroll
-                for (int i = 0; i < TM; ++i) {
-                    if (i < tm) {
-                        const double *M = ctx[i];
-                        if (KIND == KIND_HOMOG) r2v[i] = homography_r2(M, x1_0, x1_1, x2_0, x2_1);
-                        else r2v[i] = sampson_r2(M, x1_0, x1_1, x2_0, x2_1);
-                        if (r2v[i] < sq_thr) under |= 1u << i;
-                    }
-                }
-                if (KIND == KIND_RELPOSE && under) {
-                    // cheirality only for candidates under the threshold (robust/utils.cc:187-197); the normalised
-                    // bearings depend on the correspondence alone and are computed once
-                    const d3 b1 = bearing(x1_0, x1_1), b2 = bearing(x2_0, x2_1);
-#pragma unroll 1
-                    for (int i = 0; i < TM; ++i)
-                        if ((under >> i) & 1u)
-                            if (!cheirality_ok(ctx[i] + 9, ctx[i] + 13, b1, b2, 0.01)) under &= ~(1u << i);
-                }
-#pragma unroll
-                for (int i = 0; i < TM; ++i) {
-                    if (i < tm) {
-                        if ((under >> i) & 1u) {
-                            ++cnt[i];
-                            sc[i] += r2v[i];
-                        }
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < TM; ++i) {
-            const uint32_t c = warp_sum_u(cnt[i]);
-            const double v = warp_sum(sc[i]);
-            if (lane == 0) {
-                red_c[warp][i] = c;
-                red_s[warp][i] = v;
-            }
-        }
-        __syncthreads();
-        if (tid < tm) {
-            uint32_t ct = 0;
-            double st = 0.0;
-#pragma unroll
-            for (int w = 0; w < SCORE_WARPS; ++w) {
-                ct += red_c[w][tid];
-                st += red_s[w][tid];
-            }
-            st += (double)(n - (int)ct) * sq_thr; // see cta_score
-            out.counts[seg + m0 + tid] = ct;
-            out.scores[seg + m0 + tid] = st;
-        }
+        msac_score<KIND, TM>(P, ctx, tm, red, out.counts + seg + m0, out.scores + seg + m0);
     }
 }
 
@@ -948,7 +867,7 @@ template <int KIND, int NTHR>
 __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const RoundDesc R, HypOut out, int use_smem) {
     constexpr int SCR_THREADS = NTHR, SCR_WARPS = NTHR / 32; // shadow the file-scope defaults
     constexpr int MSZ = kind_model_size(KIND);
-    constexpr int CTX = (KIND == KIND_PNP) ? 12 : kind_is_relpose(KIND) ? 16 : 9;
+    constexpr int CTX = kind_ctx_size(KIND);
     constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
     extern __shared__ __align__(128) unsigned char scr_smem[];
     __shared__ __align__(8) uint64_t bar;
@@ -1081,9 +1000,8 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             double mdl[MSZ];
 #pragma unroll
             for (int k = 0; k < MSZ; ++k) mdl[k] = out.models[(size_t)(seg + m0 + tid) * MSZ + k];
-            ModelCtx<KIND> C;
-            C.init(mdl);
-            const double *cp = reinterpret_cast<const double *>(&C);
+            double cp[CTX];
+            model_ctx<KIND>(mdl, cp);
 #pragma unroll
             for (int k = 0; k < CTX; ++k) ctx[tid][k] = (float)cp[k];
             // per-model constants of the error bounds (screen_math.cuh), from the fp64 model and the problem's maxima
@@ -1093,7 +1011,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             if (KIND == KIND_PNP) scr::transfer_setup<3>(cp, cm + 2, cm, P.sq_thr, ctx[tid]);
             else if (KIND == KIND_HOMOG) scr::transfer_setup<2>(cp, cm, cm + 2, P.sq_thr, ctx[tid]);
             else scr::sampson_setup(cp, cm, P.sq_thr, ctx[tid]);
-            if (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, ctx[tid]);
+            if constexpr (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, ctx[tid]);
         }
         __syncthreads();
         uint32_t cnt[SCR_TM];
@@ -1277,12 +1195,12 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
 }
 
 // fast mode confirmation driven by the device-side candidate lists of k_select: CTA (x, a) rescores the candidates
-// x, x + gridDim.x, ... of active problem a in fp64 (same cta_score routine, hence the same bits, as everywhere else).
+// x, x + gridDim.x, ... of active problem a in fp64 (msac_score, hence the same bits as everywhere else).
 template <int KIND>
 __global__ void __launch_bounds__(SCORE_THREADS, 4)
     k_confirm(const ProblemDev *__restrict__ probs, const SelectArgs A, const double *__restrict__ models) {
     constexpr int MSZ = kind_model_size(KIND);
-    __shared__ ScoreRed red;
+    __shared__ ScoreRed<1> red;
     const int a = blockIdx.y;
     const int nc = A.n_cand[a];
     if ((int)blockIdx.x >= nc) return;
@@ -1293,13 +1211,7 @@ __global__ void __launch_bounds__(SCORE_THREADS, 4)
         double mdl[MSZ];
 #pragma unroll
         for (int k = 0; k < MSZ; ++k) mdl[k] = models[(size_t)m * MSZ + k];
-        uint32_t cnt;
-        double score;
-        cta_score<KIND>(P, mdl, P.sq_thr, &red, cnt, score);
-        if (threadIdx.x == 0) {
-            A.counts[m] = cnt;
-            A.scores[m] = score;
-        }
+        cta_score<KIND>(P, mdl, red, A.counts + m, A.scores + m);
     }
 }
 
@@ -1320,6 +1232,14 @@ static int sm_count() {
         cached[dev] = n > 0 ? n : 132;
     }
     return cached[dev];
+}
+// Calls f(std::integral_constant<int, K>{}) for the runtime kind K; unknown kinds run as KIND_HOMOG.
+template <class F> static void with_kind(int kind, F &&f) {
+    if (kind == KIND_PNP) f(std::integral_constant<int, KIND_PNP>{});
+    else if (kind == KIND_RELPOSE) f(std::integral_constant<int, KIND_RELPOSE>{});
+    else if (kind == KIND_FUND) f(std::integral_constant<int, KIND_FUND>{});
+    else if (kind == KIND_RELPOSE_TS) f(std::integral_constant<int, KIND_RELPOSE_TS>{});
+    else f(std::integral_constant<int, KIND_HOMOG>{});
 }
 
 // relpose_5pt first half and root isolation of the R.n_total samples whose bearings are in out.s5_blk (entries
@@ -1391,13 +1311,7 @@ static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int ma
 void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
                        cudaEvent_t ev_between) {
     cudaMemsetAsync(out.prob_count, 0, sizeof(int) * R.n_active, stream);
-    switch (kind) {
-    case KIND_PNP: launch_hyp_t<KIND_PNP>(R, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_RELPOSE: launch_hyp_t<KIND_RELPOSE>(R, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_FUND: launch_hyp_t<KIND_FUND>(R, out, mode, max_n_pad, stream, ev_between); break;
-    case KIND_RELPOSE_TS: launch_hyp_t<KIND_RELPOSE_TS>(R, out, mode, max_n_pad, stream, ev_between); break;
-    default: launch_hyp_t<KIND_HOMOG>(R, out, mode, max_n_pad, stream, ev_between); break;
-    }
+    with_kind(kind, [&](auto K) { launch_hyp_t<K>(R, out, mode, max_n_pad, stream, ev_between); });
 }
 void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, const double *models, cudaStream_t stream) {
     if (A.na <= 0) return;
@@ -1405,13 +1319,7 @@ void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, cons
     if (gx > 64) gx = 64;
     if (gx < 1) gx = 1;
     const dim3 grid((unsigned)gx, (unsigned)A.na, 1);
-    switch (kind) {
-    case KIND_PNP: k_confirm<KIND_PNP><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); break;
-    case KIND_RELPOSE: k_confirm<KIND_RELPOSE><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); break;
-    case KIND_FUND: k_confirm<KIND_FUND><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); break;
-    case KIND_RELPOSE_TS: k_confirm<KIND_RELPOSE_TS><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); break;
-    default: k_confirm<KIND_HOMOG><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); break;
-    }
+    with_kind(kind, [&](auto K) { k_confirm<K><<<grid, SCORE_THREADS, 0, stream>>>(probs, A, models); });
 }
 
 // ============================================================================================================
@@ -1422,13 +1330,9 @@ void launch_score_models(int kind, const ProblemDev *probs, const double *models
     if (n_models <= 0) return;
     int blocks = n_models;
     if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
-    switch (kind) {
-    case KIND_PNP: k_score<KIND_PNP><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
-    case KIND_RELPOSE: k_score<KIND_RELPOSE><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
-    case KIND_FUND: k_score<KIND_FUND><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
-    case KIND_RELPOSE_TS: k_score<KIND_RELPOSE_TS><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
-    default: k_score<KIND_HOMOG><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores); break;
-    }
+    with_kind(kind, [&](auto K) {
+        k_score<K><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores);
+    });
 }
 
 // ============================================================================================================
@@ -1446,34 +1350,20 @@ __global__ void k_inlier_mask(const ProblemDev *__restrict__ probs, const MaskDe
     for (int k = 0; k < MSZ; ++k) mdl[k] = D.model[k];
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= P.n) return;
-    if (KIND == KIND_PNP) {
-        // robust/utils.cc:374-383: Z = R*X + t ; r2 = |Z.hnormalized() - x|^2 ; inlier iff r2 < thr && Z(2) > 0
+    if constexpr (KIND == KIND_PNP) {
+        // The PnP mask keeps its own formula on purpose (DESIGN.md §3): the reference's mask (robust/utils.cc:374-383)
+        // divides, r2 = |Z.hnormalized() - x|^2 with Z = R*X + t, and tests Z(2) > 0 after the threshold, while its
+        // scorer (under_thr) multiplies by 1/z2 and skips z2 <= 0 first.  The two give different bits.
         const m3 R = quat_to_rot(mdl);
         const d3 Z = mvec(R, mk(P.p[2][k], P.p[3][k], P.p[4][k])) + mk(mdl[4], mdl[5], mdl[6]);
         const double d0 = Z.x / Z.z - P.p[0][k], d1 = Z.y / Z.z - P.p[1][k];
         const double r2 = d0 * d0 + d1 * d1;
         mask[k] = (r2 < sq_thr && Z.z > 0.0) ? 1 : 0;
-    } else if (KIND == KIND_RELPOSE_TS) { // robust/utils.cc:541-569
-        ModelCtx<KIND> C;
-        C.init(mdl);
-        const double *M = reinterpret_cast<const double *>(&C);
-        double v[TS_ARRAYS];
-        load_ts(P, k, v);
-        bool inl = tangent_r2(M, v) < sq_thr;
-        if (inl) inl = cheirality_ok(M + 9, M + 13, mk(v[0], v[1], v[2]), mk(v[3], v[4], v[5]), 0.01);
-        mask[k] = inl ? 1 : 0;
-    } else {
-        ModelCtx<KIND> C;
-        C.init(mdl);
-        const double *M = reinterpret_cast<const double *>(&C);
-        const double x1_0 = P.p[0][k], x1_1 = P.p[1][k], x2_0 = P.p[2][k], x2_1 = P.p[3][k];
-        double r2;
-        if (KIND == KIND_HOMOG) r2 = homography_r2(M, x1_0, x1_1, x2_0, x2_1);
-        else r2 = sampson_r2(M, x1_0, x1_1, x2_0, x2_1);
-        bool inl = r2 < sq_thr;
-        if (KIND == KIND_RELPOSE && inl)
-            inl = cheirality_ok(M + 9, M + 13, bearing(x1_0, x1_1), bearing(x2_0, x2_1), 0.01);
-        mask[k] = inl ? 1 : 0;
+    } else { // the scorer's test (tangent Sampson: robust/utils.cc:541-569)
+        double C[kind_ctx_size(KIND)], v[kind_corr_size(KIND)];
+        model_ctx<KIND>(mdl, C);
+        load_corr<KIND>(P, k, v);
+        mask[k] = is_inlier<KIND>(C, v, sq_thr) ? 1 : 0;
     }
 }
 // One bit per correspondence for the trip over PCIe (the host expands them to the caller's char[n]).
@@ -1492,19 +1382,14 @@ void launch_inlier_masks(int kind, const ProblemDev *probs, const MaskDesc *desc
     if (n_desc <= 0 || max_n <= 0) return;
     const int threads = 256;
     dim3 grid((max_n + threads - 1) / threads, n_desc, 1);
-    switch (kind) {
-    case KIND_PNP: k_inlier_mask<KIND_PNP><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); break;
-    case KIND_RELPOSE: k_inlier_mask<KIND_RELPOSE><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); break;
-    case KIND_FUND: k_inlier_mask<KIND_FUND><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); break;
-    case KIND_RELPOSE_TS: k_inlier_mask<KIND_RELPOSE_TS><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); break;
-    default: k_inlier_mask<KIND_HOMOG><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); break;
-    }
+    with_kind(kind, [&](auto K) { k_inlier_mask<K><<<grid, threads, 0, stream>>>(probs, descs_dev, mask_base); });
 }
 
 // ============================================================================================================
 // Levenberg-Marquardt refit: one CTA per job
 // ============================================================================================================
 constexpr int LM_THREADS = 256;
+static_assert(LM_THREADS == SCORE_THREADS, "k_lm rescores its result with msac_score");
 constexpr int LM_WARPS = LM_THREADS / 32;
 constexpr int LM_MAX_CLUSTER = 8;
 constexpr int LM_NV_MAX = 56;
@@ -1819,7 +1704,7 @@ struct LmShared {
     double red[LM_WARPS][LM_NV_MAX];
     double sums[2][LM_NV_MAX]; // CTA partial sums, double-buffered: read by the other CTAs of the cluster (DSMEM)
     double tot[LM_NV_MAX];     // cluster totals (identical in every CTA)
-    ScoreRed sred;
+    ScoreRed<1> sred;
     int wcount[LM_WARPS];
     int flag;
 };
@@ -2111,9 +1996,8 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
     bool untouched = false;
     if (prm.subset_mode != 0) {
         int *mylist = idx_scratch + (size_t)cluster_id * (size_t)scratch_stride + lo;
-        ModelCtx<KIND_RELPOSE> C;
-        if (KIND == KIND_RELPOSE && prm.subset_mode == 1) C.init(min);
-        const double *M = reinterpret_cast<const double *>(&C);
+        double C[kind_ctx_size(KIND_RELPOSE)];
+        if (KIND == KIND_RELPOSE && prm.subset_mode == 1) model_ctx<KIND_RELPOSE>(min, C);
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
         int base = 0;
         for (int t0 = lo; t0 < hi; t0 += (int)blockDim.x) {
@@ -2124,9 +2008,9 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
                     keep = mask_in[k] != 0;
                 } else if (KIND == KIND_RELPOSE) {
                     // relpose LO subset: inliers of the start pose at 5*thr^2 (estimators/relative_pose.cc:62-86)
-                    const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
-                    keep = sampson_r2(M, a0, a1, b0, b1) < prm.subset_sq_thr;
-                    if (keep) keep = cheirality_ok(M + 9, M + 13, bearing(a0, a1), bearing(b0, b1), 0.01);
+                    double v[kind_corr_size(KIND_RELPOSE)];
+                    load_corr<KIND_RELPOSE>(P, k, v);
+                    keep = is_inlier<KIND_RELPOSE>(C, v, prm.subset_sq_thr);
                 }
             }
             const unsigned bal = __ballot_sync(0xffffffffu, keep);
@@ -2284,16 +2168,10 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
     }
     __syncthreads();
     if (prm.score_after && crank == 0) {
-        uint32_t cnt;
-        double score;
         double mdl[9];
 #pragma unroll
         for (int k = 0; k < 9; ++k) mdl[k] = S.par_new[k];
-        cta_score<KIND>(P, mdl, P.sq_thr, &S.sred, cnt, score);
-        if (threadIdx.x == 0) {
-            out->count = cnt;
-            out->score = score;
-        }
+        cta_score<KIND>(P, mdl, S.sred, &out->count, &out->score);
     }
     cluster.sync(); // no CTA may exit (or start the next job) while a sibling can still read its shared memory
     } // jobs of this cluster
@@ -2327,10 +2205,9 @@ static int lm_cluster_size(int n_jobs, int max_n) {
     while (csize > 1 && n_jobs * csize > sm_count() * sm_share / 100) csize /= 2;
     return csize;
 }
-template <int KIND>
-static void launch_lm_t(const ProblemDev *probs, const LmJob *jobs, const LoJobSrc *job_src, const double *models_in,
-                        const int *n_jobs_dev, int n_jobs, int n_clusters, int csize, const char *mask_base,
-                        int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
+static void launch_lm_any(int kind, const ProblemDev *probs, const LmJob *jobs, const LoJobSrc *job_src,
+                          const double *models_in, const int *n_jobs_dev, int n_jobs, int n_clusters, int csize,
+                          const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
@@ -2344,19 +2221,10 @@ static void launch_lm_t(const ProblemDev *probs, const LmJob *jobs, const LoJobS
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, k_lm<KIND>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
-                       scratch_stride, out);
-}
-static void launch_lm_any(int kind, const ProblemDev *probs, const LmJob *jobs, const LoJobSrc *job_src,
-                          const double *models_in, const int *n_jobs_dev, int n_jobs, int n_clusters, int csize,
-                          const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
-    switch (kind) {
-    case KIND_PNP: launch_lm_t<KIND_PNP>(probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, n_clusters, csize, mask_base, idx_scratch, scratch_stride, out, stream); break;
-    case KIND_RELPOSE: launch_lm_t<KIND_RELPOSE>(probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, n_clusters, csize, mask_base, idx_scratch, scratch_stride, out, stream); break;
-    case KIND_FUND: launch_lm_t<KIND_FUND>(probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, n_clusters, csize, mask_base, idx_scratch, scratch_stride, out, stream); break;
-    case KIND_RELPOSE_TS: launch_lm_t<KIND_RELPOSE_TS>(probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, n_clusters, csize, mask_base, idx_scratch, scratch_stride, out, stream); break;
-    default: launch_lm_t<KIND_HOMOG>(probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, n_clusters, csize, mask_base, idx_scratch, scratch_stride, out, stream); break;
-    }
+    with_kind(kind, [&](auto K) {
+        cudaLaunchKernelEx(&cfg, k_lm<K>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
+                           scratch_stride, out);
+    });
 }
 void launch_lm(int kind, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in, int n_jobs,
                int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
