@@ -58,10 +58,25 @@ typedef struct plb_ransac_stats {
 
 /* PoseLib/types.h:60-95 BundleOptions (fields read by the four in-scope refiners; NIELSEN + LEVENBERG) */
 enum { PLB_LOSS_TRIVIAL = 0, PLB_LOSS_TRUNCATED = 1, PLB_LOSS_HUBER = 2, PLB_LOSS_CAUCHY = 3 };
+/* refine_intrinsics: BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params (types.h:92-94)
+ * as a bit set.  The camera parameters they select (Camera::get_param_refinement_idx, camera_models.cc:545-561: focal
+ * lengths, then principal point, then the model's extra parameters; none for the NULL camera) are refined with the pose
+ * by plb_bundle_adjust_image and plb_estimate_absolute_pose_image (AbsolutePoseRefiner, optim/absolute.h:40-171).
+ * Where the selection is non-empty the other entry points behave as follows:
+ *   - ignored, as the reference ignores them: plb_bundle_adjust (NULL camera), plb_refine_relpose,
+ *     plb_refine_fundamental, plb_refine_homography, plb_estimate_fundamental, plb_estimate_homography and
+ *     plb_estimate_relative_pose without tangent_sampson;
+ *   - PLB_ERR_NYI (CameraRelativePoseRefiner, bundle.cc:237-256): plb_refine_relpose_cameras, and
+ *     plb_estimate_relative_pose / plb_estimate_batch with tangent_sampson when either camera's selection is non-empty;
+ *   - PLB_ERR_ARG: plb_estimate_absolute_pose, which cannot return the camera (use plb_estimate_absolute_pose_image);
+ *   - plb_estimate_batch refines the camera of PnP problems and writes it into camera1 (camera1 of the other problems
+ *     is left untouched).
+ * All of this is checked before any device call.  Other bits are ignored. */
+enum { PLB_REFINE_FOCAL_LENGTH = 1, PLB_REFINE_PRINCIPAL_POINT = 2, PLB_REFINE_EXTRA_PARAMS = 4 };
 typedef struct plb_bundle_opt {
     uint64_t max_iterations;   /* 100 */
     int32_t loss_type;         /* PLB_LOSS_CAUCHY */
-    int32_t reserved;
+    int32_t refine_intrinsics; /* 0; PLB_REFINE_* bits */
     double loss_scale;         /* 1.0 */
     double gradient_tol;       /* 1e-12 */
     double step_tol;           /* 1e-8 */
@@ -158,6 +173,14 @@ int plb_estimate_absolute_pose(const double *points2D, const double *points3D, s
                                const plb_ransac_opt *ransac, const plb_bundle_opt *bundle, double max_error,
                                const plb_camera *camera, double pose_inout[7], char *inliers,
                                plb_ransac_stats *stats, plb_counters *counters);
+/* estimate_absolute_pose with the Image* of the reference (robust.cc:36-126): like plb_estimate_absolute_pose, and the
+ * final bundle adjustment also refines the camera parameters bundle->refine_intrinsics selects.  camera_inout is always
+ * written back; after a final bundle adjustment (num_inliers > 3) it went through the reference's rescale(scale) /
+ * rescale(1 / scale) round trip, which can change the last bits of parameters that were not refined. */
+int plb_estimate_absolute_pose_image(const double *points2D, const double *points3D, size_t n,
+                                     const plb_ransac_opt *ransac, const plb_bundle_opt *bundle, double max_error,
+                                     plb_camera *camera_inout, double pose_inout[7], char *inliers,
+                                     plb_ransac_stats *stats, plb_counters *counters);
 int plb_estimate_relative_pose(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                                const plb_camera *camera2, const plb_ransac_opt *ransac,
                                const plb_bundle_opt *bundle, double max_error, int tangent_sampson,
@@ -204,6 +227,11 @@ int plb_relpose_8pt_batch(size_t count, size_t n, const double *x1, const double
  * Uniform weights.  bundle_stats_out (may be NULL): {iterations, initial_cost, cost}. ------------------------- */
 int plb_bundle_adjust(const double *x_xy, const double *X_xyz, size_t n, double pose_inout[7],
                       const plb_bundle_opt *opt, double bundle_stats_out[3]);
+/* bundle.h:47 bundle_adjust(x, X, Image*, opt) (bundle.cc:95-112): the pose and the camera parameters opt->refine_intrinsics
+ * selects, points in the camera's pixel units as given (no rescaling).  Only the refined parameters of camera_inout are
+ * written. */
+int plb_bundle_adjust_image(const double *x_px, const double *X_xyz, size_t n, double pose_inout[7],
+                            plb_camera *camera_inout, const plb_bundle_opt *opt, double bundle_stats_out[3]);
 int plb_refine_relpose(const double *x1_xy, const double *x2_xy, size_t n, double pose_inout[7],
                        const plb_bundle_opt *opt, double bundle_stats_out[3]);
 /* bundle.h refine_relpose(x1, x2, ImagePair*, opt) with fixed intrinsics (bundle.cc:237-247): tangent Sampson refiner */

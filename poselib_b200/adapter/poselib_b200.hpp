@@ -54,7 +54,9 @@ template <typename BundleOptions> inline plb_bundle_opt bundle_to_c(const Bundle
     case 3: c.loss_type = PLB_LOSS_CAUCHY; break;
     default: throw std::runtime_error("poselib_b200: NYI loss type (TRUNCATED_CAUCHY / TRUNCATED_LE_ZACH)");
     }
-    c.reserved = 0;
+    c.refine_intrinsics = (o.refine_focal_length ? PLB_REFINE_FOCAL_LENGTH : 0) |
+                          (o.refine_principal_point ? PLB_REFINE_PRINCIPAL_POINT : 0) |
+                          (o.refine_extra_params ? PLB_REFINE_EXTRA_PARAMS : 0);
     c.loss_scale = o.loss_scale;
     c.gradient_tol = o.gradient_tol;
     c.step_tol = o.step_tol;
@@ -62,9 +64,8 @@ template <typename BundleOptions> inline plb_bundle_opt bundle_to_c(const Bundle
     c.initial_lambda = o.initial_lambda;
     c.min_lambda = o.min_lambda;
     c.max_lambda = o.max_lambda;
-    if (static_cast<int>(o.lambda_update) != 0 || static_cast<int>(o.damping) != 0 || o.refine_focal_length ||
-        o.refine_extra_params || o.refine_principal_point)
-        throw std::runtime_error("poselib_b200: NYI bundle option (FIXED_FACTOR / MARQUARDT / intrinsics refinement)");
+    if (static_cast<int>(o.lambda_update) != 0 || static_cast<int>(o.damping) != 0)
+        throw std::runtime_error("poselib_b200: NYI bundle option (FIXED_FACTOR / MARQUARDT)");
     return c;
 }
 template <typename RansacStats> inline RansacStats from_c(const plb_ransac_stats &s) {
@@ -86,6 +87,10 @@ template <typename Camera> inline plb_camera camera_to_c(const Camera &cam) {
     for (int i = 0; i < 8; ++i) c.params[i] = (i < (int)cam.params.size()) ? cam.params[i] : 0.0;
     if (cam.params.empty()) c.model_id = PLB_CAMERA_NULL; // "empty camera assumed to be identity" camera_models.cc:305-307
     return c;
+}
+// plb_camera -> Camera::params (the model id and the size of the parameter vector are the caller's)
+template <typename Camera> inline void camera_from_c(const plb_camera &c, Camera *cam) {
+    for (size_t i = 0; i < cam->params.size() && i < 8; ++i) cam->params[i] = c.params[i];
 }
 template <typename Pose> inline void pose_to(const Pose &p, double out[7]) {
     for (int i = 0; i < 4; ++i) out[i] = p.q(i);
@@ -182,9 +187,10 @@ RansacStats estimate_absolute_pose(const std::vector<P2> &points2D, const std::v
     plb_camera cam = detail::camera_to_c(image->camera);
     plb_ransac_stats st;
     inliers->resize(points2D.size());
-    detail::check(plb_estimate_absolute_pose(detail::raw(points2D), detail::raw(points3D), points2D.size(), &ro, &bo,
-                                             opt.max_error, &cam, m, inliers->data(), &st, nullptr));
+    detail::check(plb_estimate_absolute_pose_image(detail::raw(points2D), detail::raw(points3D), points2D.size(), &ro,
+                                                   &bo, opt.max_error, &cam, m, inliers->data(), &st, nullptr));
     detail::pose_from(m, &image->pose);
+    detail::camera_from_c(cam, &image->camera); // refined / rescaled intrinsics (robust.cc:103-123)
     return detail::from_c<RansacStats>(st);
 }
 // estimate_relative_pose(x1, x2, camera1, camera2, RelativePoseOptions, CameraPose*, inliers*)   robust.h:68-70
@@ -261,6 +267,21 @@ BundleStats bundle_adjust(const std::vector<P2> &x, const std::vector<P3> &X, Po
     plb_bundle_opt bo = detail::bundle_to_c(opt);
     detail::check(plb_bundle_adjust(detail::raw(x), detail::raw(X), x.size(), m, &bo, st));
     detail::pose_from(m, pose);
+    return detail::bundle_from_c<BundleStats>(st);
+}
+// bundle_adjust(x, X, Image*, BundleOptions, weights)   robust/bundle.h:47: the pose and the camera parameters the
+// refine_* flags select, points in the camera's pixel units
+template <typename BundleStats, typename P2, typename P3, typename Image, typename BOpt>
+BundleStats bundle_adjust_image(const std::vector<P2> &x, const std::vector<P3> &X, Image *image, const BOpt &opt,
+                                const std::vector<double> &weights = std::vector<double>()) {
+    detail::no_weights(weights);
+    double m[7], st[3];
+    detail::pose_to(image->pose, m);
+    plb_bundle_opt bo = detail::bundle_to_c(opt);
+    plb_camera cam = detail::camera_to_c(image->camera);
+    detail::check(plb_bundle_adjust_image(detail::raw(x), detail::raw(X), x.size(), m, &cam, &bo, st));
+    detail::pose_from(m, &image->pose);
+    detail::camera_from_c(cam, &image->camera);
     return detail::bundle_from_c<BundleStats>(st);
 }
 // refine_relpose(x1, x2, CameraPose*, BundleOptions, weights)   robust/bundle.h:84-86

@@ -15,7 +15,10 @@
 // reference's headers and links a client written against PoseLib's headers only.
 //
 // Entry points of those headers that are NOT on the path (generalized / hybrid / monodepth / focal-estimating variants,
-// Image- and ImagePair-based refiners with intrinsics refinement) stay with PoseLib's CPU sources.
+// Image- and ImagePair-based refiners) stay with PoseLib's CPU sources.  In particular bundle_adjust(x, X, Image*, ...)
+// is not defined here although the adapter has it (bundle_adjust_image): defining it would also replace PoseLib's CPU body
+// for its callers off the path (the focal-estimating estimators, the recalibrator) and their camera models, which the
+// device lacks.  estimate_absolute_pose below refines the camera through the adapter (refine_* flags of opt.bundle).
 #include "PoseLib/robust.h"
 #include "PoseLib/robust/bundle.h"
 #include "PoseLib/robust/ransac.h"

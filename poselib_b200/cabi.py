@@ -15,6 +15,9 @@ PLB_OK, PLB_ERR_CUDA, PLB_ERR_ARG, PLB_ERR_NYI = 0, -1, -2, -3
 KIND = {"pnp": 0, "relpose": 1, "fundamental": 2, "homography": 3}
 LOSS = {"TRIVIAL": 0, "TRUNCATED": 1, "HUBER": 2, "CAUCHY": 3}
 CAMERA = {"NULL": -1, "SIMPLE_PINHOLE": 0, "PINHOLE": 1, "SIMPLE_RADIAL": 2, "RADIAL": 3, "OPENCV": 4}
+CAMERA_NUM_PARAMS = {-1: 0, 0: 3, 1: 4, 2: 4, 3: 5, 4: 8}
+# BundleOpt.refine_intrinsics bits (refine_focal_length, refine_principal_point, refine_extra_params)
+REFINE_FOCAL_LENGTH, REFINE_PRINCIPAL_POINT, REFINE_EXTRA_PARAMS = 1, 2, 4
 
 
 class PoseLibB200Error(RuntimeError):
@@ -48,17 +51,17 @@ class RansacStats(C.Structure):
 
 class BundleOpt(C.Structure):
     """PoseLib/types.h:60-95"""
-    _fields_ = [("max_iterations", C.c_uint64), ("loss_type", C.c_int32), ("reserved", C.c_int32),
+    _fields_ = [("max_iterations", C.c_uint64), ("loss_type", C.c_int32), ("refine_intrinsics", C.c_int32),
                 ("loss_scale", C.c_double), ("gradient_tol", C.c_double), ("step_tol", C.c_double),
                 ("relative_cost_tol", C.c_double), ("initial_lambda", C.c_double),
                 ("min_lambda", C.c_double), ("max_lambda", C.c_double)]
 
     def __init__(self, max_iterations=100, loss_type="CAUCHY", loss_scale=1.0, gradient_tol=1e-12,
                  step_tol=1e-8, relative_cost_tol=1e-10, initial_lambda=1e-3, min_lambda=1e-10,
-                 max_lambda=1e10):
+                 max_lambda=1e10, refine_intrinsics=0):
         lt = LOSS[loss_type] if isinstance(loss_type, str) else int(loss_type)
-        super().__init__(max_iterations, lt, 0, loss_scale, gradient_tol, step_tol, relative_cost_tol,
-                         initial_lambda, min_lambda, max_lambda)
+        super().__init__(max_iterations, lt, int(refine_intrinsics), loss_scale, gradient_tol, step_tol,
+                         relative_cost_tol, initial_lambda, min_lambda, max_lambda)
 
 
 class Counters(C.Structure):
@@ -97,7 +100,7 @@ EXPORTS = [
     "plb_estimate_absolute_pose", "plb_estimate_relative_pose", "plb_estimate_fundamental",
     "plb_estimate_homography", "plb_p3p_batch", "plb_p3p_lambdatwist_batch", "plb_relpose_5pt_batch", "plb_relpose_5pt_poses_batch",
     "plb_relpose_7pt_batch", "plb_homography_4pt_batch", "plb_essential_matrix_8pt_batch", "plb_relpose_8pt_batch", "plb_ransac_batch", "plb_ransac_batch_multi", "plb_estimate_batch", "plb_bundle_adjust",
-    "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
+    "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
     "plb_resident_free",
 ]
 
@@ -262,6 +265,47 @@ def estimate(kind, a, b, ropt, bopt, max_error, cam1=None, cam2=None, init=None,
                                           C.c_double(max_error), mp, mk, C.byref(st), C.byref(cn))
     _check(rc)
     return {"model": _model_out(kind, m), "inliers": mask[:n], "stats": st.as_dict(), "counters": cn.as_dict()}
+
+
+def _copy_camera(cam):
+    return Camera(cam.model_id, tuple(cam.params), cam.width, cam.height)
+
+
+def _camera_params(cam):
+    return np.array(cam.params[:CAMERA_NUM_PARAMS[cam.model_id]], dtype=np.float64)
+
+
+def estimate_image(x, X, cam, ropt, bopt, max_error, init=None):
+    """estimate_absolute_pose with an Image* (robust.cc:36-126): bopt.refine_intrinsics selects camera parameters that
+    the final bundle adjustment refines with the pose.  Returns dict(model, camera [model's parameters], inliers, stats,
+    counters); `cam` is not modified."""
+    n = len(x)
+    aa, ap = _d(x)
+    ba, bp = _d(X)
+    mask = np.zeros(max(n, 1), dtype=np.int8)
+    st, cn = RansacStats(), Counters()
+    m = _init_model("pnp", init)
+    c = _copy_camera(cam)
+    _check(_lib.plb_estimate_absolute_pose_image(ap, bp, C.c_size_t(n), C.byref(ropt), C.byref(bopt),
+                                                 C.c_double(max_error), C.byref(c), m.ctypes.data_as(_P),
+                                                 mask.ctypes.data_as(C.c_char_p), C.byref(st), C.byref(cn)))
+    return {"model": m, "camera": _camera_params(c), "inliers": mask[:n], "stats": st.as_dict(),
+            "counters": cn.as_dict()}
+
+
+def refine_image(pose, x, X, cam, bopt):
+    """bundle_adjust(x, X, Image*, opt) (robust/bundle.h:47): points in the camera's pixel units, bopt.refine_intrinsics
+    selects the camera parameters refined with the pose.  Returns (pose, camera parameters, [iterations, initial_cost,
+    cost]); `cam` is not modified."""
+    n = len(x)
+    aa, ap = _d(x)
+    ba, bp = _d(X)
+    m = _init_model("pnp", pose)
+    c = _copy_camera(cam)
+    bs = np.zeros(3)
+    _check(_lib.plb_bundle_adjust_image(ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(c), C.byref(bopt),
+                                        bs.ctypes.data_as(_P)))
+    return m, _camera_params(c), bs
 
 
 def refine(kind, model, a, b, bopt):
@@ -484,5 +528,5 @@ def estimate_batch(problems, streams=8, n_gpus=-1):
         kind = p["kind"]
         m = np.array(q.model[:7] if kind in ("pnp", "relpose") else q.model[:9], dtype=np.float64)
         out.append({"model": _model_out(kind, m), "inliers": keep[i][2][:q.n].copy(), "stats": q.stats.as_dict(),
-                    "counters": q.counters.as_dict(), "status": q.status})
+                    "counters": q.counters.as_dict(), "status": q.status, "camera1": _camera_params(q.camera1)})
     return out

@@ -249,6 +249,90 @@ PLB_HD void cam_project_with_jac(const CamDev &c, double X, double Y, double Z, 
     }
 }
 
+constexpr int CAM_MAX_PARAMS = 8;
+
+// jac_params of <Model>::project_with_jac: d(u, v) / d(params), 2 x CAM_MAX_PARAMS row-major (jp[c] row u,
+// jp[CAM_MAX_PARAMS + c] row v); columns past the model's parameter count are left untouched.
+// (camera_models.cc:688-697,737-743,800-816,878-891,939-949,1011-1021,2719-2722)
+PLB_HD void cam_jac_params(const CamDev &c, double X, double Y, double Z, double *jp) {
+    const double *p = c.p;
+    double *j0 = jp, *j1 = jp + CAM_MAX_PARAMS;
+    switch (c.model) {
+    case CAMM_NULL: return;
+    case CAMM_SIMPLE_PINHOLE: {
+        const double inv_z = 1.0 / Z;
+        j0[0] = X * inv_z; j1[0] = Y * inv_z;
+        j0[1] = 1.0; j1[1] = 0.0;
+        j0[2] = 0.0; j1[2] = 1.0;
+        return;
+    }
+    case CAMM_PINHOLE: {
+        const double inv_z = 1.0 / Z;
+        j0[0] = X * inv_z; j1[0] = 0.0;
+        j0[1] = 0.0; j1[1] = Y * inv_z;
+        j0[2] = 1.0; j1[2] = 0.0;
+        j0[3] = 0.0; j1[3] = 1.0;
+        return;
+    }
+    case CAMM_SIMPLE_RADIAL:
+    case CAMM_RADIAL: {
+        const double inv_z = 1.0 / Z;
+        const double px = X * inv_z, py = Y * inv_z;
+        const double r2 = px * px + py * py;
+        const double alpha = c.model == CAMM_RADIAL ? (1.0 + p[3] * r2 + p[4] * r2 * r2) : (1.0 + p[3] * r2);
+        j0[0] = alpha * px; j1[0] = alpha * py;
+        j0[1] = 1.0; j1[1] = 0.0;
+        j0[2] = 0.0; j1[2] = 1.0;
+        j0[3] = p[0] * r2 * px; j1[3] = p[0] * r2 * py;
+        if (c.model == CAMM_RADIAL) {
+            j0[4] = p[0] * r2 * r2 * px;
+            j1[4] = p[0] * r2 * r2 * py;
+        }
+        return;
+    }
+    default: {
+        const double u = X / Z, v = Y / Z;
+        double xd, yd;
+        cam_opencv_distortion(p, u, v, xd, yd);
+        const double uv = u * v, r2 = u * u + v * v;
+        j0[0] = xd; j1[0] = 0.0;
+        j0[1] = 0.0; j1[1] = yd;
+        j0[2] = 1.0; j1[2] = 0.0;
+        j0[3] = 0.0; j1[3] = 1.0;
+        j0[4] = p[0] * (r2 * u); j1[4] = p[1] * (r2 * v);
+        j0[5] = p[0] * (r2 * r2 * u); j1[5] = p[1] * (r2 * r2 * v);
+        j0[6] = p[0] * (2.0 * uv); j1[6] = p[1] * (r2 + 2.0 * (v * v));
+        j0[7] = p[0] * (r2 + 2.0 * (u * u)); j1[7] = p[1] * (2.0 * uv);
+        return;
+    }
+    }
+}
+
+// Refinement flags of BundleOptions as one bit set (refine_focal_length, refine_principal_point, refine_extra_params)
+enum { CAM_REFINE_FOCAL = 1, CAM_REFINE_PP = 2, CAM_REFINE_EXTRA = 4 };
+
+// Camera::get_param_refinement_idx (camera_models.cc:545-561): focal indices, then principal point, then the extra
+// parameters of the model (index tables :708-710,759-761,834-836,911-913,1036-1038,2730-2732).  Returns the count.
+PLB_HD int cam_refine_idx(int model, int flags, int *idx) {
+    int nf = 0, npp = 0, ne = 0; // focal count, principal point at [nf, nf + npp), extras at [nf + npp, + ne)
+    switch (model) {
+    case CAMM_SIMPLE_PINHOLE: nf = 1; npp = 2; ne = 0; break;
+    case CAMM_PINHOLE: nf = 2; npp = 2; ne = 0; break;
+    case CAMM_SIMPLE_RADIAL: nf = 1; npp = 2; ne = 1; break;
+    case CAMM_RADIAL: nf = 1; npp = 2; ne = 2; break;
+    case CAMM_OPENCV: nf = 2; npp = 2; ne = 4; break;
+    default: return 0;
+    }
+    int m = 0;
+    if (flags & CAM_REFINE_FOCAL)
+        for (int i = 0; i < nf; ++i) idx[m++] = i;
+    if (flags & CAM_REFINE_PP)
+        for (int i = 0; i < npp; ++i) idx[m++] = nf + i;
+    if (flags & CAM_REFINE_EXTRA)
+        for (int i = 0; i < ne; ++i) idx[m++] = nf + npp + i;
+    return m;
+}
+
 // default <Model>::unproject_with_jac (camera_models.cc:456-489): bearing d and M = J^T (J J^T)^-1 (3x2 row-major)
 PLB_HD void cam_unproject_with_jac(const CamDev &c, double u, double v, double *d, double *M) {
     cam_unproject(c, u, v, d);

@@ -242,6 +242,12 @@ struct Engine {
     MapBuf<SelHeader> h_hdr;
     MapBuf<ImpRec> h_imp;
     MapBuf<LmJobOut> h_lm_out;
+    // LM jobs with camera-parameter refinement (k_lm_intr)
+    DevBuf<LmIntrJob> ijobs;
+    PinBuf<LmIntrJob> h_ijobs;
+    DevBuf<double> lmi_in;
+    PinBuf<double> h_lmi_in;
+    MapBuf<LmIntrJobOut> h_lmi_out;
     uint64_t launches = 0;
 
     int init() {
@@ -440,6 +446,12 @@ struct FinalPolish { // the post-RANSAC refinement of PoseLib/robust.cc (estimat
     // pnp only: refine in pixel*scale coordinates with the rescaled camera (robust.cc:103-123)
     const double *px_scaled = nullptr; // 2n doubles (AoS) or null
     CamDev cam{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
+    // pnp, Image* form: the camera parameters refine_idx[0..refine_m) are refined with the pose (k_lm_intr), and cam_out
+    // receives the camera after the polish, rescaled back by 1 / scale (robust.cc:103-123)
+    int refine_m = 0;
+    int refine_idx[CAM_MAX_PARAMS] = {0, 0, 0, 0, 0, 0, 0, 0};
+    plb_camera *cam_out = nullptr;
+    double scale = 1.0;
 };
 
 // ---- small host-side 3x3 helpers for the estimate_* wrappers (column-major <-> row-major) ---------------------
@@ -574,6 +586,17 @@ struct LmTask {
     const double *model;
     LmJob job;
 };
+struct LmIntrTask {
+    const double *model;
+    LmIntrJob job;
+};
+static LmIntrJob lm_intr_job(const LmJob &base, int m, const int *idx) {
+    LmIntrJob J;
+    J.base = base;
+    J.m = m;
+    for (int c = 0; c < CAM_MAX_PARAMS; ++c) J.idx[c] = c < m ? idx[c] : 0;
+    return J;
+}
 static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
     LmJob J;
     J.pidx = pidx;
@@ -587,6 +610,20 @@ static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
 static bool profiling() {
     static const bool on = std::getenv("PLB_PROFILE") != nullptr;
     return on;
+}
+
+// The camera after the polish of estimate_absolute_pose: the (refined) parameters of the rescaled camera, rescaled by
+// 1 / scale (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
+static void camera_rescale(CamDev &c, double scale);
+static void polish_camera_out(const FinalPolish &fp, const double *params) {
+    CamDev c = fp.cam;
+    for (int i = 0; i < CAM_MAX_PARAMS; ++i) c.p[i] = params[i];
+    camera_rescale(c, 1.0 / fp.scale);
+    const int np = fp.cam_out->model_id == PLB_CAMERA_SIMPLE_PINHOLE ? 3
+                   : fp.cam_out->model_id == PLB_CAMERA_RADIAL   ? 5
+                   : fp.cam_out->model_id == PLB_CAMERA_OPENCV   ? 8
+                                                                 : 4;
+    for (int i = 0; i < np; ++i) fp.cam_out->params[i] = c.p[i];
 }
 
 // A group of problems of the same kind, run in lock-step rounds: one solve launch, one score launch and one LM launch
@@ -900,6 +937,29 @@ struct Group {
         launch_lm(kind, E.probs.p, E.jobs.p, E.lm_in.p, nj, max_n, E.mask.p, E.subset.p, max_n_pad, E.h_lm_out.d, st);
         E.launches++;
         d2h += sizeof(LmJobOut) * nj;
+        return PLB_OK;
+    }
+    // The same for LM jobs that refine camera parameters too (k_lm_intr, results in E.h_lmi_out[j]).
+    int lmi_batch(const std::vector<LmIntrTask> &batch) {
+        const int nj = (int)batch.size();
+        int rc;
+        if ((rc = E.h_lmi_in.ensure(9 * (size_t)nj)) || (rc = E.h_ijobs.ensure(nj)) || (rc = E.ijobs.ensure(nj)) ||
+            (rc = E.lmi_in.ensure(9 * (size_t)nj)) || (rc = E.h_lmi_out.ensure(nj)) ||
+            (rc = E.subset.ensure((size_t)nj * max_n_pad)))
+            return rc;
+        for (int j = 0; j < nj; ++j) {
+            double *row = E.h_lmi_in.p + 9 * (size_t)j;
+            std::fill(row, row + 9, 0.0);
+            std::copy(batch[j].model, batch[j].model + 7, row);
+            E.h_ijobs.p[j] = batch[j].job;
+            E.h_ijobs.p[j].base.scratch_off = (long long)j * max_n_pad;
+        }
+        PLB_CUDA(cudaMemcpyAsync(E.ijobs.p, E.h_ijobs.p, sizeof(LmIntrJob) * nj, cudaMemcpyHostToDevice, st));
+        PLB_CUDA(cudaMemcpyAsync(E.lmi_in.p, E.h_lmi_in.p, sizeof(double) * 9 * nj, cudaMemcpyHostToDevice, st));
+        h2d += (sizeof(LmIntrJob) + sizeof(double) * 9) * nj;
+        launch_lm_intr(E.probs.p, E.ijobs.p, E.lmi_in.p, nj, max_n, E.mask.p, E.subset.p, max_n_pad, E.h_lmi_out.d, st);
+        E.launches++;
+        d2h += sizeof(LmIntrJobOut) * nj;
         return PLB_OK;
     }
     LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
@@ -1356,24 +1416,41 @@ struct Group {
         // robust.cc:103-123,296-311,573-588,736-751: LM over the inliers with the user's BundleOptions
         std::vector<LmTask> pol;
         std::vector<PState *> pol_of;
+        std::vector<LmIntrTask> ipol; // polish jobs that refine camera parameters too
+        std::vector<PState *> ipol_of;
         for (PState &S : PS) {
             if (S.n == 0 || !S.t->polish.enabled || S.stats.num_inliers <= S.t->polish.min_inliers) continue;
-            LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(S.t->polish.bundle));
+            const FinalPolish &fp = S.t->polish;
+            LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(fp.bundle));
             if (S.polish_pidx >= 0) {
                 J.pidx = S.polish_pidx;
                 J.prm.use_camera = 1;
-                J.prm.cam = S.t->polish.cam;
+                J.prm.cam = fp.cam;
             }
-            pol.push_back({S.best_model, J});
-            pol_of.push_back(&S);
+            if (fp.refine_m > 0) {
+                ipol.push_back({S.best_model, lm_intr_job(J, fp.refine_m, fp.refine_idx)});
+                ipol_of.push_back(&S);
+            } else {
+                pol.push_back({S.best_model, J});
+                pol_of.push_back(&S);
+            }
         }
         if (!pol.empty() && (rc = lm_batch(pol))) return rc;
+        if (!ipol.empty() && (rc = lmi_batch(ipol))) return rc;
         // the masks cross PCIe as bits (1/8 of the bytes) and are expanded into the caller's char[n] below
         launch_pack_mask(E.mask.p, E.mask_bits.p, mask_bytes, st);
         E.launches++;
         PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
         if ((rc = sync())) return rc;
-        for (size_t j = 0; j < pol.size(); ++j) std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
+        for (size_t j = 0; j < pol.size(); ++j) {
+            std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
+            if (pol_of[j]->t->polish.cam_out) polish_camera_out(pol_of[j]->t->polish, pol_of[j]->t->polish.cam.p);
+        }
+        for (size_t j = 0; j < ipol.size(); ++j) {
+            const LmIntrJobOut &o = E.h_lmi_out.p[j];
+            std::copy(o.pose, o.pose + 7, ipol_of[j]->best_model);
+            if (ipol_of[j]->t->polish.cam_out) polish_camera_out(ipol_of[j]->t->polish, o.cam);
+        }
         for (PState &S : PS) {
             if (S.t->inliers && S.n > 0) {
                 const uint32_t *w = E.h_mask_bits.p + (S.mask_off >> 5); // mask_off is a multiple of 32
@@ -1473,9 +1550,12 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 
 // One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
 // group (sq_thr 0, no normalisation, no pre-step beyond the cameras), then one LM job over every point.
+// PnP on an Image (bundle.cc:95-112): `proj` is the camera the points are projected with; its parameters idx[0..m) are
+// refined with the pose (k_lm_intr) and written to proj_out.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cam_a = nullptr,
-                      const CamDev *cam_b = nullptr) {
+                      const CamDev *cam_b = nullptr, const CamDev *proj = nullptr, int m = 0, const int *idx = nullptr,
+                      double *proj_out = nullptr) {
     if (n_pts == 0) return PLB_OK;
     Task t;
     t.kind = kind;
@@ -1490,16 +1570,28 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose())) return rc;
     LmParams prm = bundle_params(bopt);
     prm.subset_mode = 0;
-    lm_set_sm_share(100);
-    if ((rc = G.lm_batch({{model, lm_job(0, -1, prm)}})) || (rc = G.sync())) return rc;
-    PLB_CUDA(cudaGetLastError());
-    const LmJobOut &o = G.E.h_lm_out.p[0];
-    std::copy(o.model, o.model + G.MSZ, model);
-    if (bstats) {
-        bstats[0] = o.iterations;
-        bstats[1] = o.initial_cost;
-        bstats[2] = o.cost;
+    if (proj) {
+        prm.use_camera = proj->model != CAMM_NULL;
+        prm.cam = *proj;
     }
+    lm_set_sm_share(100);
+    const LmJob J = lm_job(0, -1, prm);
+    double st[3];
+    if (m == 0) {
+        if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        const LmJobOut &o = G.E.h_lm_out.p[0];
+        std::copy(o.model, o.model + G.MSZ, model);
+        st[0] = o.iterations, st[1] = o.initial_cost, st[2] = o.cost;
+    } else {
+        if ((rc = G.lmi_batch({{model, lm_intr_job(J, m, idx)}})) || (rc = G.sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        const LmIntrJobOut &o = G.E.h_lmi_out.p[0];
+        std::copy(o.pose, o.pose + 7, model);
+        for (int c = 0; c < m; ++c) proj_out[idx[c]] = o.cam[idx[c]];
+        st[0] = o.iterations, st[1] = o.initial_cost, st[2] = o.cost;
+    }
+    if (bstats) std::copy(st, st + 3, bstats);
     return PLB_OK;
 }
 
@@ -1556,7 +1648,7 @@ void plb_ransac_opt_default(plb_ransac_opt *o) {
 void plb_bundle_opt_default(plb_bundle_opt *o) {
     o->max_iterations = 100;
     o->loss_type = PLB_LOSS_CAUCHY;
-    o->reserved = 0;
+    o->refine_intrinsics = 0;
     o->loss_scale = 1.0;
     o->gradient_tol = 1e-12;
     o->step_tol = 1e-8;
@@ -1741,10 +1833,21 @@ static void default_stats(plb_ransac_stats *stats, plb_counters *counters) {
 // and runs the tangent-Sampson estimator with the cameras), :544-594 (fundamental), :712-757 (homography).
 // The camera pre-step (Camera::unproject / unproject_with_jac of every point) runs on the device, fused into the layout
 // kernel; normalize_points (F / H) runs here on the calling (worker) thread.
+// Camera write-back of estimate_absolute_pose (robust.cc:103-123, Image*): CAM_RET_NONE the caller cannot take the camera
+// (refinement flags -> PLB_ERR_ARG), CAM_RET_ALWAYS the Image* form, CAM_RET_REFINED only when parameters are refined.
+// BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params as a bit set
+static int refine_flags(const plb_bundle_opt *b) { return b->refine_intrinsics & (CAM_REFINE_FOCAL | CAM_REFINE_PP | CAM_REFINE_EXTRA); }
+// Camera::get_param_refinement_idx(opt) is non-empty
+static bool r_nonempty(const CamDev &c, const plb_bundle_opt *b) {
+    int idx[CAM_MAX_PARAMS];
+    return cam_refine_idx(c.model, refine_flags(b), idx) > 0;
+}
+enum { CAM_RET_NONE = 0, CAM_RET_ALWAYS = 1, CAM_RET_REFINED = 2 };
 static int estimate_prepare(int kind, const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                             const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                             double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
-                            plb_ransac_stats *stats, plb_counters *counters, EstimateJob &J) {
+                            plb_ransac_stats *stats, plb_counters *counters, EstimateJob &J,
+                            plb_camera *camera_out = nullptr, int cam_ret = CAM_RET_NONE) {
     if (int r = check_ptrs(x1, x2, ransac, model, n)) return r;
     if (!bundle) {
         g_err = "null bundle options";
@@ -1771,6 +1874,11 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
     if (kind == PLB_KIND_PNP) {
         CamDev cam;
         if (int r = camera_dev(camera1, &cam)) return r;
+        fp.refine_m = cam_refine_idx(cam.model, refine_flags(bundle), fp.refine_idx);
+        if (fp.refine_m > 0 && cam_ret == CAM_RET_NONE) {
+            g_err = "camera refinement flags need a camera to return: use plb_estimate_absolute_pose_image";
+            return PLB_ERR_ARG;
+        }
         const double scale = 1.0 / camera_focal(cam);
         fp.bundle.loss_scale = bundle->loss_scale * scale;
         fp.min_inliers = 3;
@@ -1780,6 +1888,8 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             fp.px_scaled = J.px.data();
             fp.cam = cam;
             camera_rescale(fp.cam, scale);
+            fp.scale = scale;
+            if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && fp.refine_m > 0)) fp.cam_out = camera_out;
         }
         t.kind = KIND_PNP;
         t.max_error = max_error * scale;
@@ -1791,6 +1901,10 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         CamDev c1, c2;
         if (int r = camera_dev(camera1, &c1)) return r;
         if (int r = camera_dev(camera2, &c2)) return r;
+        if (tangent_sampson && (r_nonempty(c1, bundle) || r_nonempty(c2, bundle))) {
+            g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
+            return PLB_ERR_NYI;
+        }
         const double scale = 0.5 * (1.0 / camera_focal(c1) + 1.0 / camera_focal(c2));
         fp.bundle.loss_scale = bundle->loss_scale * scale;
         fp.min_inliers = 5;
@@ -1843,10 +1957,11 @@ static void estimate_finish(EstimateJob &J, const Task &t) {
 static int estimate_single(int kind, const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                            const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                            double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
-                           plb_ransac_stats *stats, plb_counters *counters) {
+                           plb_ransac_stats *stats, plb_counters *counters, plb_camera *camera_out = nullptr,
+                           int cam_ret = CAM_RET_NONE) {
     EstimateJob J;
     if (int r = estimate_prepare(kind, x1, x2, n, camera1, camera2, ransac, bundle, max_error, real_focal_check,
-                                 tangent_sampson, model, inliers, stats, counters, J))
+                                 tangent_sampson, model, inliers, stats, counters, J, camera_out, cam_ret))
         return r;
     if (J.t.skip) return PLB_OK;
     std::vector<Task *> v{&J.t};
@@ -1860,6 +1975,19 @@ int plb_estimate_absolute_pose(const double *points2D, const double *points3D, s
                                double pose[7], char *inliers, plb_ransac_stats *stats, plb_counters *counters) {
     return estimate_single(PLB_KIND_PNP, points2D, points3D, n, camera, nullptr, ransac, bundle, max_error, 0, 0, pose,
                            inliers, stats, counters);
+}
+// robust.cc:36-126 with the Image* of the reference: the camera is read, refined by the final bundle adjustment when
+// bundle->refine_intrinsics selects parameters of its model, and written back.
+int plb_estimate_absolute_pose_image(const double *points2D, const double *points3D, size_t n,
+                                     const plb_ransac_opt *ransac, const plb_bundle_opt *bundle, double max_error,
+                                     plb_camera *camera_inout, double pose[7], char *inliers, plb_ransac_stats *stats,
+                                     plb_counters *counters) {
+    if (!camera_inout) {
+        g_err = "null camera";
+        return PLB_ERR_ARG;
+    }
+    return estimate_single(PLB_KIND_PNP, points2D, points3D, n, camera_inout, nullptr, ransac, bundle, max_error, 0, 0,
+                           pose, inliers, stats, counters, camera_inout, CAM_RET_ALWAYS);
 }
 int plb_estimate_relative_pose(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                                const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
@@ -1908,7 +2036,24 @@ int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, con
     CamDev c1, c2;
     if (int r = camera_dev(camera1, &c1)) return r;
     if (int r = camera_dev(camera2, &c2)) return r;
+    if (r_nonempty(c1, opt) || r_nonempty(c2, opt)) {
+        g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
+        return PLB_ERR_NYI;
+    }
     return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, &c1, &c2);
+}
+// robust/bundle.cc:95-112: AbsolutePoseRefiner on an Image, camera_refine_idx from the flags; points in camera units
+int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
+                            const plb_bundle_opt *opt, double bs[3]) {
+    if (!opt || !pose || !camera_inout || (n > 0 && (!x || !X))) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    CamDev cam;
+    if (int r = camera_dev(camera_inout, &cam)) return r;
+    int idx[CAM_MAX_PARAMS];
+    const int m = cam_refine_idx(cam.model, refine_flags(opt), idx);
+    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, m, idx, camera_inout->params);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {
@@ -2229,7 +2374,7 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
                 plb_estimate_problem &p = problems[i];
                 rcs[i] = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
                                           p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
-                                          &p.counters, jobs[i]);
+                                          &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED);
                 if (rcs[i] != PLB_OK) msgs[i] = g_err;
             }
         };

@@ -1709,6 +1709,23 @@ struct LmShared {
     int flag;
 };
 
+// Cluster totals of the CTA partial sums S->sums[buf][0..nv) -> S->tot[0..nv) in every CTA, CTAs in rank order
+// (the second half of cluster_sum, for partial sums that are already per CTA).
+template <class Shared> PLB_DEV void cluster_total(Shared *S, int nv, int buf, int csize) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cluster = cg::this_cluster();
+    cluster.sync();
+    if ((int)threadIdx.x < nv) {
+        double t = 0.0;
+        for (int r = 0; r < csize; ++r) {
+            const double *remote = cluster.map_shared_rank(&S->sums[buf][0], r);
+            t += remote[threadIdx.x];
+        }
+        S->tot[threadIdx.x] = t;
+    }
+    __syncthreads();
+}
+
 // Cluster-wide deterministic sum of NV per-thread values -> S->tot[0..NV) in every CTA of the cluster.
 // Order: xor-butterfly inside a warp, warps left to right, CTAs in rank order.
 template <int NV> PLB_DEV void cluster_sum(LmShared *S, const double *v, int &buf, int csize) {
@@ -1740,7 +1757,7 @@ template <int NV> PLB_DEV void cluster_sum(LmShared *S, const double *v, int &bu
 }
 
 // thread 0 -> whole CTA broadcast of a small integer (two barriers: the slot can be reused right away)
-PLB_DEV int block_bcast(LmShared *S, int v) {
+template <class Shared> PLB_DEV int block_bcast(Shared *S, int v) {
     if (threadIdx.x == 0) S->flag = v;
     __syncthreads();
     const int r = S->flag;
@@ -2250,6 +2267,365 @@ void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const
     const int nc = lm_round_max_clusters(kind, est_jobs, max_n);
     launch_lm_any(kind, probs, tmpl, job_src, models, n_jobs_dev, job_cap, nc, csize, nullptr, idx_scratch, scratch_stride,
                   out, stream);
+}
+
+// ============================================================================================================
+// LM of the absolute pose together with camera parameters: AbsolutePoseRefiner with a non-empty camera_refine_idx
+// (optim/absolute.h:40-171).  The scalar LM logic is k_lm's; the normal equations are reduced through a shared-memory
+// tile instead of per-thread packed accumulators (105 + 14 doubles per thread would not fit beside the rest).
+// ============================================================================================================
+// Parameters: the pose (6) and m <= CAM_MAX_PARAMS camera parameters, padded to LMI_NP.  The padded rows and columns of
+// JtJ and Jtr are zero, their damped diagonal is lambda and their step component zero, so the Cholesky solve, the step,
+// its norm and the predicted decrease are those of the (6 + m)-dimensional system.
+constexpr int LMI_NP = 6 + CAM_MAX_PARAMS;
+constexpr int LMI_NT = LMI_NP * (LMI_NP + 1) / 2;
+constexpr int LMI_NV = 2 + LMI_NT + LMI_NP + 1; // [loss, residual rows, JtJ (packed lower, row-major), Jtr, jac rows]
+static_assert(LMI_NV <= LM_THREADS, "one owner thread per reduced value");
+// Tile row of one point: Jacobian row u (LMI_NP) | row v (LMI_NP) | w*r_u | w*r_v | w | loss | residual row | jac row
+// | jac_params of the point (2 x CAM_MAX_PARAMS, staging for the column selection)
+enum { LMI_WR0 = 2 * LMI_NP, LMI_WR1, LMI_WT, LMI_LOSS, LMI_ROW, LMI_JROW, LMI_JP, LMI_W = LMI_JP + 2 * CAM_MAX_PARAMS };
+constexpr size_t LMI_TILE_BYTES = sizeof(double) * LMI_W * LM_THREADS;
+
+struct LmIntrShared {
+    double par[9], par_new[9];
+    double cam[CAM_MAX_PARAMS], cam_new[CAM_MAX_PARAMS];
+    double ctx[12];
+    double JtJ[LMI_NP * LMI_NP], Am[LMI_NP * LMI_NP];
+    double Jtr[LMI_NP], rhs[LMI_NP], sol[LMI_NP];
+    double sums[2][LMI_NV]; // CTA partial sums, double-buffered: read by the other CTAs of the cluster (DSMEM)
+    double tot[LMI_NV];     // cluster totals (identical in every CTA)
+    int wcount[LM_WARPS];
+    int flag;
+};
+
+// Points of this CTA's slice [lo, hi) whose mask byte is set, in point order -> mylist (the subset mode 2 of k_lm);
+// returns their number.
+PLB_DEV int lmi_mask_list(const char *mask_in, int lo, int hi, int *mylist, LmIntrShared *S) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int base = 0;
+    for (int t0 = lo; t0 < hi; t0 += (int)blockDim.x) {
+        const int k = t0 + threadIdx.x;
+        const bool keep = k < hi && mask_in[k] != 0;
+        const unsigned bal = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) S->wcount[warp] = __popc(bal);
+        __syncthreads();
+        int off = base;
+        for (int w = 0; w < warp; ++w) off += S->wcount[w];
+        int tile = 0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tile += S->wcount[w];
+        if (keep) mylist[off + __popc(bal & ((1u << lane) - 1u))] = k;
+        base += tile;
+        __syncthreads();
+    }
+    return base;
+}
+
+// One evaluation pass at the pose whose context is in S->ctx and the camera parameters cp: robust cost and residual
+// rows (compute_residual, <Model>::project) and JtJ, Jtr, jacobian rows (compute_jacobian, <Model>::project_with_jac
+// with jac_params) -> S->tot, in lm_eval_pass's layout.  Every 256 points each thread writes its point's row of the tile;
+// thread e < LMI_NV then adds value e of every row in point order.  Order of the sums: points in order inside a CTA, CTAs
+// in rank order (deterministic for a given cluster size).
+PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, int model, const double *cp, int m, const int *idx,
+                           const int *list, int lo, int na, LmIntrShared *S, double *tile, int &buf, int csize) {
+    const double *ctx = S->ctx;
+    CamDev cam;
+    cam.model = model;
+    cam.reserved = 0;
+#pragma unroll
+    for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam.p[c] = cp[c];
+    // the value this thread owns: kind 0 column sum of column a, 1 JtJ(a, b), 2 Jtr(a), -1 none (or a padded entry)
+    const int e = threadIdx.x, np = 6 + m;
+    int kind = -1, a = 0, b = 0;
+    if (e == 0) {
+        kind = 0; a = LMI_LOSS;
+    } else if (e == 1) {
+        kind = 0; a = LMI_ROW;
+    } else if (e < 2 + LMI_NT) {
+        const int t = e - 2;
+        while ((a + 1) * (a + 2) / 2 <= t) ++a;
+        b = t - a * (a + 1) / 2;
+        if (a < np) kind = 1;
+    } else if (e < 2 + LMI_NT + LMI_NP) {
+        a = e - 2 - LMI_NT;
+        if (a < np) kind = 2;
+    } else if (e == LMI_NV - 1) {
+        kind = 0; a = LMI_JROW;
+    }
+    double acc = 0.0;
+    for (int t0 = 0; t0 < na; t0 += (int)blockDim.x) {
+        const int i = t0 + threadIdx.x;
+        double *tr = tile + (size_t)threadIdx.x * LMI_W;
+        bool filled = false;
+        if (i < na) {
+            const int k = list ? list[i] : lo + i;
+            const double X0 = P.p[2][k], X1 = P.p[3][k], X2 = P.p[4][k];
+            const double Z0 = ctx[0] * X0 + ctx[1] * X1 + ctx[2] * X2 + ctx[9];
+            const double Z1 = ctx[3] * X0 + ctx[4] * X1 + ctx[5] * X2 + ctx[10];
+            const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
+            if (!(Z2 < 0)) { // optim/absolute.h:57-58,93-94
+                double xr0, xr1, zp0, zp1, Jp[2][3];
+                cam_project(cam, Z0, Z1, Z2, xr0, xr1);
+                cam_project_with_jac(cam, Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
+                const double x0 = P.p[0][k], x1 = P.p[1][k];
+                const double q0 = xr0 - x0, q1 = xr1 - x1;
+                tr[LMI_LOSS] = L.loss(q0 * q0 + q1 * q1);
+                tr[LMI_ROW] = 1.0;
+                const double r0 = zp0 - x0, r1 = zp1 - x1;
+                const double w = L.weight(r0 * r0 + r1 * r1);
+                if (w != 0) { // jacobian_accumulator.h:87-104
+                    filled = true;
+                    tr[LMI_JROW] = 1.0;
+                    tr[LMI_WT] = w;
+                    tr[LMI_WR0] = w * r0;
+                    tr[LMI_WR1] = w * r1;
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        double dZ[3];
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) dZ[c] = Jp[q][0] * ctx[c] + Jp[q][1] * ctx[3 + c] + Jp[q][2] * ctx[6 + c];
+                        double *Jr = tr + q * LMI_NP;
+                        Jr[0] = -X2 * dZ[1] + X1 * dZ[2];
+                        Jr[1] = X2 * dZ[0] - X0 * dZ[2];
+                        Jr[2] = -X1 * dZ[0] + X0 * dZ[1];
+                        Jr[3] = dZ[0]; Jr[4] = dZ[1]; Jr[5] = dZ[2];
+                    }
+                    // J.col(6 + c) = J_params.col(camera_refine_idx[c]); jac_params is staged in the row's tail
+                    cam_jac_params(cam, Z0, Z1, Z2, tr + LMI_JP);
+#pragma unroll
+                    for (int c = 0; c < LMI_NP - 6; ++c) {
+                        tr[6 + c] = c < m ? tr[LMI_JP + idx[c]] : 0.0;
+                        tr[LMI_NP + 6 + c] = c < m ? tr[LMI_JP + CAM_MAX_PARAMS + idx[c]] : 0.0;
+                    }
+                } else {
+                    tr[LMI_JROW] = 0.0;
+                }
+            } else {
+                tr[LMI_LOSS] = 0.0;
+                tr[LMI_ROW] = 0.0;
+                tr[LMI_JROW] = 0.0;
+            }
+        } else {
+            tr[LMI_LOSS] = 0.0;
+            tr[LMI_ROW] = 0.0;
+            tr[LMI_JROW] = 0.0;
+        }
+        if (!filled) { // no Jacobian contribution: a zero row (reference: add_jacobian returns early)
+            for (int c = 0; c < 2 * LMI_NP; ++c) tr[c] = 0.0;
+            tr[LMI_WT] = 0.0;
+            tr[LMI_WR0] = 0.0;
+            tr[LMI_WR1] = 0.0;
+        }
+        __syncthreads();
+        const int rows = min_i((int)blockDim.x, na - t0);
+        if (kind == 0) {
+            for (int r = 0; r < rows; ++r) acc += tile[r * LMI_W + a];
+        } else if (kind == 1) {
+            for (int r = 0; r < rows; ++r) {
+                const double *q = tile + r * LMI_W;
+                acc += q[LMI_WT] * (q[a] * q[b] + q[LMI_NP + a] * q[LMI_NP + b]);
+            }
+        } else if (kind == 2) {
+            for (int r = 0; r < rows; ++r) {
+                const double *q = tile + r * LMI_W;
+                acc += q[a] * q[LMI_WR0] + q[LMI_NP + a] * q[LMI_WR1];
+            }
+        }
+        __syncthreads();
+    }
+    if (e < LMI_NV) S->sums[buf][e] = acc;
+    cluster_total(S, LMI_NV, buf, csize);
+    buf ^= 1;
+}
+
+// llt_solve with the size at run time and the factor written over A (shared memory), in llt_solve's operation order:
+// unrolled at compile time, a 14 x 14 factor in registers would crowd out the evaluation pass (spills).
+PLB_DEV void llt_solve_n(double *A, const double *rhs, double *x, int n) {
+    for (int j = 0; j < n; ++j) {
+        double d = A[j * n + j];
+        for (int k = 0; k < j; ++k) d -= A[j * n + k] * A[j * n + k];
+        const double ljj = sqrt(d);
+        A[j * n + j] = ljj;
+        for (int i = j + 1; i < n; ++i) {
+            double s = A[i * n + j];
+            for (int k = 0; k < j; ++k) s -= A[i * n + k] * A[j * n + k];
+            A[i * n + j] = s / ljj;
+        }
+    }
+    for (int i = 0; i < n; ++i) {
+        double s = rhs[i];
+        for (int k = 0; k < i; ++k) s -= A[i * n + k] * x[k];
+        x[i] = s / A[i * n + i];
+    }
+    for (int i = n - 1; i >= 0; --i) {
+        double s = x[i];
+        for (int k = i + 1; k < n; ++k) s -= A[k * n + i] * x[k];
+        x[i] = s / A[i * n + i];
+    }
+}
+
+// One thread-block cluster per job, as k_lm (the LM scalar logic of optim/lm_impl.h:56-140 runs redundantly in every
+// CTA on identical cluster totals).  Output: refined pose and camera parameters.
+__global__ void __launch_bounds__(LM_THREADS, 1)
+    k_lm_intr(const ProblemDev *__restrict__ probs, const LmIntrJob *__restrict__ jobs, const double *__restrict__ models_in,
+              int n_jobs, const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *outs) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cluster = cg::this_cluster();
+    __shared__ LmIntrShared S;
+    extern __shared__ double lmi_tile[];
+    const int csize = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
+    const int n_clusters = (int)gridDim.x / csize, cluster_id = (int)blockIdx.x / csize;
+    int buf = 0;
+    for (int job = cluster_id; job < n_jobs; job += n_clusters) {
+    const LmIntrJob &JI = jobs[job];
+    const ProblemDev P = probs[JI.base.pidx];
+    const LmParams prm = JI.base.prm;
+    const int m = JI.m, model = prm.cam.model;
+    int idx[CAM_MAX_PARAMS];
+#pragma unroll
+    for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[c] = JI.idx[c];
+    const char *mask_in = (JI.base.mask_off >= 0) ? mask_base + JI.base.mask_off : nullptr;
+    const double *min = models_in + (size_t)job * 9;
+    LmIntrJobOut *out = outs + job;
+    LossFn L;
+    L.type = prm.loss_type;
+    L.thr = prm.loss_scale;
+    L.sq_thr = prm.loss_scale * prm.loss_scale;
+    L.inv_sq_thr = 1.0 / L.sq_thr;
+
+    const int chunk = (((P.n + csize - 1) / csize) + 31) & ~31;
+    const int lo = min_i(crank * chunk, P.n), hi = min_i(lo + chunk, P.n);
+    int na = hi - lo;
+    const int *list = nullptr;
+    if (prm.subset_mode != 0) {
+        int *mylist = idx_scratch + (size_t)cluster_id * (size_t)scratch_stride + lo;
+        na = lmi_mask_list(mask_in, lo, hi, mylist, &S);
+        list = mylist;
+    }
+    if (threadIdx.x == 0) {
+        for (int k = 0; k < 7; ++k) S.par[k] = min[k];
+        for (int k = 7; k < 9; ++k) S.par[k] = 0.0;
+        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = prm.cam.p[c];
+        lm_build_ctx<KIND_PNP>(S.par, S.ctx, nullptr, true);
+    }
+    __syncthreads();
+
+    int iterations = 0;
+    double cost = 0.0, initial_cost = 0.0;
+    // scalar LM state (thread 0 of every CTA); rc mirrors NormalAccumulator::residual_count
+    double lambda = prm.initial_lambda, nu = 2.0, rc = 0.0;
+    bool recompute_jac = true;
+    lmi_eval_pass(P, L, model, S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+    if (threadIdx.x == 0) {
+        cost = S.tot[0] * (1.0 / fmax(1.0, S.tot[1]));
+        initial_cost = cost;
+        int t = 0;
+        for (int i = 0; i < LMI_NP; ++i)
+            for (int j = 0; j <= i; ++j) S.JtJ[i * LMI_NP + j] = S.tot[2 + t++];
+        for (int i = 0; i < LMI_NP; ++i) S.Jtr[i] = S.tot[2 + LMI_NT + i];
+        rc = S.tot[2 + LMI_NT + LMI_NP];
+    }
+    for (int it = 0; it < prm.max_iterations; ++it) {
+        iterations = it;
+        int stop = 0;
+        if (threadIdx.x == 0) {
+            if (recompute_jac) {
+                double g = 0.0;
+                for (int i = 0; i < LMI_NP; ++i) g += S.Jtr[i] * S.Jtr[i];
+                const double grad_norm = (1.0 / fmax(1.0, rc)) * sqrt(g);
+                if (grad_norm < prm.gradient_tol) stop = 1;
+            }
+            if (!stop) {
+                const double scale = 1.0 / fmax(1.0, rc);
+                for (int i = 0; i < LMI_NP; ++i)
+                    for (int j = 0; j <= i; ++j) S.Am[i * LMI_NP + j] = scale * S.JtJ[i * LMI_NP + j];
+                for (int i = 0; i < LMI_NP; ++i) S.Am[i * LMI_NP + i] += lambda;
+                for (int i = 0; i < LMI_NP; ++i) S.rhs[i] = -(scale * S.Jtr[i]);
+                llt_solve_n(S.Am, S.rhs, S.sol, LMI_NP);
+                double sn = 0.0;
+                for (int i = 0; i < LMI_NP; ++i) sn += S.sol[i] * S.sol[i];
+                if (sqrt(sn) < prm.step_tol) stop = 1;
+            }
+            if (!stop) { // AbsolutePoseRefiner::step (optim/absolute.h:146-160)
+                lm_step<KIND_PNP>(S.par, S.sol, nullptr, S.par_new);
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam_new[c] = S.cam[c];
+                for (int c = 0; c < m; ++c) S.cam_new[idx[c]] += S.sol[6 + c];
+                lm_build_ctx<KIND_PNP>(S.par_new, S.ctx, nullptr, true);
+            }
+        }
+        if (block_bcast(&S, stop)) break;
+        lmi_eval_pass(P, L, model, S.cam_new, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+        int brk = 0;
+        if (threadIdx.x == 0) {
+            rc = S.tot[1];
+            const double cost_new = S.tot[0] * (1.0 / fmax(1.0, rc));
+            if (cost_new < cost) {
+                const double cost_decrease = cost - cost_new;
+                for (int k = 0; k < 9; ++k) S.par[k] = S.par_new[k];
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = S.cam_new[c];
+                cost = cost_new;
+                recompute_jac = true;
+                const double scale = 1.0 / fmax(1.0, rc);
+                double pred = 0.0;
+                for (int i = 0; i < LMI_NP; ++i) pred += S.sol[i] * (lambda * S.sol[i] + scale * S.Jtr[i]);
+                pred = -pred;
+                if (pred > 0) {
+                    const double rho = cost_decrease / pred;
+                    const double factor = 1.0 - pow(2.0 * rho - 1.0, 3.0);
+                    lambda *= fmax(1.0 / 3.0, factor);
+                } else {
+                    lambda *= 1.0 / 3.0;
+                }
+                nu = 2.0;
+                lambda = fmax(prm.min_lambda, lambda);
+                if (cost > 0 && cost_decrease / cost < prm.relative_cost_tol) brk = 1;
+                // the Jacobian pass the reference would run next at the accepted parameters
+                int t = 0;
+                for (int i = 0; i < LMI_NP; ++i)
+                    for (int j = 0; j <= i; ++j) S.JtJ[i * LMI_NP + j] = S.tot[2 + t++];
+                for (int i = 0; i < LMI_NP; ++i) S.Jtr[i] = S.tot[2 + LMI_NT + i];
+                if (!brk && it + 1 < prm.max_iterations) rc = S.tot[2 + LMI_NT + LMI_NP];
+            } else {
+                recompute_jac = false;
+                lambda *= nu;
+                nu *= 2.0;
+                lambda = fmin(prm.max_lambda, lambda);
+            }
+            if (it + 1 >= prm.max_iterations && !brk) iterations = it + 1;
+        }
+        if (block_bcast(&S, brk)) break;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && crank == 0) {
+        for (int k = 0; k < 7; ++k) out->pose[k] = S.par[k];
+        for (int c = 0; c < CAM_MAX_PARAMS; ++c) out->cam[c] = S.cam[c];
+        out->iterations = iterations;
+        out->reserved = 0;
+        out->cost = cost;
+        out->initial_cost = initial_cost;
+    }
+    cluster.sync(); // no CTA may exit (or start the next job) while a sibling can still read its shared memory
+    } // jobs of this cluster
+}
+
+void launch_lm_intr(const ProblemDev *probs, const LmIntrJob *jobs_dev, const double *models_in, int n_jobs, int max_n,
+                    const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *out, cudaStream_t stream) {
+    if (n_jobs <= 0) return;
+    cudaFuncSetAttribute(k_lm_intr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LMI_TILE_BYTES);
+    const int csize = lm_cluster_size(n_jobs, max_n);
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)(n_jobs * csize), 1, 1);
+    cfg.blockDim = dim3((unsigned)LM_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = LMI_TILE_BYTES;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)csize;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, k_lm_intr, probs, jobs_dev, models_in, n_jobs, mask_base, idx_scratch, scratch_stride, out);
 }
 
 // ============================================================================================================

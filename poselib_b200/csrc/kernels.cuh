@@ -179,6 +179,20 @@ struct LmJobOut {
     int iterations;
     double cost, initial_cost;
 };
+// LM job of AbsolutePoseRefiner with camera parameters (optim/absolute.h:40-171): the pose (models_in, 7 of 9 doubles)
+// and the parameters idx[0..m) of base.prm.cam are refined together; base.prm.use_camera and score_after are not read.
+struct LmIntrJob {
+    LmJob base;
+    int m;                    // 1..CAM_MAX_PARAMS
+    int idx[CAM_MAX_PARAMS];  // Camera::get_param_refinement_idx (cam_refine_idx)
+};
+struct LmIntrJobOut {
+    double pose[7];
+    double cam[CAM_MAX_PARAMS];
+    int iterations;
+    int reserved;
+    double initial_cost, cost;
+};
 // Pre-step of one problem: caller layout (AoS doubles, device copies) -> resident SoA arrays.
 //   mode 0: plain transposition (points already calibrated / normalised)
 //   mode 1: Camera::unproject to 2D of a (cam_a) and, for 2D-2D kinds, of b (cam_b)   (robust.cc:40-43,287-292)
@@ -230,6 +244,10 @@ void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const
                      const double *models, const int *n_jobs_dev, int job_cap, int est_jobs, int max_n,
                      int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream);
 int lm_round_max_clusters(int kind, int est_jobs, int max_n);
+// PnP LM with camera-parameter refinement: one thread-block cluster per job, models_in n_jobs * 9 doubles, idx_scratch
+// n_jobs * scratch_stride ints (subset mode 2).
+void launch_lm_intr(const ProblemDev *probs, const LmIntrJob *jobs_dev, const double *models_in, int n_jobs, int max_n,
+                    const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *out, cudaStream_t stream);
 // Share of the SMs (percent) the LO clusters launched from this host thread may cover (50: batch groups, 100: a lone call).
 void lm_set_sm_share(int pct);
 // Device-side sampling of a round: one warp per active problem draws its B samples into samples[(g0+s)*K ..] from
