@@ -12,6 +12,7 @@
 // There is no CPU compute path: without a CUDA device every compute entry point fails with PLB_ERR_CUDA.
 #include "../../include/poselib_b200.h"
 #include "kernels.cuh"
+#include "screen_math.cuh"
 
 #include <sched.h>
 
@@ -211,7 +212,7 @@ struct Engine {
     DevBuf<int> n_models, first_slot, prefix, cand_slot, cand_sample, n_cand, n_models_tot;
     DevBuf<uint32_t> counts, fcounts, fborder;
     DevBuf<double> scores;
-    DevBuf<float> fscores, ferr;
+    DevBuf<float> fscores, ferr, fctx;
     DevBuf<LmJob> lo_tmpl;
     DevBuf<LoJobSrc> job_src;
     PinBuf<SamplerDev> h_smp;
@@ -1220,7 +1221,8 @@ struct Group {
         out.model_prob = E.model_prob.p;
         if (mode == 1) {
             if ((rc = E.fcounts.ensure(cap_models)) || (rc = E.fscores.ensure(cap_models)) ||
-                (rc = E.fborder.ensure(cap_models)) || (rc = E.ferr.ensure(cap_models)))
+                (rc = E.fborder.ensure(cap_models)) || (rc = E.ferr.ensure(cap_models)) ||
+                (rc = E.fctx.ensure(cap_models * scr::CTX_FLOATS)))
                 return rc;
             out.fcounts = E.fcounts.p;
             out.fscores = E.fscores.p;
@@ -1242,9 +1244,10 @@ struct Group {
         launch_sample(E.rp.p, na, E.smp.p + (size_t)smp_cur * NP, E.smp.p + (size_t)(smp_cur ^ 1) * NP, E.samples.p, st);
         E.launches++;
         mark(PH_SAMPLE);
-        launch_hypotheses(kind, R, out, mode, max_n_pad, st, E.ev2);
+        launch_hypotheses(kind, R, out, mode, max_n_pad, E.fctx.p, st, E.ev2);
         PLB_CUDA(cudaEventRecord(E.ev1, st));
-        E.launches += kind_is_relpose(kind) ? 5 : 2; // one solve kernel (5pt: k5_gather, k5_prep_lane, k5_roots, k5_back) + scoring
+        // one solve kernel (5pt: k5_gather, k5_prep_lane, k5_roots, k5_back) + scoring (fast mode: k_screen_ctx + k_screen)
+        E.launches += (kind_is_relpose(kind) ? 5 : 2) + (mode == 1 && kind != KIND_RELPOSE_TS ? 1 : 0);
         SelectArgs SA;
         SA.rp = E.rp.p;
         SA.na = na;

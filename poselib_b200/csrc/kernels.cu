@@ -816,6 +816,41 @@ constexpr int SCR_THREADS = 512;
 constexpr int SCR_WARPS = SCR_THREADS / 32;
 constexpr int SCR_TM = 8;
 constexpr int SCR_RQ_TAKE = 8; // cases a lane may queue per pass of the warp-compacted handling
+constexpr int SCR_PB = 4;      // correspondences per thread and step of the streaming pass
+constexpr int SCR_CTX_THREADS = 128;
+
+// The fp32 screening constants of every model of the round (scr::CTX_FLOATS floats per model slot, fctx), one
+// thread per model: the fp32 model from model_ctx and the per-model constants of the error bounds (screen_math.cuh),
+// from the fp64 model and the problem's coordinate maxima.  Entries a kind does not use are 0.
+template <int KIND>
+__global__ void __launch_bounds__(SCR_CTX_THREADS) k_screen_ctx(const RoundDesc R, const HypOut out, float *__restrict__ fctx) {
+    constexpr int MSZ = kind_model_size(KIND);
+    constexpr int CTX = kind_ctx_size(KIND);
+    constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
+    const int a = blockIdx.y;
+    const int m = blockIdx.x * SCR_CTX_THREADS + threadIdx.x;
+    if (m >= out.prob_count[a]) return;
+    const ProblemDev &P = R.probs[R.active[a]];
+    const size_t slot = (size_t)out.seg_base[a] + m;
+    double mdl[MSZ];
+#pragma unroll
+    for (int k = 0; k < MSZ; ++k) mdl[k] = out.models[slot * MSZ + k];
+    double cp[CTX];
+    model_ctx<KIND>(mdl, cp);
+    float c[scr::CTX_FLOATS];
+#pragma unroll
+    for (int k = 0; k < scr::CTX_FLOATS; ++k) c[k] = k < CTX ? (float)cp[k] : 0.f;
+    float cm[5];
+#pragma unroll
+    for (int j = 0; j < NARR; ++j) cm[j] = P.cmax[j];
+    if (KIND == KIND_PNP) scr::transfer_setup<3>(cp, cm + 2, cm, P.sq_thr, c);
+    else if (KIND == KIND_HOMOG) scr::transfer_setup<2>(cp, cm, cm + 2, P.sq_thr, c);
+    else scr::sampson_setup(cp, cm, P.sq_thr, c);
+    if constexpr (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, c);
+    float4 *dst = reinterpret_cast<float4 *>(fctx + slot * scr::CTX_FLOATS);
+#pragma unroll
+    for (int k = 0; k < scr::CTX_FLOATS / 4; ++k) dst[k] = make_float4(c[4 * k], c[4 * k + 1], c[4 * k + 2], c[4 * k + 3]);
+}
 
 PLB_DEV uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 PLB_DEV void mbar_init(uint64_t *bar, int count) {
@@ -831,6 +866,10 @@ PLB_DEV void tma_bulk_g2s(void *dst_smem, const void *src_gmem, uint32_t bytes, 
                  "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+PLB_DEV void cp_async16(void *dst_smem, const void *src_gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
+}
+PLB_DEV void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 PLB_DEV void mbar_wait(uint64_t *bar, uint32_t phase) {
     asm volatile("{\n"
                  ".reg .pred P1;\n"
@@ -860,22 +899,35 @@ PLB_DEV float warp_sum_f(float v) {
     return v;
 }
 
+// Padded length of one staged array: the streaming pass then runs whole steps of SCR_PB correspondences per thread.
+template <int NTHR> constexpr __host__ __device__ int scr_stage_len(int n) {
+    return (n + SCR_PB * NTHR - 1) / (SCR_PB * NTHR) * (SCR_PB * NTHR);
+}
+
 // NTHR: threads per CTA.  512 (one CTA per SM next to a 160 KB staging buffer) for the large problems the kernel was
 // shaped for; 128 (four CTAs per SM) for small ones (BASELINE config 1: 200 correspondences), where a 512-thread CTA
-// leaves most threads without a correspondence and the per-tile setup / reduction is what costs.
+// leaves most threads without a correspondence.
+//
+// The pipeline of one CTA over its tiles of SCR_TM models, with one barrier per tile:
+//   * the model constants come ready-made from fctx (k_screen_ctx); tile t+1's are copied (cp.async) into the other
+//     half of the double-buffered ctx[] while tile t streams, and waited for just before the tile's barrier;
+//   * the warps' partial records of tile t go to one half of the double-buffered red_* / s_border; the cross-warp sums
+//     and the record writes of tile t are done by threads 0..SCR_TM-1 at the start of tile t+1 (the last tile of a
+//     problem right after its barrier), always in warp order, so the records do not depend on timing;
+//   * on the shared-memory path the staged arrays are padded with NaN to whole streaming steps (scr_stage_len), so there
+//     is no remainder pass; the global-memory path runs one guarded step for the last < SCR_PB correspondences.
 template <int KIND, int NTHR>
-__global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const RoundDesc R, HypOut out, int use_smem) {
+__global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const RoundDesc R, HypOut out, const float *__restrict__ fctx, int use_smem) {
     constexpr int SCR_THREADS = NTHR, SCR_WARPS = NTHR / 32; // shadow the file-scope defaults
-    constexpr int MSZ = kind_model_size(KIND);
-    constexpr int CTX = kind_ctx_size(KIND);
     constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
+    constexpr int CTX_V4 = scr::CTX_FLOATS / 4;
     extern __shared__ __align__(128) unsigned char scr_smem[];
     __shared__ __align__(8) uint64_t bar;
-    __shared__ __align__(16) float ctx[SCR_TM][scr::CTX_FLOATS];
-    __shared__ float red_s[SCR_WARPS][SCR_TM];
-    __shared__ float red_e[SCR_WARPS][SCR_TM];
-    __shared__ uint32_t red_c[SCR_WARPS][SCR_TM];
-    __shared__ uint32_t s_border[SCR_TM];
+    __shared__ __align__(16) float ctx[2][SCR_TM][scr::CTX_FLOATS];
+    __shared__ float red_s[2][SCR_WARPS][SCR_TM];
+    __shared__ float red_e[2][SCR_WARPS][SCR_TM];
+    __shared__ uint32_t red_c[2][SCR_WARPS][SCR_TM];
+    __shared__ uint32_t s_border[2][SCR_TM];
     __shared__ uint16_t rq[SCR_WARPS][32 * SCR_RQ_TAKE]; // per-warp queue of recorded cases: lane << 8 | bit << 3 | model
     // ---- static, cost-balanced partition of the round's (problem, tile) list over the CTAs of the grid ------------
     // cost of a tile = correspondences of its problem; CTA c owns the tiles whose start cost lies in
@@ -956,6 +1008,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
         s_Sa = s_first_pre;
         if (use_smem) mbar_init(&bar, 1);
     }
+    if (tid < 2 * SCR_TM) s_border[tid / SCR_TM][tid % SCR_TM] = 0u; // then reset by each tile's record writer
     __syncthreads();
     uint32_t phase = 0;
     for (int a = s_first; a <= s_last; ++a) {
@@ -974,46 +1027,75 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     if (t_begin >= t_end) continue;
     const float thr = (float)P.sq_thr;
     const int seg = out.seg_base[a];
+    // copy the constants of the tile of models starting at m0f (cp.async, 16 B per thread; waited for before the
+    // barrier that precedes their first use)
+    auto fetch_ctx = [&](int b, int m0f) {
+        const int tmf = (count - m0f < SCR_TM) ? (count - m0f) : SCR_TM;
+        if (tid < tmf * CTX_V4) cp_async16(&ctx[b][0][0] + 4 * tid, fctx + (size_t)(seg + m0f) * scr::CTX_FLOATS + 4 * tid);
+    };
+    // cross-warp sums of the tile of models starting at m0f (partials in half b), by thread tid < that tile's size
+    auto write_record = [&](int b, int m0f) {
+        uint32_t ct = 0;
+        float st = 0.f, et = 0.f;
+#pragma unroll
+        for (int w = 0; w < SCR_WARPS; ++w) {
+            ct += red_c[b][w][tid];
+            st += red_s[b][w][tid];
+            et += red_e[b][w][tid];
+        }
+        st += (float)n * thr; // the per-correspondence sums hold (r2 - thr) of the inliers only
+        // + the rounding of the fp32 sums themselves: at most n/SCR_THREADS + 24 additions deep over terms of
+        //   magnitude <= thr each (ct of them), and the final n * thr product and addition.  The padding below adds no
+        //   term (a padded correspondence is never recorded), and the correspondence -> (lane, bit) mapping and the
+        //   queue order are those of a pass over the n correspondences alone, so the depth is unchanged.
+        const float depth = (float)(n / SCR_THREADS + 24);
+        et = et * (1.f + 1e-5f) + scr::U * thr * (depth * (float)ct + 2.2f * (float)n);
+        out.fcounts[seg + m0f + tid] = ct;
+        out.fscores[seg + m0f + tid] = st;
+        out.fborder[seg + m0f + tid] = s_border[b][tid];
+        out.ferr[seg + m0f + tid] = et * (1.f + 1e-5f);
+        s_border[b][tid] = 0u;
+    };
+    fetch_ctx(0, t_begin * SCR_TM);
     const float *arr[NARR];
+    int n_str = n; // correspondences the streaming pass runs over (padded on the shared-memory path)
     if (use_smem) {
         float *pts = reinterpret_cast<float *>(scr_smem);
+        const int n_st = scr_stage_len<NTHR>(n);
         __syncthreads(); // every thread is done with the previous problem's arrays
         if (tid == 0) {
             const uint32_t bytes = (uint32_t)n_pad * 4u;
             mbar_expect_tx(&bar, bytes * NARR);
 #pragma unroll
-            for (int c = 0; c < NARR; ++c) tma_bulk_g2s(pts + (size_t)c * n_pad, P.f[c], bytes, &bar);
+            for (int c = 0; c < NARR; ++c) tma_bulk_g2s(pts + (size_t)c * n_st, P.f[c], bytes, &bar);
         }
         mbar_wait(&bar, phase);
         phase ^= 1u;
+        // NaN padding of [n, n_st) of every array, written after this thread saw the bulk copies complete and made
+        // visible to all by the barrier below.  A padded correspondence is never recorded: every test of the streaming
+        // pass is an ordered comparison, false when an operand is NaN, and NaN coordinates make every operand NaN
+        //   relpose, fundamental: C, D and so g are NaN  ->  sampson_maybe's  g <= thr' D  is false;
+        //   homography: w is NaN  ->  z = fma(thr_s', |w|, c') is NaN  ->  transfer_maybe's  z > 0  is false;
+        //   pnp: the depth z2 is NaN  ->  z is NaN  ->  z > 0  is false.
+        // This holds whatever the model constants are, infinite ones included.
+        for (int i = n + tid; i < n_st; i += SCR_THREADS)
 #pragma unroll
-        for (int c = 0; c < NARR; ++c) arr[c] = pts + (size_t)c * n_pad;
+            for (int c = 0; c < NARR; ++c) pts[(size_t)c * n_st + i] = __int_as_float(0x7fc00000);
+#pragma unroll
+        for (int c = 0; c < NARR; ++c) arr[c] = pts + (size_t)c * n_st;
+        n_str = n_st;
     } else {
 #pragma unroll
         for (int c = 0; c < NARR; ++c) arr[c] = P.f[c];
     }
-    for (int m0 = t_begin * SCR_TM; m0 < t_end * SCR_TM; m0 += SCR_TM) {
+    cp_async_wait_all();
+    __syncthreads();
+    int b = 0;
+    for (int m0 = t_begin * SCR_TM; m0 < t_end * SCR_TM; m0 += SCR_TM, b ^= 1) {
         const int tm = (count - m0 < SCR_TM) ? (count - m0) : SCR_TM;
-        __syncthreads();
-        if (tid < SCR_TM) s_border[tid] = 0u;
-        if (tid < tm) {
-            double mdl[MSZ];
-#pragma unroll
-            for (int k = 0; k < MSZ; ++k) mdl[k] = out.models[(size_t)(seg + m0 + tid) * MSZ + k];
-            double cp[CTX];
-            model_ctx<KIND>(mdl, cp);
-#pragma unroll
-            for (int k = 0; k < CTX; ++k) ctx[tid][k] = (float)cp[k];
-            // per-model constants of the error bounds (screen_math.cuh), from the fp64 model and the problem's maxima
-            float cm[5];
-#pragma unroll
-            for (int c = 0; c < NARR; ++c) cm[c] = P.cmax[c];
-            if (KIND == KIND_PNP) scr::transfer_setup<3>(cp, cm + 2, cm, P.sq_thr, ctx[tid]);
-            else if (KIND == KIND_HOMOG) scr::transfer_setup<2>(cp, cm, cm + 2, P.sq_thr, ctx[tid]);
-            else scr::sampson_setup(cp, cm, P.sq_thr, ctx[tid]);
-            if constexpr (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, ctx[tid]);
-        }
-        __syncthreads();
+        if (m0 + SCR_TM < t_end * SCR_TM) fetch_ctx(b ^ 1, m0 + SCR_TM);
+        if (m0 > t_begin * SCR_TM && tid < SCR_TM) write_record(b ^ 1, m0 - SCR_TM); // only a problem's last tile is partial
+        const float(*cx)[scr::CTX_FLOATS] = ctx[b];
         uint32_t cnt[SCR_TM];
         float sc[SCR_TM], er[SCR_TM];
 #pragma unroll
@@ -1031,52 +1113,44 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             // decision, is it provably the fp64 decision, cheirality, division, accumulation of score and error bound)
             // are handled afterwards in a compacted loop in which every lane pops one of ITS recorded cases per
             // iteration — handled inline they cost a divergent detour for the whole warp whenever one lane of 32 hits.
-            constexpr int SCR_PB = 4;
             auto maybe = [&](const float *M, const float *p) -> bool {
                 if (KIND == KIND_PNP) return scr::transfer_maybe<true>(M, scr::pnp_terms(M, p[0], p[1], p[2], p[3], p[4]));
                 if (KIND == KIND_HOMOG) return scr::transfer_maybe<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]));
                 return scr::sampson_maybe(M, p[0], p[1], p[2], p[3]);
             };
-            for (int base = 0; base < n; base += 32 * SCR_THREADS) {
-                const int lim = min_i(n, base + 32 * SCR_THREADS);
+            for (int base = 0; base < n_str; base += 32 * SCR_THREADS) {
+                const int lim = min_i(n_str, base + 32 * SCR_THREADS);
                 uint32_t hit[SCR_TM];
 #pragma unroll
                 for (int i = 0; i < SCR_TM; ++i) hit[i] = 0u;
                 int k0 = base + tid;
                 uint32_t qbit = 1u;
-                for (; k0 + (SCR_PB - 1) * SCR_THREADS < lim; k0 += SCR_THREADS * SCR_PB, qbit <<= SCR_PB) {
+                // GUARDED: correspondences at or past lim read as NaN (never recorded, see the padding above)
+                auto step = [&](auto guarded) {
                     float p[SCR_PB][NARR];
 #pragma unroll
                     for (int j = 0; j < SCR_PB; ++j) {
                         const int k = k0 + j * SCR_THREADS;
 #pragma unroll
-                        for (int c = 0; c < NARR; ++c) p[j][c] = arr[c][k];
+                        for (int c = 0; c < NARR; ++c) p[j][c] = (!decltype(guarded)::value || k < lim) ? arr[c][k] : __int_as_float(0x7fc00000);
                     }
 #pragma unroll
                     for (int i = 0; i < SCR_TM; ++i) {
                         if (i < tm) {
                             float Mr[20]; // [0..11] model, [16..19] constants of the streaming test
-                            lds_v4(ctx[i], Mr);
-                            lds_v4(ctx[i] + 4, Mr + 4);
-                            lds_v4(ctx[i] + 8, Mr + 8);
-                            lds_v4(ctx[i] + 16, Mr + 16);
+                            lds_v4(cx[i], Mr);
+                            lds_v4(cx[i] + 4, Mr + 4);
+                            lds_v4(cx[i] + 8, Mr + 8);
+                            lds_v4(cx[i] + 16, Mr + 16);
 #pragma unroll
                             for (int j = 0; j < SCR_PB; ++j)
                                 if (maybe(Mr, p[j])) hit[i] |= qbit << j;
                         }
                     }
-                }
-                for (; k0 < lim; k0 += SCR_THREADS, qbit <<= 1) { // remainder
-                    float p[NARR];
-#pragma unroll
-                    for (int c = 0; c < NARR; ++c) p[c] = arr[c][k0];
-#pragma unroll
-                    for (int i = 0; i < SCR_TM; ++i) {
-                        if (i < tm) {
-                            if (maybe(ctx[i], p)) hit[i] |= qbit;
-                        }
-                    }
-                }
+                };
+                for (; k0 + (SCR_PB - 1) * SCR_THREADS < lim; k0 += SCR_THREADS * SCR_PB, qbit <<= SCR_PB)
+                    step(std::false_type{});
+                if (!use_smem && k0 < lim) step(std::true_type{}); // the last < SCR_PB correspondences of this lane
                 // Handling of the recorded cases, compacted across the WARP: the lanes list their cases (model, bit, lane)
                 // in a per-warp queue in shared memory — at most SCR_RQ_TAKE per lane and pass, so the queue cannot
                 // overflow — and the warp then works through the queue 32 entries at a time.  A case is evaluated by
@@ -1121,7 +1195,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                         float p[NARR];
 #pragma unroll
                         for (int c = 0; c < NARR; ++c) p[c] = arr[c][k];
-                        const float *M = ctx[mi];
+                        const float *M = cx[mi];
                         bool plain = false, border = false;
                         float v = 0.f, e = 0.f;
                         if (KIND == KIND_PNP) {
@@ -1142,7 +1216,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                                 plain = plain && ok;
                             }
                         }
-                        if (border) atomicAdd(&s_border[mi], 1u);
+                        if (border) atomicAdd(&s_border[b][mi], 1u);
                         if (plain || border) {
 #pragma unroll
                             for (int i = 0; i < SCR_TM; ++i)
@@ -1165,32 +1239,17 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             const float v = warp_sum_f(sc[i]);
             const float ev = warp_sum_f(er[i]);
             if (lane == 0) {
-                red_c[warp][i] = c;
-                red_s[warp][i] = v;
-                red_e[warp][i] = ev;
+                red_c[b][warp][i] = c;
+                red_s[b][warp][i] = v;
+                red_e[b][warp][i] = ev;
             }
         }
+        cp_async_wait_all(); // the next tile's constants
         __syncthreads();
-        if (tid < tm) {
-            uint32_t ct = 0;
-            float st = 0.f, et = 0.f;
-#pragma unroll
-            for (int w = 0; w < SCR_WARPS; ++w) {
-                ct += red_c[w][tid];
-                st += red_s[w][tid];
-                et += red_e[w][tid];
-            }
-            st += (float)n * thr; // the per-correspondence sums hold (r2 - thr) of the inliers only
-            // + the rounding of the fp32 sums themselves: at most n/SCR_THREADS + 24 additions deep over terms of
-            //   magnitude <= thr each (ct of them), and the final n * thr product and addition
-            const float depth = (float)(n / SCR_THREADS + 24);
-            et = et * (1.f + 1e-5f) + scr::U * thr * (depth * (float)ct + 2.2f * (float)n);
-            out.fcounts[seg + m0 + tid] = ct;
-            out.fscores[seg + m0 + tid] = st;
-            out.fborder[seg + m0 + tid] = s_border[tid];
-            out.ferr[seg + m0 + tid] = et * (1.f + 1e-5f);
-        }
     }
+    // the problem's last tile (the next problem starts with a barrier before any of its tiles writes red_* / s_border)
+    const int m_last = (t_end - 1) * SCR_TM;
+    if (tid < ((count - m_last < SCR_TM) ? (count - m_last) : SCR_TM)) write_record(b ^ 1, m_last);
     } // problems of this CTA
 }
 
@@ -1256,7 +1315,7 @@ static void launch_5pt_prep_roots(const RoundDesc &R, const HypOut &out, cudaStr
 }
 
 template <int KIND>
-static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
+static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, float *fctx, cudaStream_t stream,
                          cudaEvent_t ev_between) {
     if constexpr (KIND == KIND_RELPOSE_TS) mode = 0; // no fp32 screening copy of the 18-array layout: exact scoring
     if constexpr (kind_is_relpose(KIND)) {
@@ -1283,13 +1342,17 @@ static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int ma
         if (gx < 1) gx = 1;
         k_score_tiled<KIND><<<dim3(gx, R.n_active, 1), SCORE_THREADS, 0, stream>>>(R, out);
     } else if constexpr (KIND != KIND_RELPOSE_TS) {
-        // fp32 screening: one CTA holds one problem's fp32 arrays in shared memory (TMA) and strides over its tiles
+        // fp32 screening: the constants of every model once, then one CTA holds one problem's fp32 arrays in shared
+        // memory (TMA) and strides over its tiles
+        k_screen_ctx<KIND><<<dim3((out.max_seg_cap + SCR_CTX_THREADS - 1) / SCR_CTX_THREADS, R.n_active, 1),
+                             SCR_CTX_THREADS, 0, stream>>>(R, out, fctx);
         constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
-        const size_t bytes = (size_t)NARR * (size_t)max_n_pad * 4;
+        const bool small = max_n_pad <= 2048; // few correspondences per problem: 128-thread CTAs, four per SM
+        const size_t bytes =
+            (size_t)NARR * (size_t)(small ? scr_stage_len<128>(max_n_pad) : scr_stage_len<512>(max_n_pad)) * 4;
         const int use_smem = bytes <= 200 * 1024 ? 1 : 0;
         static bool attr_done_dev[MAX_DEVICES] = {false};
         bool &attr_done = attr_done_dev[cur_dev()];
-        const bool small = max_n_pad <= 2048; // few correspondences per problem: 128-thread CTAs, four per SM
         auto kern = small ? k_screen<KIND, 128> : k_screen<KIND, 512>;
         const int nthr = small ? 128 : 512;
         if (!attr_done) {
@@ -1305,13 +1368,13 @@ static void launch_hyp_t(const RoundDesc &R, const HypOut &out, int mode, int ma
         int gx = per_sm * sm_count();
         if ((long long)gx > tiles) gx = (int)tiles;
         if (gx < 1) gx = 1;
-        kern<<<gx, nthr, use_smem ? bytes : 0, stream>>>(R, out, use_smem);
+        kern<<<gx, nthr, use_smem ? bytes : 0, stream>>>(R, out, fctx, use_smem);
     }
 }
-void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
-                       cudaEvent_t ev_between) {
+void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, float *fctx,
+                       cudaStream_t stream, cudaEvent_t ev_between) {
     cudaMemsetAsync(out.prob_count, 0, sizeof(int) * R.n_active, stream);
-    with_kind(kind, [&](auto K) { launch_hyp_t<K>(R, out, mode, max_n_pad, stream, ev_between); });
+    with_kind(kind, [&](auto K) { launch_hyp_t<K>(R, out, mode, max_n_pad, fctx, stream, ev_between); });
 }
 void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, const double *models, cudaStream_t stream) {
     if (A.na <= 0) return;

@@ -228,9 +228,10 @@ void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream
 void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream);
 // Solve + score kernels of one round (kind = kind of every problem of the group); *out.overflow must be zeroed.
 // mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (the candidates k_select lists are
-// rescored exactly by launch_confirm).
-void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, cudaStream_t stream,
-                       cudaEvent_t ev_between = nullptr);
+// rescored exactly by launch_confirm).  fctx (mode 1): scratch of scr::CTX_FLOATS floats per model slot for the
+// screening constants of the round's models.
+void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, float *fctx,
+                       cudaStream_t stream, cudaEvent_t ev_between = nullptr);
 // Exact fp64 scoring of an explicit list of n_models models (stride MSZ) with problem indices.
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
                          uint32_t *counts, double *scores, cudaStream_t stream);
