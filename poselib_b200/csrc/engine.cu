@@ -243,12 +243,7 @@ struct Engine {
     MapBuf<SelHeader> h_hdr;
     MapBuf<ImpRec> h_imp;
     MapBuf<LmJobOut> h_lm_out;
-    // LM jobs with camera-parameter refinement (k_lm_intr)
-    DevBuf<LmIntrJob> ijobs;
-    PinBuf<LmIntrJob> h_ijobs;
-    DevBuf<double> lmi_in;
-    PinBuf<double> h_lmi_in;
-    MapBuf<LmIntrJobOut> h_lmi_out;
+    MapBuf<double> h_cam_out; // CAM_MAX_PARAMS per LM job: the camera of a job that refines it
     uint64_t launches = 0;
 
     int init() {
@@ -447,10 +442,9 @@ struct FinalPolish { // the post-RANSAC refinement of PoseLib/robust.cc (estimat
     // pnp only: refine in pixel*scale coordinates with the rescaled camera (robust.cc:103-123)
     const double *px_scaled = nullptr; // 2n doubles (AoS) or null
     CamDev cam{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
-    // pnp, Image* form: the camera parameters refine_idx[0..refine_m) are refined with the pose (k_lm_intr), and cam_out
+    // pnp, Image* form: CAM_REFINE_* flags of the camera parameters refined with the pose (LmJob::cam_refine), and cam_out
     // receives the camera after the polish, rescaled back by 1 / scale (robust.cc:103-123)
-    int refine_m = 0;
-    int refine_idx[CAM_MAX_PARAMS] = {0, 0, 0, 0, 0, 0, 0, 0};
+    int cam_refine = 0;
     plb_camera *cam_out = nullptr;
     double scale = 1.0;
 };
@@ -587,21 +581,16 @@ struct LmTask {
     const double *model;
     LmJob job;
 };
-struct LmIntrTask {
-    const double *model;
-    LmIntrJob job;
-};
-static LmIntrJob lm_intr_job(const LmJob &base, int m, const int *idx) {
-    LmIntrJob J;
-    J.base = base;
-    J.m = m;
-    for (int c = 0; c < CAM_MAX_PARAMS; ++c) J.idx[c] = c < m ? idx[c] : 0;
-    return J;
+// Camera::get_param_refinement_idx of the camera and the refinement flags is non-empty
+static bool refines_camera(const CamDev &c, int flags) {
+    int idx[CAM_MAX_PARAMS];
+    return cam_refine_idx(c.model, flags, idx) > 0;
 }
+static bool refines_camera(const LmJob &J) { return refines_camera(J.prm.cam, J.cam_refine); }
 static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
     LmJob J;
     J.pidx = pidx;
-    J.reserved = 0;
+    J.cam_refine = 0;
     J.mask_off = mask_off;
     J.scratch_off = 0;
     J.prm = prm;
@@ -916,14 +905,18 @@ struct Group {
         return PLB_OK;
     }
 
-    // Stages a batch of LM jobs (job j: start model batch[j].model, results in E.h_lm_out[j]) and launches them in one
-    // k_lm launch.  The caller synchronises.
+    // Stages a batch of LM jobs (job j: start model batch[j].model, results in E.h_lm_out[j]) and launches one k_lm per
+    // refiner: the jobs that refine the camera come last and write it to row j of E.h_cam_out.  The caller synchronises.
     int lm_batch(const std::vector<LmTask> &batch) {
         const int nj = (int)batch.size();
+        const int n_fixed = (int)(std::partition_point(batch.begin(), batch.end(),
+                                                       [](const LmTask &t) { return !refines_camera(t.job); }) -
+                                  batch.begin());
         int rc;
         if ((rc = E.h_lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_jobs.ensure(nj)) || (rc = E.jobs.ensure(nj)) ||
             (rc = E.lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_lm_out.ensure(nj)) ||
-            (rc = E.subset.ensure((size_t)nj * max_n_pad)))
+            (rc = E.subset.ensure((size_t)nj * max_n_pad)) ||
+            (n_fixed < nj && (rc = E.h_cam_out.ensure((size_t)nj * CAM_MAX_PARAMS))))
             return rc;
         for (int j = 0; j < nj; ++j) {
             double *row = E.h_lm_in.p + 9 * (size_t)j;
@@ -935,32 +928,14 @@ struct Group {
         PLB_CUDA(cudaMemcpyAsync(E.jobs.p, E.h_jobs.p, sizeof(LmJob) * nj, cudaMemcpyHostToDevice, st));
         PLB_CUDA(cudaMemcpyAsync(E.lm_in.p, E.h_lm_in.p, sizeof(double) * 9 * nj, cudaMemcpyHostToDevice, st));
         h2d += (sizeof(LmJob) + sizeof(double) * 9) * nj;
-        launch_lm(kind, E.probs.p, E.jobs.p, E.lm_in.p, nj, max_n, E.mask.p, E.subset.p, max_n_pad, E.h_lm_out.d, st);
-        E.launches++;
-        d2h += sizeof(LmJobOut) * nj;
-        return PLB_OK;
-    }
-    // The same for LM jobs that refine camera parameters too (k_lm_intr, results in E.h_lmi_out[j]).
-    int lmi_batch(const std::vector<LmIntrTask> &batch) {
-        const int nj = (int)batch.size();
-        int rc;
-        if ((rc = E.h_lmi_in.ensure(9 * (size_t)nj)) || (rc = E.h_ijobs.ensure(nj)) || (rc = E.ijobs.ensure(nj)) ||
-            (rc = E.lmi_in.ensure(9 * (size_t)nj)) || (rc = E.h_lmi_out.ensure(nj)) ||
-            (rc = E.subset.ensure((size_t)nj * max_n_pad)))
-            return rc;
-        for (int j = 0; j < nj; ++j) {
-            double *row = E.h_lmi_in.p + 9 * (size_t)j;
-            std::fill(row, row + 9, 0.0);
-            std::copy(batch[j].model, batch[j].model + 7, row);
-            E.h_ijobs.p[j] = batch[j].job;
-            E.h_ijobs.p[j].base.scratch_off = (long long)j * max_n_pad;
+        for (int cam = 0; cam < 2; ++cam) {
+            const int j0 = cam ? n_fixed : 0, n = cam ? nj - n_fixed : n_fixed;
+            if (n == 0) continue;
+            launch_lm(kind, cam, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
+                      max_n_pad, E.h_lm_out.d + j0, cam ? E.h_cam_out.d + (size_t)j0 * CAM_MAX_PARAMS : nullptr, st);
+            E.launches++;
         }
-        PLB_CUDA(cudaMemcpyAsync(E.ijobs.p, E.h_ijobs.p, sizeof(LmIntrJob) * nj, cudaMemcpyHostToDevice, st));
-        PLB_CUDA(cudaMemcpyAsync(E.lmi_in.p, E.h_lmi_in.p, sizeof(double) * 9 * nj, cudaMemcpyHostToDevice, st));
-        h2d += (sizeof(LmIntrJob) + sizeof(double) * 9) * nj;
-        launch_lm_intr(E.probs.p, E.ijobs.p, E.lmi_in.p, nj, max_n, E.mask.p, E.subset.p, max_n_pad, E.h_lmi_out.d, st);
-        E.launches++;
-        d2h += sizeof(LmIntrJobOut) * nj;
+        d2h += sizeof(LmJobOut) * nj + sizeof(double) * CAM_MAX_PARAMS * (nj - n_fixed);
         return PLB_OK;
     }
     LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
@@ -1419,40 +1394,32 @@ struct Group {
         // robust.cc:103-123,296-311,573-588,736-751: LM over the inliers with the user's BundleOptions
         std::vector<LmTask> pol;
         std::vector<PState *> pol_of;
-        std::vector<LmIntrTask> ipol; // polish jobs that refine camera parameters too
-        std::vector<PState *> ipol_of;
-        for (PState &S : PS) {
-            if (S.n == 0 || !S.t->polish.enabled || S.stats.num_inliers <= S.t->polish.min_inliers) continue;
-            const FinalPolish &fp = S.t->polish;
-            LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(fp.bundle));
-            if (S.polish_pidx >= 0) {
-                J.pidx = S.polish_pidx;
-                J.prm.use_camera = 1;
-                J.prm.cam = fp.cam;
-            }
-            if (fp.refine_m > 0) {
-                ipol.push_back({S.best_model, lm_intr_job(J, fp.refine_m, fp.refine_idx)});
-                ipol_of.push_back(&S);
-            } else {
+        for (int cam = 0; cam < 2; ++cam) // the jobs that refine the camera last (lm_batch)
+            for (PState &S : PS) {
+                if (S.n == 0 || !S.t->polish.enabled || S.stats.num_inliers <= S.t->polish.min_inliers) continue;
+                const FinalPolish &fp = S.t->polish;
+                LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(fp.bundle));
+                if (S.polish_pidx >= 0) {
+                    J.pidx = S.polish_pidx;
+                    J.prm.use_camera = 1;
+                    J.prm.cam = fp.cam;
+                }
+                J.cam_refine = fp.cam_refine;
+                if (refines_camera(J) != (cam == 1)) continue;
                 pol.push_back({S.best_model, J});
                 pol_of.push_back(&S);
             }
-        }
         if (!pol.empty() && (rc = lm_batch(pol))) return rc;
-        if (!ipol.empty() && (rc = lmi_batch(ipol))) return rc;
         // the masks cross PCIe as bits (1/8 of the bytes) and are expanded into the caller's char[n] below
         launch_pack_mask(E.mask.p, E.mask_bits.p, mask_bytes, st);
         E.launches++;
         PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
         if ((rc = sync())) return rc;
         for (size_t j = 0; j < pol.size(); ++j) {
+            const FinalPolish &fp = pol_of[j]->t->polish;
             std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
-            if (pol_of[j]->t->polish.cam_out) polish_camera_out(pol_of[j]->t->polish, pol_of[j]->t->polish.cam.p);
-        }
-        for (size_t j = 0; j < ipol.size(); ++j) {
-            const LmIntrJobOut &o = E.h_lmi_out.p[j];
-            std::copy(o.pose, o.pose + 7, ipol_of[j]->best_model);
-            if (ipol_of[j]->t->polish.cam_out) polish_camera_out(ipol_of[j]->t->polish, o.cam);
+            if (fp.cam_out)
+                polish_camera_out(fp, refines_camera(pol[j].job) ? E.h_cam_out.p + j * CAM_MAX_PARAMS : fp.cam.p);
         }
         for (PState &S : PS) {
             if (S.t->inliers && S.n > 0) {
@@ -1553,11 +1520,11 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 
 // One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
 // group (sq_thr 0, no normalisation, no pre-step beyond the cameras), then one LM job over every point.
-// PnP on an Image (bundle.cc:95-112): `proj` is the camera the points are projected with; its parameters idx[0..m) are
-// refined with the pose (k_lm_intr) and written to proj_out.
+// PnP on an Image (bundle.cc:95-112): `proj` is the camera the points are projected with; the parameters the flags
+// cam_refine select are refined with the pose and written to proj_out.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cam_a = nullptr,
-                      const CamDev *cam_b = nullptr, const CamDev *proj = nullptr, int m = 0, const int *idx = nullptr,
+                      const CamDev *cam_b = nullptr, const CamDev *proj = nullptr, int cam_refine = 0,
                       double *proj_out = nullptr) {
     if (n_pts == 0) return PLB_OK;
     Task t;
@@ -1578,23 +1545,20 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
         prm.cam = *proj;
     }
     lm_set_sm_share(100);
-    const LmJob J = lm_job(0, -1, prm);
-    double st[3];
-    if (m == 0) {
-        if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
-        PLB_CUDA(cudaGetLastError());
-        const LmJobOut &o = G.E.h_lm_out.p[0];
-        std::copy(o.model, o.model + G.MSZ, model);
-        st[0] = o.iterations, st[1] = o.initial_cost, st[2] = o.cost;
-    } else {
-        if ((rc = G.lmi_batch({{model, lm_intr_job(J, m, idx)}})) || (rc = G.sync())) return rc;
-        PLB_CUDA(cudaGetLastError());
-        const LmIntrJobOut &o = G.E.h_lmi_out.p[0];
-        std::copy(o.pose, o.pose + 7, model);
-        for (int c = 0; c < m; ++c) proj_out[idx[c]] = o.cam[idx[c]];
-        st[0] = o.iterations, st[1] = o.initial_cost, st[2] = o.cost;
+    LmJob J = lm_job(0, -1, prm);
+    J.cam_refine = cam_refine;
+    if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
+    PLB_CUDA(cudaGetLastError());
+    const LmJobOut &o = G.E.h_lm_out.p[0];
+    std::copy(o.model, o.model + G.MSZ, model);
+    int idx[CAM_MAX_PARAMS];
+    const int m = cam_refine_idx(prm.cam.model, cam_refine, idx);
+    for (int c = 0; c < m; ++c) proj_out[idx[c]] = G.E.h_cam_out.p[idx[c]];
+    if (bstats) {
+        bstats[0] = o.iterations;
+        bstats[1] = o.initial_cost;
+        bstats[2] = o.cost;
     }
-    if (bstats) std::copy(st, st + 3, bstats);
     return PLB_OK;
 }
 
@@ -1840,11 +1804,6 @@ static void default_stats(plb_ransac_stats *stats, plb_counters *counters) {
 // (refinement flags -> PLB_ERR_ARG), CAM_RET_ALWAYS the Image* form, CAM_RET_REFINED only when parameters are refined.
 // BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params as a bit set
 static int refine_flags(const plb_bundle_opt *b) { return b->refine_intrinsics & (CAM_REFINE_FOCAL | CAM_REFINE_PP | CAM_REFINE_EXTRA); }
-// Camera::get_param_refinement_idx(opt) is non-empty
-static bool r_nonempty(const CamDev &c, const plb_bundle_opt *b) {
-    int idx[CAM_MAX_PARAMS];
-    return cam_refine_idx(c.model, refine_flags(b), idx) > 0;
-}
 enum { CAM_RET_NONE = 0, CAM_RET_ALWAYS = 1, CAM_RET_REFINED = 2 };
 static int estimate_prepare(int kind, const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                             const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
@@ -1877,8 +1836,9 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
     if (kind == PLB_KIND_PNP) {
         CamDev cam;
         if (int r = camera_dev(camera1, &cam)) return r;
-        fp.refine_m = cam_refine_idx(cam.model, refine_flags(bundle), fp.refine_idx);
-        if (fp.refine_m > 0 && cam_ret == CAM_RET_NONE) {
+        fp.cam_refine = refine_flags(bundle);
+        const bool refined = refines_camera(cam, fp.cam_refine);
+        if (refined && cam_ret == CAM_RET_NONE) {
             g_err = "camera refinement flags need a camera to return: use plb_estimate_absolute_pose_image";
             return PLB_ERR_ARG;
         }
@@ -1892,7 +1852,7 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             fp.cam = cam;
             camera_rescale(fp.cam, scale);
             fp.scale = scale;
-            if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && fp.refine_m > 0)) fp.cam_out = camera_out;
+            if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && refined)) fp.cam_out = camera_out;
         }
         t.kind = KIND_PNP;
         t.max_error = max_error * scale;
@@ -1904,7 +1864,7 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         CamDev c1, c2;
         if (int r = camera_dev(camera1, &c1)) return r;
         if (int r = camera_dev(camera2, &c2)) return r;
-        if (tangent_sampson && (r_nonempty(c1, bundle) || r_nonempty(c2, bundle))) {
+        if (tangent_sampson && (refines_camera(c1, refine_flags(bundle)) || refines_camera(c2, refine_flags(bundle)))) {
             g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
             return PLB_ERR_NYI;
         }
@@ -2039,7 +1999,7 @@ int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, con
     CamDev c1, c2;
     if (int r = camera_dev(camera1, &c1)) return r;
     if (int r = camera_dev(camera2, &c2)) return r;
-    if (r_nonempty(c1, opt) || r_nonempty(c2, opt)) {
+    if (refines_camera(c1, refine_flags(opt)) || refines_camera(c2, refine_flags(opt))) {
         g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
         return PLB_ERR_NYI;
     }
@@ -2054,9 +2014,7 @@ int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double p
     }
     CamDev cam;
     if (int r = camera_dev(camera_inout, &cam)) return r;
-    int idx[CAM_MAX_PARAMS];
-    const int m = cam_refine_idx(cam.model, refine_flags(opt), idx);
-    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, m, idx, camera_inout->params);
+    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, refine_flags(opt), camera_inout->params);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {

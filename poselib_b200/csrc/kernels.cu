@@ -7,8 +7,8 @@
 //                      MSAC scoring of every model of a round over all correspondences (exact fp64 / fp32 screening)
 //   k_score            exact scoring of explicit models (initial models)
 //   k_confirm          exact rescoring of the fast-mode candidates of a round
-//   k_lm<KIND>         Levenberg-Marquardt refit (LO step + final polish): one CTA per job, block-wide reductions of
-//                      the normal equations, scalar LM logic on thread 0
+//   k_lm<KIND, CAM>    Levenberg-Marquardt refit (LO step + final polish): one cluster per job, cluster-wide reductions
+//                      of the normal equations, scalar LM logic on thread 0; CAM refines PnP camera parameters too
 //   k_inlier_mask      final inlier masks
 //   Every exact score (k_score_tiled, k_score, k_confirm, the rescoring in k_lm) comes from one routine, msac_score,
 //   and every fp64 inlier decision (those, k_inlier_mask, the LO subset in k_lm) from one test per kind, under_thr
@@ -1760,21 +1760,47 @@ template <int NP> struct JacAcc {
     }
 };
 
-struct LmShared {
+// The refiner with camera parameters (AbsolutePoseRefiner with a non-empty camera_refine_idx, optim/absolute.h:40-171):
+// the pose (6) and m <= CAM_MAX_PARAMS camera parameters, padded to LMI_NP.  The padded rows and columns of JtJ and Jtr
+// are zero, their damped diagonal is lambda and their step component zero, so the Cholesky solve, the step, its norm
+// and the predicted decrease are those of the (6 + m)-dimensional system.
+constexpr int LMI_NP = 6 + CAM_MAX_PARAMS;
+constexpr int LMI_NT = LMI_NP * (LMI_NP + 1) / 2;
+constexpr int LMI_NV = 2 + LMI_NT + LMI_NP + 1; // [loss, residual rows, JtJ (packed lower, row-major), Jtr, jac rows]
+static_assert(LMI_NV <= LM_THREADS, "one owner thread per reduced value");
+// Tile row of one point: Jacobian row u (LMI_NP) | row v (LMI_NP) | w*r_u | w*r_v | w | loss | residual row | jac row
+// | jac_params of the point (2 x CAM_MAX_PARAMS, staging for the column selection)
+enum { LMI_WR0 = 2 * LMI_NP, LMI_WR1, LMI_WT, LMI_LOSS, LMI_ROW, LMI_JROW, LMI_JP, LMI_W = LMI_JP + 2 * CAM_MAX_PARAMS };
+constexpr size_t LMI_TILE_BYTES = sizeof(double) * LMI_W * LM_THREADS;
+
+// Shared memory of one k_lm CTA that both refiners use: the parameters, the scalar LM state of thread 0 (JtJ and its
+// damped copy Am NP x NP row-major, lower triangle used) and the cluster reduction of NV values.
+template <int NP, int NV> struct LmCore {
     double par[9], par_new[9];
-    double ctx[80];
-    double tb[6], tb_new[6];
-    double red[LM_WARPS][LM_NV_MAX];
-    double sums[2][LM_NV_MAX]; // CTA partial sums, double-buffered: read by the other CTAs of the cluster (DSMEM)
-    double tot[LM_NV_MAX];     // cluster totals (identical in every CTA)
-    ScoreRed<1> sred;
+    double tb[6], tb_new[6]; // relpose: tangent basis of par / par_new
+    double JtJ[NP * NP], Am[NP * NP], Jtr[NP], rhs[NP], sol[NP];
+    double sums[2][NV]; // CTA partial sums, double-buffered: read by the other CTAs of the cluster (DSMEM)
+    double tot[NV];     // cluster totals (identical in every CTA)
     int wcount[LM_WARPS];
     int flag;
 };
+// fixed camera: per-warp partial sums of the packed normal equations (cluster_sum), the rescoring of the result
+template <int NP> struct LmShared : LmCore<NP, LM_NV_MAX> {
+    double ctx[80];
+    double red[LM_WARPS][LM_NV_MAX];
+    ScoreRed<1> sred;
+};
+// camera refinement: the camera parameters of par / par_new and the refined indices idx[0..m); the tile rows of
+// lmi_eval_pass are dynamic shared memory
+struct LmCamShared : LmCore<LMI_NP, LMI_NV> {
+    double ctx[12];
+    double cam[CAM_MAX_PARAMS], cam_new[CAM_MAX_PARAMS];
+    int idx[CAM_MAX_PARAMS];
+    int m;
+};
 
-// Cluster totals of the CTA partial sums S->sums[buf][0..nv) -> S->tot[0..nv) in every CTA, CTAs in rank order
-// (the second half of cluster_sum, for partial sums that are already per CTA).
-template <class Shared> PLB_DEV void cluster_total(Shared *S, int nv, int buf, int csize) {
+// Cluster totals of the CTA partial sums S->sums[buf][0..nv) -> S->tot[0..nv) in every CTA, CTAs in rank order.
+template <class Shared> PLB_DEV void cluster_total(Shared *S, int nv, int &buf, int csize) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     cluster.sync();
@@ -1787,13 +1813,12 @@ template <class Shared> PLB_DEV void cluster_total(Shared *S, int nv, int buf, i
         S->tot[threadIdx.x] = t;
     }
     __syncthreads();
+    buf ^= 1;
 }
 
 // Cluster-wide deterministic sum of NV per-thread values -> S->tot[0..NV) in every CTA of the cluster.
 // Order: xor-butterfly inside a warp, warps left to right, CTAs in rank order.
-template <int NV> PLB_DEV void cluster_sum(LmShared *S, const double *v, int &buf, int csize) {
-    namespace cg = cooperative_groups;
-    cg::cluster_group cluster = cg::this_cluster();
+template <int NV, class Shared> PLB_DEV void cluster_sum(Shared *S, const double *v, int &buf, int csize) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
@@ -1806,17 +1831,7 @@ template <int NV> PLB_DEV void cluster_sum(LmShared *S, const double *v, int &bu
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += S->red[w][threadIdx.x];
         S->sums[buf][threadIdx.x] = s;
     }
-    cluster.sync();
-    if (threadIdx.x < NV) {
-        double t = 0.0;
-        for (int r = 0; r < csize; ++r) {
-            const double *remote = cluster.map_shared_rank(&S->sums[buf][0], r);
-            t += remote[threadIdx.x];
-        }
-        S->tot[threadIdx.x] = t;
-    }
-    __syncthreads();
-    buf ^= 1;
+    cluster_total(S, NV, buf, csize);
 }
 
 // thread 0 -> whole CTA broadcast of a small integer (two barriers: the slot can be reused right away)
@@ -1834,7 +1849,7 @@ template <class Shared> PLB_DEV int block_bcast(Shared *S, int v) {
 // Output layout in S->tot: [0] loss sum, [1] residual rows, [2..2+NT) JtJ, [2+NT..2+NT+NP) Jtr, [2+NT+NP] jac rows.
 template <int KIND>
 PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn &L, const int *list, int lo, int na,
-                          LmShared *S, int &buf, int csize) {
+                          LmShared<LmDims<KIND>::NP> *S, int &buf, int csize) {
     constexpr int NP = LmDims<KIND>::NP;
     constexpr int NT = NP * (NP + 1) / 2;
     const double *ctx = S->ctx;
@@ -2002,394 +2017,13 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn
     cluster_sum<NV>(S, v, buf, csize);
 }
 
-// lower Cholesky solve of (A) x = rhs, only the lower triangle of A read (jacobian_accumulator.h:145-154)
-template <int NP> PLB_DEV void llt_solve(const double *A, const double *rhs, double *x) {
-    double Lm[NP * NP];
-    for (int j = 0; j < NP; ++j) {
-        double d = A[j * NP + j];
-        for (int k = 0; k < j; ++k) d -= Lm[j * NP + k] * Lm[j * NP + k];
-        const double ljj = sqrt(d);
-        Lm[j * NP + j] = ljj;
-        for (int i = j + 1; i < NP; ++i) {
-            double s = A[i * NP + j];
-            for (int k = 0; k < j; ++k) s -= Lm[i * NP + k] * Lm[j * NP + k];
-            Lm[i * NP + j] = s / ljj;
-        }
-    }
-    double y[NP];
-    for (int i = 0; i < NP; ++i) {
-        double s = rhs[i];
-        for (int k = 0; k < i; ++k) s -= Lm[i * NP + k] * y[k];
-        y[i] = s / Lm[i * NP + i];
-    }
-    for (int i = NP - 1; i >= 0; --i) {
-        double s = y[i];
-        for (int k = i + 1; k < NP; ++k) s -= Lm[k * NP + i] * x[k];
-        x[i] = s / Lm[i * NP + i];
-    }
-}
-
-// One thread-block CLUSTER per job (1..8 CTAs of 256 threads, DSMEM reductions); CTA r owns the correspondences
-// [r*chunk, (r+1)*chunk).  Every CTA runs the scalar LM logic (optim/lm_impl.h:56-140) redundantly on identical
-// cluster totals, so no broadcast between CTAs is needed.  The reference evaluates the residual of a trial step and,
-// if accepted, the Jacobian at the same parameters in a second pass; here both come from one pass.
-template <int KIND>
-__global__ void __launch_bounds__(LM_THREADS, 1)
-    k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
-         const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
-         int *idx_scratch, int scratch_stride, LmJobOut *outs) {
-    namespace cg = cooperative_groups;
-    cg::cluster_group cluster = cg::this_cluster();
-    constexpr int NP = LmDims<KIND>::NP;
-    constexpr int NT = NP * (NP + 1) / 2;
-    constexpr int MSZ = kind_model_size(KIND);
-    __shared__ LmShared S;
-    const int csize = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
-    // The grid is a set of clusters that walk the job list: explicit jobs (jobs[j], model j of models_in, stride 9) or
-    // the LO jobs k_pass1 listed on the device (template jobs[job_src[j].pidx], model slot job_src[j].slot of the
-    // round's model list, stride MSZ; the count is read from device memory and clamped to n_jobs).
-    const int n_clusters = (int)gridDim.x / csize, cluster_id = (int)blockIdx.x / csize;
-    int nj = n_jobs;
-    if (n_jobs_dev) {
-        const int v = *n_jobs_dev;
-        if (v < nj) nj = v;
-    }
-    int buf = 0;
-    for (int job = cluster_id; job < nj; job += n_clusters) {
-    const LmJob &J = job_src ? jobs[job_src[job].pidx] : jobs[job];
-    const ProblemDev P = probs[J.pidx];
-    const LmParams prm = J.prm;
-    const char *mask_in = (J.mask_off >= 0) ? mask_base + J.mask_off : nullptr;
-    const double *min = job_src ? models_in + (size_t)job_src[job].slot * MSZ : models_in + (size_t)job * 9;
-    LmJobOut *out = outs + job;
-    LossFn L;
-    L.type = prm.loss_type;
-    L.thr = prm.loss_scale;
-    L.sq_thr = prm.loss_scale * prm.loss_scale;
-    L.inv_sq_thr = 1.0 / L.sq_thr;
-
-    // ---- this CTA's slice and its active-point list ------------------------------------------------------------
-    const int chunk = (((P.n + csize - 1) / csize) + 31) & ~31;
-    const int lo = min_i(crank * chunk, P.n), hi = min_i(lo + chunk, P.n);
-    int na = hi - lo;
-    const int *list = nullptr;
-    bool untouched = false;
-    if (prm.subset_mode != 0) {
-        int *mylist = idx_scratch + (size_t)cluster_id * (size_t)scratch_stride + lo;
-        double C[kind_ctx_size(KIND_RELPOSE)];
-        if (KIND == KIND_RELPOSE && prm.subset_mode == 1) model_ctx<KIND_RELPOSE>(min, C);
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        int base = 0;
-        for (int t0 = lo; t0 < hi; t0 += (int)blockDim.x) {
-            const int k = t0 + threadIdx.x;
-            bool keep = false;
-            if (k < hi) {
-                if (prm.subset_mode == 2) {
-                    keep = mask_in[k] != 0;
-                } else if (KIND == KIND_RELPOSE) {
-                    // relpose LO subset: inliers of the start pose at 5*thr^2 (estimators/relative_pose.cc:62-86)
-                    double v[kind_corr_size(KIND_RELPOSE)];
-                    load_corr<KIND_RELPOSE>(P, k, v);
-                    keep = is_inlier<KIND_RELPOSE>(C, v, prm.subset_sq_thr);
-                }
-            }
-            const unsigned bal = __ballot_sync(0xffffffffu, keep);
-            if (lane == 0) S.wcount[warp] = __popc(bal);
-            __syncthreads();
-            int off = base;
-            for (int w = 0; w < warp; ++w) off += S.wcount[w];
-            int tile = 0;
-            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tile += S.wcount[w];
-            if (keep) mylist[off + __popc(bal & ((1u << lane) - 1u))] = k;
-            base += tile;
-            __syncthreads();
-        }
-        na = base;
-        list = mylist;
-        __syncthreads();
-        if (KIND == KIND_RELPOSE && prm.subset_mode == 1) {
-            double c[1] = {threadIdx.x == 0 ? (double)na : 0.0};
-            cluster_sum<1>(&S, c, buf, csize);
-            untouched = !(S.tot[0] > 5.0);
-        }
-    }
-
-    // ---- initial parameters
-    if (threadIdx.x == 0) {
-        if (KIND == KIND_FUND) {
-            m3 F, U, V;
-#pragma unroll
-            for (int k = 0; k < 9; ++k) F.a[3 * (k % 3) + k / 3] = min[k];
-            double sv[3];
-            svd3_dev(F, U, sv, V);
-            if (det3(U) < 0)
-                for (int k = 0; k < 9; ++k) U.a[k] = -U.a[k];
-            if (det3(V) < 0)
-                for (int k = 0; k < 9; ++k) V.a[k] = -V.a[k];
-            rot_to_quat(U, S.par);
-            rot_to_quat(V, S.par + 4);
-            S.par[8] = sv[1] / sv[0];
-        } else {
-            for (int k = 0; k < MSZ; ++k) S.par[k] = min[k];
-            for (int k = MSZ; k < 9; ++k) S.par[k] = 0.0;
-        }
-    }
-    __syncthreads();
-
-    int iterations = 0;
-    double cost = 0.0, initial_cost = 0.0;
-    if (!untouched) {
-        // scalar LM state (thread 0 of every CTA); rc mirrors NormalAccumulator::residual_count
-        double lambda = prm.initial_lambda, nu = 2.0, rc = 0.0;
-        double JtJ[NP * NP], Jtr[NP], sol[NP];
-        bool recompute_jac = true;
-        if (threadIdx.x == 0) lm_build_ctx<KIND>(S.par, S.ctx, S.tb, true);
-        __syncthreads();
-        lm_eval_pass<KIND>(P, prm, L, list, lo, na, &S, buf, csize);
-        if (threadIdx.x == 0) {
-            cost = S.tot[0] * (1.0 / fmax(1.0, S.tot[1])); // acc.get_residual() after the residual pass
-            initial_cost = cost;
-            int t = 0;
-            for (int i = 0; i < NP; ++i)
-                for (int j = 0; j <= i; ++j) JtJ[i * NP + j] = S.tot[2 + t++];
-            for (int i = 0; i < NP; ++i) Jtr[i] = S.tot[2 + NT + i];
-            rc = S.tot[2 + NT + NP]; // residual_count after the Jacobian pass
-        }
-        for (int it = 0; it < prm.max_iterations; ++it) {
-            iterations = it;
-            int stop = 0;
-            if (threadIdx.x == 0) {
-                if (recompute_jac) {
-                    double g = 0.0;
-                    for (int i = 0; i < NP; ++i) g += Jtr[i] * Jtr[i];
-                    const double grad_norm = (1.0 / fmax(1.0, rc)) * sqrt(g);
-                    if (grad_norm < prm.gradient_tol) stop = 1;
-                }
-                if (!stop) {
-                    const double scale = 1.0 / fmax(1.0, rc);
-                    double Am[NP * NP], rhs[NP];
-                    for (int i = 0; i < NP; ++i)
-                        for (int j = 0; j <= i; ++j) Am[i * NP + j] = scale * JtJ[i * NP + j];
-                    for (int i = 0; i < NP; ++i) Am[i * NP + i] += lambda;
-                    for (int i = 0; i < NP; ++i) rhs[i] = -(scale * Jtr[i]);
-                    llt_solve<NP>(Am, rhs, sol);
-                    double sn = 0.0;
-                    for (int i = 0; i < NP; ++i) sn += sol[i] * sol[i];
-                    if (sqrt(sn) < prm.step_tol) stop = 1;
-                }
-                if (!stop) {
-                    lm_step<KIND>(S.par, sol, S.tb, S.par_new);
-                    lm_build_ctx<KIND>(S.par_new, S.ctx, S.tb_new, true);
-                }
-            }
-            if (block_bcast(&S, stop)) break;
-            lm_eval_pass<KIND>(P, prm, L, list, lo, na, &S, buf, csize);
-            int brk = 0;
-            if (threadIdx.x == 0) {
-                rc = S.tot[1]; // residual_count after the residual pass of the trial point
-                const double cost_new = S.tot[0] * (1.0 / fmax(1.0, rc));
-                if (cost_new < cost) {
-                    const double cost_decrease = cost - cost_new;
-                    for (int k = 0; k < 9; ++k) S.par[k] = S.par_new[k];
-                    for (int k = 0; k < 6; ++k) S.tb[k] = S.tb_new[k];
-                    cost = cost_new;
-                    recompute_jac = true;
-                    const double scale = 1.0 / fmax(1.0, rc);
-                    double pred = 0.0;
-                    for (int i = 0; i < NP; ++i) pred += sol[i] * (lambda * sol[i] + scale * Jtr[i]);
-                    pred = -pred;
-                    if (pred > 0) {
-                        const double rho = cost_decrease / pred;
-                        const double factor = 1.0 - pow(2.0 * rho - 1.0, 3.0);
-                        lambda *= fmax(1.0 / 3.0, factor);
-                    } else {
-                        lambda *= 1.0 / 3.0;
-                    }
-                    nu = 2.0;
-                    lambda = fmax(prm.min_lambda, lambda);
-                    if (cost > 0 && cost_decrease / cost < prm.relative_cost_tol) brk = 1;
-                    // the Jacobian pass the reference would run next at the accepted parameters
-                    int t = 0;
-                    for (int i = 0; i < NP; ++i)
-                        for (int j = 0; j <= i; ++j) JtJ[i * NP + j] = S.tot[2 + t++];
-                    for (int i = 0; i < NP; ++i) Jtr[i] = S.tot[2 + NT + i];
-                    if (!brk && it + 1 < prm.max_iterations) rc = S.tot[2 + NT + NP];
-                } else {
-                    recompute_jac = false;
-                    lambda *= nu;
-                    nu *= 2.0;
-                    lambda = fmin(prm.max_lambda, lambda);
-                }
-                if (it + 1 >= prm.max_iterations && !brk) iterations = it + 1;
-            }
-            if (block_bcast(&S, brk)) break;
-        }
-    }
-    // ---- output (CTA 0 of the cluster)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        if (KIND == KIND_FUND) {
-            if (untouched) {
-                for (int k = 0; k < 9; ++k) S.par_new[k] = min[k];
-            } else {
-                const m3 F = ff_to_F(S.par);
-                for (int k = 0; k < 9; ++k) S.par_new[k] = F.a[3 * (k % 3) + k / 3];
-            }
-        } else {
-            for (int k = 0; k < MSZ; ++k) S.par_new[k] = untouched ? min[k] : S.par[k];
-            for (int k = MSZ; k < 9; ++k) S.par_new[k] = 0.0;
-        }
-        if (crank == 0) {
-            for (int k = 0; k < 9; ++k) out->model[k] = S.par_new[k];
-            out->iterations = iterations;
-            out->cost = cost;
-            out->initial_cost = initial_cost;
-        }
-    }
-    __syncthreads();
-    if (prm.score_after && crank == 0) {
-        double mdl[9];
-#pragma unroll
-        for (int k = 0; k < 9; ++k) mdl[k] = S.par_new[k];
-        cta_score<KIND>(P, mdl, S.sred, &out->count, &out->score);
-    }
-    cluster.sync(); // no CTA may exit (or start the next job) while a sibling can still read its shared memory
-    } // jobs of this cluster
-}
-
-// k_lm needs ~255 registers per thread: one 256-thread CTA (one job, or one slice of a job's cluster) per SM.
-static thread_local int t_lm_sm_share = 50;
-void lm_set_sm_share(int pct) { t_lm_sm_share = (pct > 0 && pct <= 100) ? pct : 50; }
-static int lm_cluster_size(int n_jobs, int max_n) {
-    static const int per_cta = [] { // correspondences per CTA before another CTA of the cluster pays off
-        const char *e = std::getenv("PLB_LM_PER_CTA");
-        const int v = e ? std::atoi(e) : 0;
-        return v > 0 ? v : 2048;
-    }();
-    int csize = (max_n + per_cta - 1) / per_cta;
-    if (csize < 1) csize = 1;
-    if (csize > LM_MAX_CLUSTER) csize = LM_MAX_CLUSTER;
-    if (csize > 4 && csize < 8) csize = 4;
-    if (csize == 3) csize = 2;
-    // k_lm needs the whole register file of an SM per CTA: with many jobs in one launch (batch groups) wide clusters
-    // only take SMs away from the co-running hypothesis kernels, so the cluster shrinks as the job count grows
-    // SMs (percent of the device) the LO clusters of one launch may cover: half when other lock-step groups share the GPU
-    // (their hypothesis kernels want the other half: +5 % on the batch workload), all of it for a call that runs alone
-    // (C4 single call 2.7 -> 2.2 ms).  PLB_LM_SM_PCT overrides.
-    static const int forced = [] {
-        const char *e = std::getenv("PLB_LM_SM_PCT");
-        const int v = e ? std::atoi(e) : 0;
-        return (v > 0 && v <= 100) ? v : 0;
-    }();
-    const int sm_share = forced ? forced : t_lm_sm_share;
-    while (csize > 1 && n_jobs * csize > sm_count() * sm_share / 100) csize /= 2;
-    return csize;
-}
-static void launch_lm_any(int kind, const ProblemDev *probs, const LmJob *jobs, const LoJobSrc *job_src,
-                          const double *models_in, const int *n_jobs_dev, int n_jobs, int n_clusters, int csize,
-                          const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
-    cfg.blockDim = dim3((unsigned)LM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)csize;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    with_kind(kind, [&](auto K) {
-        cudaLaunchKernelEx(&cfg, k_lm<K>, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
-                           scratch_stride, out);
-    });
-}
-void launch_lm(int kind, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in, int n_jobs,
-               int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
-    if (n_jobs <= 0) return;
-    const int csize = lm_cluster_size(n_jobs, max_n);
-    launch_lm_any(kind, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base, idx_scratch,
-                  scratch_stride, out, stream);
-}
-// Clusters of a round's LO launch: at most one wave (a k_lm CTA owns an SM), at most the estimated number of jobs.
-int lm_round_max_clusters(int kind, int est_jobs, int max_n) {
-    (void)kind;
-    if (est_jobs < 1) est_jobs = 1;
-    const int csize = lm_cluster_size(est_jobs, max_n);
-    int nc = sm_count() / csize;
-    if (nc > est_jobs) nc = est_jobs;
-    return nc < 1 ? 1 : nc;
-}
-void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const LoJobSrc *job_src,
-                     const double *models, const int *n_jobs_dev, int job_cap, int est_jobs, int max_n,
-                     int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
-    if (est_jobs < 1) est_jobs = 1;
-    const int csize = lm_cluster_size(est_jobs, max_n);
-    const int nc = lm_round_max_clusters(kind, est_jobs, max_n);
-    launch_lm_any(kind, probs, tmpl, job_src, models, n_jobs_dev, job_cap, nc, csize, nullptr, idx_scratch, scratch_stride,
-                  out, stream);
-}
-
-// ============================================================================================================
-// LM of the absolute pose together with camera parameters: AbsolutePoseRefiner with a non-empty camera_refine_idx
-// (optim/absolute.h:40-171).  The scalar LM logic is k_lm's; the normal equations are reduced through a shared-memory
-// tile instead of per-thread packed accumulators (105 + 14 doubles per thread would not fit beside the rest).
-// ============================================================================================================
-// Parameters: the pose (6) and m <= CAM_MAX_PARAMS camera parameters, padded to LMI_NP.  The padded rows and columns of
-// JtJ and Jtr are zero, their damped diagonal is lambda and their step component zero, so the Cholesky solve, the step,
-// its norm and the predicted decrease are those of the (6 + m)-dimensional system.
-constexpr int LMI_NP = 6 + CAM_MAX_PARAMS;
-constexpr int LMI_NT = LMI_NP * (LMI_NP + 1) / 2;
-constexpr int LMI_NV = 2 + LMI_NT + LMI_NP + 1; // [loss, residual rows, JtJ (packed lower, row-major), Jtr, jac rows]
-static_assert(LMI_NV <= LM_THREADS, "one owner thread per reduced value");
-// Tile row of one point: Jacobian row u (LMI_NP) | row v (LMI_NP) | w*r_u | w*r_v | w | loss | residual row | jac row
-// | jac_params of the point (2 x CAM_MAX_PARAMS, staging for the column selection)
-enum { LMI_WR0 = 2 * LMI_NP, LMI_WR1, LMI_WT, LMI_LOSS, LMI_ROW, LMI_JROW, LMI_JP, LMI_W = LMI_JP + 2 * CAM_MAX_PARAMS };
-constexpr size_t LMI_TILE_BYTES = sizeof(double) * LMI_W * LM_THREADS;
-
-struct LmIntrShared {
-    double par[9], par_new[9];
-    double cam[CAM_MAX_PARAMS], cam_new[CAM_MAX_PARAMS];
-    double ctx[12];
-    double JtJ[LMI_NP * LMI_NP], Am[LMI_NP * LMI_NP];
-    double Jtr[LMI_NP], rhs[LMI_NP], sol[LMI_NP];
-    double sums[2][LMI_NV]; // CTA partial sums, double-buffered: read by the other CTAs of the cluster (DSMEM)
-    double tot[LMI_NV];     // cluster totals (identical in every CTA)
-    int wcount[LM_WARPS];
-    int flag;
-};
-
-// Points of this CTA's slice [lo, hi) whose mask byte is set, in point order -> mylist (the subset mode 2 of k_lm);
-// returns their number.
-PLB_DEV int lmi_mask_list(const char *mask_in, int lo, int hi, int *mylist, LmIntrShared *S) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int base = 0;
-    for (int t0 = lo; t0 < hi; t0 += (int)blockDim.x) {
-        const int k = t0 + threadIdx.x;
-        const bool keep = k < hi && mask_in[k] != 0;
-        const unsigned bal = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) S->wcount[warp] = __popc(bal);
-        __syncthreads();
-        int off = base;
-        for (int w = 0; w < warp; ++w) off += S->wcount[w];
-        int tile = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tile += S->wcount[w];
-        if (keep) mylist[off + __popc(bal & ((1u << lane) - 1u))] = k;
-        base += tile;
-        __syncthreads();
-    }
-    return base;
-}
-
 // One evaluation pass at the pose whose context is in S->ctx and the camera parameters cp: robust cost and residual
 // rows (compute_residual, <Model>::project) and JtJ, Jtr, jacobian rows (compute_jacobian, <Model>::project_with_jac
 // with jac_params) -> S->tot, in lm_eval_pass's layout.  Every 256 points each thread writes its point's row of the tile;
 // thread e < LMI_NV then adds value e of every row in point order.  Order of the sums: points in order inside a CTA, CTAs
 // in rank order (deterministic for a given cluster size).
 PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, int model, const double *cp, int m, const int *idx,
-                           const int *list, int lo, int na, LmIntrShared *S, double *tile, int &buf, int csize) {
+                           const int *list, int lo, int na, LmCamShared *S, double *tile, int &buf, int csize) {
     const double *ctx = S->ctx;
     CamDev cam;
     cam.model = model;
@@ -2497,189 +2131,347 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, int model, cons
     }
     if (e < LMI_NV) S->sums[buf][e] = acc;
     cluster_total(S, LMI_NV, buf, csize);
-    buf ^= 1;
 }
 
-// llt_solve with the size at run time and the factor written over A (shared memory), in llt_solve's operation order:
-// unrolled at compile time, a 14 x 14 factor in registers would crowd out the evaluation pass (spills).
+// Lower Cholesky solve of (A) x = rhs, n x n row-major, only the lower triangle of A read and the factor written over it
+// (jacobian_accumulator.h:145-154).  Unrolled for the fixed-camera sizes (n <= 8): the step is on the critical path of
+// every LM iteration, and as loops over shared memory it makes the LO of small problems half as slow again.  The 14 x 14
+// camera system stays a loop: unrolled, it would take the registers of the evaluation pass (spills).
 PLB_DEV void llt_solve_n(double *A, const double *rhs, double *x, int n) {
+#pragma unroll 8
     for (int j = 0; j < n; ++j) {
         double d = A[j * n + j];
+#pragma unroll 8
         for (int k = 0; k < j; ++k) d -= A[j * n + k] * A[j * n + k];
         const double ljj = sqrt(d);
         A[j * n + j] = ljj;
+#pragma unroll 8
         for (int i = j + 1; i < n; ++i) {
             double s = A[i * n + j];
+#pragma unroll 8
             for (int k = 0; k < j; ++k) s -= A[i * n + k] * A[j * n + k];
             A[i * n + j] = s / ljj;
         }
     }
+#pragma unroll 8
     for (int i = 0; i < n; ++i) {
         double s = rhs[i];
+#pragma unroll 8
         for (int k = 0; k < i; ++k) s -= A[i * n + k] * x[k];
         x[i] = s / A[i * n + i];
     }
+#pragma unroll 8
     for (int i = n - 1; i >= 0; --i) {
         double s = x[i];
+#pragma unroll 8
         for (int k = i + 1; k < n; ++k) s -= A[k * n + i] * x[k];
         x[i] = s / A[i * n + i];
     }
 }
 
-// One thread-block cluster per job, as k_lm (the LM scalar logic of optim/lm_impl.h:56-140 runs redundantly in every
-// CTA on identical cluster totals).  Output: refined pose and camera parameters.
+// The points k of this CTA's slice [lo, hi) with keep(k), in point order -> list; returns their number.
+template <class Shared, class Keep> PLB_DEV int lm_compact(Shared *S, int lo, int hi, int *list, Keep keep) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int base = 0;
+    for (int t0 = lo; t0 < hi; t0 += (int)blockDim.x) {
+        const int k = t0 + threadIdx.x;
+        const bool kept = k < hi && keep(k);
+        const unsigned bal = __ballot_sync(0xffffffffu, kept);
+        if (lane == 0) S->wcount[warp] = __popc(bal);
+        __syncthreads();
+        int off = base;
+        for (int w = 0; w < warp; ++w) off += S->wcount[w];
+        int tile = 0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tile += S->wcount[w];
+        if (kept) list[off + __popc(bal & ((1u << lane) - 1u))] = k;
+        base += tile;
+        __syncthreads();
+    }
+    return base;
+}
+
+// One thread-block CLUSTER per job (1..8 CTAs of 256 threads, DSMEM reductions); CTA r owns the correspondences
+// [r*chunk, (r+1)*chunk).  Every CTA runs the scalar LM logic (optim/lm_impl.h:56-140) redundantly on identical
+// cluster totals, so no broadcast between CTAs is needed.  The reference evaluates the residual of a trial step and,
+// if accepted, the Jacobian at the same parameters in a second pass; here both come from one pass.
+// Two refiners: the fixed-camera one of every kind (lm_eval_pass: per-thread packed normal equations, cluster_sum), and
+// CAM, AbsolutePoseRefiner with the camera parameters cam_refine_idx(prm.cam.model, job.cam_refine) refined with the
+// pose (lmi_eval_pass: the shared-memory tile summed in point order, which ~255 registers of per-thread accumulators
+// for 14 parameters would not leave room for).  CAM writes the camera of job j to cam_outs[j * CAM_MAX_PARAMS ..].
+template <int KIND, bool CAM>
 __global__ void __launch_bounds__(LM_THREADS, 1)
-    k_lm_intr(const ProblemDev *__restrict__ probs, const LmIntrJob *__restrict__ jobs, const double *__restrict__ models_in,
-              int n_jobs, const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *outs) {
+    k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
+         const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
+         int *idx_scratch, int scratch_stride, LmJobOut *outs, double *cam_outs) {
+    static_assert(!CAM || KIND == KIND_PNP, "camera refinement is the absolute pose refiner's");
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    __shared__ LmIntrShared S;
-    extern __shared__ double lmi_tile[];
+    constexpr int NP = CAM ? LMI_NP : LmDims<KIND>::NP;
+    constexpr int NT = NP * (NP + 1) / 2;
+    constexpr int MSZ = kind_model_size(KIND);
+    __shared__ std::conditional_t<CAM, LmCamShared, LmShared<NP>> S;
+    extern __shared__ double lmi_tile[]; // CAM: LMI_TILE_BYTES
     const int csize = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
+    // The grid is a set of clusters that walk the job list: explicit jobs (jobs[j], model j of models_in, stride 9) or
+    // the LO jobs k_pass1 listed on the device (template jobs[job_src[j].pidx], model slot job_src[j].slot of the
+    // round's model list, stride MSZ; the count is read from device memory and clamped to n_jobs).
     const int n_clusters = (int)gridDim.x / csize, cluster_id = (int)blockIdx.x / csize;
+    int nj = n_jobs;
+    if (n_jobs_dev) {
+        const int v = *n_jobs_dev;
+        if (v < nj) nj = v;
+    }
     int buf = 0;
-    for (int job = cluster_id; job < n_jobs; job += n_clusters) {
-    const LmIntrJob &JI = jobs[job];
-    const ProblemDev P = probs[JI.base.pidx];
-    const LmParams prm = JI.base.prm;
-    const int m = JI.m, model = prm.cam.model;
-    int idx[CAM_MAX_PARAMS];
-#pragma unroll
-    for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[c] = JI.idx[c];
-    const char *mask_in = (JI.base.mask_off >= 0) ? mask_base + JI.base.mask_off : nullptr;
-    const double *min = models_in + (size_t)job * 9;
-    LmIntrJobOut *out = outs + job;
+    for (int job = cluster_id; job < nj; job += n_clusters) {
+    const LmJob &J = job_src ? jobs[job_src[job].pidx] : jobs[job];
+    const ProblemDev P = probs[J.pidx];
+    const LmParams prm = J.prm;
+    const char *mask_in = (J.mask_off >= 0) ? mask_base + J.mask_off : nullptr;
+    const double *min = job_src ? models_in + (size_t)job_src[job].slot * MSZ : models_in + (size_t)job * 9;
+    LmJobOut *out = outs + job;
     LossFn L;
     L.type = prm.loss_type;
     L.thr = prm.loss_scale;
     L.sq_thr = prm.loss_scale * prm.loss_scale;
     L.inv_sq_thr = 1.0 / L.sq_thr;
 
+    // ---- this CTA's slice and its active-point list ------------------------------------------------------------
     const int chunk = (((P.n + csize - 1) / csize) + 31) & ~31;
     const int lo = min_i(crank * chunk, P.n), hi = min_i(lo + chunk, P.n);
     int na = hi - lo;
     const int *list = nullptr;
+    bool untouched = false;
     if (prm.subset_mode != 0) {
         int *mylist = idx_scratch + (size_t)cluster_id * (size_t)scratch_stride + lo;
-        na = lmi_mask_list(mask_in, lo, hi, mylist, &S);
+        double C[kind_ctx_size(KIND_RELPOSE)];
+        if (KIND == KIND_RELPOSE && prm.subset_mode == 1) model_ctx<KIND_RELPOSE>(min, C);
+        na = lm_compact(&S, lo, hi, mylist, [&](int k) {
+            if (prm.subset_mode == 2) return mask_in[k] != 0;
+            if (KIND != KIND_RELPOSE) return false;
+            // relpose LO subset: inliers of the start pose at 5*thr^2 (estimators/relative_pose.cc:62-86)
+            double v[kind_corr_size(KIND_RELPOSE)];
+            load_corr<KIND_RELPOSE>(P, k, v);
+            return is_inlier<KIND_RELPOSE>(C, v, prm.subset_sq_thr);
+        });
         list = mylist;
+        __syncthreads();
+        if constexpr (KIND == KIND_RELPOSE) {
+            if (prm.subset_mode == 1) {
+                double c[1] = {threadIdx.x == 0 ? (double)na : 0.0};
+                cluster_sum<1>(&S, c, buf, csize);
+                untouched = !(S.tot[0] > 5.0);
+            }
+        }
     }
+
+    // ---- initial parameters
     if (threadIdx.x == 0) {
-        for (int k = 0; k < 7; ++k) S.par[k] = min[k];
-        for (int k = 7; k < 9; ++k) S.par[k] = 0.0;
-        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = prm.cam.p[c];
-        lm_build_ctx<KIND_PNP>(S.par, S.ctx, nullptr, true);
+        if (KIND == KIND_FUND) {
+            m3 F, U, V;
+#pragma unroll
+            for (int k = 0; k < 9; ++k) F.a[3 * (k % 3) + k / 3] = min[k];
+            double sv[3];
+            svd3_dev(F, U, sv, V);
+            if (det3(U) < 0)
+                for (int k = 0; k < 9; ++k) U.a[k] = -U.a[k];
+            if (det3(V) < 0)
+                for (int k = 0; k < 9; ++k) V.a[k] = -V.a[k];
+            rot_to_quat(U, S.par);
+            rot_to_quat(V, S.par + 4);
+            S.par[8] = sv[1] / sv[0];
+        } else {
+            for (int k = 0; k < MSZ; ++k) S.par[k] = min[k];
+            for (int k = MSZ; k < 9; ++k) S.par[k] = 0.0;
+        }
+        if constexpr (CAM) {
+            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = prm.cam.p[c];
+            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.idx[c] = 0;
+            S.m = cam_refine_idx(prm.cam.model, J.cam_refine, S.idx);
+        }
     }
     __syncthreads();
+    int m = 0, idx[CAM_MAX_PARAMS]; // CAM: the refined camera parameters, in registers for the evaluation pass
+    if constexpr (CAM) {
+        m = S.m;
+#pragma unroll
+        for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[c] = S.idx[c];
+    }
+    // one evaluation pass at par (trial: par_new), totals in S.tot
+    auto eval = [&](bool trial) {
+        if constexpr (CAM)
+            lmi_eval_pass(P, L, prm.cam.model, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+        else
+            lm_eval_pass<KIND>(P, prm, L, list, lo, na, &S, buf, csize);
+    };
 
     int iterations = 0;
     double cost = 0.0, initial_cost = 0.0;
-    // scalar LM state (thread 0 of every CTA); rc mirrors NormalAccumulator::residual_count
-    double lambda = prm.initial_lambda, nu = 2.0, rc = 0.0;
-    bool recompute_jac = true;
-    lmi_eval_pass(P, L, model, S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
-    if (threadIdx.x == 0) {
-        cost = S.tot[0] * (1.0 / fmax(1.0, S.tot[1]));
-        initial_cost = cost;
-        int t = 0;
-        for (int i = 0; i < LMI_NP; ++i)
-            for (int j = 0; j <= i; ++j) S.JtJ[i * LMI_NP + j] = S.tot[2 + t++];
-        for (int i = 0; i < LMI_NP; ++i) S.Jtr[i] = S.tot[2 + LMI_NT + i];
-        rc = S.tot[2 + LMI_NT + LMI_NP];
-    }
-    for (int it = 0; it < prm.max_iterations; ++it) {
-        iterations = it;
-        int stop = 0;
+    if (!untouched) {
+        // scalar LM state (thread 0 of every CTA); rc mirrors NormalAccumulator::residual_count
+        double lambda = prm.initial_lambda, nu = 2.0, rc = 0.0;
+        bool recompute_jac = true;
+        if (threadIdx.x == 0) lm_build_ctx<KIND>(S.par, S.ctx, S.tb, true);
+        __syncthreads();
+        eval(false);
         if (threadIdx.x == 0) {
-            if (recompute_jac) {
-                double g = 0.0;
-                for (int i = 0; i < LMI_NP; ++i) g += S.Jtr[i] * S.Jtr[i];
-                const double grad_norm = (1.0 / fmax(1.0, rc)) * sqrt(g);
-                if (grad_norm < prm.gradient_tol) stop = 1;
-            }
-            if (!stop) {
-                const double scale = 1.0 / fmax(1.0, rc);
-                for (int i = 0; i < LMI_NP; ++i)
-                    for (int j = 0; j <= i; ++j) S.Am[i * LMI_NP + j] = scale * S.JtJ[i * LMI_NP + j];
-                for (int i = 0; i < LMI_NP; ++i) S.Am[i * LMI_NP + i] += lambda;
-                for (int i = 0; i < LMI_NP; ++i) S.rhs[i] = -(scale * S.Jtr[i]);
-                llt_solve_n(S.Am, S.rhs, S.sol, LMI_NP);
-                double sn = 0.0;
-                for (int i = 0; i < LMI_NP; ++i) sn += S.sol[i] * S.sol[i];
-                if (sqrt(sn) < prm.step_tol) stop = 1;
-            }
-            if (!stop) { // AbsolutePoseRefiner::step (optim/absolute.h:146-160)
-                lm_step<KIND_PNP>(S.par, S.sol, nullptr, S.par_new);
-                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam_new[c] = S.cam[c];
-                for (int c = 0; c < m; ++c) S.cam_new[idx[c]] += S.sol[6 + c];
-                lm_build_ctx<KIND_PNP>(S.par_new, S.ctx, nullptr, true);
-            }
+            cost = S.tot[0] * (1.0 / fmax(1.0, S.tot[1])); // acc.get_residual() after the residual pass
+            initial_cost = cost;
+            int t = 0;
+            for (int i = 0; i < NP; ++i)
+                for (int j = 0; j <= i; ++j) S.JtJ[i * NP + j] = S.tot[2 + t++];
+            for (int i = 0; i < NP; ++i) S.Jtr[i] = S.tot[2 + NT + i];
+            rc = S.tot[2 + NT + NP]; // residual_count after the Jacobian pass
         }
-        if (block_bcast(&S, stop)) break;
-        lmi_eval_pass(P, L, model, S.cam_new, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
-        int brk = 0;
-        if (threadIdx.x == 0) {
-            rc = S.tot[1];
-            const double cost_new = S.tot[0] * (1.0 / fmax(1.0, rc));
-            if (cost_new < cost) {
-                const double cost_decrease = cost - cost_new;
-                for (int k = 0; k < 9; ++k) S.par[k] = S.par_new[k];
-                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = S.cam_new[c];
-                cost = cost_new;
-                recompute_jac = true;
-                const double scale = 1.0 / fmax(1.0, rc);
-                double pred = 0.0;
-                for (int i = 0; i < LMI_NP; ++i) pred += S.sol[i] * (lambda * S.sol[i] + scale * S.Jtr[i]);
-                pred = -pred;
-                if (pred > 0) {
-                    const double rho = cost_decrease / pred;
-                    const double factor = 1.0 - pow(2.0 * rho - 1.0, 3.0);
-                    lambda *= fmax(1.0 / 3.0, factor);
-                } else {
-                    lambda *= 1.0 / 3.0;
+        for (int it = 0; it < prm.max_iterations; ++it) {
+            iterations = it;
+            int stop = 0;
+            if (threadIdx.x == 0) {
+                if (recompute_jac) {
+                    double g = 0.0;
+                    for (int i = 0; i < NP; ++i) g += S.Jtr[i] * S.Jtr[i];
+                    const double grad_norm = (1.0 / fmax(1.0, rc)) * sqrt(g);
+                    if (grad_norm < prm.gradient_tol) stop = 1;
                 }
-                nu = 2.0;
-                lambda = fmax(prm.min_lambda, lambda);
-                if (cost > 0 && cost_decrease / cost < prm.relative_cost_tol) brk = 1;
-                // the Jacobian pass the reference would run next at the accepted parameters
-                int t = 0;
-                for (int i = 0; i < LMI_NP; ++i)
-                    for (int j = 0; j <= i; ++j) S.JtJ[i * LMI_NP + j] = S.tot[2 + t++];
-                for (int i = 0; i < LMI_NP; ++i) S.Jtr[i] = S.tot[2 + LMI_NT + i];
-                if (!brk && it + 1 < prm.max_iterations) rc = S.tot[2 + LMI_NT + LMI_NP];
-            } else {
-                recompute_jac = false;
-                lambda *= nu;
-                nu *= 2.0;
-                lambda = fmin(prm.max_lambda, lambda);
+                if (!stop) {
+                    const double scale = 1.0 / fmax(1.0, rc);
+                    for (int i = 0; i < NP; ++i)
+                        for (int j = 0; j <= i; ++j) S.Am[i * NP + j] = scale * S.JtJ[i * NP + j];
+                    for (int i = 0; i < NP; ++i) S.Am[i * NP + i] += lambda;
+                    for (int i = 0; i < NP; ++i) S.rhs[i] = -(scale * S.Jtr[i]);
+                    llt_solve_n(S.Am, S.rhs, S.sol, NP);
+                    double sn = 0.0;
+                    for (int i = 0; i < NP; ++i) sn += S.sol[i] * S.sol[i];
+                    if (sqrt(sn) < prm.step_tol) stop = 1;
+                }
+                if (!stop) {
+                    lm_step<KIND>(S.par, S.sol, S.tb, S.par_new);
+                    if constexpr (CAM) { // AbsolutePoseRefiner::step (optim/absolute.h:146-160)
+                        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam_new[c] = S.cam[c];
+                        for (int c = 0; c < S.m; ++c) S.cam_new[S.idx[c]] += S.sol[6 + c];
+                    }
+                    lm_build_ctx<KIND>(S.par_new, S.ctx, S.tb_new, true);
+                }
             }
-            if (it + 1 >= prm.max_iterations && !brk) iterations = it + 1;
+            if (block_bcast(&S, stop)) break;
+            eval(true);
+            int brk = 0;
+            if (threadIdx.x == 0) {
+                rc = S.tot[1]; // residual_count after the residual pass of the trial point
+                const double cost_new = S.tot[0] * (1.0 / fmax(1.0, rc));
+                if (cost_new < cost) {
+                    const double cost_decrease = cost - cost_new;
+                    for (int k = 0; k < 9; ++k) S.par[k] = S.par_new[k];
+                    for (int k = 0; k < 6; ++k) S.tb[k] = S.tb_new[k];
+                    if constexpr (CAM)
+                        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = S.cam_new[c];
+                    cost = cost_new;
+                    recompute_jac = true;
+                    const double scale = 1.0 / fmax(1.0, rc);
+                    double pred = 0.0;
+                    for (int i = 0; i < NP; ++i) pred += S.sol[i] * (lambda * S.sol[i] + scale * S.Jtr[i]);
+                    pred = -pred;
+                    if (pred > 0) {
+                        const double rho = cost_decrease / pred;
+                        const double factor = 1.0 - pow(2.0 * rho - 1.0, 3.0);
+                        lambda *= fmax(1.0 / 3.0, factor);
+                    } else {
+                        lambda *= 1.0 / 3.0;
+                    }
+                    nu = 2.0;
+                    lambda = fmax(prm.min_lambda, lambda);
+                    if (cost > 0 && cost_decrease / cost < prm.relative_cost_tol) brk = 1;
+                    // the Jacobian pass the reference would run next at the accepted parameters
+                    int t = 0;
+                    for (int i = 0; i < NP; ++i)
+                        for (int j = 0; j <= i; ++j) S.JtJ[i * NP + j] = S.tot[2 + t++];
+                    for (int i = 0; i < NP; ++i) S.Jtr[i] = S.tot[2 + NT + i];
+                    if (!brk && it + 1 < prm.max_iterations) rc = S.tot[2 + NT + NP];
+                } else {
+                    recompute_jac = false;
+                    lambda *= nu;
+                    nu *= 2.0;
+                    lambda = fmin(prm.max_lambda, lambda);
+                }
+                if (it + 1 >= prm.max_iterations && !brk) iterations = it + 1;
+            }
+            if (block_bcast(&S, brk)) break;
         }
-        if (block_bcast(&S, brk)) break;
+    }
+    // ---- output (CTA 0 of the cluster)
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        if (KIND == KIND_FUND) {
+            if (untouched) {
+                for (int k = 0; k < 9; ++k) S.par_new[k] = min[k];
+            } else {
+                const m3 F = ff_to_F(S.par);
+                for (int k = 0; k < 9; ++k) S.par_new[k] = F.a[3 * (k % 3) + k / 3];
+            }
+        } else {
+            for (int k = 0; k < MSZ; ++k) S.par_new[k] = untouched ? min[k] : S.par[k];
+            for (int k = MSZ; k < 9; ++k) S.par_new[k] = 0.0;
+        }
+        if (crank == 0) {
+            for (int k = 0; k < 9; ++k) out->model[k] = S.par_new[k];
+            out->iterations = iterations;
+            out->cost = cost;
+            out->initial_cost = initial_cost;
+            if constexpr (CAM)
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam_outs[(size_t)job * CAM_MAX_PARAMS + c] = S.cam[c];
+        }
     }
     __syncthreads();
-    if (threadIdx.x == 0 && crank == 0) {
-        for (int k = 0; k < 7; ++k) out->pose[k] = S.par[k];
-        for (int c = 0; c < CAM_MAX_PARAMS; ++c) out->cam[c] = S.cam[c];
-        out->iterations = iterations;
-        out->reserved = 0;
-        out->cost = cost;
-        out->initial_cost = initial_cost;
+    if constexpr (!CAM) {
+        if (prm.score_after && crank == 0) {
+            double mdl[9];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) mdl[k] = S.par_new[k];
+            cta_score<KIND>(P, mdl, S.sred, &out->count, &out->score);
+        }
     }
     cluster.sync(); // no CTA may exit (or start the next job) while a sibling can still read its shared memory
     } // jobs of this cluster
 }
 
-void launch_lm_intr(const ProblemDev *probs, const LmIntrJob *jobs_dev, const double *models_in, int n_jobs, int max_n,
-                    const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *out, cudaStream_t stream) {
-    if (n_jobs <= 0) return;
-    cudaFuncSetAttribute(k_lm_intr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LMI_TILE_BYTES);
-    const int csize = lm_cluster_size(n_jobs, max_n);
+// k_lm needs ~255 registers per thread: one 256-thread CTA (one job, or one slice of a job's cluster) per SM.
+static thread_local int t_lm_sm_share = 50;
+void lm_set_sm_share(int pct) { t_lm_sm_share = (pct > 0 && pct <= 100) ? pct : 50; }
+static int lm_cluster_size(int n_jobs, int max_n) {
+    static const int per_cta = [] { // correspondences per CTA before another CTA of the cluster pays off
+        const char *e = std::getenv("PLB_LM_PER_CTA");
+        const int v = e ? std::atoi(e) : 0;
+        return v > 0 ? v : 2048;
+    }();
+    int csize = (max_n + per_cta - 1) / per_cta;
+    if (csize < 1) csize = 1;
+    if (csize > LM_MAX_CLUSTER) csize = LM_MAX_CLUSTER;
+    if (csize > 4 && csize < 8) csize = 4;
+    if (csize == 3) csize = 2;
+    // k_lm needs the whole register file of an SM per CTA: with many jobs in one launch (batch groups) wide clusters
+    // only take SMs away from the co-running hypothesis kernels, so the cluster shrinks as the job count grows
+    // SMs (percent of the device) the LO clusters of one launch may cover: half when other lock-step groups share the GPU
+    // (their hypothesis kernels want the other half: +5 % on the batch workload), all of it for a call that runs alone
+    // (C4 single call 2.7 -> 2.2 ms).  PLB_LM_SM_PCT overrides.
+    static const int forced = [] {
+        const char *e = std::getenv("PLB_LM_SM_PCT");
+        const int v = e ? std::atoi(e) : 0;
+        return (v > 0 && v <= 100) ? v : 0;
+    }();
+    const int sm_share = forced ? forced : t_lm_sm_share;
+    while (csize > 1 && n_jobs * csize > sm_count() * sm_share / 100) csize /= 2;
+    return csize;
+}
+// A grid of n_clusters clusters of csize CTAs over a job list: k_lm<kind> of the fixed-camera refiner, or with
+// refine_camera the absolute pose refiner with camera parameters.
+static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs,
+                          const LoJobSrc *job_src, const double *models_in, const int *n_jobs_dev, int n_jobs,
+                          int n_clusters, int csize, const char *mask_base, int *idx_scratch, int scratch_stride,
+                          LmJobOut *out, double *cam_out, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(n_jobs * csize), 1, 1);
+    cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
     cfg.blockDim = dim3((unsigned)LM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = LMI_TILE_BYTES;
+    cfg.dynamicSmemBytes = refine_camera ? LMI_TILE_BYTES : 0;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -2688,7 +2480,42 @@ void launch_lm_intr(const ProblemDev *probs, const LmIntrJob *jobs_dev, const do
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, k_lm_intr, probs, jobs_dev, models_in, n_jobs, mask_base, idx_scratch, scratch_stride, out);
+    auto launch = [&](auto kernel) {
+        cudaLaunchKernelEx(&cfg, kernel, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
+                           scratch_stride, out, cam_out);
+    };
+    if (refine_camera) {
+        cudaFuncSetAttribute(k_lm<KIND_PNP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LMI_TILE_BYTES);
+        launch(k_lm<KIND_PNP, true>);
+    } else {
+        with_kind(kind, [&](auto K) { launch(k_lm<K, false>); });
+    }
+}
+void launch_lm(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in,
+               int n_jobs, int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out,
+               double *cam_out, cudaStream_t stream) {
+    if (n_jobs <= 0) return;
+    const int csize = lm_cluster_size(n_jobs, max_n);
+    launch_lm_any(kind, refine_camera, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base,
+                  idx_scratch, scratch_stride, out, cam_out, stream);
+}
+// Clusters of a round's LO launch: at most one wave (a k_lm CTA owns an SM), at most the estimated number of jobs.
+int lm_round_max_clusters(int kind, int est_jobs, int max_n) {
+    (void)kind;
+    if (est_jobs < 1) est_jobs = 1;
+    const int csize = lm_cluster_size(est_jobs, max_n);
+    int nc = sm_count() / csize;
+    if (nc > est_jobs) nc = est_jobs;
+    return nc < 1 ? 1 : nc;
+}
+void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const LoJobSrc *job_src,
+                     const double *models, const int *n_jobs_dev, int job_cap, int est_jobs, int max_n,
+                     int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream) {
+    if (est_jobs < 1) est_jobs = 1;
+    const int csize = lm_cluster_size(est_jobs, max_n);
+    const int nc = lm_round_max_clusters(kind, est_jobs, max_n);
+    launch_lm_any(kind, false, probs, tmpl, job_src, models, n_jobs_dev, job_cap, nc, csize, nullptr, idx_scratch,
+                  scratch_stride, out, nullptr, stream);
 }
 
 // ============================================================================================================

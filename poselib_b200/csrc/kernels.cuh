@@ -167,7 +167,8 @@ struct LmParams {
 };
 struct LmJob {
     int pidx;               // index into probs[]
-    int reserved;
+    int cam_refine;         // KIND_PNP: CAM_REFINE_* flags; a job with a non-empty cam_refine_idx(prm.cam.model, cam_refine)
+                            // refines those camera parameters with the pose (AbsolutePoseRefiner, optim/absolute.h:40-171)
     long long mask_off;     // offset into the mask buffer (subset_mode 2), else -1
     long long scratch_off;  // offset (ints) into idx_scratch for the active-point list (subset modes 1, 2)
     LmParams prm;
@@ -178,20 +179,6 @@ struct LmJobOut {
     uint32_t count;
     int iterations;
     double cost, initial_cost;
-};
-// LM job of AbsolutePoseRefiner with camera parameters (optim/absolute.h:40-171): the pose (models_in, 7 of 9 doubles)
-// and the parameters idx[0..m) of base.prm.cam are refined together; base.prm.use_camera and score_after are not read.
-struct LmIntrJob {
-    LmJob base;
-    int m;                    // 1..CAM_MAX_PARAMS
-    int idx[CAM_MAX_PARAMS];  // Camera::get_param_refinement_idx (cam_refine_idx)
-};
-struct LmIntrJobOut {
-    double pose[7];
-    double cam[CAM_MAX_PARAMS];
-    int iterations;
-    int reserved;
-    double initial_cost, cost;
 };
 // Pre-step of one problem: caller layout (AoS doubles, device copies) -> resident SoA arrays.
 //   mode 0: plain transposition (points already calibrated / normalised)
@@ -235,9 +222,11 @@ void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode
 // Exact fp64 scoring of an explicit list of n_models models (stride MSZ) with problem indices.
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
                          uint32_t *counts, double *scores, cudaStream_t stream);
-// LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.
-void launch_lm(int kind, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in, int n_jobs,
-               int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream);
+// LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.  refine_camera (KIND_PNP): every job
+// refines camera parameters with the pose (LmJob::cam_refine) and writes its camera to cam_out[j * CAM_MAX_PARAMS ..].
+void launch_lm(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in,
+               int n_jobs, int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out,
+               double *cam_out, cudaStream_t stream);
 // LO jobs of a round, listed on the device by k_pass1: job j refines model slot job_src[j].slot of the round's model
 // list (stride MSZ) with the template tmpl[job_src[j].pidx]; *n_jobs_dev jobs.  A persistent grid of clusters walks the
 // list; est_jobs (host estimate) only sizes the clusters / the grid.
@@ -245,10 +234,6 @@ void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const
                      const double *models, const int *n_jobs_dev, int job_cap, int est_jobs, int max_n,
                      int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream);
 int lm_round_max_clusters(int kind, int est_jobs, int max_n);
-// PnP LM with camera-parameter refinement: one thread-block cluster per job, models_in n_jobs * 9 doubles, idx_scratch
-// n_jobs * scratch_stride ints (subset mode 2).
-void launch_lm_intr(const ProblemDev *probs, const LmIntrJob *jobs_dev, const double *models_in, int n_jobs, int max_n,
-                    const char *mask_base, int *idx_scratch, int scratch_stride, LmIntrJobOut *out, cudaStream_t stream);
 // Share of the SMs (percent) the LO clusters launched from this host thread may cover (50: batch groups, 100: a lone call).
 void lm_set_sm_share(int pct);
 // Device-side sampling of a round: one warp per active problem draws its B samples into samples[(g0+s)*K ..] from
