@@ -61,12 +61,14 @@ enum { PLB_LOSS_TRIVIAL = 0, PLB_LOSS_TRUNCATED = 1, PLB_LOSS_HUBER = 2, PLB_LOS
 /* refine_intrinsics: BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params (types.h:92-94)
  * as a bit set.  The camera parameters they select (Camera::get_param_refinement_idx, camera_models.cc:545-561: focal
  * lengths, then principal point, then the model's extra parameters; none for the NULL camera) are refined with the pose
- * by plb_bundle_adjust_image and plb_estimate_absolute_pose_image (AbsolutePoseRefiner, optim/absolute.h:40-171).
+ * by plb_bundle_adjust_image and plb_estimate_absolute_pose_image (AbsolutePoseRefiner, optim/absolute.h:40-171), and,
+ * for each of the two cameras, by plb_refine_relpose_pair and plb_estimate_relative_pose_pair with tangent_sampson
+ * (CameraRelativePoseRefiner, bundle.cc:237-256, optim/relative.h:268-483).
  * Where the selection is non-empty the other entry points behave as follows:
  *   - ignored, as the reference ignores them: plb_bundle_adjust (NULL camera), plb_refine_relpose,
  *     plb_refine_fundamental, plb_refine_homography, plb_estimate_fundamental, plb_estimate_homography and
  *     plb_estimate_relative_pose without tangent_sampson;
- *   - PLB_ERR_NYI (CameraRelativePoseRefiner, bundle.cc:237-256): plb_refine_relpose_cameras, and
+ *   - PLB_ERR_NYI, as these cannot return the cameras: plb_refine_relpose_cameras (use plb_refine_relpose_pair), and
  *     plb_estimate_relative_pose / plb_estimate_batch with tangent_sampson when either camera's selection is non-empty;
  *   - PLB_ERR_ARG: plb_estimate_absolute_pose, which cannot return the camera (use plb_estimate_absolute_pose_image);
  *   - plb_estimate_batch refines the camera of PnP problems and writes it into camera1 (camera1 of the other problems
@@ -186,6 +188,17 @@ int plb_estimate_relative_pose(const double *x1, const double *x2, size_t n, con
                                const plb_bundle_opt *bundle, double max_error, int tangent_sampson,
                                double pose_inout[7], char *inliers, plb_ransac_stats *stats,
                                plb_counters *counters);
+/* estimate_relative_pose with the cameras in/out (robust.cc:242-314): like plb_estimate_relative_pose, and with
+ * tangent_sampson and a non-empty selection of bundle->refine_intrinsics in either camera, the final bundle adjustment
+ * (num_inliers > 5) runs CameraRelativePoseRefiner on x * scale with the rescaled cameras.  Pose, inlier mask and stats
+ * are the reference's; RANSAC itself (its LO included) keeps the cameras fixed, as the reference does.  The one addition:
+ * the refined cameras are written back to camera1_inout / camera2_inout through rescale(1 / scale); the reference
+ * computes them and discards them.  Otherwise the cameras are left untouched. */
+int plb_estimate_relative_pose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                                    plb_camera *camera2_inout, const plb_ransac_opt *ransac,
+                                    const plb_bundle_opt *bundle, double max_error, int tangent_sampson,
+                                    double pose_inout[7], char *inliers, plb_ransac_stats *stats,
+                                    plb_counters *counters);
 int plb_estimate_fundamental(const double *x1, const double *x2, size_t n, const plb_ransac_opt *ransac,
                              const plb_bundle_opt *bundle, double max_error, int real_focal_check,
                              double F_inout[9], char *inliers, plb_ransac_stats *stats, plb_counters *counters);
@@ -238,6 +251,13 @@ int plb_refine_relpose(const double *x1_xy, const double *x2_xy, size_t n, doubl
 int plb_refine_relpose_cameras(const double *x1_px, const double *x2_px, size_t n, const plb_camera *camera1,
                                const plb_camera *camera2, double pose_inout[7], const plb_bundle_opt *opt,
                                double bundle_stats_out[3]);
+/* bundle.h refine_relpose(x1, x2, ImagePair*, opt) (bundle.cc:237-256): the pose and, in each camera, the parameters
+ * opt->refine_intrinsics selects (CameraRelativePoseRefiner, separate intrinsics), pixels as given (no rescaling).  Only
+ * the refined parameters of camera1_inout / camera2_inout are written.  Where neither selection is non-empty it is
+ * plb_refine_relpose_cameras. */
+int plb_refine_relpose_pair(const double *x1_px, const double *x2_px, size_t n, plb_camera *camera1_inout,
+                            plb_camera *camera2_inout, double pose_inout[7], const plb_bundle_opt *opt,
+                            double bundle_stats_out[3]);
 int plb_refine_fundamental(const double *x1_xy, const double *x2_xy, size_t n, double F_inout[9],
                            const plb_bundle_opt *opt, double bundle_stats_out[3]);
 int plb_refine_homography(const double *x1_xy, const double *x2_xy, size_t n, double H_inout[9],

@@ -194,6 +194,8 @@ RansacStats estimate_absolute_pose(const std::vector<P2> &points2D, const std::v
     return detail::from_c<RansacStats>(st);
 }
 // estimate_relative_pose(x1, x2, camera1, camera2, RelativePoseOptions, CameraPose*, inliers*)   robust.h:68-70
+// With tangent_sampson and refine_* flags the final bundle adjustment refines the cameras too (robust.cc:262-282); like
+// the reference, the refined cameras are computed on copies and discarded.
 template <typename RansacStats, typename P2, typename Camera, typename Opt, typename Pose>
 RansacStats estimate_relative_pose(const std::vector<P2> &x1, const std::vector<P2> &x2, const Camera &camera1,
                                    const Camera &camera2, const Opt &opt, Pose *pose, std::vector<char> *inliers) {
@@ -204,9 +206,15 @@ RansacStats estimate_relative_pose(const std::vector<P2> &x1, const std::vector<
     plb_camera c1 = detail::camera_to_c(camera1), c2 = detail::camera_to_c(camera2);
     plb_ransac_stats st;
     inliers->resize(x1.size());
-    detail::check(plb_estimate_relative_pose(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, &ro, &bo,
-                                             opt.max_error, opt.tangent_sampson ? 1 : 0, m, inliers->data(), &st,
-                                             nullptr));
+    const bool refine_cameras = opt.tangent_sampson && (bo.refine_intrinsics & (PLB_REFINE_FOCAL_LENGTH |
+                                                                                  PLB_REFINE_PRINCIPAL_POINT |
+                                                                                  PLB_REFINE_EXTRA_PARAMS)) != 0;
+    detail::check(refine_cameras
+                      ? plb_estimate_relative_pose_pair(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, &ro, &bo,
+                                                        opt.max_error, 1, m, inliers->data(), &st, nullptr)
+                      : plb_estimate_relative_pose(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, &ro, &bo,
+                                                   opt.max_error, opt.tangent_sampson ? 1 : 0, m, inliers->data(), &st,
+                                                   nullptr));
     detail::pose_from(m, pose);
     return detail::from_c<RansacStats>(st);
 }
@@ -294,6 +302,22 @@ BundleStats refine_relpose(const std::vector<P2> &x1, const std::vector<P2> &x2,
     plb_bundle_opt bo = detail::bundle_to_c(opt);
     detail::check(plb_refine_relpose(detail::raw(x1), detail::raw(x2), x1.size(), m, &bo, st));
     detail::pose_from(m, pose);
+    return detail::bundle_from_c<BundleStats>(st);
+}
+// refine_relpose(x1, x2, ImagePair*, BundleOptions, weights)   robust/bundle.cc:237-256: the pose and, in each camera,
+// the parameters the refine_* flags select, pixels as given
+template <typename BundleStats, typename P2, typename ImagePair, typename BOpt>
+BundleStats refine_relpose_pair(const std::vector<P2> &x1, const std::vector<P2> &x2, ImagePair *pair, const BOpt &opt,
+                                const std::vector<double> &weights = std::vector<double>()) {
+    detail::no_weights(weights);
+    double m[7], st[3];
+    detail::pose_to(pair->pose, m);
+    plb_bundle_opt bo = detail::bundle_to_c(opt);
+    plb_camera c1 = detail::camera_to_c(pair->camera1), c2 = detail::camera_to_c(pair->camera2);
+    detail::check(plb_refine_relpose_pair(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, m, &bo, st));
+    detail::pose_from(m, &pair->pose);
+    detail::camera_from_c(c1, &pair->camera1);
+    detail::camera_from_c(c2, &pair->camera2);
     return detail::bundle_from_c<BundleStats>(st);
 }
 // refine_fundamental(x1, x2, Matrix3d*, BundleOptions, weights)   robust/bundle.h:132-134

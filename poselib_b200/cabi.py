@@ -97,10 +97,10 @@ EXPORTS = [
     "plb_ransac_opt_default", "plb_bundle_opt_default", "plb_last_error", "plb_device_count", "plb_set_device",
     "plb_set_mode", "plb_host_sample_table", "plb_device_sample_table", "plb_host_dynamic_max_iter", "plb_ransac_pnp", "plb_ransac_relpose", "plb_ransac_relpose_cameras", "plb_ransac_fundamental",
     "plb_ransac_homography",
-    "plb_estimate_absolute_pose", "plb_estimate_relative_pose", "plb_estimate_fundamental",
+    "plb_estimate_absolute_pose", "plb_estimate_relative_pose", "plb_estimate_relative_pose_pair", "plb_estimate_fundamental",
     "plb_estimate_homography", "plb_p3p_batch", "plb_p3p_lambdatwist_batch", "plb_relpose_5pt_batch", "plb_relpose_5pt_poses_batch",
     "plb_relpose_7pt_batch", "plb_homography_4pt_batch", "plb_essential_matrix_8pt_batch", "plb_relpose_8pt_batch", "plb_ransac_batch", "plb_ransac_batch_multi", "plb_estimate_batch", "plb_bundle_adjust",
-    "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
+    "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_relpose_pair", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
     "plb_resident_free",
 ]
 
@@ -293,6 +293,25 @@ def estimate_image(x, X, cam, ropt, bopt, max_error, init=None):
             "counters": cn.as_dict()}
 
 
+def estimate_relative_pose_pair(x1, x2, cam1, cam2, ropt, bopt, max_error, tangent_sampson=True, init=None):
+    """estimate_relative_pose with the cameras in/out: with tangent_sampson, bopt.refine_intrinsics selects camera
+    parameters the final bundle adjustment refines with the pose.  Returns dict(model, camera1, camera2 [the models'
+    parameters], inliers, stats, counters); cam1 / cam2 are not modified."""
+    n = len(x1)
+    aa, ap = _d(x1)
+    ba, bp = _d(x2)
+    mask = np.zeros(max(n, 1), dtype=np.int8)
+    st, cn = RansacStats(), Counters()
+    m = _init_model("relpose", init)
+    c1, c2 = _copy_camera(cam1), _copy_camera(cam2)
+    _check(_lib.plb_estimate_relative_pose_pair(ap, bp, C.c_size_t(n), C.byref(c1), C.byref(c2), C.byref(ropt),
+                                                C.byref(bopt), C.c_double(max_error), int(tangent_sampson),
+                                                m.ctypes.data_as(_P), mask.ctypes.data_as(C.c_char_p), C.byref(st),
+                                                C.byref(cn)))
+    return {"model": m, "camera1": _camera_params(c1), "camera2": _camera_params(c2), "inliers": mask[:n],
+            "stats": st.as_dict(), "counters": cn.as_dict()}
+
+
 def refine_image(pose, x, X, cam, bopt):
     """bundle_adjust(x, X, Image*, opt) (robust/bundle.h:47): points in the camera's pixel units, bopt.refine_intrinsics
     selects the camera parameters refined with the pose.  Returns (pose, camera parameters, [iterations, initial_cost,
@@ -306,6 +325,21 @@ def refine_image(pose, x, X, cam, bopt):
     _check(_lib.plb_bundle_adjust_image(ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(c), C.byref(bopt),
                                         bs.ctypes.data_as(_P)))
     return m, _camera_params(c), bs
+
+
+def refine_relpose_pair(pose, x1, x2, cam1, cam2, bopt):
+    """refine_relpose(x1, x2, ImagePair*, opt) (bundle.cc:237-256): pixels as given, bopt.refine_intrinsics selects the
+    parameters of each camera refined with the pose.  Returns (pose, camera 1 parameters, camera 2 parameters,
+    [iterations, initial_cost, cost]); cam1 / cam2 are not modified."""
+    n = len(x1)
+    aa, ap = _d(x1)
+    ba, bp = _d(x2)
+    m = _init_model("relpose", pose)
+    c1, c2 = _copy_camera(cam1), _copy_camera(cam2)
+    bs = np.zeros(3)
+    _check(_lib.plb_refine_relpose_pair(ap, bp, C.c_size_t(n), C.byref(c1), C.byref(c2), m.ctypes.data_as(_P),
+                                        C.byref(bopt), bs.ctypes.data_as(_P)))
+    return m, _camera_params(c1), _camera_params(c2), bs
 
 
 def refine(kind, model, a, b, bopt):

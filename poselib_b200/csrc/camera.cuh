@@ -353,4 +353,20 @@ PLB_HD void cam_unproject_with_jac(const CamDev &c, double u, double v, double *
         for (int q = 0; q < 2; ++q) M[2 * i + q] = J[i] * Bi[q] + J[3 + i] * Bi[2 + q];
 }
 
+// default <Model>::unproject_with_jac with jac_params (camera_models.cc:456-489): d, M as above and
+// dp = d(bearing) / d(params), 3 x CAM_MAX_PARAMS row-major, = -M * jac_params of project_with_jac at d; columns past
+// the model's parameter count are left untouched.  The reference has two orders: -(J^T B^-1) Jp with a jac_point
+// (:480-483) and -J^T B^-1 Jp without (:486-488).  Negation is exact and commutes with every rounding, so both give
+// these bits.
+PLB_HD void cam_unproject_with_jac_params(const CamDev &c, double u, double v, double *d, double *M, double *dp) {
+    cam_unproject_with_jac(c, u, v, d, M);
+    double jp[2 * CAM_MAX_PARAMS];
+    cam_jac_params(c, d[0], d[1], d[2], jp);
+    const int np = c.model == CAMM_NULL ? 0 : c.model == CAMM_SIMPLE_PINHOLE ? 3 : c.model == CAMM_RADIAL ? 5
+                   : c.model == CAMM_OPENCV ? 8 : 4;
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < np; ++j)
+            dp[CAM_MAX_PARAMS * i + j] = (-M[2 * i]) * jp[j] + (-M[2 * i + 1]) * jp[CAM_MAX_PARAMS + j];
+}
+
 } // namespace plb

@@ -439,13 +439,16 @@ struct FinalPolish { // the post-RANSAC refinement of PoseLib/robust.cc (estimat
     bool enabled = false;
     plb_bundle_opt bundle;
     size_t min_inliers = 0; // run iff stats.num_inliers > min_inliers
-    // pnp only: refine in pixel*scale coordinates with the rescaled camera (robust.cc:103-123)
-    const double *px_scaled = nullptr; // 2n doubles (AoS) or null
+    // pnp: refine in pixel*scale coordinates with the rescaled camera (robust.cc:103-123); relpose tangent Sampson with
+    // camera refinement: x1*scale (px_scaled) and x2*scale (px2_scaled), the pixels the problem's arrays come from
+    // (robust.cc:255-282).  2n doubles (AoS) each, or null
+    const double *px_scaled = nullptr, *px2_scaled = nullptr;
     CamDev cam{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
-    // pnp, Image* form: CAM_REFINE_* flags of the camera parameters refined with the pose (LmJob::cam_refine), and cam_out
-    // receives the camera after the polish, rescaled back by 1 / scale (robust.cc:103-123)
+    // Image* / ImagePair* forms: CAM_REFINE_* flags of the camera parameters refined with the pose (LmJob::cam_refine),
+    // and cam_out receives the camera (relpose: both cameras, from Task::cam_a / cam_b) after the polish, rescaled back by
+    // 1 / scale (robust.cc:103-123)
     int cam_refine = 0;
-    plb_camera *cam_out = nullptr;
+    plb_camera *cam_out = nullptr, *cam2_out = nullptr;
     double scale = 1.0;
 };
 
@@ -586,7 +589,6 @@ static bool refines_camera(const CamDev &c, int flags) {
     int idx[CAM_MAX_PARAMS];
     return cam_refine_idx(c.model, flags, idx) > 0;
 }
-static bool refines_camera(const LmJob &J) { return refines_camera(J.prm.cam, J.cam_refine); }
 static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
     LmJob J;
     J.pidx = pidx;
@@ -602,18 +604,17 @@ static bool profiling() {
     return on;
 }
 
-// The camera after the polish of estimate_absolute_pose: the (refined) parameters of the rescaled camera, rescaled by
-// 1 / scale (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
+// The camera after the polish of estimate_absolute_pose: the (refined) parameters of the rescaled camera `cam`, rescaled
+// by 1 / scale into `out` (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
 static void camera_rescale(CamDev &c, double scale);
-static void polish_camera_out(const FinalPolish &fp, const double *params) {
-    CamDev c = fp.cam;
+static void polish_camera_out(CamDev c, double scale, const double *params, plb_camera *out) {
     for (int i = 0; i < CAM_MAX_PARAMS; ++i) c.p[i] = params[i];
-    camera_rescale(c, 1.0 / fp.scale);
-    const int np = fp.cam_out->model_id == PLB_CAMERA_SIMPLE_PINHOLE ? 3
-                   : fp.cam_out->model_id == PLB_CAMERA_RADIAL   ? 5
-                   : fp.cam_out->model_id == PLB_CAMERA_OPENCV   ? 8
-                                                                 : 4;
-    for (int i = 0; i < np; ++i) fp.cam_out->params[i] = c.p[i];
+    camera_rescale(c, 1.0 / scale);
+    const int np = out->model_id == PLB_CAMERA_SIMPLE_PINHOLE ? 3
+                   : out->model_id == PLB_CAMERA_RADIAL   ? 5
+                   : out->model_id == PLB_CAMERA_OPENCV   ? 8
+                                                          : 4;
+    for (int i = 0; i < np; ++i) out->params[i] = c.p[i];
 }
 
 // A group of problems of the same kind, run in lock-step rounds: one solve launch, one score launch and one LM launch
@@ -737,6 +738,7 @@ struct Group {
                 px_elems += 2 * (size_t)S.n_pad;
                 ++n_polish_pnp;
             }
+            if (kind == KIND_RELPOSE_TS && S.t->polish.px_scaled) px_elems += 4 * (size_t)S.n_pad;
         }
         n_probdev = NP + n_polish_pnp;
         if ((rc = E.h_in.ensure(in_doubles + px_elems)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
@@ -759,6 +761,7 @@ struct Group {
             PState &S = PS[i];
             ProblemDev &P = E.h_probs.p[i];
             std::memset(&P, 0, sizeof(P));
+            P.cam[0].model = P.cam[1].model = CAMM_NULL;
             P.n = S.n;
             P.kind = kind;
             P.sq_thr = S.t->max_error * S.t->max_error;
@@ -824,6 +827,19 @@ struct Group {
                 PP.p[1] = E.px64.p + px_off + S.n_pad;
                 px_off += 2 * (size_t)S.n_pad;
                 ++ipol;
+            }
+            if (kind == KIND_RELPOSE_TS && S.t->polish.px_scaled) {
+                // the pixels of both images as SoA for the camera-refining refiner, with the cameras of the pre-step
+                double *hp = E.h_in.p + in_doubles + px_off;
+                const double *src[2] = {S.t->polish.px_scaled, S.t->polish.px2_scaled};
+                for (int c = 0; c < 4; ++c) {
+                    for (int k = 0; k < S.n; ++k) hp[c * (size_t)S.n_pad + k] = src[c >> 1][2 * k + (c & 1)];
+                    for (int k = S.n; k < S.n_pad; ++k) hp[c * (size_t)S.n_pad + k] = 0.0;
+                    P.p[c] = E.px64.p + px_off + c * (size_t)S.n_pad;
+                }
+                P.cam[0] = S.t->cam_a;
+                P.cam[1] = S.t->cam_b;
+                px_off += 4 * (size_t)S.n_pad;
             }
         }
         // The lock-step groups of a batch call start together; left alone, their host->device copies interleave on the
@@ -906,17 +922,25 @@ struct Group {
     }
 
     // Stages a batch of LM jobs (job j: start model batch[j].model, results in E.h_lm_out[j]) and launches one k_lm per
-    // refiner: the jobs that refine the camera come last and write it to row j of E.h_cam_out.  The caller synchronises.
+    // refiner: the jobs that refine the camera come last and write their kind_cam_count(kind) cameras to row j of
+    // E.h_cam_out.  The caller synchronises.
+    // A job refines camera parameters when the flags select some of its camera (PnP: prm.cam) or cameras (tangent
+    // Sampson: the problem's two cameras, ProblemDev::cam)
+    bool refines_camera(const LmJob &J) const {
+        if (kind != KIND_RELPOSE_TS) return plb::refines_camera(J.prm.cam, J.cam_refine);
+        const ProblemDev &P = E.h_probs.p[J.pidx];
+        return plb::refines_camera(P.cam[0], J.cam_refine) || plb::refines_camera(P.cam[1], J.cam_refine);
+    }
     int lm_batch(const std::vector<LmTask> &batch) {
-        const int nj = (int)batch.size();
+        const int nj = (int)batch.size(), nc = kind_cam_count(kind);
         const int n_fixed = (int)(std::partition_point(batch.begin(), batch.end(),
-                                                       [](const LmTask &t) { return !refines_camera(t.job); }) -
+                                                       [&](const LmTask &t) { return !refines_camera(t.job); }) -
                                   batch.begin());
         int rc;
         if ((rc = E.h_lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_jobs.ensure(nj)) || (rc = E.jobs.ensure(nj)) ||
             (rc = E.lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_lm_out.ensure(nj)) ||
             (rc = E.subset.ensure((size_t)nj * max_n_pad)) ||
-            (n_fixed < nj && (rc = E.h_cam_out.ensure((size_t)nj * CAM_MAX_PARAMS))))
+            (n_fixed < nj && (rc = E.h_cam_out.ensure((size_t)nj * nc * CAM_MAX_PARAMS))))
             return rc;
         for (int j = 0; j < nj; ++j) {
             double *row = E.h_lm_in.p + 9 * (size_t)j;
@@ -932,10 +956,10 @@ struct Group {
             const int j0 = cam ? n_fixed : 0, n = cam ? nj - n_fixed : n_fixed;
             if (n == 0) continue;
             launch_lm(kind, cam, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
-                      max_n_pad, E.h_lm_out.d + j0, cam ? E.h_cam_out.d + (size_t)j0 * CAM_MAX_PARAMS : nullptr, st);
+                      max_n_pad, E.h_lm_out.d + j0, cam ? E.h_cam_out.d + (size_t)j0 * nc * CAM_MAX_PARAMS : nullptr, st);
             E.launches++;
         }
-        d2h += sizeof(LmJobOut) * nj + sizeof(double) * CAM_MAX_PARAMS * (nj - n_fixed);
+        d2h += sizeof(LmJobOut) * nj + sizeof(double) * nc * CAM_MAX_PARAMS * (nj - n_fixed);
         return PLB_OK;
     }
     LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
@@ -1416,10 +1440,19 @@ struct Group {
         PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
         if ((rc = sync())) return rc;
         for (size_t j = 0; j < pol.size(); ++j) {
-            const FinalPolish &fp = pol_of[j]->t->polish;
+            const Task &t = *pol_of[j]->t;
+            const FinalPolish &fp = t.polish;
             std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
-            if (fp.cam_out)
-                polish_camera_out(fp, refines_camera(pol[j].job) ? E.h_cam_out.p + j * CAM_MAX_PARAMS : fp.cam.p);
+            const bool refined = refines_camera(pol[j].job);
+            const double *cams = refined ? E.h_cam_out.p + j * kind_cam_count(kind) * CAM_MAX_PARAMS : nullptr;
+            if (kind == KIND_RELPOSE_TS) { // the pair's refined cameras (only where the polish refined them)
+                if (fp.cam_out && refined) {
+                    polish_camera_out(t.cam_a, fp.scale, cams, fp.cam_out);
+                    polish_camera_out(t.cam_b, fp.scale, cams + CAM_MAX_PARAMS, fp.cam2_out);
+                }
+            } else if (fp.cam_out) {
+                polish_camera_out(fp.cam, fp.scale, refined ? cams : fp.cam.p, fp.cam_out);
+            }
         }
         for (PState &S : PS) {
             if (S.t->inliers && S.n > 0) {
@@ -1521,11 +1554,13 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 // One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
 // group (sq_thr 0, no normalisation, no pre-step beyond the cameras), then one LM job over every point.
 // PnP on an Image (bundle.cc:95-112): `proj` is the camera the points are projected with; the parameters the flags
-// cam_refine select are refined with the pose and written to proj_out.
+// cam_refine select are refined with the pose and written to params_out[0].
+// Tangent Sampson on an ImagePair (bundle.cc:237-256): the parameters of cam_a / cam_b the flags select are refined with
+// the pose and written to params_out[0] / params_out[1]; without a selection it is the fixed-camera refiner.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cam_a = nullptr,
                       const CamDev *cam_b = nullptr, const CamDev *proj = nullptr, int cam_refine = 0,
-                      double *proj_out = nullptr) {
+                      double *const *params_out = nullptr) {
     if (n_pts == 0) return PLB_OK;
     Task t;
     t.kind = kind;
@@ -1534,6 +1569,11 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     t.n = n_pts;
     if (cam_a) t.cam_a = *cam_a;
     if (cam_b) t.cam_b = *cam_b;
+    const bool pair_refined = kind == KIND_RELPOSE_TS && (refines_camera(t.cam_a, cam_refine) || refines_camera(t.cam_b, cam_refine));
+    if (pair_refined) { // the pixels as given (no rescaling)
+        t.polish.px_scaled = a;
+        t.polish.px2_scaled = b;
+    }
     std::vector<Task *> v{&t};
     Group G(kind, v);
     int rc;
@@ -1551,9 +1591,13 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     PLB_CUDA(cudaGetLastError());
     const LmJobOut &o = G.E.h_lm_out.p[0];
     std::copy(o.model, o.model + G.MSZ, model);
-    int idx[CAM_MAX_PARAMS];
-    const int m = cam_refine_idx(prm.cam.model, cam_refine, idx);
-    for (int c = 0; c < m; ++c) proj_out[idx[c]] = G.E.h_cam_out.p[idx[c]];
+    const CamDev *cams[2] = {kind == KIND_PNP ? &prm.cam : &t.cam_a, &t.cam_b};
+    if (kind == KIND_PNP || pair_refined)
+        for (int i = 0; i < kind_cam_count(kind); ++i) {
+            int idx[CAM_MAX_PARAMS];
+            const int m = cam_refine_idx(cams[i]->model, cam_refine, idx);
+            for (int c = 0; c < m; ++c) params_out[i][idx[c]] = G.E.h_cam_out.p[i * CAM_MAX_PARAMS + idx[c]];
+        }
     if (bstats) {
         bstats[0] = o.iterations;
         bstats[1] = o.initial_cost;
@@ -1783,7 +1827,7 @@ int plb_ransac_homography(const double *x1, const double *x2, size_t n, const pl
 struct EstimateJob {
     Task t;
     int api_kind = 0; // PLB_KIND_*
-    std::vector<double> px;
+    std::vector<double> px, px2;
     HM3 T1, T2;
     bool normalised = false;
     double *model = nullptr;
@@ -1809,7 +1853,8 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
                             const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                             double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
                             plb_ransac_stats *stats, plb_counters *counters, EstimateJob &J,
-                            plb_camera *camera_out = nullptr, int cam_ret = CAM_RET_NONE) {
+                            plb_camera *camera_out = nullptr, int cam_ret = CAM_RET_NONE,
+                            plb_camera *camera2_out = nullptr) {
     if (int r = check_ptrs(x1, x2, ransac, model, n)) return r;
     if (!bundle) {
         g_err = "null bundle options";
@@ -1864,8 +1909,9 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         CamDev c1, c2;
         if (int r = camera_dev(camera1, &c1)) return r;
         if (int r = camera_dev(camera2, &c2)) return r;
-        if (tangent_sampson && (refines_camera(c1, refine_flags(bundle)) || refines_camera(c2, refine_flags(bundle)))) {
-            g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
+        const bool refined = tangent_sampson && (refines_camera(c1, refine_flags(bundle)) || refines_camera(c2, refine_flags(bundle)));
+        if (refined && !camera2_out) {
+            g_err = "NYI: camera refinement needs cameras to return: use plb_estimate_relative_pose_pair";
             return PLB_ERR_NYI;
         }
         const double scale = 0.5 * (1.0 / camera_focal(c1) + 1.0 / camera_focal(c2));
@@ -1880,6 +1926,20 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             t.kind = KIND_RELPOSE_TS;
             t.pre_mode = 2;
             t.pre_scale = scale;
+            if (refined) { // the polish refines the cameras on x * scale with the rescaled cameras (robust.cc:262-282)
+                J.px.resize(2 * n);
+                J.px2.resize(2 * n);
+                for (size_t k = 0; k < 2 * n; ++k) {
+                    J.px[k] = x1[k] * scale;
+                    J.px2[k] = x2[k] * scale;
+                }
+                fp.px_scaled = J.px.data();
+                fp.px2_scaled = J.px2.data();
+                fp.cam_refine = refine_flags(bundle);
+                fp.scale = scale;
+                fp.cam_out = camera_out;
+                fp.cam2_out = camera2_out;
+            }
         } else {
             t.kind = KIND_RELPOSE;
             t.pre_mode = (c1.model != CAMM_NULL || c2.model != CAMM_NULL) ? 1 : 0;
@@ -1921,10 +1981,10 @@ static int estimate_single(int kind, const double *x1, const double *x2, size_t 
                            const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                            double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
                            plb_ransac_stats *stats, plb_counters *counters, plb_camera *camera_out = nullptr,
-                           int cam_ret = CAM_RET_NONE) {
+                           int cam_ret = CAM_RET_NONE, plb_camera *camera2_out = nullptr) {
     EstimateJob J;
     if (int r = estimate_prepare(kind, x1, x2, n, camera1, camera2, ransac, bundle, max_error, real_focal_check,
-                                 tangent_sampson, model, inliers, stats, counters, J, camera_out, cam_ret))
+                                 tangent_sampson, model, inliers, stats, counters, J, camera_out, cam_ret, camera2_out))
         return r;
     if (J.t.skip) return PLB_OK;
     std::vector<Task *> v{&J.t};
@@ -1958,6 +2018,21 @@ int plb_estimate_relative_pose(const double *x1, const double *x2, size_t n, con
                                plb_ransac_stats *stats, plb_counters *counters) {
     return estimate_single(PLB_KIND_RELPOSE, x1, x2, n, camera1, camera2, ransac, bundle, max_error, 0, tangent_sampson,
                            pose, inliers, stats, counters);
+}
+// robust.cc:242-314 with the ImagePair of the reference: like plb_estimate_relative_pose, and with tangent_sampson the
+// final bundle adjustment also refines the parameters bundle->refine_intrinsics selects in either camera, which are then
+// written back (the one addition to the reference, which computes them and discards them).
+int plb_estimate_relative_pose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                                    plb_camera *camera2_inout, const plb_ransac_opt *ransac,
+                                    const plb_bundle_opt *bundle, double max_error, int tangent_sampson,
+                                    double pose[7], char *inliers, plb_ransac_stats *stats, plb_counters *counters) {
+    if (!camera1_inout || !camera2_inout) {
+        g_err = "null camera";
+        return PLB_ERR_ARG;
+    }
+    return estimate_single(PLB_KIND_RELPOSE, x1, x2, n, camera1_inout, camera2_inout, ransac, bundle, max_error, 0,
+                           tangent_sampson, pose, inliers, stats, counters, camera1_inout, CAM_RET_REFINED,
+                           camera2_inout);
 }
 int plb_estimate_fundamental(const double *x1, const double *x2, size_t n, const plb_ransac_opt *ransac,
                              const plb_bundle_opt *bundle, double max_error, int real_focal_check, double F[9],
@@ -2000,7 +2075,7 @@ int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, con
     if (int r = camera_dev(camera1, &c1)) return r;
     if (int r = camera_dev(camera2, &c2)) return r;
     if (refines_camera(c1, refine_flags(opt)) || refines_camera(c2, refine_flags(opt))) {
-        g_err = "NYI: camera refinement in the relative pose bundle adjustment (CameraRelativePoseRefiner)";
+        g_err = "NYI: camera refinement needs cameras to return: use plb_refine_relpose_pair";
         return PLB_ERR_NYI;
     }
     return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, &c1, &c2);
@@ -2014,7 +2089,22 @@ int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double p
     }
     CamDev cam;
     if (int r = camera_dev(camera_inout, &cam)) return r;
-    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, refine_flags(opt), camera_inout->params);
+    double *out[1] = {camera_inout->params};
+    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, refine_flags(opt), out);
+}
+// robust/bundle.cc:237-256: refine_relpose(x1, x2, ImagePair*, opt), CameraRelativePoseRefiner with the parameters the
+// flags select in either camera (shared_camera false); pixels as given, only the refined parameters written
+int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                            plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
+    if (!opt || !pose || !camera1_inout || !camera2_inout || (n > 0 && (!x1 || !x2))) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    CamDev c1, c2;
+    if (int r = camera_dev(camera1_inout, &c1)) return r;
+    if (int r = camera_dev(camera2_inout, &c2)) return r;
+    double *out[2] = {camera1_inout->params, camera2_inout->params};
+    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, &c1, &c2, nullptr, refine_flags(opt), out);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {

@@ -1760,18 +1760,33 @@ template <int NP> struct JacAcc {
     }
 };
 
-// The refiner with camera parameters (AbsolutePoseRefiner with a non-empty camera_refine_idx, optim/absolute.h:40-171):
-// the pose (6) and m <= CAM_MAX_PARAMS camera parameters, padded to LMI_NP.  The padded rows and columns of JtJ and Jtr
-// are zero, their damped diagonal is lambda and their step component zero, so the Cholesky solve, the step, its norm
-// and the predicted decrease are those of the (6 + m)-dimensional system.
-constexpr int LMI_NP = 6 + CAM_MAX_PARAMS;
-constexpr int LMI_NT = LMI_NP * (LMI_NP + 1) / 2;
-constexpr int LMI_NV = 2 + LMI_NT + LMI_NP + 1; // [loss, residual rows, JtJ (packed lower, row-major), Jtr, jac rows]
-static_assert(LMI_NV <= LM_THREADS, "one owner thread per reduced value");
-// Tile row of one point: Jacobian row u (LMI_NP) | row v (LMI_NP) | w*r_u | w*r_v | w | loss | residual row | jac row
-// | jac_params of the point (2 x CAM_MAX_PARAMS, staging for the column selection)
-enum { LMI_WR0 = 2 * LMI_NP, LMI_WR1, LMI_WT, LMI_LOSS, LMI_ROW, LMI_JROW, LMI_JP, LMI_W = LMI_JP + 2 * CAM_MAX_PARAMS };
-constexpr size_t LMI_TILE_BYTES = sizeof(double) * LMI_W * LM_THREADS;
+// The refiners with camera parameters: the pose and, per camera, m <= CAM_MAX_PARAMS parameters, padded to NP.
+//   KIND_PNP        AbsolutePoseRefiner with a non-empty camera_refine_idx (optim/absolute.h:40-171): pose 6, one
+//                   camera, a 2-dim residual per point
+//   KIND_RELPOSE_TS CameraRelativePoseRefiner, shared_intrinsics false (optim/relative.h:268-483, bundle.cc:249-254):
+//                   rotation 3, tangent translation 2, camera 1 then camera 2, a 1-dim residual per point
+// The padded rows and columns of JtJ and Jtr are zero, their damped diagonal is lambda and their step component zero, so
+// the Cholesky solve, the step, its norm and the predicted decrease are those of the unpadded system.
+// Tile row of one point: R Jacobian rows (NP each) | w*r (R) | w | loss | residual row | jac row | staging (STAGE):
+//   PnP : jac_params of the point (2 x CAM_MAX_PARAMS)
+//   TS  : jac_params of unproject_with_jac at x1, at x2 and at the finite-difference point (3 x 3 x CAM_MAX_PARAMS)
+template <int KIND> struct LmCamDims;
+template <> struct LmCamDims<KIND_PNP> {
+    static constexpr int NPOSE = 6, NCAM = 1, R = 2, STAGE = 2 * CAM_MAX_PARAMS, CTX = 12;
+};
+template <> struct LmCamDims<KIND_RELPOSE_TS> {
+    static constexpr int NPOSE = 5, NCAM = 2, R = 1, STAGE = 9 * CAM_MAX_PARAMS, CTX = 9 + 45;
+};
+template <int KIND> struct LmCamLayout : LmCamDims<KIND> {
+    using D = LmCamDims<KIND>;
+    static constexpr int NP = D::NPOSE + D::NCAM * CAM_MAX_PARAMS;
+    static constexpr int NT = NP * (NP + 1) / 2;
+    static constexpr int NV = 2 + NT + NP + 1; // [loss, residual rows, JtJ (packed lower, row-major), Jtr, jac rows]
+    static constexpr int WR = D::R * NP, WT = WR + D::R, LOSS = WT + 1, ROW = LOSS + 1, JROW = ROW + 1, JP = JROW + 1,
+                         W = JP + D::STAGE;
+    static constexpr size_t TILE_BYTES = sizeof(double) * W * LM_THREADS;
+    static_assert(NV <= LM_THREADS, "one owner thread per reduced value");
+};
 
 // Shared memory of one k_lm CTA that both refiners use: the parameters, the scalar LM state of thread 0 (JtJ and its
 // damped copy Am NP x NP row-major, lower triangle used) and the cluster reduction of NV values.
@@ -1790,13 +1805,14 @@ template <int NP> struct LmShared : LmCore<NP, LM_NV_MAX> {
     double red[LM_WARPS][LM_NV_MAX];
     ScoreRed<1> sred;
 };
-// camera refinement: the camera parameters of par / par_new and the refined indices idx[0..m); the tile rows of
-// lmi_eval_pass are dynamic shared memory
-struct LmCamShared : LmCore<LMI_NP, LMI_NV> {
-    double ctx[12];
-    double cam[CAM_MAX_PARAMS], cam_new[CAM_MAX_PARAMS];
-    int idx[CAM_MAX_PARAMS];
-    int m;
+// camera refinement: the camera parameters of par / par_new and the refined indices idx[i][0..m[i]) of every camera;
+// the tile rows of lmi_eval_pass are dynamic shared memory
+template <int KIND> struct LmCamShared : LmCore<LmCamLayout<KIND>::NP, LmCamLayout<KIND>::NV> {
+    static constexpr int NC = LmCamDims<KIND>::NCAM;
+    double ctx[LmCamDims<KIND>::CTX];
+    double cam[NC][CAM_MAX_PARAMS], cam_new[NC][CAM_MAX_PARAMS];
+    int idx[NC][CAM_MAX_PARAMS];
+    int m[NC];
 };
 
 // Cluster totals of the CTA partial sums S->sums[buf][0..nv) -> S->tot[0..nv) in every CTA, CTAs in rank order.
@@ -2017,120 +2033,252 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn
     cluster_sum<NV>(S, v, buf, csize);
 }
 
-// One evaluation pass at the pose whose context is in S->ctx and the camera parameters cp: robust cost and residual
-// rows (compute_residual, <Model>::project) and JtJ, Jtr, jacobian rows (compute_jacobian, <Model>::project_with_jac
-// with jac_params) -> S->tot, in lm_eval_pass's layout.  Every 256 points each thread writes its point's row of the tile;
-// thread e < LMI_NV then adds value e of every row in point order.  Order of the sums: points in order inside a CTA, CTAs
-// in rank order (deterministic for a given cluster size).
-PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, int model, const double *cp, int m, const int *idx,
-                           const int *list, int lo, int na, LmCamShared *S, double *tile, int &buf, int csize) {
-    const double *ctx = S->ctx;
-    CamDev cam;
-    cam.model = model;
-    cam.reserved = 0;
+// Tangent-Sampson row of one correspondence for CameraRelativePoseRefiner::compute_jacobian (optim/relative.h:333-437):
+// the pose columns tr[0..5) and the camera columns tr[5 ..) of the tile row, from the pixels (a0, a1), (b0, b1), the
+// bearings d1, d2 and the unprojection Jacobians M1, M2 at cameras c1, c2, C and J_C of tangent_terms.  The jac_params
+// of both points are staged at st (d1_p) and st + 3 * CAM_MAX_PARAMS (d2_p); st + 6 * CAM_MAX_PARAMS is the scratch of
+// the finite-difference points.  Operation order of the reference on mini-Eigen (products and dots left to right).
+template <int NP>
+PLB_DEV void ts_cam_row(const double *E, const double *D, const CamDev &c1, const CamDev &c2, double a0, double a1,
+                        double b0, double b1, const double *d1, const double *d2, const double *M1, const double *M2,
+                        double C, const double *JC, const int (*idx)[CAM_MAX_PARAMS], const int *m, double *st,
+                        double *tr) {
+    const double nJ_C = sqrt((JC[0] * JC[0] + JC[2] * JC[2]) + (JC[1] * JC[1] + JC[3] * JC[3]));
+    const double inv = 1.0 / nJ_C;
+    const double s = C * inv * inv;
+    {
+        double dF[9];
 #pragma unroll
-    for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam.p[c] = cp[c];
+        for (int c = 0; c < 3; ++c)
+#pragma unroll
+            for (int rr = 0; rr < 3; ++rr) {
+                double e = d1[c] * d2[rr];
+                e -= s * (JC[0] * M1[2 * c] * d2[rr] + JC[1] * M1[2 * c + 1] * d2[rr] + JC[2] * M2[2 * rr] * d1[c] +
+                          JC[3] * M2[2 * rr + 1] * d1[c]);
+                dF[3 * c + rr] = e * inv;
+            }
+#pragma unroll
+        for (int p = 0; p < 5; ++p) {
+            double t = 0.0;
+#pragma unroll
+            for (int q = 0; q < 9; ++q) t += dF[q] * D[5 * q + p];
+            tr[p] = t;
+        }
+    }
+    constexpr double eps = 1e-6;
+    const double sig = (-s) * inv; // -s * inv_nJ_C of J_M11 .. J_M22
+    double *tmp = st + 6 * CAM_MAX_PARAMS;
+    int col = 5;
+#pragma unroll 1
+    for (int cam = 0; cam < 2; ++cam) {
+        // this camera's point d, its partner's point e, its M and the partner's M: J_d = (e^T G - s (d^T G^T Mo Mo^T G)) inv
+        // with G = E (camera 1) or E^T (camera 2); J_Mq = sig * Mc.col(q)^T G^T e e^T G
+        const double *d = cam ? d2 : d1, *e = cam ? d1 : d2, *Mc = cam ? M2 : M1, *Mo = cam ? M1 : M2;
+        auto G = [&](int r, int c) { return cam ? E[3 * c + r] : E[3 * r + c]; };
+        double Jd[3], JM[2][3];
+        {
+            double a[3], b[2], c[3];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) a[j] = d[0] * G(j, 0) + d[1] * G(j, 1) + d[2] * G(j, 2); // d^T G^T
+#pragma unroll
+            for (int q = 0; q < 2; ++q) b[q] = a[0] * Mo[q] + a[1] * Mo[2 + q] + a[2] * Mo[4 + q];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) c[j] = b[0] * Mo[2 * j] + b[1] * Mo[2 * j + 1];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                const double eg = e[0] * G(0, j) + e[1] * G(1, j) + e[2] * G(2, j);
+                const double cg = c[0] * G(0, j) + c[1] * G(1, j) + c[2] * G(2, j);
+                Jd[j] = (eg - s * cg) * inv;
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            double g[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) g[k] = sig * Mc[2 * k + q];
+            double h[3];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) h[j] = g[0] * G(j, 0) + g[1] * G(j, 1) + g[2] * G(j, 2); // (..) G^T
+            const double hs = h[0] * e[0] + h[1] * e[1] + h[2] * e[2];
+            double u[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) u[k] = hs * e[k];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) JM[q][j] = u[0] * G(0, j) + u[1] * G(1, j) + u[2] * G(2, j);
+        }
+        const CamDev &cc = cam ? c2 : c1;
+        const double *dp = st + 3 * CAM_MAX_PARAMS * cam;
+        const double x0 = cam ? b0 : a0, x1 = cam ? b1 : a1;
+        for (int i = 0; i < m[cam]; ++i) {
+            const int j = idx[cam][i];
+            tr[col + i] = Jd[0] * dp[j] + Jd[1] * dp[CAM_MAX_PARAMS + j] + Jd[2] * dp[2 * CAM_MAX_PARAMS + j];
+        }
+#pragma unroll 1
+        for (int q = 0; q < 2; ++q) { // x + eps e_q: dp_e = (jac_params(x + eps e_q) - d_p) / eps
+            double dd[3], dM[6];
+            cam_unproject_with_jac_params(cc, q == 0 ? x0 + eps : x0, q == 1 ? x1 + eps : x1, dd, dM, tmp);
+            for (int i = 0; i < m[cam]; ++i) {
+                const int j = idx[cam][i];
+                double f[3];
+#pragma unroll
+                for (int r = 0; r < 3; ++r) f[r] = (tmp[CAM_MAX_PARAMS * r + j] - dp[CAM_MAX_PARAMS * r + j]) / eps;
+                tr[col + i] += JM[q][0] * f[0] + JM[q][1] * f[1] + JM[q][2] * f[2];
+            }
+        }
+        col += m[cam];
+    }
+    for (; col < NP; ++col) tr[col] = 0.0;
+}
+
+// One evaluation pass at the pose whose context is in S->ctx and the camera parameters cp[i] of camera i: robust cost
+// and residual rows (compute_residual) and JtJ, Jtr, jacobian rows (compute_jacobian) -> S->tot, in lm_eval_pass's
+// layout.
+//   PnP : <Model>::project / project_with_jac with jac_params (optim/absolute.h:55-143)
+//   TS  : unproject_with_jac of both pixels at the (trial) cameras, the tangent Sampson residual, the pose columns of
+//         the fixed-camera refiner and the camera columns of ts_cam_row (optim/relative.h:289-441)
+// Every 256 points each thread writes its point's row of the tile; thread e < NV then adds value e of every row in point
+// order.  Order of the sums: points in order inside a CTA, CTAs in rank order (deterministic for a given cluster size).
+template <int KIND>
+PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *cams, const double (*cp)[CAM_MAX_PARAMS],
+                           const int *m, const int (*idx)[CAM_MAX_PARAMS], const int *list, int lo, int na,
+                           LmCamShared<KIND> *S, double *tile, int &buf, int csize) {
+    using Y = LmCamLayout<KIND>;
+    constexpr int NP = Y::NP, NC = Y::NCAM;
+    const double *ctx = S->ctx;
+    CamDev cam[NC];
+#pragma unroll
+    for (int i = 0; i < NC; ++i) {
+        cam[i].model = cams[i].model;
+        cam[i].reserved = 0;
+#pragma unroll
+        for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam[i].p[c] = cp[i][c];
+    }
     // the value this thread owns: kind 0 column sum of column a, 1 JtJ(a, b), 2 Jtr(a), -1 none (or a padded entry)
-    const int e = threadIdx.x, np = 6 + m;
+    int np = Y::NPOSE;
+#pragma unroll
+    for (int i = 0; i < NC; ++i) np += m[i];
+    const int e = threadIdx.x;
     int kind = -1, a = 0, b = 0;
     if (e == 0) {
-        kind = 0; a = LMI_LOSS;
+        kind = 0; a = Y::LOSS;
     } else if (e == 1) {
-        kind = 0; a = LMI_ROW;
-    } else if (e < 2 + LMI_NT) {
+        kind = 0; a = Y::ROW;
+    } else if (e < 2 + Y::NT) {
         const int t = e - 2;
         while ((a + 1) * (a + 2) / 2 <= t) ++a;
         b = t - a * (a + 1) / 2;
         if (a < np) kind = 1;
-    } else if (e < 2 + LMI_NT + LMI_NP) {
-        a = e - 2 - LMI_NT;
+    } else if (e < 2 + Y::NT + NP) {
+        a = e - 2 - Y::NT;
         if (a < np) kind = 2;
-    } else if (e == LMI_NV - 1) {
-        kind = 0; a = LMI_JROW;
+    } else if (e == Y::NV - 1) {
+        kind = 0; a = Y::JROW;
     }
     double acc = 0.0;
     for (int t0 = 0; t0 < na; t0 += (int)blockDim.x) {
         const int i = t0 + threadIdx.x;
-        double *tr = tile + (size_t)threadIdx.x * LMI_W;
+        double *tr = tile + (size_t)threadIdx.x * Y::W;
         bool filled = false;
+        tr[Y::LOSS] = 0.0;
+        tr[Y::ROW] = 0.0;
+        tr[Y::JROW] = 0.0;
         if (i < na) {
             const int k = list ? list[i] : lo + i;
-            const double X0 = P.p[2][k], X1 = P.p[3][k], X2 = P.p[4][k];
-            const double Z0 = ctx[0] * X0 + ctx[1] * X1 + ctx[2] * X2 + ctx[9];
-            const double Z1 = ctx[3] * X0 + ctx[4] * X1 + ctx[5] * X2 + ctx[10];
-            const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
-            if (!(Z2 < 0)) { // optim/absolute.h:57-58,93-94
-                double xr0, xr1, zp0, zp1, Jp[2][3];
-                cam_project(cam, Z0, Z1, Z2, xr0, xr1);
-                cam_project_with_jac(cam, Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
-                const double x0 = P.p[0][k], x1 = P.p[1][k];
-                const double q0 = xr0 - x0, q1 = xr1 - x1;
-                tr[LMI_LOSS] = L.loss(q0 * q0 + q1 * q1);
-                tr[LMI_ROW] = 1.0;
-                const double r0 = zp0 - x0, r1 = zp1 - x1;
-                const double w = L.weight(r0 * r0 + r1 * r1);
-                if (w != 0) { // jacobian_accumulator.h:87-104
-                    filled = true;
-                    tr[LMI_JROW] = 1.0;
-                    tr[LMI_WT] = w;
-                    tr[LMI_WR0] = w * r0;
-                    tr[LMI_WR1] = w * r1;
+            if constexpr (KIND == KIND_PNP) {
+                const double X0 = P.p[2][k], X1 = P.p[3][k], X2 = P.p[4][k];
+                const double Z0 = ctx[0] * X0 + ctx[1] * X1 + ctx[2] * X2 + ctx[9];
+                const double Z1 = ctx[3] * X0 + ctx[4] * X1 + ctx[5] * X2 + ctx[10];
+                const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
+                if (!(Z2 < 0)) { // optim/absolute.h:57-58,93-94
+                    double xr0, xr1, zp0, zp1, Jp[2][3];
+                    cam_project(cam[0], Z0, Z1, Z2, xr0, xr1);
+                    cam_project_with_jac(cam[0], Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
+                    const double x0 = P.p[0][k], x1 = P.p[1][k];
+                    const double q0 = xr0 - x0, q1 = xr1 - x1;
+                    tr[Y::LOSS] = L.loss(q0 * q0 + q1 * q1);
+                    tr[Y::ROW] = 1.0;
+                    const double r0 = zp0 - x0, r1 = zp1 - x1;
+                    const double w = L.weight(r0 * r0 + r1 * r1);
+                    if (w != 0) { // jacobian_accumulator.h:87-104
+                        filled = true;
+                        tr[Y::JROW] = 1.0;
+                        tr[Y::WT] = w;
+                        tr[Y::WR] = w * r0;
+                        tr[Y::WR + 1] = w * r1;
 #pragma unroll
-                    for (int q = 0; q < 2; ++q) {
-                        double dZ[3];
+                        for (int q = 0; q < 2; ++q) {
+                            double dZ[3];
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) dZ[c] = Jp[q][0] * ctx[c] + Jp[q][1] * ctx[3 + c] + Jp[q][2] * ctx[6 + c];
-                        double *Jr = tr + q * LMI_NP;
-                        Jr[0] = -X2 * dZ[1] + X1 * dZ[2];
-                        Jr[1] = X2 * dZ[0] - X0 * dZ[2];
-                        Jr[2] = -X1 * dZ[0] + X0 * dZ[1];
-                        Jr[3] = dZ[0]; Jr[4] = dZ[1]; Jr[5] = dZ[2];
+                            for (int c = 0; c < 3; ++c)
+                                dZ[c] = Jp[q][0] * ctx[c] + Jp[q][1] * ctx[3 + c] + Jp[q][2] * ctx[6 + c];
+                            double *Jr = tr + q * NP;
+                            Jr[0] = -X2 * dZ[1] + X1 * dZ[2];
+                            Jr[1] = X2 * dZ[0] - X0 * dZ[2];
+                            Jr[2] = -X1 * dZ[0] + X0 * dZ[1];
+                            Jr[3] = dZ[0]; Jr[4] = dZ[1]; Jr[5] = dZ[2];
+                        }
+                        // J.col(6 + c) = J_params.col(camera_refine_idx[c]); jac_params is staged in the row's tail
+                        cam_jac_params(cam[0], Z0, Z1, Z2, tr + Y::JP);
+#pragma unroll
+                        for (int c = 0; c < NP - 6; ++c) {
+                            tr[6 + c] = c < m[0] ? tr[Y::JP + idx[0][c]] : 0.0;
+                            tr[NP + 6 + c] = c < m[0] ? tr[Y::JP + CAM_MAX_PARAMS + idx[0][c]] : 0.0;
+                        }
                     }
-                    // J.col(6 + c) = J_params.col(camera_refine_idx[c]); jac_params is staged in the row's tail
-                    cam_jac_params(cam, Z0, Z1, Z2, tr + LMI_JP);
-#pragma unroll
-                    for (int c = 0; c < LMI_NP - 6; ++c) {
-                        tr[6 + c] = c < m ? tr[LMI_JP + idx[c]] : 0.0;
-                        tr[LMI_NP + 6 + c] = c < m ? tr[LMI_JP + CAM_MAX_PARAMS + idx[c]] : 0.0;
-                    }
-                } else {
-                    tr[LMI_JROW] = 0.0;
                 }
-            } else {
-                tr[LMI_LOSS] = 0.0;
-                tr[LMI_ROW] = 0.0;
-                tr[LMI_JROW] = 0.0;
+            } else { // KIND_RELPOSE_TS
+                const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
+                double d1[3], d2[3], M1[6], M2[6];
+                cam_unproject_with_jac_params(cam[0], a0, a1, d1, M1, tr + Y::JP);
+                cam_unproject_with_jac_params(cam[1], b0, b1, d2, M2, tr + Y::JP + 3 * CAM_MAX_PARAMS);
+                double C, JC[4];
+                tangent_terms(ctx, d1, d2, M1, M2, C, JC);
+                {
+                    const double nJc_sq = (JC[2] * JC[2] + JC[3] * JC[3]) + (JC[0] * JC[0] + JC[1] * JC[1]);
+                    const double rr = C / sqrt(nJc_sq);
+                    tr[Y::LOSS] = L.loss(rr * rr);
+                    tr[Y::ROW] = 1.0;
+                }
+                const double nJ_C = sqrt((JC[0] * JC[0] + JC[2] * JC[2]) + (JC[1] * JC[1] + JC[3] * JC[3]));
+                const double r = C * (1.0 / nJ_C);
+                const double w = L.weight(r * r);
+                if (w != 0) { // jacobian_accumulator.h:125-141
+                    filled = true;
+                    tr[Y::JROW] = 1.0;
+                    tr[Y::WT] = w;
+                    tr[Y::WR] = w * r;
+                    ts_cam_row<NP>(ctx, ctx + 9, cam[0], cam[1], a0, a1, b0, b1, d1, d2, M1, M2, C, JC, idx, m,
+                                   tr + Y::JP, tr);
+                }
             }
-        } else {
-            tr[LMI_LOSS] = 0.0;
-            tr[LMI_ROW] = 0.0;
-            tr[LMI_JROW] = 0.0;
         }
         if (!filled) { // no Jacobian contribution: a zero row (reference: add_jacobian returns early)
-            for (int c = 0; c < 2 * LMI_NP; ++c) tr[c] = 0.0;
-            tr[LMI_WT] = 0.0;
-            tr[LMI_WR0] = 0.0;
-            tr[LMI_WR1] = 0.0;
+            for (int c = 0; c < Y::R * NP; ++c) tr[c] = 0.0;
+            tr[Y::WT] = 0.0;
+#pragma unroll
+            for (int q = 0; q < Y::R; ++q) tr[Y::WR + q] = 0.0;
         }
         __syncthreads();
         const int rows = min_i((int)blockDim.x, na - t0);
         if (kind == 0) {
-            for (int r = 0; r < rows; ++r) acc += tile[r * LMI_W + a];
+            for (int r = 0; r < rows; ++r) acc += tile[r * Y::W + a];
         } else if (kind == 1) {
             for (int r = 0; r < rows; ++r) {
-                const double *q = tile + r * LMI_W;
-                acc += q[LMI_WT] * (q[a] * q[b] + q[LMI_NP + a] * q[LMI_NP + b]);
+                const double *q = tile + r * Y::W;
+                if constexpr (Y::R == 2) acc += q[Y::WT] * (q[a] * q[b] + q[NP + a] * q[NP + b]);
+                else acc += q[Y::WT] * (q[a] * q[b]);
             }
         } else if (kind == 2) {
             for (int r = 0; r < rows; ++r) {
-                const double *q = tile + r * LMI_W;
-                acc += q[a] * q[LMI_WR0] + q[LMI_NP + a] * q[LMI_WR1];
+                const double *q = tile + r * Y::W;
+                if constexpr (Y::R == 2) acc += q[a] * q[Y::WR] + q[NP + a] * q[Y::WR + 1];
+                else acc += q[a] * q[Y::WR];
             }
         }
         __syncthreads();
     }
-    if (e < LMI_NV) S->sums[buf][e] = acc;
-    cluster_total(S, LMI_NV, buf, csize);
+    if (e < Y::NV) S->sums[buf][e] = acc;
+    cluster_total(S, Y::NV, buf, csize);
 }
 
 // Lower Cholesky solve of (A) x = rhs, n x n row-major, only the lower triangle of A read and the factor written over it
@@ -2195,22 +2343,26 @@ template <class Shared, class Keep> PLB_DEV int lm_compact(Shared *S, int lo, in
 // cluster totals, so no broadcast between CTAs is needed.  The reference evaluates the residual of a trial step and,
 // if accepted, the Jacobian at the same parameters in a second pass; here both come from one pass.
 // Two refiners: the fixed-camera one of every kind (lm_eval_pass: per-thread packed normal equations, cluster_sum), and
-// CAM, AbsolutePoseRefiner with the camera parameters cam_refine_idx(prm.cam.model, job.cam_refine) refined with the
-// pose (lmi_eval_pass: the shared-memory tile summed in point order, which ~255 registers of per-thread accumulators
-// for 14 parameters would not leave room for).  CAM writes the camera of job j to cam_outs[j * CAM_MAX_PARAMS ..].
+// CAM, the refiner with camera parameters (lmi_eval_pass: the shared-memory tile summed in point order, which ~255
+// registers of per-thread accumulators for 14 or 21 parameters would not leave room for):
+//   KIND_PNP        AbsolutePoseRefiner, the parameters cam_refine_idx(prm.cam.model, job.cam_refine) of prm.cam
+//   KIND_RELPOSE_TS CameraRelativePoseRefiner, cam_refine_idx(P.cam[i].model, job.cam_refine) of both cameras P.cam[i]
+// CAM writes camera i of job j to cam_outs[(j * kind_cam_count(KIND) + i) * CAM_MAX_PARAMS ..].
+template <int KIND, bool CAM> struct LmNP { static constexpr int v = LmDims<KIND>::NP; };
+template <int KIND> struct LmNP<KIND, true> { static constexpr int v = LmCamLayout<KIND>::NP; };
 template <int KIND, bool CAM>
 __global__ void __launch_bounds__(LM_THREADS, 1)
     k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
          const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
          int *idx_scratch, int scratch_stride, LmJobOut *outs, double *cam_outs) {
-    static_assert(!CAM || KIND == KIND_PNP, "camera refinement is the absolute pose refiner's");
+    static_assert(!CAM || KIND == KIND_PNP || KIND == KIND_RELPOSE_TS, "camera refinement: absolute and tangent-Sampson relative pose");
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    constexpr int NP = CAM ? LMI_NP : LmDims<KIND>::NP;
+    constexpr int NP = LmNP<KIND, CAM>::v;
     constexpr int NT = NP * (NP + 1) / 2;
     constexpr int MSZ = kind_model_size(KIND);
-    __shared__ std::conditional_t<CAM, LmCamShared, LmShared<NP>> S;
-    extern __shared__ double lmi_tile[]; // CAM: LMI_TILE_BYTES
+    __shared__ std::conditional_t<CAM, LmCamShared<KIND>, LmShared<NP>> S;
+    extern __shared__ double lmi_tile[]; // CAM: LmCamLayout<KIND>::TILE_BYTES
     const int csize = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
     // The grid is a set of clusters that walk the job list: explicit jobs (jobs[j], model j of models_in, stride 9) or
     // the LO jobs k_pass1 listed on the device (template jobs[job_src[j].pidx], model slot job_src[j].slot of the
@@ -2284,22 +2436,32 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
             for (int k = MSZ; k < 9; ++k) S.par[k] = 0.0;
         }
         if constexpr (CAM) {
-            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = prm.cam.p[c];
-            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.idx[c] = 0;
-            S.m = cam_refine_idx(prm.cam.model, J.cam_refine, S.idx);
+            for (int i = 0; i < kind_cam_count(KIND); ++i) {
+                const CamDev &c0 = KIND == KIND_PNP ? prm.cam : P.cam[i];
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[i][c] = c0.p[c];
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.idx[i][c] = 0;
+                S.m[i] = cam_refine_idx(c0.model, J.cam_refine, S.idx[i]);
+            }
         }
     }
     __syncthreads();
-    int m = 0, idx[CAM_MAX_PARAMS]; // CAM: the refined camera parameters, in registers for the evaluation pass
+    constexpr int NC = kind_cam_count(KIND);
+    // CAM: the cameras' models and refined parameters, in registers for the evaluation pass
+    int m[NC] = {}, idx[NC][CAM_MAX_PARAMS];
+    CamDev cams[NC];
     if constexpr (CAM) {
-        m = S.m;
 #pragma unroll
-        for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[c] = S.idx[c];
+        for (int i = 0; i < NC; ++i) {
+            cams[i].model = KIND == KIND_PNP ? prm.cam.model : P.cam[i].model;
+            m[i] = S.m[i];
+#pragma unroll
+            for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[i][c] = S.idx[i][c];
+        }
     }
     // one evaluation pass at par (trial: par_new), totals in S.tot
     auto eval = [&](bool trial) {
         if constexpr (CAM)
-            lmi_eval_pass(P, L, prm.cam.model, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+            lmi_eval_pass<KIND>(P, L, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
         else
             lm_eval_pass<KIND>(P, prm, L, list, lo, na, &S, buf, csize);
     };
@@ -2345,9 +2507,13 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
                 }
                 if (!stop) {
                     lm_step<KIND>(S.par, S.sol, S.tb, S.par_new);
-                    if constexpr (CAM) { // AbsolutePoseRefiner::step (optim/absolute.h:146-160)
-                        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam_new[c] = S.cam[c];
-                        for (int c = 0; c < S.m; ++c) S.cam_new[S.idx[c]] += S.sol[6 + c];
+                    if constexpr (CAM) { // AbsolutePoseRefiner::step (optim/absolute.h:146-160), relative.h:443-468
+                        int off = LmCamDims<KIND>::NPOSE;
+                        for (int i = 0; i < NC; ++i) {
+                            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam_new[i][c] = S.cam[i][c];
+                            for (int c = 0; c < S.m[i]; ++c) S.cam_new[i][S.idx[i][c]] += S.sol[off + c];
+                            off += S.m[i];
+                        }
                     }
                     lm_build_ctx<KIND>(S.par_new, S.ctx, S.tb_new, true);
                 }
@@ -2363,7 +2529,8 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
                     for (int k = 0; k < 9; ++k) S.par[k] = S.par_new[k];
                     for (int k = 0; k < 6; ++k) S.tb[k] = S.tb_new[k];
                     if constexpr (CAM)
-                        for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[c] = S.cam_new[c];
+                        for (int i = 0; i < NC; ++i)
+                            for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[i][c] = S.cam_new[i][c];
                     cost = cost_new;
                     recompute_jac = true;
                     const double scale = 1.0 / fmax(1.0, rc);
@@ -2417,7 +2584,8 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
             out->cost = cost;
             out->initial_cost = initial_cost;
             if constexpr (CAM)
-                for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam_outs[(size_t)job * CAM_MAX_PARAMS + c] = S.cam[c];
+                for (int i = 0; i < NC; ++i)
+                    for (int c = 0; c < CAM_MAX_PARAMS; ++c) cam_outs[((size_t)job * NC + i) * CAM_MAX_PARAMS + c] = S.cam[i][c];
         }
     }
     __syncthreads();
@@ -2462,7 +2630,7 @@ static int lm_cluster_size(int n_jobs, int max_n) {
     return csize;
 }
 // A grid of n_clusters clusters of csize CTAs over a job list: k_lm<kind> of the fixed-camera refiner, or with
-// refine_camera the absolute pose refiner with camera parameters.
+// refine_camera the refiner with camera parameters of the kind (KIND_PNP or KIND_RELPOSE_TS).
 static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs,
                           const LoJobSrc *job_src, const double *models_in, const int *n_jobs_dev, int n_jobs,
                           int n_clusters, int csize, const char *mask_base, int *idx_scratch, int scratch_stride,
@@ -2471,7 +2639,10 @@ static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs,
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
     cfg.blockDim = dim3((unsigned)LM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = refine_camera ? LMI_TILE_BYTES : 0;
+    const size_t tile = !refine_camera                 ? 0
+                        : kind == KIND_RELPOSE_TS ? LmCamLayout<KIND_RELPOSE_TS>::TILE_BYTES
+                                                  : LmCamLayout<KIND_PNP>::TILE_BYTES;
+    cfg.dynamicSmemBytes = tile;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -2485,8 +2656,9 @@ static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs,
                            scratch_stride, out, cam_out);
     };
     if (refine_camera) {
-        cudaFuncSetAttribute(k_lm<KIND_PNP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LMI_TILE_BYTES);
-        launch(k_lm<KIND_PNP, true>);
+        auto cam_kernel = kind == KIND_RELPOSE_TS ? k_lm<KIND_RELPOSE_TS, true> : k_lm<KIND_PNP, true>;
+        cudaFuncSetAttribute(cam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile);
+        launch(cam_kernel);
     } else {
         with_kind(kind, [&](auto K) { launch(k_lm<K, false>); });
     }

@@ -26,6 +26,9 @@ struct ProblemDev {
     int n_pad;      // array stride of ts
     const double *ts;
     const float *cmax; // max |coordinate| of every SoA array (fp64 values rounded up): error bounds of the fp32 screening
+    // RELPOSE_TS with camera refinement: p[0..3] = x1.x x1.y x2.x x2.y (the pixels ts was computed from, SoA, stride
+    // n_pad) and the cameras of the two images; otherwise p[] is null and the cameras are CAMM_NULL
+    CamDev cam[2];
 };
 
 constexpr __host__ __device__ bool kind_is_relpose(int kind) { return kind == KIND_RELPOSE || kind == KIND_RELPOSE_TS; }
@@ -167,8 +170,10 @@ struct LmParams {
 };
 struct LmJob {
     int pidx;               // index into probs[]
-    int cam_refine;         // KIND_PNP: CAM_REFINE_* flags; a job with a non-empty cam_refine_idx(prm.cam.model, cam_refine)
-                            // refines those camera parameters with the pose (AbsolutePoseRefiner, optim/absolute.h:40-171)
+    int cam_refine;         // CAM_REFINE_* flags.  KIND_PNP: a job with a non-empty cam_refine_idx(prm.cam.model, cam_refine)
+                            // refines those camera parameters with the pose (AbsolutePoseRefiner, optim/absolute.h:40-171).
+                            // KIND_RELPOSE_TS: a job where either camera of its problem (ProblemDev::cam) has a non-empty
+                            // selection refines both selections with the pose (CameraRelativePoseRefiner, relative.h:268-483)
     long long mask_off;     // offset into the mask buffer (subset_mode 2), else -1
     long long scratch_off;  // offset (ints) into idx_scratch for the active-point list (subset modes 1, 2)
     LmParams prm;
@@ -222,8 +227,10 @@ void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode
 // Exact fp64 scoring of an explicit list of n_models models (stride MSZ) with problem indices.
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
                          uint32_t *counts, double *scores, cudaStream_t stream);
-// LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.  refine_camera (KIND_PNP): every job
-// refines camera parameters with the pose (LmJob::cam_refine) and writes its camera to cam_out[j * CAM_MAX_PARAMS ..].
+// LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.  refine_camera (KIND_PNP,
+// KIND_RELPOSE_TS): every job refines camera parameters with the pose (LmJob::cam_refine) and writes its
+// kind_cam_count(kind) cameras to cam_out[(j * kind_cam_count(kind) + i) * CAM_MAX_PARAMS ..].
+constexpr __host__ __device__ int kind_cam_count(int kind) { return kind == KIND_RELPOSE_TS ? 2 : 1; }
 void launch_lm(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in,
                int n_jobs, int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out,
                double *cam_out, cudaStream_t stream);

@@ -1,0 +1,80 @@
+"""Single-call latency of the relative-pose camera refinement on the GPU.
+
+Inputs: C2-sized two-view problems (10 000 correspondences, 30 % inliers) with RADIAL and OPENCV cameras on both
+images.  Timed, each as the median of --reps synchronised calls after --warmup calls (host clock; every call returns
+after its device work is done):
+  * plb_estimate_relative_pose_pair with tangent_sampson, refine flags 0 and 7;
+  * plb_refine_relpose_pair with flags 0 and 7 on the inlier set of the flags-0 estimate.
+Prints one JSON line per measurement, after one line with the card's name, power limit and max SM clock.
+
+    python tools/relpose_pair_timing.py [--reps 9] [--warmup 3]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+from poselib_b200 import cabi  # noqa: E402
+import make_relpose_intrinsics_golden as RG  # noqa: E402
+
+N, INLIER_RATIO, MAX_ERROR = 10000, 0.3, 1.0
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True, check=True).stdout.splitlines()[0]
+    name, power, clock = [s.strip() for s in q.split(",")]
+    return dict(card=name, power_limit=power, max_sm_clock=clock)
+
+
+def median_ms(fn, reps, warmup):
+    for _ in range(warmup):
+        fn()
+    t = []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        fn()
+        t.append(1e3 * (time.perf_counter() - t0))
+    return float(np.median(t)), float(min(t)), float(max(t))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=9)
+    ap.add_argument("--warmup", type=int, default=3)
+    a = ap.parse_args()
+    if a.reps < 7:
+        sys.exit("--reps must be at least 7")
+    if cabi.device_count() == 0:
+        sys.exit("no CUDA device: nothing is measured")
+    print(json.dumps(card()))
+    ro = cabi.RansacOpt(max_iterations=10000, min_iterations=100, seed=0)
+    for model in ("RADIAL", "OPENCV"):
+        mid = RG.MODELS[model]
+        x1, x2, pose0, c1, c2 = RG.pair_problem(mid, mid, N, 1234 + mid, outliers=1.0 - INLIER_RATIO)
+        cam1, cam2 = cabi.Camera(model, tuple(c1)), cabi.Camera(model, tuple(c2))
+        base = cabi.estimate_relative_pose_pair(x1, x2, cam1, cam2, ro, cabi.BundleOpt(), MAX_ERROR)
+        keep = base["inliers"].astype(bool)
+        for flags in (0, 7):
+            b = cabi.BundleOpt(refine_intrinsics=flags)
+            med, lo, hi = median_ms(lambda: cabi.estimate_relative_pose_pair(x1, x2, cam1, cam2, ro, b, MAX_ERROR),
+                                    a.reps, a.warmup)
+            print(json.dumps(dict(call="plb_estimate_relative_pose_pair", camera=model, n=N, flags=flags,
+                                  num_inliers=int(keep.sum()), median_ms=med, min_ms=lo, max_ms=hi)))
+        for flags in (0, 7):
+            b = cabi.BundleOpt(refine_intrinsics=flags)
+            med, lo, hi = median_ms(lambda: cabi.refine_relpose_pair(base["model"], x1[keep], x2[keep], cam1, cam2, b),
+                                    a.reps, a.warmup)
+            print(json.dumps(dict(call="plb_refine_relpose_pair", camera=model, n=int(keep.sum()), flags=flags,
+                                  median_ms=med, min_ms=lo, max_ms=hi)))
+
+
+if __name__ == "__main__":
+    main()
