@@ -1245,8 +1245,8 @@ struct Group {
         mark(PH_SAMPLE);
         launch_hypotheses(kind, R, out, mode, max_n_pad, E.fctx.p, st, E.ev2);
         PLB_CUDA(cudaEventRecord(E.ev1, st));
-        // one solve kernel (5pt: k5_gather, k5_prep_lane, k5_roots, k5_back) + scoring (fast mode: k_screen_ctx + k_screen)
-        E.launches += (kind_is_relpose(kind) ? 5 : 2) + (mode == 1 && kind != KIND_RELPOSE_TS ? 1 : 0);
+        // one solve kernel (5pt: k5_gather, k5_null, k5_elim, k5_roots, k5_back) + scoring (fast mode: k_screen_ctx + k_screen)
+        E.launches += (kind_is_relpose(kind) ? 6 : 2) + (mode == 1 && kind != KIND_RELPOSE_TS ? 1 : 0);
         SelectArgs SA;
         SA.rp = E.rp.p;
         SA.na = na;

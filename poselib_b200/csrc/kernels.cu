@@ -1,7 +1,7 @@
 // poselib_b200 — CUDA kernels of the LO-RANSAC hot path for sm_90a (H100).
 //
 //   k_transpose        caller AoS doubles -> SoA fp64 (+ fp32 copy) in HBM, coalesced both ways
-//   k_solve_lane<KIND> / k7_solve_lane / k5_gather -> k5_prep_lane -> k5_roots -> k5_back
+//   k_solve_lane<KIND> / k7_solve_lane / k5_gather -> k5_null -> k5_elim -> k5_roots -> k5_back
 //                      minimal solvers of a round, one thread per minimal sample (the 5-point solver in phases)
 //   k_score_tiled / k_screen
 //                      MSAC scoring of every model of a round over all correspondences (exact fp64 / fp32 screening)
@@ -13,8 +13,8 @@
 //   Every exact score (k_score_tiled, k_score, k_confirm, the rescoring in k_lm) comes from one routine, msac_score,
 //   and every fp64 inlier decision (those, k_inlier_mask, the LO subset in k_lm) from one test per kind, under_thr
 //   (+ cheirality for the relpose kinds); the PnP mask alone keeps the reference's own formula.
-//   k_solver_batch     the solvers/*.h surface: one thread per instance (relpose_5pt: k5_load -> k5_prep_lane ->
-//                      k5_roots -> k5_solver_out)
+//   k_solver_batch     the solvers/*.h surface: one thread per instance (relpose_5pt: k5_load -> k5_null -> k5_elim
+//                      -> k5_roots -> k5_solver_out)
 //
 // Compiled with -fmad=false (see device_math.cuh).  Reference citations are relative to /root/reference.
 #include "kernels.cuh"
@@ -538,16 +538,17 @@ __global__ void __launch_bounds__(K7L_THREADS) k7_solve_lane(const RoundDesc R, 
 // The 5-point solver is a large body of code; as one kernel, warps at different places of it starve on instruction
 // fetch.  Split into phases, each kernel's code is small and every phase maps its threads to the work it has:
 //   k5_gather    : thread = sample          the sample's bearings
-//   k5_prep_lane : thread = sample          pivoted-QR nullspace, trace constraints, LU, determinant polynomial
+//   k5_null      : thread = sample          pivoted-QR nullspace
+//   k5_elim      : thread = sample          trace constraints, LU, determinant polynomial
 //   k5_roots     : lane   = sample          Sturm bracketing + Ridders/Newton, warp-cooperative
 //   k5_back      : lane   = (sample, root)  back-substitution, motion decomposition, cheirality
-// The solver surface (k5_load, k5_solver_out) runs k5_prep_lane and k5_roots on the caller's instances.
+// The solver surface (k5_load, k5_solver_out) runs k5_null, k5_elim and k5_roots on the caller's instances.
 constexpr int S5_BLK = 105;
 
 // Bearings of the 5 sampled correspondences of every sample (estimators/relative_pose.cc:51-54,90-94) into the
 // entry-major per-sample block (entries 75..104).  Its chain of dependent global loads (problem slot -> problem ->
-// sample ids -> points) is a kernel of its own, at full occupancy: inside k5_prep_lane (4 warps per SM) it was 19 % of
-// that kernel's time.
+// sample ids -> points) is a kernel of its own, at full occupancy: inside the first-half kernel (4 warps per SM) it was
+// 19 % of that kernel's time.
 __global__ void __launch_bounds__(256) k5_gather(const RoundDesc R, HypOut out) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= R.n_total) return;
@@ -575,25 +576,23 @@ __global__ void __launch_bounds__(256) k5_gather(const RoundDesc R, HypOut out) 
     }
 }
 
-// First half with ONE THREAD PER SAMPLE (solver5_lane.cuh): the nullspace basis and the quadratic blocks live in
-// registers (compile-time monomial tables); shared memory holds only the LEFT 10 x 10 block of the elimination matrix
-// (dynamic pivot rows) plus 10 doubles of scratch per thread, the right-hand sides are parked in global memory (L2)
-// while the block is factored and come back column by column.  111 doubles per thread (odd: the 32 lanes of a warp
-// spread over all bank pairs) x 256 threads = 222 KB: one CTA, 8 warps per SM.
-constexpr int PREPL_THREADS = 256;
-constexpr int PREPL_STRIDE = 111;
-constexpr size_t PREPL_SMEM = sizeof(double) * PREPL_STRIDE * PREPL_THREADS;
-// Of R, only n_total is read.  (With an int parameter in its place the compiler schedules this kernel differently.)
-__global__ void __launch_bounds__(PREPL_THREADS, 1) k5_prep_lane(const RoundDesc R, HypOut out) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    double *W = reinterpret_cast<double *>(smem_raw) + (size_t)threadIdx.x * PREPL_STRIDE;
-    double *CL = W, *S = W + 100;
-    int g = blockIdx.x * PREPL_THREADS + threadIdx.x;
-    const bool live = g < R.n_total;
-    if (!live) g = R.n_total - 1; // idle threads of the last CTA redo the last sample (same values, harmless stores)
-    const size_t nt = (size_t)R.n_total;
-    double *blk = out.s5_blk + g;   // entry-major: blk[e * n_total]
-    double *park = out.s5_park + g; // right-hand sides, entry-major: park[(row * 10 + column) * n_total]
+// First half with ONE THREAD PER SAMPLE (solver5_lane.cuh), in two kernels split at the nullspace.  As one kernel its
+// 200 KB of straight-line code starved on instruction fetch, and the nullspace, which needs far fewer registers, ran at
+// the occupancy the elimination imposes.
+//
+// k5_null: the 9 x 5 epipolar matrix in a 45-double slice of shared memory (odd stride: the 32 lanes of a warp spread
+// over all bank pairs; the pivoted QR indexes it dynamically), its nullspace basis Nb straight from registers to
+// entries 39..74 of the sample's block, where k5_elim and k5_back read it.  Four CTAs of 128 threads, 16 warps per SM
+// (128 registers, no spills; 7 % faster on the H100 than 12 warps at 162 registers).
+constexpr int NULL_THREADS = 128;
+constexpr int NULL_STRIDE = 45;
+__global__ void __launch_bounds__(NULL_THREADS, 4) k5_null(const int n_total, HypOut out) {
+    __shared__ double sW[NULL_THREADS * NULL_STRIDE];
+    double *W = sW + threadIdx.x * NULL_STRIDE;
+    const int g = blockIdx.x * NULL_THREADS + threadIdx.x;
+    if (g >= n_total) return;
+    const size_t nt = (size_t)n_total;
+    double *blk = out.s5_blk + g; // entry-major: blk[e * n_total]
     {
         double xs[30]; // the sample's bearings, written by k5_gather: 30 independent coalesced loads
 #pragma unroll
@@ -605,16 +604,33 @@ __global__ void __launch_bounds__(PREPL_THREADS, 1) k5_prep_lane(const RoundDesc
             W[e] = xs[3 * i + k / 3] * xs[15 + 3 * i + k % 3];
         }
     }
-    lane5::nullspace_9x5(W, W + 45);
+    // Nb[4 * k + r] = entry k of basis vector r
+    lane5::nullspace_basis<5>(W, [&](int r, int k, double v) { blk[(39 + 4 * k + r) * nt] = v; });
+}
+
+// k5_elim: Nb (registers) -> trace / determinant constraints -> elimination -> determinant polynomial.  The quadratic
+// blocks live in registers (compile-time monomial tables); shared memory holds only the LEFT 10 x 10 block of the
+// elimination matrix (dynamic pivot rows) plus 10 doubles of scratch per thread, the right-hand sides are parked in
+// global memory (L2) while the block is factored and come back column by column.  111 doubles per thread (odd) x 256
+// threads = 222 KB: one CTA, 8 warps per SM.
+constexpr int ELIM_THREADS = 256;
+constexpr int ELIM_STRIDE = 111;
+constexpr size_t ELIM_SMEM = sizeof(double) * ELIM_STRIDE * ELIM_THREADS;
+// Of R, only n_total is read.  (With an int parameter in its place the compiler schedules this kernel differently.)
+__global__ void __launch_bounds__(ELIM_THREADS, 1) k5_elim(const RoundDesc R, HypOut out) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    double *W = reinterpret_cast<double *>(smem_raw) + (size_t)threadIdx.x * ELIM_STRIDE;
+    double *CL = W, *S = W + 100;
+    int g = blockIdx.x * ELIM_THREADS + threadIdx.x;
+    const bool live = g < R.n_total;
+    if (!live) g = R.n_total - 1; // idle threads of the last CTA redo the last sample (same values, harmless stores)
+    const size_t nt = (size_t)R.n_total;
+    double *blk = out.s5_blk + g;   // entry-major: blk[e * n_total]
+    double *park = out.s5_park + g; // right-hand sides, entry-major: park[(row * 10 + column) * n_total]
     {
         double Nb[36];
 #pragma unroll
-        for (int e = 0; e < 36; ++e) {
-            const int r = e / 9, k = e % 9;
-            Nb[4 * k + r] = W[45 + 9 * r + k];
-        }
-#pragma unroll
-        for (int e = 0; e < 36; ++e) blk[(39 + e) * nt] = Nb[e];
+        for (int e = 0; e < 36; ++e) Nb[e] = blk[(39 + e) * nt];
         lane5::build_coeffs(Nb, [&](int row, auto cc, double v) {
             constexpr int ci = decltype(cc)::value;
             if constexpr (ci < 10) CL[row * 10 + ci] = v;
@@ -704,7 +720,7 @@ __global__ void __launch_bounds__(128) k5_back(const RoundDesc R, HypOut out) {
         double cand[4][7];
         unsigned mask = 0;
         if (valid) {
-            const StridedD blk{out.s5_blk + g, (size_t)R.n_total}; // entry-major (k5_prep_lane)
+            const StridedD blk{out.s5_blk + g, (size_t)R.n_total}; // entry-major (k5_null, k5_elim)
             double E[9];
             backsub_5pt(blk, blk + 39, out.s5_roots[(size_t)g * 10 + r], E);
             mask = motions_from_E(E, blk + 75, blk + 90, 5, cand);
@@ -1306,11 +1322,12 @@ template <class F> static void with_kind(int kind, F &&f) {
 static void launch_5pt_prep_roots(const RoundDesc &R, const HypOut &out, cudaStream_t stream) {
     static bool attr_set[MAX_DEVICES] = {false};
     if (!attr_set[cur_dev()]) {
-        cudaFuncSetAttribute(k5_prep_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PREPL_SMEM);
+        cudaFuncSetAttribute(k5_elim, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ELIM_SMEM);
         attr_set[cur_dev()] = true;
     }
     const int n = R.n_total;
-    k5_prep_lane<<<(unsigned)((n + PREPL_THREADS - 1) / PREPL_THREADS), PREPL_THREADS, PREPL_SMEM, stream>>>(R, out);
+    k5_null<<<(unsigned)((n + NULL_THREADS - 1) / NULL_THREADS), NULL_THREADS, 0, stream>>>(n, out);
+    k5_elim<<<(unsigned)((n + ELIM_THREADS - 1) / ELIM_THREADS), ELIM_THREADS, ELIM_SMEM, stream>>>(R, out);
     k5_roots<<<(n + ROOTS_THREADS - 1) / ROOTS_THREADS, ROOTS_THREADS, 0, stream>>>(n, out);
 }
 
@@ -2916,7 +2933,7 @@ __global__ void __launch_bounds__(K7L_THREADS)
 }
 
 // relpose_5pt: the caller's bearings (5 x 3 doubles per side and instance) into entries 75..104 of the entry-major
-// per-instance block, where k5_prep_lane and k5_back expect the sample's bearings.
+// per-instance block, where k5_null and k5_back expect the sample's bearings.
 __global__ void __launch_bounds__(256) k5_load(int n, const double *__restrict__ a, const double *__restrict__ b,
                                                HypOut s5) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -3000,7 +3017,7 @@ int launch_solver_batch(int kind, int variant, size_t count, const double *a, co
         launch_5pt_prep_roots(R, s5, stream);
         if (variant == 0) k5_solver_out<0><<<(n + 127) / 128, 128, 0, stream>>>(n, s5, out, n_out);
         else k5_solver_out<1><<<(n + 127) / 128, 128, 0, stream>>>(n, s5, out, n_out);
-        return 4;
+        return 5;
     }
     case KIND_FUND: launch_solver_t<KIND_FUND, 0>(count, a, b, out, n_out, flags, stream); return 1;
     default: launch_solver_t<KIND_HOMOG, 0>(count, a, b, out, n_out, flags, stream); return 1;

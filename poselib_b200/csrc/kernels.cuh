@@ -70,7 +70,7 @@ struct HypOut {
     float *ferr;       // fast mode: bound of |score32 - score64|
     // relpose_5pt phase buffers (device), sized for the round's n_total samples:
     double *s5_blk;   // 105 x n_total, entry-major (blk[e * n_total + g]): A (39) | Nb (36) | sample bearings x1s,x2s (30)
-    double *s5_park;  // 100 x n_total, entry-major: right-hand sides of the elimination, parked by k5_prep_lane
+    double *s5_park;  // 100 x n_total, entry-major: right-hand sides of the elimination, parked by k5_elim
     double *s5_cpoly; // 11 x n_total, coefficient-major (cpoly[c * n_total + g])
     double *s5_roots; // per sample 10 doubles
     int *s5_nroots;   // per sample

@@ -66,11 +66,11 @@ constexpr Tables make_tables() {
 constexpr Tables TB = make_tables();
 
 // ---- nullspace of the 9 x C epipolar matrix (C = 5: relpose_5pt, C = 7: relpose_7pt) --------------------------------------------------------------------------
-// a: 9 C doubles, column-major (a[c * 9 + r]), overwritten; qn: 9 (9 - C) doubles, qn[9 * s + r] = entry r of the s-th
-// basis vector = column C + s of the Householder Q of the full-pivoting QR (relpose_5pt.cc:167-168, relpose_7pt.cc:18-19):
-// Eigen's pivot rule (largest |entry|, first in column-major order on ties), reflectors and order of the row
-// transpositions.
-template <int COLS> PLB_L5 void nullspace_9xC(double *a, double *qn) {
+// a: 9 C doubles, column-major (a[c * 9 + r]), overwritten; put(s, r, v) receives entry r of the s-th basis vector =
+// column C + s of the Householder Q of the full-pivoting QR (relpose_5pt.cc:167-168, relpose_7pt.cc:18-19): Eigen's
+// pivot rule (largest |entry|, first in column-major order on ties), reflectors and order of the row transpositions.
+// s and r are compile-time after unrolling, so the basis can go straight to registers or to its final place.
+template <int COLS, class Sink> PLB_L5 void nullspace_basis(double *a, Sink &&put) {
     constexpr int ROWS = 9;
     double tau_k[COLS];
     int rt_k[COLS];
@@ -207,7 +207,11 @@ template <int COLS> PLB_L5 void nullspace_9xC(double *a, double *qn) {
 #pragma unroll
     for (int s = 0; s < ROWS - COLS; ++s)
 #pragma unroll
-        for (int r = 0; r < ROWS; ++r) qn[s * ROWS + r] = q[s][r];
+        for (int r = 0; r < ROWS; ++r) put(s, r, q[s][r]);
+}
+// qn: 9 (9 - C) doubles, qn[9 * s + r] = entry r of the s-th basis vector
+template <int COLS> PLB_L5 void nullspace_9xC(double *a, double *qn) {
+    nullspace_basis<COLS>(a, [&](int s, int r, double v) { qn[9 * s + r] = v; });
 }
 PLB_L5 void nullspace_9x5(double *a, double *qn) { nullspace_9xC<5>(a, qn); }
 
@@ -496,8 +500,8 @@ PLB_L5 void det_poly(const double *A, double *cp) {
 }
 #undef PLB_L5_P
 
-// Whole first half on plain arrays (the host test's entry; the device kernel strings the same pieces together with its
-// shared-memory slice and a parking buffer in global memory).  W: >= 210 doubles; xs: the 5 + 5 bearings (x1s | x2s).
+// Whole first half on plain arrays (the host test's entry; the device kernels k5_null and k5_elim string the same pieces
+// together with their shared-memory slices and a parking buffer in global memory).  W: >= 210 doubles; xs: the 5 + 5 bearings (x1s | x2s).
 PLB_L5 void solve_5pt_poly_lane(double *W, const double *xs, double *Nb, double *A, double *cp) {
     // 9 x 5 epipolar constraints (:163-166): entry 3a+b of column i = x1[i][a] * x2[i][b]
 #pragma unroll
