@@ -60,7 +60,8 @@ typedef struct plb_ransac_stats {
 enum { PLB_LOSS_TRIVIAL = 0, PLB_LOSS_TRUNCATED = 1, PLB_LOSS_HUBER = 2, PLB_LOSS_CAUCHY = 3 };
 /* refine_intrinsics: BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params (types.h:92-94)
  * as a bit set.  The camera parameters they select (Camera::get_param_refinement_idx, camera_models.cc:545-561: focal
- * lengths, then principal point, then the model's extra parameters; none for the NULL camera) are refined with the pose
+ * lengths, then principal point, then the model's extra parameters — k1..p2 of OPENCV, k / k1, k2 of the radial,
+ * fisheye and division models; none for the NULL camera, no extras for the pinhole models) are refined with the pose
  * by plb_bundle_adjust_image and plb_estimate_absolute_pose_image (AbsolutePoseRefiner, optim/absolute.h:40-171), and,
  * for each of the two cameras, by plb_refine_relpose_pair and plb_estimate_relative_pose_pair with tangent_sampson
  * (CameraRelativePoseRefiner, bundle.cc:237-256, optim/relative.h:268-483).
@@ -108,15 +109,21 @@ typedef struct plb_counters {
     uint64_t rounds;           /* lock-step rounds (= host synchronisations inside the loop) of the problem's group */
 } plb_counters;
 
-/* misc/camera_models.h:39-157 Camera, restricted to the six models on the path (others -> PLB_ERR_NYI, like the
- * reference's "NYI" throw, camera_models.cc:184-185).  Ids are the reference's CameraModelId values. */
+/* misc/camera_models.h:39-157 Camera, restricted to the ten models on the path below.  Ids are the reference's
+ * CameraModelId values.  The reference's other models -> PLB_ERR_NYI, like the reference's "NYI" throw
+ * (camera_models.cc:184-185): OPENCV_FISHEYE (5), FULL_OPENCV (6), FOV (7), THIN_PRISM_FISHEYE (10),
+ * RAD_TAN_THIN_PRISM_FISHEYE (11), RADIAL_1D (99) and SPHERICAL (100). */
 enum {
     PLB_CAMERA_NULL = -1,
-    PLB_CAMERA_SIMPLE_PINHOLE = 0, /* f, cx, cy */
-    PLB_CAMERA_PINHOLE = 1,        /* fx, fy, cx, cy */
-    PLB_CAMERA_SIMPLE_RADIAL = 2,  /* f, cx, cy, k */
-    PLB_CAMERA_RADIAL = 3,         /* f, cx, cy, k1, k2 */
-    PLB_CAMERA_OPENCV = 4          /* fx, fy, cx, cy, k1, k2, p1, p2 */
+    PLB_CAMERA_SIMPLE_PINHOLE = 0,         /* f, cx, cy */
+    PLB_CAMERA_PINHOLE = 1,                /* fx, fy, cx, cy */
+    PLB_CAMERA_SIMPLE_RADIAL = 2,          /* f, cx, cy, k */
+    PLB_CAMERA_RADIAL = 3,                 /* f, cx, cy, k1, k2 */
+    PLB_CAMERA_OPENCV = 4,                 /* fx, fy, cx, cy, k1, k2, p1, p2 */
+    PLB_CAMERA_SIMPLE_RADIAL_FISHEYE = 8,  /* f, cx, cy, k */
+    PLB_CAMERA_RADIAL_FISHEYE = 9,         /* f, cx, cy, k1, k2 */
+    PLB_CAMERA_DIVISION = 101,             /* fx, fy, cx, cy, k */
+    PLB_CAMERA_SIMPLE_DIVISION = 102       /* f, cx, cy, k */
 };
 typedef struct plb_camera {
     int32_t model_id;

@@ -77,7 +77,7 @@ template <typename RansacStats> inline RansacStats from_c(const plb_ransac_stats
     r.model_score = s.model_score;
     return r;
 }
-// misc/camera_models.h:59-157 -> plb_camera (six models on the path; others raise NYI inside the library)
+// misc/camera_models.h:59-157 -> plb_camera (the ten models of include/poselib_b200.h are on the path; others raise NYI inside the library)
 template <typename Camera> inline plb_camera camera_to_c(const Camera &cam) {
     plb_camera c;
     c.model_id = cam.model_id;

@@ -14,8 +14,9 @@ LIB_PATH = os.path.join(_HERE, "libposelib_b200.so")
 PLB_OK, PLB_ERR_CUDA, PLB_ERR_ARG, PLB_ERR_NYI = 0, -1, -2, -3
 KIND = {"pnp": 0, "relpose": 1, "fundamental": 2, "homography": 3}
 LOSS = {"TRIVIAL": 0, "TRUNCATED": 1, "HUBER": 2, "CAUCHY": 3}
-CAMERA = {"NULL": -1, "SIMPLE_PINHOLE": 0, "PINHOLE": 1, "SIMPLE_RADIAL": 2, "RADIAL": 3, "OPENCV": 4}
-CAMERA_NUM_PARAMS = {-1: 0, 0: 3, 1: 4, 2: 4, 3: 5, 4: 8}
+CAMERA = {"NULL": -1, "SIMPLE_PINHOLE": 0, "PINHOLE": 1, "SIMPLE_RADIAL": 2, "RADIAL": 3, "OPENCV": 4,
+          "SIMPLE_RADIAL_FISHEYE": 8, "RADIAL_FISHEYE": 9, "DIVISION": 101, "SIMPLE_DIVISION": 102}
+CAMERA_NUM_PARAMS = {-1: 0, 0: 3, 1: 4, 2: 4, 3: 5, 4: 8, 8: 4, 9: 5, 101: 5, 102: 4}
 # BundleOpt.refine_intrinsics bits (refine_focal_length, refine_principal_point, refine_extra_params)
 REFINE_FOCAL_LENGTH, REFINE_PRINCIPAL_POINT, REFINE_EXTRA_PARAMS = 1, 2, 4
 

@@ -606,14 +606,10 @@ static bool profiling() {
 
 // The camera after the polish of estimate_absolute_pose: the (refined) parameters of the rescaled camera `cam`, rescaled
 // by 1 / scale into `out` (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
-static void camera_rescale(CamDev &c, double scale);
 static void polish_camera_out(CamDev c, double scale, const double *params, plb_camera *out) {
     for (int i = 0; i < CAM_MAX_PARAMS; ++i) c.p[i] = params[i];
-    camera_rescale(c, 1.0 / scale);
-    const int np = out->model_id == PLB_CAMERA_SIMPLE_PINHOLE ? 3
-                   : out->model_id == PLB_CAMERA_RADIAL   ? 5
-                   : out->model_id == PLB_CAMERA_OPENCV   ? 8
-                                                          : 4;
+    cam_rescale(c, 1.0 / scale);
+    const int np = cam_num_params(out->model_id);
     for (int i = 0; i < np; ++i) out->params[i] = c.p[i];
 }
 
@@ -915,7 +911,9 @@ struct Group {
         if (n_up) {
             PLB_CUDA(cudaMemsetAsync(E.cmax.p, 0, sizeof(float) * 5 * (size_t)NP, st));
             PLB_CUDA(cudaMemcpyAsync(E.tdesc.p, E.h_tdesc.p, sizeof(TransposeDesc) * n_up, cudaMemcpyHostToDevice, st));
-            launch_transpose(E.tdesc.p, n_up, max_n_pad, st);
+            bool xcam = false;
+            for (int i = 0; i < n_up; ++i) xcam = xcam || cam_is_x(E.h_tdesc.p[i].cam_a.model) || cam_is_x(E.h_tdesc.p[i].cam_b.model);
+            launch_transpose(E.tdesc.p, n_up, max_n_pad, xcam, st);
             E.launches++;
         }
         return PLB_OK;
@@ -930,6 +928,13 @@ struct Group {
         if (kind != KIND_RELPOSE_TS) return plb::refines_camera(J.prm.cam, J.cam_refine);
         const ProblemDev &P = E.h_probs.p[J.pidx];
         return plb::refines_camera(P.cam[0], J.cam_refine) || plb::refines_camera(P.cam[1], J.cam_refine);
+    }
+    // A job evaluates a fisheye or division camera: its prm.cam (PnP) or the problem's cameras (tangent Sampson)
+    bool uses_x_camera(const LmJob &J) const {
+        if (J.prm.use_camera && cam_is_x(J.prm.cam.model)) return true;
+        if (kind != KIND_RELPOSE_TS) return false;
+        const ProblemDev &P = E.h_probs.p[J.pidx];
+        return cam_is_x(P.cam[0].model) || cam_is_x(P.cam[1].model);
     }
     int lm_batch(const std::vector<LmTask> &batch) {
         const int nj = (int)batch.size(), nc = kind_cam_count(kind);
@@ -955,7 +960,9 @@ struct Group {
         for (int cam = 0; cam < 2; ++cam) {
             const int j0 = cam ? n_fixed : 0, n = cam ? nj - n_fixed : n_fixed;
             if (n == 0) continue;
-            launch_lm(kind, cam, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
+            bool xcam = false;
+            for (int j = j0; j < j0 + n; ++j) xcam = xcam || uses_x_camera(batch[j].job);
+            launch_lm(kind, cam, xcam, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
                       max_n_pad, E.h_lm_out.d + j0, cam ? E.h_cam_out.d + (size_t)j0 * nc * CAM_MAX_PARAMS : nullptr, st);
             E.launches++;
         }
@@ -1606,38 +1613,21 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     return PLB_OK;
 }
 
-// plb_camera -> CamDev; models outside the six on the path are rejected like Camera::unproject's "NYI"
+// plb_camera -> CamDev; models outside the ten on the path (cam_layout) are rejected like Camera::unproject's "NYI"
 // (misc/camera_models.cc:176-188)
 static int camera_dev(const plb_camera *c, CamDev *out) {
     out->model = CAMM_NULL;
     out->reserved = 0;
     for (int i = 0; i < 8; ++i) out->p[i] = 0.0;
     if (!c || c->model_id == PLB_CAMERA_NULL) return PLB_OK;
-    int np = 0;
-    switch (c->model_id) {
-    case PLB_CAMERA_SIMPLE_PINHOLE: np = 3; break;
-    case PLB_CAMERA_PINHOLE: np = 4; break;
-    case PLB_CAMERA_SIMPLE_RADIAL: np = 4; break;
-    case PLB_CAMERA_RADIAL: np = 5; break;
-    case PLB_CAMERA_OPENCV: np = 8; break;
-    default: g_err = "NYI: camera model not supported by the CUDA path (undistort on the host first)"; return PLB_ERR_NYI;
+    CamLayout L;
+    if (!cam_layout(c->model_id, L)) {
+        g_err = "NYI: camera model not supported by the CUDA path (undistort on the host first)";
+        return PLB_ERR_NYI;
     }
     out->model = c->model_id;
-    for (int i = 0; i < np; ++i) out->p[i] = c->params[i];
+    for (int i = 0; i < L.np(); ++i) out->p[i] = c->params[i];
     return PLB_OK;
-}
-static double camera_focal(const CamDev &c) { // Camera::focal() camera_models.cc:304-324
-    switch (c.model) {
-    case CAMM_NULL: return 1.0;
-    case CAMM_PINHOLE:
-    case CAMM_OPENCV: return 0.0 + c.p[0] / 2 + c.p[1] / 2;
-    default: return 0.0 + c.p[0] / 1;
-    }
-}
-static void camera_rescale(CamDev &c, double scale) { // Camera::rescale camera_models.cc:432-454
-    if (c.model == CAMM_NULL) return;
-    const int k = (c.model == CAMM_PINHOLE || c.model == CAMM_OPENCV) ? 4 : 3; // focal_idx then principal_point_idx
-    for (int i = 0; i < k; ++i) c.p[i] *= scale;
 }
 
 } // namespace plb
@@ -1887,7 +1877,7 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             g_err = "camera refinement flags need a camera to return: use plb_estimate_absolute_pose_image";
             return PLB_ERR_ARG;
         }
-        const double scale = 1.0 / camera_focal(cam);
+        const double scale = 1.0 / cam_focal(cam);
         fp.bundle.loss_scale = bundle->loss_scale * scale;
         fp.min_inliers = 3;
         if (cam.model != CAMM_NULL) { // the polish runs on pixels*scale with the rescaled camera (robust.cc:103-123)
@@ -1895,7 +1885,7 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             for (size_t k = 0; k < 2 * n; ++k) J.px[k] = x1[k] * scale;
             fp.px_scaled = J.px.data();
             fp.cam = cam;
-            camera_rescale(fp.cam, scale);
+            cam_rescale(fp.cam, scale);
             fp.scale = scale;
             if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && refined)) fp.cam_out = camera_out;
         }
@@ -1914,13 +1904,13 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             g_err = "NYI: camera refinement needs cameras to return: use plb_estimate_relative_pose_pair";
             return PLB_ERR_NYI;
         }
-        const double scale = 0.5 * (1.0 / camera_focal(c1) + 1.0 / camera_focal(c2));
+        const double scale = 0.5 * (1.0 / cam_focal(c1) + 1.0 / cam_focal(c2));
         fp.bundle.loss_scale = bundle->loss_scale * scale;
         fp.min_inliers = 5;
         t.max_error = max_error * scale;
         if (tangent_sampson) {
-            camera_rescale(c1, scale);
-            camera_rescale(c2, scale);
+            cam_rescale(c1, scale);
+            cam_rescale(c2, scale);
             model[0] = 1.0; // ransac.cc:159-160: the start pose is reset even when score_initial_model is set
             for (int i = 1; i < 7; ++i) model[i] = 0.0;
             t.kind = KIND_RELPOSE_TS;
@@ -2481,7 +2471,7 @@ int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts
     D.scale = 1.0;
     PLB_CUDA(cudaMemsetAsync(R->cmax.p, 0, sizeof(float) * 8, E.stream));
     PLB_CUDA(cudaMemcpyAsync(E.tdesc.p, E.h_tdesc.p, sizeof(TransposeDesc), cudaMemcpyHostToDevice, E.stream));
-    launch_transpose(E.tdesc.p, 1, n_pad, E.stream);
+    launch_transpose(E.tdesc.p, 1, n_pad, false, E.stream);
     PLB_CUDA(cudaStreamSynchronize(E.stream));
     R->n = n;
     R->n_pad = n_pad;

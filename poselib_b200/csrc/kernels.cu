@@ -44,7 +44,8 @@ PLB_DEV void coord_max(float *cmax, int c, double v) {
     const unsigned m = __reduce_max_sync(0xffffffffu, bits);
     if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned *>(cmax) + c, m);
 }
-__global__ void k_transpose(const TransposeDesc *__restrict__ descs) {
+// X: some camera of the launch is a fisheye or division model (camera.cuh)
+template <bool X> __global__ void k_transpose(const TransposeDesc *__restrict__ descs) {
     const TransposeDesc &d = descs[blockIdx.y];
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= d.n_pad) return;
@@ -53,23 +54,23 @@ __global__ void k_transpose(const TransposeDesc *__restrict__ descs) {
     if (d.mode == 2) {
         // tangent-Sampson pre-step: scaled pixels -> unit bearing + unprojection Jacobian of both images
         double v[9];
-        cam_unproject_with_jac(d.cam_a, a0 * d.scale, a1 * d.scale, v, v + 3);
+        cam_unproject_with_jac<X>(d.cam_a, a0 * d.scale, a1 * d.scale, v, v + 3);
 #pragma unroll
         for (int j = 0; j < 3; ++j) d.s64[(size_t)j * d.n_pad + k] = v[j];
 #pragma unroll
         for (int j = 0; j < 6; ++j) d.s64[(size_t)(6 + j) * d.n_pad + k] = v[3 + j];
         const double b0 = d.b[2 * (size_t)idx], b1 = d.b[2 * (size_t)idx + 1];
-        cam_unproject_with_jac(d.cam_b, b0 * d.scale, b1 * d.scale, v, v + 3);
+        cam_unproject_with_jac<X>(d.cam_b, b0 * d.scale, b1 * d.scale, v, v + 3);
 #pragma unroll
         for (int j = 0; j < 3; ++j) d.s64[(size_t)(3 + j) * d.n_pad + k] = v[j];
 #pragma unroll
         for (int j = 0; j < 6; ++j) d.s64[(size_t)(12 + j) * d.n_pad + k] = v[3 + j];
         return;
     }
-    if (d.mode == 1) cam_unproject2(d.cam_a, a0, a1, a0, a1);
+    if (d.mode == 1) cam_unproject2<X>(d.cam_a, a0, a1, a0, a1);
     if (d.mode == 1 && d.b_dim == 2) {
         double b0, b1;
-        cam_unproject2(d.cam_b, d.b[2 * (size_t)idx], d.b[2 * (size_t)idx + 1], b0, b1);
+        cam_unproject2<X>(d.cam_b, d.b[2 * (size_t)idx], d.b[2 * (size_t)idx + 1], b0, b1);
         d.s64[0 * (size_t)d.n_pad + k] = a0;
         d.s64[1 * (size_t)d.n_pad + k] = a1;
         d.s64[2 * (size_t)d.n_pad + k] = b0;
@@ -175,11 +176,14 @@ void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream
     if (n_desc <= 0) return;
     k_normalize<<<n_desc, NORM_THREADS, 0, stream>>>(descs_dev);
 }
-void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream) {
+void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, bool xcam, cudaStream_t stream) {
     if (n_desc <= 0) return;
     const int threads = 256;
     dim3 grid((max_n_pad + threads - 1) / threads, n_desc, 1);
-    k_transpose<<<grid, threads, 0, stream>>>(descs_dev);
+    if (xcam)
+        k_transpose<true><<<grid, threads, 0, stream>>>(descs_dev);
+    else
+        k_transpose<false><<<grid, threads, 0, stream>>>(descs_dev);
 }
 
 // ============================================================================================================
@@ -1880,7 +1884,7 @@ template <class Shared> PLB_DEV int block_bcast(Shared *S, int v) {
 // refiners) AND the normal equations JtJ (lower triangle, packed row-major), Jtr + count of non-zero-weight rows
 // (compute_jacobian), accumulated separately exactly as two passes of the reference would.
 // Output layout in S->tot: [0] loss sum, [1] residual rows, [2..2+NT) JtJ, [2+NT..2+NT+NP) Jtr, [2+NT+NP] jac rows.
-template <int KIND>
+template <int KIND, bool X = false>
 PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn &L, const int *list, int lo, int na,
                           LmShared<LmDims<KIND>::NP> *S, int &buf, int csize) {
     constexpr int NP = LmDims<KIND>::NP;
@@ -1899,8 +1903,8 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn
             if (Z2 < 0) continue; // optim/absolute.h:57-58,93-94
             double zp0, zp1, xr0, xr1, Jp[2][3];
             if (prm.use_camera) { // <Model>::project for the residual, ::project_with_jac for the Jacobian pass
-                cam_project(prm.cam, Z0, Z1, Z2, xr0, xr1); // (optim/absolute.h:59-61,97-104)
-                cam_project_with_jac(prm.cam, Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
+                cam_project<X>(prm.cam, Z0, Z1, Z2, xr0, xr1); // (optim/absolute.h:59-61,97-104)
+                cam_project_with_jac<X>(prm.cam, Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
             } else { // NullCameraModel (camera_models.cc:2708-2722)
                 zp0 = Z0 / Z2;
                 zp1 = Z1 / Z2;
@@ -2055,7 +2059,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn
 // bearings d1, d2 and the unprojection Jacobians M1, M2 at cameras c1, c2, C and J_C of tangent_terms.  The jac_params
 // of both points are staged at st (d1_p) and st + 3 * CAM_MAX_PARAMS (d2_p); st + 6 * CAM_MAX_PARAMS is the scratch of
 // the finite-difference points.  Operation order of the reference on mini-Eigen (products and dots left to right).
-template <int NP>
+template <int NP, bool X = false>
 PLB_DEV void ts_cam_row(const double *E, const double *D, const CamDev &c1, const CamDev &c2, double a0, double a1,
                         double b0, double b1, const double *d1, const double *d2, const double *M1, const double *M2,
                         double C, const double *JC, const int (*idx)[CAM_MAX_PARAMS], const int *m, double *st,
@@ -2133,7 +2137,7 @@ PLB_DEV void ts_cam_row(const double *E, const double *D, const CamDev &c1, cons
 #pragma unroll 1
         for (int q = 0; q < 2; ++q) { // x + eps e_q: dp_e = (jac_params(x + eps e_q) - d_p) / eps
             double dd[3], dM[6];
-            cam_unproject_with_jac_params(cc, q == 0 ? x0 + eps : x0, q == 1 ? x1 + eps : x1, dd, dM, tmp);
+            cam_unproject_with_jac_params<X>(cc, q == 0 ? x0 + eps : x0, q == 1 ? x1 + eps : x1, dd, dM, tmp);
             for (int i = 0; i < m[cam]; ++i) {
                 const int j = idx[cam][i];
                 double f[3];
@@ -2155,7 +2159,7 @@ PLB_DEV void ts_cam_row(const double *E, const double *D, const CamDev &c1, cons
 //         the fixed-camera refiner and the camera columns of ts_cam_row (optim/relative.h:289-441)
 // Every 256 points each thread writes its point's row of the tile; thread e < NV then adds value e of every row in point
 // order.  Order of the sums: points in order inside a CTA, CTAs in rank order (deterministic for a given cluster size).
-template <int KIND>
+template <int KIND, bool X = false>
 PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *cams, const double (*cp)[CAM_MAX_PARAMS],
                            const int *m, const int (*idx)[CAM_MAX_PARAMS], const int *list, int lo, int na,
                            LmCamShared<KIND> *S, double *tile, int &buf, int csize) {
@@ -2208,8 +2212,8 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                 const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
                 if (!(Z2 < 0)) { // optim/absolute.h:57-58,93-94
                     double xr0, xr1, zp0, zp1, Jp[2][3];
-                    cam_project(cam[0], Z0, Z1, Z2, xr0, xr1);
-                    cam_project_with_jac(cam[0], Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
+                    cam_project<X>(cam[0], Z0, Z1, Z2, xr0, xr1);
+                    cam_project_with_jac<X>(cam[0], Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
                     const double x0 = P.p[0][k], x1 = P.p[1][k];
                     const double q0 = xr0 - x0, q1 = xr1 - x1;
                     tr[Y::LOSS] = L.loss(q0 * q0 + q1 * q1);
@@ -2235,7 +2239,7 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                             Jr[3] = dZ[0]; Jr[4] = dZ[1]; Jr[5] = dZ[2];
                         }
                         // J.col(6 + c) = J_params.col(camera_refine_idx[c]); jac_params is staged in the row's tail
-                        cam_jac_params(cam[0], Z0, Z1, Z2, tr + Y::JP);
+                        cam_jac_params<X>(cam[0], Z0, Z1, Z2, tr + Y::JP);
 #pragma unroll
                         for (int c = 0; c < NP - 6; ++c) {
                             tr[6 + c] = c < m[0] ? tr[Y::JP + idx[0][c]] : 0.0;
@@ -2246,8 +2250,8 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
             } else { // KIND_RELPOSE_TS
                 const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
                 double d1[3], d2[3], M1[6], M2[6];
-                cam_unproject_with_jac_params(cam[0], a0, a1, d1, M1, tr + Y::JP);
-                cam_unproject_with_jac_params(cam[1], b0, b1, d2, M2, tr + Y::JP + 3 * CAM_MAX_PARAMS);
+                cam_unproject_with_jac_params<X>(cam[0], a0, a1, d1, M1, tr + Y::JP);
+                cam_unproject_with_jac_params<X>(cam[1], b0, b1, d2, M2, tr + Y::JP + 3 * CAM_MAX_PARAMS);
                 double C, JC[4];
                 tangent_terms(ctx, d1, d2, M1, M2, C, JC);
                 {
@@ -2264,7 +2268,7 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                     tr[Y::JROW] = 1.0;
                     tr[Y::WT] = w;
                     tr[Y::WR] = w * r;
-                    ts_cam_row<NP>(ctx, ctx + 9, cam[0], cam[1], a0, a1, b0, b1, d1, d2, M1, M2, C, JC, idx, m,
+                    ts_cam_row<NP, X>(ctx, ctx + 9, cam[0], cam[1], a0, a1, b0, b1, d1, d2, M1, M2, C, JC, idx, m,
                                    tr + Y::JP, tr);
                 }
             }
@@ -2367,7 +2371,7 @@ template <class Shared, class Keep> PLB_DEV int lm_compact(Shared *S, int lo, in
 // CAM writes camera i of job j to cam_outs[(j * kind_cam_count(KIND) + i) * CAM_MAX_PARAMS ..].
 template <int KIND, bool CAM> struct LmNP { static constexpr int v = LmDims<KIND>::NP; };
 template <int KIND> struct LmNP<KIND, true> { static constexpr int v = LmCamLayout<KIND>::NP; };
-template <int KIND, bool CAM>
+template <int KIND, bool CAM, bool X = false>
 __global__ void __launch_bounds__(LM_THREADS, 1)
     k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
          const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
@@ -2478,9 +2482,9 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
     // one evaluation pass at par (trial: par_new), totals in S.tot
     auto eval = [&](bool trial) {
         if constexpr (CAM)
-            lmi_eval_pass<KIND>(P, L, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+            lmi_eval_pass<KIND, X>(P, L, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
         else
-            lm_eval_pass<KIND>(P, prm, L, list, lo, na, &S, buf, csize);
+            lm_eval_pass<KIND, X>(P, prm, L, list, lo, na, &S, buf, csize);
     };
 
     int iterations = 0;
@@ -2648,7 +2652,7 @@ static int lm_cluster_size(int n_jobs, int max_n) {
 }
 // A grid of n_clusters clusters of csize CTAs over a job list: k_lm<kind> of the fixed-camera refiner, or with
 // refine_camera the refiner with camera parameters of the kind (KIND_PNP or KIND_RELPOSE_TS).
-static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs,
+static void launch_lm_any(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs,
                           const LoJobSrc *job_src, const double *models_in, const int *n_jobs_dev, int n_jobs,
                           int n_clusters, int csize, const char *mask_base, int *idx_scratch, int scratch_stride,
                           LmJobOut *out, double *cam_out, cudaStream_t stream) {
@@ -2672,20 +2676,25 @@ static void launch_lm_any(int kind, bool refine_camera, const ProblemDev *probs,
         cudaLaunchKernelEx(&cfg, kernel, probs, jobs, job_src, models_in, n_jobs_dev, n_jobs, mask_base, idx_scratch,
                            scratch_stride, out, cam_out);
     };
+    // xcam: a camera of the jobs is a fisheye or division model.  Only the refiners that evaluate cameras have an X
+    // instantiation: the PnP refiners (prm.cam, the camera refiner's camera) and the tangent-Sampson camera refiner.
     if (refine_camera) {
-        auto cam_kernel = kind == KIND_RELPOSE_TS ? k_lm<KIND_RELPOSE_TS, true> : k_lm<KIND_PNP, true>;
+        auto cam_kernel = kind == KIND_RELPOSE_TS ? (xcam ? k_lm<KIND_RELPOSE_TS, true, true> : k_lm<KIND_RELPOSE_TS, true>)
+                                                  : (xcam ? k_lm<KIND_PNP, true, true> : k_lm<KIND_PNP, true>);
         cudaFuncSetAttribute(cam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile);
         launch(cam_kernel);
+    } else if (xcam && kind == KIND_PNP) {
+        launch(k_lm<KIND_PNP, false, true>);
     } else {
         with_kind(kind, [&](auto K) { launch(k_lm<K, false>); });
     }
 }
-void launch_lm(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in,
-               int n_jobs, int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out,
-               double *cam_out, cudaStream_t stream) {
+void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs_dev,
+               const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
+               int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream) {
     if (n_jobs <= 0) return;
     const int csize = lm_cluster_size(n_jobs, max_n);
-    launch_lm_any(kind, refine_camera, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base,
+    launch_lm_any(kind, refine_camera, xcam, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base,
                   idx_scratch, scratch_stride, out, cam_out, stream);
 }
 // Clusters of a round's LO launch: at most one wave (a k_lm CTA owns an SM), at most the estimated number of jobs.
@@ -2703,7 +2712,7 @@ void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const
     if (est_jobs < 1) est_jobs = 1;
     const int csize = lm_cluster_size(est_jobs, max_n);
     const int nc = lm_round_max_clusters(kind, est_jobs, max_n);
-    launch_lm_any(kind, false, probs, tmpl, job_src, models, n_jobs_dev, job_cap, nc, csize, nullptr, idx_scratch,
+    launch_lm_any(kind, false, false, probs, tmpl, job_src, models, n_jobs_dev, job_cap, nc, csize, nullptr, idx_scratch,
                   scratch_stride, out, nullptr, stream);
 }
 

@@ -217,7 +217,8 @@ struct MaskDesc {
 // normalize_points for n_desc problems (descriptors in device memory), one CTA each.
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream);
 // AoS (caller layout) -> SoA fp64 + fp32 for n_desc problems (descriptors in device memory), camera pre-step fused.
-void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream);
+// xcam: some camera of the descriptors is a fisheye or division model (the kernel's instantiation that evaluates them)
+void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, bool xcam, cudaStream_t stream);
 // Solve + score kernels of one round (kind = kind of every problem of the group); *out.overflow must be zeroed.
 // mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (the candidates k_select lists are
 // rescored exactly by launch_confirm).  fctx (mode 1): scratch of scr::CTX_FLOATS floats per model slot for the
@@ -231,9 +232,10 @@ void launch_score_models(int kind, const ProblemDev *probs, const double *models
 // KIND_RELPOSE_TS): every job refines camera parameters with the pose (LmJob::cam_refine) and writes its
 // kind_cam_count(kind) cameras to cam_out[(j * kind_cam_count(kind) + i) * CAM_MAX_PARAMS ..].
 constexpr __host__ __device__ int kind_cam_count(int kind) { return kind == KIND_RELPOSE_TS ? 2 : 1; }
-void launch_lm(int kind, bool refine_camera, const ProblemDev *probs, const LmJob *jobs_dev, const double *models_in,
-               int n_jobs, int max_n, const char *mask_base, int *idx_scratch, int scratch_stride, LmJobOut *out,
-               double *cam_out, cudaStream_t stream);
+// xcam: some camera of the jobs (prm.cam, or the problem's cameras) is a fisheye or division model
+void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs_dev,
+               const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
+               int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream);
 // LO jobs of a round, listed on the device by k_pass1: job j refines model slot job_src[j].slot of the round's model
 // list (stride MSZ) with the template tmpl[job_src[j].pidx]; *n_jobs_dev jobs.  A persistent grid of clusters walks the
 // list; est_jobs (host estimate) only sizes the clusters / the grid.
