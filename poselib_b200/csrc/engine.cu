@@ -18,6 +18,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <chrono>
 #include <condition_variable>
 #include <functional>
@@ -412,8 +413,6 @@ static LmParams lo_params(int kind, double max_error) {
     p.max_lambda = 1e10;
     p.subset_mode = (kind == KIND_RELPOSE) ? 1 : 0;
     p.subset_sq_thr = 5 * (max_error * max_error); // estimators/relative_pose.cc:70
-    p.use_camera = 0;
-    p.cam.model = CAMM_NULL;
     p.score_after = 1;
     return p;
 }
@@ -430,7 +429,6 @@ static LmParams bundle_params(const plb_bundle_opt &b) {
     p.min_lambda = b.min_lambda;
     p.max_lambda = b.max_lambda;
     p.subset_mode = 2;
-    p.cam.model = CAMM_NULL;
     p.score_after = 0;
     return p;
 }
@@ -439,17 +437,16 @@ struct FinalPolish { // the post-RANSAC refinement of PoseLib/robust.cc (estimat
     bool enabled = false;
     plb_bundle_opt bundle;
     size_t min_inliers = 0; // run iff stats.num_inliers > min_inliers
-    // pnp: refine in pixel*scale coordinates with the rescaled camera (robust.cc:103-123); relpose tangent Sampson with
-    // camera refinement: x1*scale (px_scaled) and x2*scale (px2_scaled), the pixels the problem's arrays come from
-    // (robust.cc:255-282).  2n doubles (AoS) each, or null
-    const double *px_scaled = nullptr, *px2_scaled = nullptr;
-    CamDev cam{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
-    // Image* / ImagePair* forms: CAM_REFINE_* flags of the camera parameters refined with the pose (LmJob::cam_refine),
-    // and cam_out receives the camera (relpose: both cameras, from Task::cam_a / cam_b) after the polish, rescaled back by
-    // 1 / scale (robust.cc:103-123)
-    int cam_refine = 0;
-    plb_camera *cam_out = nullptr, *cam2_out = nullptr;
+    // The cameras the bundle evaluates, kind_cam_count(kind) of them, rescaled by `scale`; CAMM_NULL when it evaluates
+    // none.  With a camera the bundle runs on the task's polish problem, whose pixels are the caller's times scale: pnp
+    // robust.cc:103-123, relpose tangent Sampson with camera refinement :255-282.
+    CamDev cam[2] = {{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}}, {CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}}};
     double scale = 1.0;
+    // Image* / ImagePair* forms: CAM_REFINE_* flags of the camera parameters refined with the pose (LmJob::cam_refine),
+    // and cam_out[i] (or null) receives cam[i] after the polish, rescaled back by 1 / scale (robust.cc:103-123)
+    int cam_refine = 0;
+    plb_camera *cam_out[2] = {nullptr, nullptr};
+    bool evaluates_camera() const { return cam[0].model != CAMM_NULL || cam[1].model != CAMM_NULL; }
 };
 
 // ---- small host-side 3x3 helpers for the estimate_* wrappers (column-major <-> row-major) ---------------------
@@ -604,8 +601,8 @@ static bool profiling() {
     return on;
 }
 
-// The camera after the polish of estimate_absolute_pose: the (refined) parameters of the rescaled camera `cam`, rescaled
-// by 1 / scale into `out` (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
+// A camera after the final polish: the (refined) parameters of the rescaled camera `c`, rescaled by 1 / scale into `out`
+// (robust.cc:121-122; the round trip can change last bits even when nothing was refined).
 static void polish_camera_out(CamDev c, double scale, const double *params, plb_camera *out) {
     for (int i = 0; i < CAM_MAX_PARAMS; ++i) c.p[i] = params[i];
     cam_rescale(c, 1.0 / scale);
@@ -718,7 +715,8 @@ struct Group {
     // ---- device layout of the group: SoA arrays of every non-resident problem, masks, ProblemDev table -------------
     // Stages the caller's arrays and issues their host -> device copies; the layout kernel runs in transpose().
     int upload() {
-        int rc, n_polish_pnp = 0;
+        int rc, n_polish = 0;
+        const int nc = kind_cam_count(kind);
         for (PState &S : PS) {
             if (S.n == 0) continue;
             if (!S.t->res) {
@@ -730,14 +728,13 @@ struct Group {
             mask_bytes += (size_t)S.n_pad;
             max_n = std::max(max_n, S.n);
             max_n_pad = std::max(max_n_pad, S.n_pad);
-            if (kind == KIND_PNP && S.t->polish.enabled && S.t->polish.px_scaled) {
-                px_elems += 2 * (size_t)S.n_pad;
-                ++n_polish_pnp;
+            if (S.t->polish.evaluates_camera()) {
+                px_elems += 2 * (size_t)nc * S.n_pad;
+                ++n_polish;
             }
-            if (kind == KIND_RELPOSE_TS && S.t->polish.px_scaled) px_elems += 4 * (size_t)S.n_pad;
         }
-        n_probdev = NP + n_polish_pnp;
-        if ((rc = E.h_in.ensure(in_doubles + px_elems)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
+        n_probdev = NP + n_polish;
+        if ((rc = E.h_in.ensure(in_doubles)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
             (rc = E.soa32.ensure(soa_elems)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
             (rc = E.mask_bits.ensure(mask_bytes / 32 + 1)) || (rc = E.h_mask_bits.ensure(mask_bytes / 32 + 1)) ||
             (rc = E.work.ensure(8)) || (rc = E.probs.ensure(n_probdev)) ||
@@ -771,6 +768,7 @@ struct Group {
                     P.f[c] = S.t->res->soa32.p + (size_t)c * S.n_pad;
                 }
                 P.cmax = S.t->res->cmax.p;
+                assert(!S.t->polish.evaluates_camera()); // plb_resident_create takes no camera
             } else {
                 S.in_off = (long long)in_off;
                 if (host_pinned(S.t->a) && host_pinned(S.t->b)) {
@@ -805,37 +803,19 @@ struct Group {
                         P.f[c] = D.s32 + (size_t)c * S.n_pad;
                     }
                 }
+                const FinalPolish &fp = S.t->polish;
+                D.px = fp.evaluates_camera() ? E.px64.p + px_off : nullptr;
+                D.px_scale = fp.scale;
+                if (D.px) { // the polish problem: this one with the polish cameras and their pixels
+                    S.polish_pidx = NP + ipol++;
+                    ProblemDev &PP = E.h_probs.p[S.polish_pidx];
+                    PP = P;
+                    for (int c = 0; c < 2 * nc; ++c) PP.p[c] = D.px + (size_t)c * S.n_pad;
+                    for (int c = 0; c < nc; ++c) PP.cam[c] = fp.cam[c];
+                    px_off += 2 * (size_t)nc * S.n_pad;
+                }
                 in_off += (size_t)in_arr * S.n;
                 soa_off += (size_t)n_arr * S.n_pad;
-            }
-            if (kind == KIND_PNP && S.t->polish.enabled && S.t->polish.px_scaled) {
-                // scaled pixels staged as SoA by the host (O(N) once); extra ProblemDev for the polish job
-                double *hp = E.h_in.p + in_doubles + px_off;
-                for (int k = 0; k < S.n; ++k) {
-                    hp[k] = S.t->polish.px_scaled[2 * k];
-                    hp[S.n_pad + k] = S.t->polish.px_scaled[2 * k + 1];
-                }
-                for (int k = S.n; k < S.n_pad; ++k) hp[k] = hp[S.n_pad + k] = 0.0;
-                S.polish_pidx = NP + ipol;
-                ProblemDev &PP = E.h_probs.p[NP + ipol];
-                PP = P;
-                PP.p[0] = E.px64.p + px_off;
-                PP.p[1] = E.px64.p + px_off + S.n_pad;
-                px_off += 2 * (size_t)S.n_pad;
-                ++ipol;
-            }
-            if (kind == KIND_RELPOSE_TS && S.t->polish.px_scaled) {
-                // the pixels of both images as SoA for the camera-refining refiner, with the cameras of the pre-step
-                double *hp = E.h_in.p + in_doubles + px_off;
-                const double *src[2] = {S.t->polish.px_scaled, S.t->polish.px2_scaled};
-                for (int c = 0; c < 4; ++c) {
-                    for (int k = 0; k < S.n; ++k) hp[c * (size_t)S.n_pad + k] = src[c >> 1][2 * k + (c & 1)];
-                    for (int k = S.n; k < S.n_pad; ++k) hp[c * (size_t)S.n_pad + k] = 0.0;
-                    P.p[c] = E.px64.p + px_off + c * (size_t)S.n_pad;
-                }
-                P.cam[0] = S.t->cam_a;
-                P.cam[1] = S.t->cam_b;
-                px_off += 4 * (size_t)S.n_pad;
             }
         }
         // The lock-step groups of a batch call start together; left alone, their host->device copies interleave on the
@@ -852,10 +832,6 @@ struct Group {
             PLB_CUDA(cudaMemcpyAsync(E.in.p + off, E.h_in.p + off, sizeof(double) * len, cudaMemcpyHostToDevice, st));
             h2d += sizeof(double) * len;
             i = j;
-        }
-        if (px_elems) {
-            PLB_CUDA(cudaMemcpyAsync(E.px64.p, E.h_in.p + in_doubles, sizeof(double) * px_elems, cudaMemcpyHostToDevice, st));
-            h2d += sizeof(double) * px_elems;
         }
         return PLB_OK;
     }
@@ -922,19 +898,17 @@ struct Group {
     // Stages a batch of LM jobs (job j: start model batch[j].model, results in E.h_lm_out[j]) and launches one k_lm per
     // refiner: the jobs that refine the camera come last and write their kind_cam_count(kind) cameras to row j of
     // E.h_cam_out.  The caller synchronises.
-    // A job refines camera parameters when the flags select some of its camera (PnP: prm.cam) or cameras (tangent
-    // Sampson: the problem's two cameras, ProblemDev::cam)
+    // A job refines camera parameters when the flags select some of a camera of its problem (ProblemDev::cam)
     bool refines_camera(const LmJob &J) const {
-        if (kind != KIND_RELPOSE_TS) return plb::refines_camera(J.prm.cam, J.cam_refine);
-        const ProblemDev &P = E.h_probs.p[J.pidx];
-        return plb::refines_camera(P.cam[0], J.cam_refine) || plb::refines_camera(P.cam[1], J.cam_refine);
+        for (int i = 0; i < kind_cam_count(kind); ++i)
+            if (plb::refines_camera(E.h_probs.p[J.pidx].cam[i], J.cam_refine)) return true;
+        return false;
     }
-    // A job evaluates a fisheye or division camera: its prm.cam (PnP) or the problem's cameras (tangent Sampson)
+    // A job evaluates a fisheye or division camera
     bool uses_x_camera(const LmJob &J) const {
-        if (J.prm.use_camera && cam_is_x(J.prm.cam.model)) return true;
-        if (kind != KIND_RELPOSE_TS) return false;
-        const ProblemDev &P = E.h_probs.p[J.pidx];
-        return cam_is_x(P.cam[0].model) || cam_is_x(P.cam[1].model);
+        for (int i = 0; i < kind_cam_count(kind); ++i)
+            if (cam_is_x(E.h_probs.p[J.pidx].cam[i].model)) return true;
+        return false;
     }
     int lm_batch(const std::vector<LmTask> &batch) {
         const int nj = (int)batch.size(), nc = kind_cam_count(kind);
@@ -1429,12 +1403,7 @@ struct Group {
             for (PState &S : PS) {
                 if (S.n == 0 || !S.t->polish.enabled || S.stats.num_inliers <= S.t->polish.min_inliers) continue;
                 const FinalPolish &fp = S.t->polish;
-                LmJob J = lm_job(S.pidx, S.mask_off, bundle_params(fp.bundle));
-                if (S.polish_pidx >= 0) {
-                    J.pidx = S.polish_pidx;
-                    J.prm.use_camera = 1;
-                    J.prm.cam = fp.cam;
-                }
+                LmJob J = lm_job(S.polish_pidx >= 0 ? S.polish_pidx : S.pidx, S.mask_off, bundle_params(fp.bundle));
                 J.cam_refine = fp.cam_refine;
                 if (refines_camera(J) != (cam == 1)) continue;
                 pol.push_back({S.best_model, J});
@@ -1447,19 +1416,14 @@ struct Group {
         PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
         if ((rc = sync())) return rc;
         for (size_t j = 0; j < pol.size(); ++j) {
-            const Task &t = *pol_of[j]->t;
-            const FinalPolish &fp = t.polish;
+            const FinalPolish &fp = pol_of[j]->t->polish;
             std::copy(E.h_lm_out.p[j].model, E.h_lm_out.p[j].model + MSZ, pol_of[j]->best_model);
             const bool refined = refines_camera(pol[j].job);
-            const double *cams = refined ? E.h_cam_out.p + j * kind_cam_count(kind) * CAM_MAX_PARAMS : nullptr;
-            if (kind == KIND_RELPOSE_TS) { // the pair's refined cameras (only where the polish refined them)
-                if (fp.cam_out && refined) {
-                    polish_camera_out(t.cam_a, fp.scale, cams, fp.cam_out);
-                    polish_camera_out(t.cam_b, fp.scale, cams + CAM_MAX_PARAMS, fp.cam2_out);
-                }
-            } else if (fp.cam_out) {
-                polish_camera_out(fp.cam, fp.scale, refined ? cams : fp.cam.p, fp.cam_out);
-            }
+            for (int i = 0; i < kind_cam_count(kind); ++i)
+                if (fp.cam_out[i])
+                    polish_camera_out(fp.cam[i], fp.scale,
+                                      refined ? E.h_cam_out.p + (j * kind_cam_count(kind) + i) * CAM_MAX_PARAMS : fp.cam[i].p,
+                                      fp.cam_out[i]);
         }
         for (PState &S : PS) {
             if (S.t->inliers && S.n > 0) {
@@ -1559,14 +1523,14 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 }
 
 // One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
-// group (sq_thr 0, no normalisation, no pre-step beyond the cameras), then one LM job over every point.
-// PnP on an Image (bundle.cc:95-112): `proj` is the camera the points are projected with; the parameters the flags
-// cam_refine select are refined with the pose and written to params_out[0].
-// Tangent Sampson on an ImagePair (bundle.cc:237-256): the parameters of cam_a / cam_b the flags select are refined with
-// the pose and written to params_out[0] / params_out[1]; without a selection it is the fixed-camera refiner.
+// group (sq_thr 0, no normalisation, no pre-step beyond the tangent-Sampson one), then one LM job over every point.
+// cams (or null): the kind_cam_count(kind) cameras of the points, in their units (scale 1); the parameters the flags
+// cam_refine select are refined with the pose and written to params_out[i].
+// PnP on an Image (bundle.cc:95-112): the points are projected with cams[0].
+// Tangent Sampson on an ImagePair (bundle.cc:237-256): cams[0] / cams[1] unproject the points; without a selection it is
+// the fixed-camera refiner.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
-                      const plb_bundle_opt &bopt, double *bstats, const CamDev *cam_a = nullptr,
-                      const CamDev *cam_b = nullptr, const CamDev *proj = nullptr, int cam_refine = 0,
+                      const plb_bundle_opt &bopt, double *bstats, const CamDev *cams = nullptr, int cam_refine = 0,
                       double *const *params_out = nullptr) {
     if (n_pts == 0) return PLB_OK;
     Task t;
@@ -1574,35 +1538,31 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     t.a = a;
     t.b = b;
     t.n = n_pts;
-    if (cam_a) t.cam_a = *cam_a;
-    if (cam_b) t.cam_b = *cam_b;
-    const bool pair_refined = kind == KIND_RELPOSE_TS && (refines_camera(t.cam_a, cam_refine) || refines_camera(t.cam_b, cam_refine));
-    if (pair_refined) { // the pixels as given (no rescaling)
-        t.polish.px_scaled = a;
-        t.polish.px2_scaled = b;
+    const int nc = kind_cam_count(kind);
+    if (kind == KIND_RELPOSE_TS) { // the cameras of the pre-step
+        t.cam_a = cams[0];
+        t.cam_b = cams[1];
     }
+    // the bundle evaluates the cameras: PnP always, tangent Sampson only to refine them (else ts carries them)
+    if (cams && (kind == KIND_PNP || refines_camera(cams[0], cam_refine) || refines_camera(cams[1], cam_refine)))
+        std::copy(cams, cams + nc, t.polish.cam);
     std::vector<Task *> v{&t};
     Group G(kind, v);
     int rc;
     if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose())) return rc;
     LmParams prm = bundle_params(bopt);
     prm.subset_mode = 0;
-    if (proj) {
-        prm.use_camera = proj->model != CAMM_NULL;
-        prm.cam = *proj;
-    }
     lm_set_sm_share(100);
-    LmJob J = lm_job(0, -1, prm);
+    LmJob J = lm_job(G.PS[0].polish_pidx >= 0 ? G.PS[0].polish_pidx : 0, -1, prm);
     J.cam_refine = cam_refine;
     if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
     PLB_CUDA(cudaGetLastError());
     const LmJobOut &o = G.E.h_lm_out.p[0];
     std::copy(o.model, o.model + G.MSZ, model);
-    const CamDev *cams[2] = {kind == KIND_PNP ? &prm.cam : &t.cam_a, &t.cam_b};
-    if (kind == KIND_PNP || pair_refined)
-        for (int i = 0; i < kind_cam_count(kind); ++i) {
+    if (G.refines_camera(J))
+        for (int i = 0; i < nc; ++i) {
             int idx[CAM_MAX_PARAMS];
-            const int m = cam_refine_idx(cams[i]->model, cam_refine, idx);
+            const int m = cam_refine_idx(cams[i].model, cam_refine, idx);
             for (int c = 0; c < m; ++c) params_out[i][idx[c]] = G.E.h_cam_out.p[i * CAM_MAX_PARAMS + idx[c]];
         }
     if (bstats) {
@@ -1817,7 +1777,6 @@ int plb_ransac_homography(const double *x1, const double *x2, size_t n, const pl
 struct EstimateJob {
     Task t;
     int api_kind = 0; // PLB_KIND_*
-    std::vector<double> px, px2;
     HM3 T1, T2;
     bool normalised = false;
     double *model = nullptr;
@@ -1832,8 +1791,8 @@ static void default_stats(plb_ransac_stats *stats, plb_counters *counters) {
 }
 // robust.cc:36-126 (absolute pose, no focal estimation), :242-314 (relative pose; tangent_sampson keeps the scaled pixels
 // and runs the tangent-Sampson estimator with the cameras), :544-594 (fundamental), :712-757 (homography).
-// The camera pre-step (Camera::unproject / unproject_with_jac of every point) runs on the device, fused into the layout
-// kernel; normalize_points (F / H) runs here on the calling (worker) thread.
+// The camera pre-step (Camera::unproject / unproject_with_jac of every point) and the scaling of the polish pixels run on
+// the device, fused into the layout kernel, and normalize_points (F / H) in k_normalize: nothing here is O(N).
 // Camera write-back of estimate_absolute_pose (robust.cc:103-123, Image*): CAM_RET_NONE the caller cannot take the camera
 // (refinement flags -> PLB_ERR_ARG), CAM_RET_ALWAYS the Image* form, CAM_RET_REFINED only when parameters are refined.
 // BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params as a bit set
@@ -1881,13 +1840,10 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         fp.bundle.loss_scale = bundle->loss_scale * scale;
         fp.min_inliers = 3;
         if (cam.model != CAMM_NULL) { // the polish runs on pixels*scale with the rescaled camera (robust.cc:103-123)
-            J.px.resize(2 * n);
-            for (size_t k = 0; k < 2 * n; ++k) J.px[k] = x1[k] * scale;
-            fp.px_scaled = J.px.data();
-            fp.cam = cam;
-            cam_rescale(fp.cam, scale);
+            fp.cam[0] = cam;
+            cam_rescale(fp.cam[0], scale);
             fp.scale = scale;
-            if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && refined)) fp.cam_out = camera_out;
+            if (cam_ret == CAM_RET_ALWAYS || (cam_ret == CAM_RET_REFINED && refined)) fp.cam_out[0] = camera_out;
         }
         t.kind = KIND_PNP;
         t.max_error = max_error * scale;
@@ -1917,18 +1873,12 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
             t.pre_mode = 2;
             t.pre_scale = scale;
             if (refined) { // the polish refines the cameras on x * scale with the rescaled cameras (robust.cc:262-282)
-                J.px.resize(2 * n);
-                J.px2.resize(2 * n);
-                for (size_t k = 0; k < 2 * n; ++k) {
-                    J.px[k] = x1[k] * scale;
-                    J.px2[k] = x2[k] * scale;
-                }
-                fp.px_scaled = J.px.data();
-                fp.px2_scaled = J.px2.data();
+                fp.cam[0] = c1;
+                fp.cam[1] = c2;
                 fp.cam_refine = refine_flags(bundle);
                 fp.scale = scale;
-                fp.cam_out = camera_out;
-                fp.cam2_out = camera2_out;
+                fp.cam_out[0] = camera_out;
+                fp.cam_out[1] = camera2_out;
             }
         } else {
             t.kind = KIND_RELPOSE;
@@ -2061,14 +2011,14 @@ int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, con
         g_err = "null argument";
         return PLB_ERR_ARG;
     }
-    CamDev c1, c2;
-    if (int r = camera_dev(camera1, &c1)) return r;
-    if (int r = camera_dev(camera2, &c2)) return r;
-    if (refines_camera(c1, refine_flags(opt)) || refines_camera(c2, refine_flags(opt))) {
+    CamDev cams[2];
+    if (int r = camera_dev(camera1, &cams[0])) return r;
+    if (int r = camera_dev(camera2, &cams[1])) return r;
+    if (refines_camera(cams[0], refine_flags(opt)) || refines_camera(cams[1], refine_flags(opt))) {
         g_err = "NYI: camera refinement needs cameras to return: use plb_refine_relpose_pair";
         return PLB_ERR_NYI;
     }
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, &c1, &c2);
+    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams);
 }
 // robust/bundle.cc:95-112: AbsolutePoseRefiner on an Image, camera_refine_idx from the flags; points in camera units
 int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
@@ -2080,7 +2030,7 @@ int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double p
     CamDev cam;
     if (int r = camera_dev(camera_inout, &cam)) return r;
     double *out[1] = {camera_inout->params};
-    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, nullptr, nullptr, &cam, refine_flags(opt), out);
+    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, &cam, refine_flags(opt), out);
 }
 // robust/bundle.cc:237-256: refine_relpose(x1, x2, ImagePair*, opt), CameraRelativePoseRefiner with the parameters the
 // flags select in either camera (shared_camera false); pixels as given, only the refined parameters written
@@ -2090,11 +2040,11 @@ int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_ca
         g_err = "null argument";
         return PLB_ERR_ARG;
     }
-    CamDev c1, c2;
-    if (int r = camera_dev(camera1_inout, &c1)) return r;
-    if (int r = camera_dev(camera2_inout, &c2)) return r;
+    CamDev cams[2];
+    if (int r = camera_dev(camera1_inout, &cams[0])) return r;
+    if (int r = camera_dev(camera2_inout, &cams[1])) return r;
     double *out[2] = {camera1_inout->params, camera2_inout->params};
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, &c1, &c2, nullptr, refine_flags(opt), out);
+    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, refine_flags(opt), out);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {
@@ -2382,9 +2332,8 @@ int plb_ransac_batch_multi(plb_problem *problems, size_t count, int n_gpus, int 
 }
 
 // Batch form of the four estimate_* entry points (robust.h:45-46,68-70,112-113,133-134): pixels + cameras in, the
-// pre-step of every problem (threshold scaling, camera unprojection on the device, normalize_points on the worker
-// threads), LO-RANSAC in lock-step groups per kind (tangent-Sampson problems form their own groups), final bundle and
-// un-normalisation.  n_gpus: 0 = all devices of the process, k = the first k, -1 = the calling thread's device only.
+// pre-step of every problem (threshold scaling, camera unprojection and normalize_points on the device), LO-RANSAC in
+// lock-step groups per kind (tangent-Sampson problems form their own groups), final bundle and un-normalisation.  n_gpus: 0 = all devices of the process, k = the first k, -1 = the calling thread's device only.
 int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
     if (count == 0) return PLB_OK;
     if (!problems) {
@@ -2405,30 +2354,15 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
     else
         for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
     std::vector<EstimateJob> jobs(count);
-    std::vector<int> rcs(count, PLB_OK);
-    std::vector<std::string> msgs(count);
-    {
-        // the O(N) host part of the pre-step (normalize_points, pixel scaling) in parallel on the worker threads
-        const int nt = (int)std::min<size_t>(count, (size_t)std::max(1, usable_cpus()));
-        auto prep = [&](int w) {
-            for (size_t i = (size_t)w; i < count; i += (size_t)nt) {
-                plb_estimate_problem &p = problems[i];
-                rcs[i] = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
-                                          p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
-                                          &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED);
-                if (rcs[i] != PLB_OK) msgs[i] = g_err;
-            }
-        };
-        if (nt == 1) prep(0);
-        else worker_pool().run(nt, prep);
-    }
-    for (size_t i = 0; i < count; ++i)
-        if (rcs[i] != PLB_OK) {
-            g_err = msgs[i];
-            for (size_t j = 0; j < count; ++j) problems[j].status = rcs[i];
-            return rcs[i];
+    for (size_t i = 0; i < count; ++i) {
+        plb_estimate_problem &p = problems[i];
+        if (int r = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
+                                     p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
+                                     &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED)) {
+            for (size_t j = 0; j < count; ++j) problems[j].status = r;
+            return r;
         }
-    // the tasks point into their EstimateJob (normalised copies, scaled pixels), which stays alive until the end of the call
+    }
     std::vector<Task> tasks(count);
     std::vector<int> dev_of(count, -1);
     for (size_t i = 0; i < count; ++i) tasks[i] = jobs[i].t;

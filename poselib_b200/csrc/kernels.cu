@@ -51,6 +51,14 @@ template <bool X> __global__ void k_transpose(const TransposeDesc *__restrict__ 
     if (k >= d.n_pad) return;
     const int idx = (k < d.n) ? k : (d.n - 1); // pad by repeating the last point (never read by the kernels)
     double a0 = d.a[2 * (size_t)idx], a1 = d.a[2 * (size_t)idx + 1];
+    if (d.px) { // before mode 1 unprojects a0, a1 in place
+        d.px[k] = a0 * d.px_scale;
+        d.px[(size_t)d.n_pad + k] = a1 * d.px_scale;
+        if (d.b_dim == 2) {
+            d.px[2 * (size_t)d.n_pad + k] = d.b[2 * (size_t)idx] * d.px_scale;
+            d.px[3 * (size_t)d.n_pad + k] = d.b[2 * (size_t)idx + 1] * d.px_scale;
+        }
+    }
     if (d.mode == 2) {
         // tangent-Sampson pre-step: scaled pixels -> unit bearing + unprojection Jacobian of both images
         double v[9];
@@ -1885,7 +1893,7 @@ template <class Shared> PLB_DEV int block_bcast(Shared *S, int v) {
 // (compute_jacobian), accumulated separately exactly as two passes of the reference would.
 // Output layout in S->tot: [0] loss sum, [1] residual rows, [2..2+NT) JtJ, [2+NT..2+NT+NP) Jtr, [2+NT+NP] jac rows.
 template <int KIND, bool X = false>
-PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn &L, const int *list, int lo, int na,
+PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list, int lo, int na,
                           LmShared<LmDims<KIND>::NP> *S, int &buf, int csize) {
     constexpr int NP = LmDims<KIND>::NP;
     constexpr int NT = NP * (NP + 1) / 2;
@@ -1902,9 +1910,9 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LmParams &prm, const LossFn
             const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
             if (Z2 < 0) continue; // optim/absolute.h:57-58,93-94
             double zp0, zp1, xr0, xr1, Jp[2][3];
-            if (prm.use_camera) { // <Model>::project for the residual, ::project_with_jac for the Jacobian pass
-                cam_project<X>(prm.cam, Z0, Z1, Z2, xr0, xr1); // (optim/absolute.h:59-61,97-104)
-                cam_project_with_jac<X>(prm.cam, Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
+            if (P.cam[0].model != CAMM_NULL) { // <Model>::project for the residual, ::project_with_jac for the Jacobian pass
+                cam_project<X>(P.cam[0], Z0, Z1, Z2, xr0, xr1); // (optim/absolute.h:59-61,97-104)
+                cam_project_with_jac<X>(P.cam[0], Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
             } else { // NullCameraModel (camera_models.cc:2708-2722)
                 zp0 = Z0 / Z2;
                 zp1 = Z1 / Z2;
@@ -2366,8 +2374,8 @@ template <class Shared, class Keep> PLB_DEV int lm_compact(Shared *S, int lo, in
 // Two refiners: the fixed-camera one of every kind (lm_eval_pass: per-thread packed normal equations, cluster_sum), and
 // CAM, the refiner with camera parameters (lmi_eval_pass: the shared-memory tile summed in point order, which ~255
 // registers of per-thread accumulators for 14 or 21 parameters would not leave room for):
-//   KIND_PNP        AbsolutePoseRefiner, the parameters cam_refine_idx(prm.cam.model, job.cam_refine) of prm.cam
-//   KIND_RELPOSE_TS CameraRelativePoseRefiner, cam_refine_idx(P.cam[i].model, job.cam_refine) of both cameras P.cam[i]
+//   KIND_PNP        AbsolutePoseRefiner, KIND_RELPOSE_TS CameraRelativePoseRefiner: the parameters
+//                   cam_refine_idx(P.cam[i].model, job.cam_refine) of every camera P.cam[i] of the job's problem
 // CAM writes camera i of job j to cam_outs[(j * kind_cam_count(KIND) + i) * CAM_MAX_PARAMS ..].
 template <int KIND, bool CAM> struct LmNP { static constexpr int v = LmDims<KIND>::NP; };
 template <int KIND> struct LmNP<KIND, true> { static constexpr int v = LmCamLayout<KIND>::NP; };
@@ -2458,10 +2466,9 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
         }
         if constexpr (CAM) {
             for (int i = 0; i < kind_cam_count(KIND); ++i) {
-                const CamDev &c0 = KIND == KIND_PNP ? prm.cam : P.cam[i];
-                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[i][c] = c0.p[c];
+                for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.cam[i][c] = P.cam[i].p[c];
                 for (int c = 0; c < CAM_MAX_PARAMS; ++c) S.idx[i][c] = 0;
-                S.m[i] = cam_refine_idx(c0.model, J.cam_refine, S.idx[i]);
+                S.m[i] = cam_refine_idx(P.cam[i].model, J.cam_refine, S.idx[i]);
             }
         }
     }
@@ -2473,7 +2480,7 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
     if constexpr (CAM) {
 #pragma unroll
         for (int i = 0; i < NC; ++i) {
-            cams[i].model = KIND == KIND_PNP ? prm.cam.model : P.cam[i].model;
+            cams[i].model = P.cam[i].model;
             m[i] = S.m[i];
 #pragma unroll
             for (int c = 0; c < CAM_MAX_PARAMS; ++c) idx[i][c] = S.idx[i][c];
@@ -2484,7 +2491,7 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
         if constexpr (CAM)
             lmi_eval_pass<KIND, X>(P, L, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
         else
-            lm_eval_pass<KIND, X>(P, prm, L, list, lo, na, &S, buf, csize);
+            lm_eval_pass<KIND, X>(P, L, list, lo, na, &S, buf, csize);
     };
 
     int iterations = 0;
@@ -2677,7 +2684,7 @@ static void launch_lm_any(int kind, bool refine_camera, bool xcam, const Problem
                            scratch_stride, out, cam_out);
     };
     // xcam: a camera of the jobs is a fisheye or division model.  Only the refiners that evaluate cameras have an X
-    // instantiation: the PnP refiners (prm.cam, the camera refiner's camera) and the tangent-Sampson camera refiner.
+    // instantiation: the PnP refiners and the tangent-Sampson camera refiner.
     if (refine_camera) {
         auto cam_kernel = kind == KIND_RELPOSE_TS ? (xcam ? k_lm<KIND_RELPOSE_TS, true, true> : k_lm<KIND_RELPOSE_TS, true>)
                                                   : (xcam ? k_lm<KIND_PNP, true, true> : k_lm<KIND_PNP, true>);

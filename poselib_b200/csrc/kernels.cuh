@@ -26,8 +26,10 @@ struct ProblemDev {
     int n_pad;      // array stride of ts
     const double *ts;
     const float *cmax; // max |coordinate| of every SoA array (fp64 values rounded up): error bounds of the fp32 screening
-    // RELPOSE_TS with camera refinement: p[0..3] = x1.x x1.y x2.x x2.y (the pixels ts was computed from, SoA, stride
-    // n_pad) and the cameras of the two images; otherwise p[] is null and the cameras are CAMM_NULL
+    // The cameras k_lm evaluates, cam[0 .. kind_cam_count(kind)); CAMM_NULL for a problem whose jobs use no camera.
+    // Only the polish problem of a task whose final bundle evaluates a camera has them: a copy of the task's problem
+    // whose p[0 .. 2 * kind_cam_count(kind)) are the pixels in the units of these cameras (PnP: x.x x.y; RELPOSE_TS:
+    // x1.x x1.y x2.x x2.y, stride n_pad; written by k_transpose).
     CamDev cam[2];
 };
 
@@ -164,16 +166,14 @@ struct LmParams {
     int subset_mode; // 0: all points; 1: relpose LO subset (Sampson+cheirality inliers at subset_sq_thr of the start pose,
                      //    return untouched if <= 5, estimators/relative_pose.cc:70-76); 2: use given mask
     double subset_sq_thr;
-    int use_camera;  // pnp final polish: project with `cam` (rescaled intrinsics) instead of the null camera
-    CamDev cam;
     int score_after; // score the refined model with sq_thr of the problem (count, score)
 };
 struct LmJob {
     int pidx;               // index into probs[]
-    int cam_refine;         // CAM_REFINE_* flags.  KIND_PNP: a job with a non-empty cam_refine_idx(prm.cam.model, cam_refine)
-                            // refines those camera parameters with the pose (AbsolutePoseRefiner, optim/absolute.h:40-171).
-                            // KIND_RELPOSE_TS: a job where either camera of its problem (ProblemDev::cam) has a non-empty
-                            // selection refines both selections with the pose (CameraRelativePoseRefiner, relative.h:268-483)
+    int cam_refine;         // CAM_REFINE_* flags.  A job where some camera of its problem (ProblemDev::cam) has a non-empty
+                            // cam_refine_idx(model, cam_refine) refines every such selection with the pose: KIND_PNP
+                            // AbsolutePoseRefiner (optim/absolute.h:40-171), KIND_RELPOSE_TS CameraRelativePoseRefiner
+                            // (relative.h:268-483)
     long long mask_off;     // offset into the mask buffer (subset_mode 2), else -1
     long long scratch_off;  // offset (ints) into idx_scratch for the active-point list (subset modes 1, 2)
     LmParams prm;
@@ -190,6 +190,8 @@ struct LmJobOut {
 //   mode 1: Camera::unproject to 2D of a (cam_a) and, for 2D-2D kinds, of b (cam_b)   (robust.cc:40-43,287-292)
 //   mode 2: a*scale, b*scale -> unproject_with_jac -> the 18 RELPOSE_TS arrays (robust.cc:255-266,
 //           estimators/relative_pose.h:80-81); s32 unused
+// px (or null): the pixels of the polish problem (ProblemDev::cam), a*px_scale and, for 2D-2D kinds, b*px_scale, as
+// SoA arrays of stride n_pad
 struct TransposeDesc {
     const double *a, *b; // 2n and b_dim*n doubles
     double *s64;
@@ -198,6 +200,8 @@ struct TransposeDesc {
     int n, n_pad, b_dim, mode;
     double scale;
     CamDev cam_a, cam_b;
+    double *px;
+    double px_scale;
 };
 // normalize_points of one problem (robust/utils.cc:584-644, shared scale), in place on the uploaded AoS doubles.
 struct NormDesc {
@@ -232,7 +236,7 @@ void launch_score_models(int kind, const ProblemDev *probs, const double *models
 // KIND_RELPOSE_TS): every job refines camera parameters with the pose (LmJob::cam_refine) and writes its
 // kind_cam_count(kind) cameras to cam_out[(j * kind_cam_count(kind) + i) * CAM_MAX_PARAMS ..].
 constexpr __host__ __device__ int kind_cam_count(int kind) { return kind == KIND_RELPOSE_TS ? 2 : 1; }
-// xcam: some camera of the jobs (prm.cam, or the problem's cameras) is a fisheye or division model
+// xcam: some camera of the jobs' problems (ProblemDev::cam) is a fisheye or division model
 void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs_dev,
                const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
                int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream);
