@@ -1529,10 +1529,11 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 // PnP on an Image (bundle.cc:95-112): the points are projected with cams[0].
 // Tangent Sampson on an ImagePair (bundle.cc:237-256): cams[0] / cams[1] unproject the points; without a selection it is
 // the fixed-camera refiner.
+// No points is not special: the job runs with empty slices and reports what lm_impl reports for an empty problem
+// (iterations 0, costs 0; the fundamental refiner returns the matrix its factorisation reconstructs).
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cams = nullptr, int cam_refine = 0,
                       double *const *params_out = nullptr) {
-    if (n_pts == 0) return PLB_OK;
     Task t;
     t.kind = kind;
     t.a = a;
