@@ -37,7 +37,7 @@ PLB_DEV int min_i(int a, int b) { return a < b ? a : b; }
 // Per-problem maximum |coordinate| of every SoA array (of the fp64 values, rounded up to float): the error bounds of the
 // fp32 screening pass are built on them (screen_math.cuh).  All 32 lanes of a warp call it (n_pad is a multiple of 32).
 // NaN coordinates order above every finite value as unsigned bit patterns, so they poison the maximum (and with it the
-// bounds: every model of such a problem is rescored exactly).
+// bounds: the setups then set scr::REC_ERR0 = +inf and every model of such a problem is rescored exactly).
 PLB_DEV void coord_max(float *cmax, int c, double v) {
     if (!cmax) return;
     const unsigned bits = __float_as_uint(scr::f_up(fabs(v)));
@@ -846,6 +846,7 @@ constexpr int SCR_TM = 8;
 constexpr int SCR_RQ_TAKE = 8; // cases a lane may queue per pass of the warp-compacted handling
 constexpr int SCR_PB = 4;      // correspondences per thread and step of the streaming pass
 constexpr int SCR_CTX_THREADS = 128;
+static_assert(SCR_RQ_TAKE == scr::RQ_TAKE && SCR_TM == scr::REC_TM, "the depth bound of scr::record_depth");
 
 // The fp32 screening constants of every model of the round (scr::CTX_FLOATS floats per model slot, fctx), one
 // thread per model: the fp32 model from model_ctx and the per-model constants of the error bounds (screen_math.cuh),
@@ -1072,16 +1073,17 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             et += red_e[b][w][tid];
         }
         st += (float)n * thr; // the per-correspondence sums hold (r2 - thr) of the inliers only
-        // + the rounding of the fp32 sums themselves: at most n/SCR_THREADS + 24 additions deep over terms of
-        //   magnitude <= thr each (ct of them), and the final n * thr product and addition.  The padding below adds no
-        //   term (a padded correspondence is never recorded), and the correspondence -> (lane, bit) mapping and the
-        //   queue order are those of a pass over the n correspondences alone, so the depth is unchanged.
-        const float depth = (float)(n / SCR_THREADS + 24);
-        et = et * (1.f + 1e-5f) + scr::U * thr * (depth * (float)ct + 2.2f * (float)n);
+        // + the rounding of the fp32 sums themselves (scr::record_err): their depth follows from the queue pass, which
+        //   lets any lane of a warp add a recorded case to its sums.  The padding below adds no term (a padded
+        //   correspondence is never recorded) and no chunk, and the correspondence -> (lane, bit) mapping and the queue
+        //   order are those of a pass over the n correspondences alone, so the depth is unchanged.
+        const uint32_t bd = s_border[b][tid];
         out.fcounts[seg + m0f + tid] = ct;
         out.fscores[seg + m0f + tid] = st;
-        out.fborder[seg + m0f + tid] = s_border[b][tid];
-        out.ferr[seg + m0f + tid] = et * (1.f + 1e-5f);
+        out.fborder[seg + m0f + tid] = bd;
+        // + REC_ERR0: +inf for a model whose fp32 evaluation the bounds do not cover (overflow, non-finite data bounds)
+        out.ferr[seg + m0f + tid] = scr::record_err(et, ct, bd, thr, n, SCR_THREADS) +
+                                    fctx[(size_t)(seg + m0f + tid) * scr::CTX_FLOATS + scr::REC_ERR0];
         s_border[b][tid] = 0u;
     };
     fetch_ctx(0, t_begin * SCR_TM);

@@ -83,8 +83,21 @@ enum {
     T_THRS_HI = 21, // sqrt(thr) rounded up
     T_ED = 22,      // e_d
     T_EW = 23,      // e_w
-    T_ERR_K = 24    // 9 thr_s c
+    T_ERR_K = 24,   // 9 thr_s c
+    // both: added to the record's err — 0, or +inf when the model's fp32 evaluation is not covered by the bounds
+    REC_ERR0 = 25
 };
+
+// The bounds assume finite fp32 arithmetic.  A NaN or infinite coordinate maximum (a NaN coordinate orders above every
+// finite value in k_transpose's maximum), a model constant that does not fit fp32, or an intermediate that can overflow
+// (num, t, z^2 ...) can turn a correspondence's tests into NaN, which the streaming test reads as "certainly an outlier",
+// or into inf, which transfer_point reads as "certainly outside".  The setups bound every such intermediate in fp64 from
+// the same constants; a model whose bound exceeds 2^100 (2^28 below FLT_MAX, which covers the few sums and (1 + k u)
+// factors on top), or is NaN through the data, gets REC_ERR0 = +inf: its record makes no claim and k_select rescores it.
+// A NaN model entry needs no guard: it reaches every residual, so the fp64 test rejects every correspondence, and so does
+// the streaming test; the record 0 +- 0 is exact (the minimal solvers emit such models for degenerate samples).
+SCR_HD float overflow_guard(bool nan_model, bool fits) { return (nan_model || fits) ? 0.f : INFINITY; }
+constexpr double SCR_FIT = 1.2676506002282294e30; // 2^100
 
 // ============================================================================================================
 // Sampson error (robust/utils.cc:158-239):  C = x2^T E x1,  D = (E x1)_0^2 + (E x1)_1^2 + (E^T x2)_0^2 + (E^T x2)_1^2,
@@ -123,6 +136,11 @@ SCR_HD void sampson_setup(const double *M, const float *cmax, double sq_thr, flo
     ctx[S_BETA_P] = f_up(beta * (1.0 + 64.0 * Ud));
     ctx[S_ERR_K] = f_up((4.0 * beta + 2.0 * thr_hi * betaD) * (1.0 + 8.0 * Ud));
     ctx[S_DMIN] = f_up(4.0 * betaD);
+    // |C| <= S, D <= 4 Amax^2, t <= thr D, the model entries themselves (NaN fails every comparison)
+    double msum = 0.0;
+    for (int k = 0; k < 9; ++k) msum += fabs(M[k]);
+    ctx[REC_ERR0] = overflow_guard(msum != msum, msum <= SCR_FIT && S * S <= SCR_FIT && 4.0 * Amax * Amax * fmax(1.0, thr_hi) <= SCR_FIT &&
+                                   alpha * S + beta <= SCR_FIT && ctx[S_ERR_K] <= SCR_FIT);
 }
 struct SampsonTerms {
     float C, D;
@@ -252,6 +270,13 @@ template <int J> SCR_HD void transfer_setup(const double *M, const float *xmax, 
     ctx[T_THRS_P] = f_up(thr_s * (1.0 + 8.0 * Ud));
     ctx[T_C_P] = f_up(c * (1.0 + 8.0 * Ud));
     ctx[T_ERR_K] = f_up(9.0 * thr_s * c * (1.0 + 8.0 * Ud));
+    // |h_r| <= R_r, |w| <= R_2, |d_r| <= R_r + ymax_r R_2 (num), w^2 and thr w^2, z <= thr_s R_2 + c (z^2), the model entries
+    double msum = 0.0;
+    for (int k = 0; k < 3 * (J + 1); ++k) msum += fabs(M[k]);
+    const double d0 = R[0] + (double)ymax[0] * R[2], d1 = R[1] + (double)ymax[1] * R[2], z = thr_s * R[2] + c;
+    ctx[REC_ERR0] = overflow_guard(msum != msum, msum <= SCR_FIT && d0 * d0 + d1 * d1 <= SCR_FIT &&
+                                   R[2] * R[2] * fmax(1.0, thr_s * thr_s) <= SCR_FIT && z * z <= SCR_FIT &&
+                                   (double)ctx[T_ERR_K] <= SCR_FIT);
 }
 struct TransferTerms {
     float num, w;
@@ -302,6 +327,45 @@ SCR_HD void transfer_point(const float *ctx, TransferTerms T, bool &plain, bool 
     v = fmaf(T.num, rw * rw, -thr);
     e = fmaf(ctx[T_ERR_K], rw, 16.f * U * thr);
     if (!(wa > 2.f * e_w)) e = INFINITY;
+}
+
+// ============================================================================================================
+// Rounding of the record's own fp32 sums (k_screen, write_record).  A term that passes through d additions carries at
+// most d factors (1 + delta), so a sum whose terms are at most d additions deep is off by at most gamma_d sum |terms|.
+// The depth of one model's sums in a CTA of NTHR threads:
+//   * per lane: the terms that lane added itself.  The queue pass hands a recorded case to whichever lane picks it up,
+//     not to the lane that owns the correspondence, so a lane's share is NOT n / NTHR: per pass of the queue a lane
+//     handles at most RQ_TAKE entries (the queue holds at most 32 RQ_TAKE), and a chunk of 32 NTHR correspondences needs
+//     at most 32 TM / RQ_TAKE passes (a lane has at most TM models x 32 bits of cases, and it queues min(its cases,
+//     RQ_TAKE) per pass), so a lane adds at most 32 TM = 256 terms per chunk to any one sum.  Neither can it add more
+//     terms than the sum has: count32 for the score, count32 + border for the error bound (plain or border cases);
+//   * the warp butterfly (5 levels), the cross-warp sum (NTHR / 32 additions) and the final + n thr (1).
+//   depth = min(terms, 256 chunks) + 5 + NTHR / 32 + 1.
+// For d u <= 1/16:  gamma_d = d u / (1 - d u) <= 16/15 d u, and a sum of nonnegative terms S computed as S^ satisfies
+// S <= S^ / (1 - gamma_d) = S^ (1 + d u / (1 - 2 d u)) <= S^ (1 + 8/7 d u); 1.25 d u covers both.  Deeper sums (2^20
+// terms per lane: a problem of more than 67 M correspondences) make no claim.
+// The NaN padding of the shared-memory path adds no term and no chunk (it pads to a multiple of 4 NTHR).
+// ============================================================================================================
+constexpr int RQ_TAKE = 8; // SCR_RQ_TAKE of k_screen: cases a lane queues per pass
+constexpr int REC_TM = 8;  // SCR_TM of k_screen: models per tile
+SCR_HD int record_depth(uint32_t terms, int n, int nthr) {
+    const long long chunks = ((long long)n + 32LL * nthr - 1) / (32LL * nthr);
+    const long long per_chunk = 32LL * REC_TM; // (32 REC_TM / RQ_TAKE passes) x RQ_TAKE entries
+    long long lane = (long long)terms < per_chunk * chunks ? (long long)terms : per_chunk * chunks;
+    if (lane > (1LL << 24)) lane = 1LL << 24;
+    return (int)lane + 5 + nthr / 32 + 1;
+}
+// 1.25 d u: bound of gamma_d and of 1 / (1 - gamma_d) - 1 (see above); infinite beyond d = 2^20
+SCR_HD float sum_rel_err(int depth) { return depth <= (1 << 20) ? 1.25f * U * (float)depth : INFINITY; }
+// The record's err from the sum e_sum of the per-correspondence bounds of count32 + border cases:
+//   |score64 - score32| <= (true sum of the e) + gamma_ds count32 thr + 2.2 u n thr,
+// the last term for the rounding of the product n thr and of its addition (|v| <= thr for every inlier term v, and
+// |score32| <= n thr); the outer 1e-5 covers the fp32 evaluation of this expression itself (a handful of roundings).
+SCR_HD float record_err(float e_sum, uint32_t count, uint32_t border, float thr, int n, int nthr) {
+    const float gs = sum_rel_err(record_depth(count, n, nthr));
+    const float ge = sum_rel_err(record_depth(count + border, n, nthr));
+    const float et = e_sum * (1.f + ge) + thr * (gs * (float)count + 2.2f * U * (float)n);
+    return et * (1.f + 1e-5f);
 }
 
 } // namespace scr
