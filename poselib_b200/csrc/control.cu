@@ -204,6 +204,10 @@ void launch_sample(const RoundProb *rp, int na, const SamplerDev *st_in, Sampler
 // candidate selection: ordered scan per problem
 // ============================================================================================================
 constexpr int SEL_THREADS = 256, SEL_WARPS = SEL_THREADS / 32, SEL_SPT = 4;
+// k_select marks a sample's candidates in one 64-bit mask (bit m = model m of the sample)
+static_assert(kind_max_models(KIND_PNP) <= 64 && kind_max_models(KIND_RELPOSE) <= 64 && kind_max_models(KIND_FUND) <= 64 &&
+                  kind_max_models(KIND_HOMOG) <= 64 && kind_max_models(KIND_RELPOSE_TS) <= 64,
+              "a sample's models must fit the candidate mask of k_select");
 
 // Interval [c_lo, c_hi] x [s_lo, s_hi] that contains the exact (fp64) record of model `slot`.
 CTL_DEV void model_interval(const SelectArgs &A, int slot, double &c_lo, double &c_hi, double &s_lo, double &s_hi,

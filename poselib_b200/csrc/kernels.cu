@@ -784,6 +784,14 @@ __global__ void __launch_bounds__(128) k5_back(const RoundDesc R, HypOut out) {
     }
 }
 
+// Models the scoring kernels evaluate in active problem a's segment.  prob_count[a] keeps the whole atomicAdd total
+// even when the segment overflowed (the solve kernels then set out.overflow and drop the samples that did not fit), so
+// it is clamped to the segment: an overflowed round is redone, but its scoring must stay inside the problem's slots.
+__device__ __forceinline__ int seg_models(const HypOut &out, int a) {
+    const int c = out.prob_count[a], cap = __ldg(out.seg_cap + a);
+    return c < cap ? c : cap;
+}
+
 // Score kernel: persistent grid of 256-thread CTAs, one CTA scores one model at a time over all correspondences of
 // the model's problem.
 template <int KIND>
@@ -814,7 +822,7 @@ __global__ void __launch_bounds__(SCORE_THREADS, 2)
     __shared__ double ctx[TM][CTX_MAX];
     __shared__ ScoreRed<TM> red;
     const int a = blockIdx.y;
-    const int count = out.prob_count[a];
+    const int count = seg_models(out, a);
     const int tid = threadIdx.x;
     if (blockIdx.x * TM >= count) return;
     const ProblemDev P = R.probs[R.active[a]];
@@ -858,7 +866,7 @@ __global__ void __launch_bounds__(SCR_CTX_THREADS) k_screen_ctx(const RoundDesc 
     constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
     const int a = blockIdx.y;
     const int m = blockIdx.x * SCR_CTX_THREADS + threadIdx.x;
-    if (m >= out.prob_count[a]) return;
+    if (m >= seg_models(out, a)) return;
     const ProblemDev &P = R.probs[R.active[a]];
     const size_t slot = (size_t)out.seg_base[a] + m;
     double mdl[MSZ];
@@ -968,7 +976,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     __shared__ long long s_first_pre, s_total, s_clo, s_chi, s_Sa;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int na = R.n_active;
-    auto tiles_of = [&](int a) -> int { return (out.prob_count[a] + SCR_TM - 1) / SCR_TM; };
+    auto tiles_of = [&](int a) -> int { return (seg_models(out, a) + SCR_TM - 1) / SCR_TM; };
     auto n_of = [&](int a) -> int { return R.probs[R.active[a]].n; };
     const int per = (na + SCR_THREADS - 1) / SCR_THREADS;
     const int own_lo = min_i(tid * per, na), own_hi = min_i(own_lo + per, na);
@@ -1041,7 +1049,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     __syncthreads();
     uint32_t phase = 0;
     for (int a = s_first; a <= s_last; ++a) {
-    const int count = out.prob_count[a];
+    const int count = seg_models(out, a);
     const ProblemDev P = R.probs[R.active[a]];
     const int n = P.n, n_pad = (n + 31) & ~31;
     int t_begin = 0, t_end = 0;
@@ -2397,11 +2405,13 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
     const int csize = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
     // The grid is a set of clusters that walk the job list: explicit jobs (jobs[j], model j of models_in, stride 9) or
     // the LO jobs k_pass1 listed on the device (template jobs[job_src[j].pidx], model slot job_src[j].slot of the
-    // round's model list, stride MSZ; the count is read from device memory and clamped to n_jobs).
+    // round's model list, stride MSZ; the count is read from device memory and clamped to n_jobs).  For the LO launch of
+    // a round n_jobs_dev is &ctl[CTL_JOB_TOTAL] of the round's control words: a round whose records overflowed
+    // (CTL_FLAGS: k_pass1 left job entries unwritten) is redone by the host, so no job of it runs.
     const int n_clusters = (int)gridDim.x / csize, cluster_id = (int)blockIdx.x / csize;
     int nj = n_jobs;
     if (n_jobs_dev) {
-        const int v = *n_jobs_dev;
+        const int v = n_jobs_dev[CTL_FLAGS - CTL_JOB_TOTAL] != 0 ? 0 : n_jobs_dev[0];
         if (v < nj) nj = v;
     }
     int buf = 0;

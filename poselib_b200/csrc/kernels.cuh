@@ -241,8 +241,10 @@ void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs,
                const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
                int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream);
 // LO jobs of a round, listed on the device by k_pass1: job j refines model slot job_src[j].slot of the round's model
-// list (stride MSZ) with the template tmpl[job_src[j].pidx]; *n_jobs_dev jobs.  A persistent grid of clusters walks the
-// list; est_jobs (host estimate) only sizes the clusters / the grid.
+// list (stride MSZ) with the template tmpl[job_src[j].pidx]; *n_jobs_dev jobs.  n_jobs_dev is &ctl[CTL_JOB_TOTAL] of the
+// round's control words: when the round's CTL_FLAGS word is set no job runs and no job_src entry is read (k_pass1
+// left entries unwritten; the round is redone).  A persistent grid of clusters walks the list; est_jobs (host
+// estimate) only sizes the clusters / the grid.
 void launch_lm_round(int kind, const ProblemDev *probs, const LmJob *tmpl, const LoJobSrc *job_src,
                      const double *models, const int *n_jobs_dev, int job_cap, int est_jobs, int max_n,
                      int *idx_scratch, int scratch_stride, LmJobOut *out, cudaStream_t stream);
