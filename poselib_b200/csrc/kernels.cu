@@ -925,6 +925,15 @@ PLB_DEV void mbar_wait(uint64_t *bar, uint32_t phase) {
 PLB_DEV void lds_v4(const float *p, float *o) {
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]) : "r"(smem_u32(p)));
 }
+PLB_DEV float lds_f(uint32_t saddr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
+    return v;
+}
+// h |= bit if c, as one predicated LOP3 on c's predicate (left to itself the compiler selects bit-or-0 first and ORs that)
+PLB_DEV void or_if(uint32_t &h, bool c, uint32_t bit) {
+    asm("{\n.reg .pred p;\nsetp.ne.u32 p, %1, 0;\n@p or.b32 %0, %0, %2;\n}" : "+r"(h) : "r"((uint32_t)c), "r"(bit));
+}
 PLB_DEV float2 lds_f2(const float2 *p) {
     float2 v;
     asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)));
@@ -1096,6 +1105,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     };
     fetch_ctx(0, t_begin * SCR_TM);
     const float *arr[NARR];
+    uint32_t sarr[NARR] = {}; // shared-memory addresses of the staged arrays (the streaming pass reads them with LDS)
     int n_str = n; // correspondences the streaming pass runs over (padded on the shared-memory path)
     if (use_smem) {
         float *pts = reinterpret_cast<float *>(scr_smem);
@@ -1112,7 +1122,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
         // NaN padding of [n, n_st) of every array, written after this thread saw the bulk copies complete and made
         // visible to all by the barrier below.  A padded correspondence is never recorded: every test of the streaming
         // pass is an ordered comparison, false when an operand is NaN, and NaN coordinates make every operand NaN
-        //   relpose, fundamental: C, D and so g are NaN  ->  sampson_maybe's  g <= thr' D  is false;
+        //   relpose, fundamental: C is NaN  ->  sampson_maybe_c's  |C| <= K  is false;
         //   homography: w is NaN  ->  z = fma(thr_s', |w|, c') is NaN  ->  transfer_maybe's  z > 0  is false;
         //   pnp: the depth z2 is NaN  ->  z is NaN  ->  z > 0  is false.
         // This holds whatever the model constants are, infinite ones included.
@@ -1120,7 +1130,10 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
 #pragma unroll
             for (int c = 0; c < NARR; ++c) pts[(size_t)c * n_st + i] = __int_as_float(0x7fc00000);
 #pragma unroll
-        for (int c = 0; c < NARR; ++c) arr[c] = pts + (size_t)c * n_st;
+        for (int c = 0; c < NARR; ++c) {
+            arr[c] = pts + (size_t)c * n_st;
+            sarr[c] = smem_u32(arr[c]);
+        }
         n_str = n_st;
     } else {
 #pragma unroll
@@ -1145,16 +1158,16 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
         {
             // sc[i] accumulates sum over inliers of (r2 - thr); n*thr is added at the end.
             // The streaming pass is branch-free: the residual terms, one test "could this correspondence be an inlier
-            // of model i in fp64" (the plain fp32 test widened by the rigorous error bound, screen_math.cuh) and a
-            // predicated OR that records the correspondence in a per-lane bit mask.  SCR_PB correspondences per thread
+            // of model i in fp64" (screen_math.cuh: for the Sampson kinds |C| <= K, a bound over the coordinate box that
+            // needs neither D nor E^T x2; for the transfer kinds the plain fp32 test widened by the rigorous error bound)
+            // and a predicated OR that records the correspondence in a per-lane bit mask.  SCR_PB correspondences per thread
             // per step reuse the model constants fetched (broadcast) from shared memory.  The recorded cases (plain
             // decision, is it provably the fp64 decision, cheirality, division, accumulation of score and error bound)
             // are handled afterwards in a compacted loop in which every lane pops one of ITS recorded cases per
             // iteration — handled inline they cost a divergent detour for the whole warp whenever one lane of 32 hits.
-            auto maybe = [&](const float *M, const float *p) -> bool {
+            auto transfer_maybe = [&](const float *M, const float *p) -> bool {
                 if (KIND == KIND_PNP) return scr::transfer_maybe<true>(M, scr::pnp_terms(M, p[0], p[1], p[2], p[3], p[4]));
-                if (KIND == KIND_HOMOG) return scr::transfer_maybe<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]));
-                return scr::sampson_maybe(M, p[0], p[1], p[2], p[3]);
+                return scr::transfer_maybe<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]));
             };
             for (int base = 0; base < n_str; base += 32 * SCR_THREADS) {
                 const int lim = min_i(n_str, base + 32 * SCR_THREADS);
@@ -1163,32 +1176,52 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                 for (int i = 0; i < SCR_TM; ++i) hit[i] = 0u;
                 int k0 = base + tid;
                 uint32_t qbit = 1u;
-                // GUARDED: correspondences at or past lim read as NaN (never recorded, see the padding above)
-                auto step = [&](auto guarded) {
+                // GUARDED: correspondences at or past lim read as NaN (never recorded, see the padding above);
+                // STAGED: the arrays are in shared memory (sarr), read with LDS rather than generic loads
+                auto step = [&](auto guarded, auto staged) {
                     float p[SCR_PB][NARR];
+                    uint32_t bit[SCR_PB];
 #pragma unroll
                     for (int j = 0; j < SCR_PB; ++j) {
                         const int k = k0 + j * SCR_THREADS;
+                        bit[j] = qbit << j;
 #pragma unroll
-                        for (int c = 0; c < NARR; ++c) p[j][c] = (!decltype(guarded)::value || k < lim) ? arr[c][k] : __int_as_float(0x7fc00000);
+                        for (int c = 0; c < NARR; ++c) {
+                            if (decltype(staged)::value) p[j][c] = lds_f(sarr[c] + 4u * (uint32_t)k);
+                            else p[j][c] = (!decltype(guarded)::value || k < lim) ? arr[c][k] : __int_as_float(0x7fc00000);
+                        }
                     }
 #pragma unroll
                     for (int i = 0; i < SCR_TM; ++i) {
-                        if (i < tm) {
+                        if (i >= tm) continue;
+                        if constexpr (KIND == KIND_RELPOSE || KIND == KIND_FUND) {
+                            float E[12]; // [0..8] the model; |C^| <= K is all the test reads
+                            lds_v4(cx[i], E);
+                            lds_v4(cx[i] + 4, E + 4);
+                            E[8] = lds_f(smem_u32(cx[i] + 8));
+                            const float K = lds_f(smem_u32(cx[i] + scr::S_CK));
+#pragma unroll
+                            for (int j = 0; j < SCR_PB; ++j)
+                                or_if(hit[i], scr::sampson_maybe_c(E, K, p[j][0], p[j][1], p[j][2], p[j][3]), bit[j]);
+                        } else {
                             float Mr[20]; // [0..11] model, [16..19] constants of the streaming test
                             lds_v4(cx[i], Mr);
                             lds_v4(cx[i] + 4, Mr + 4);
                             lds_v4(cx[i] + 8, Mr + 8);
                             lds_v4(cx[i] + 16, Mr + 16);
 #pragma unroll
-                            for (int j = 0; j < SCR_PB; ++j)
-                                if (maybe(Mr, p[j])) hit[i] |= qbit << j;
+                            for (int j = 0; j < SCR_PB; ++j) or_if(hit[i], transfer_maybe(Mr, p[j]), bit[j]);
                         }
                     }
                 };
-                for (; k0 + (SCR_PB - 1) * SCR_THREADS < lim; k0 += SCR_THREADS * SCR_PB, qbit <<= SCR_PB)
-                    step(std::false_type{});
-                if (!use_smem && k0 < lim) step(std::true_type{}); // the last < SCR_PB correspondences of this lane
+                auto stream = [&](auto staged) {
+                    for (; k0 + (SCR_PB - 1) * SCR_THREADS < lim; k0 += SCR_THREADS * SCR_PB, qbit <<= SCR_PB)
+                        step(std::false_type{}, staged);
+                    // the last < SCR_PB correspondences of this lane (the staged arrays are padded to whole steps)
+                    if (!decltype(staged)::value && k0 < lim) step(std::true_type{}, staged);
+                };
+                if (use_smem) stream(std::true_type{});
+                else stream(std::false_type{});
                 // Handling of the recorded cases, compacted across the WARP: the lanes list their cases (model, bit, lane)
                 // in a per-warp queue in shared memory — at most SCR_RQ_TAKE per lane and pass, so the queue cannot
                 // overflow — and the warp then works through the queue 32 entries at a time.  A case is evaluated by

@@ -85,7 +85,9 @@ enum {
     T_EW = 23,      // e_w
     T_ERR_K = 24,   // 9 thr_s c
     // both: added to the record's err — 0, or +inf when the model's fp32 evaluation is not covered by the bounds
-    REC_ERR0 = 25
+    REC_ERR0 = 25,
+    // Sampson kinds: the streaming test |C^| <= K (sampson_maybe_c)
+    S_CK = 26
 };
 
 // The bounds assume finite fp32 arithmetic.  A NaN or infinite coordinate maximum (a NaN coordinate orders above every
@@ -115,16 +117,40 @@ constexpr double SCR_FIT = 1.2676506002282294e30; // 2^100
 //   => | (num - t) - (C^2 - thr D) | <= E_f = alpha |C^| + kappa (num + t) + beta,
 //      alpha = 2 eC, kappa = 20u (24u used: covers the fp32 evaluation of E_f itself), beta = eC^2 + thr beta_D (1 + 4u).
 // ============================================================================================================
+// The streaming test of k_screen only needs C^.  Over the coordinate box |e_r| <= A_r and |f_c| <= B_c, so
+//   D <= G = A_0^2 + A_1^2 + B_0^2 + B_1^2,  and with the rounding of D^ above  D^ <= (G + beta_D) / (1 - 13u) <= Dmax,
+//   Dmax = (G + beta_D)(1 + 16u)   (14u for the division, the rest for the fp64 evaluation).
+// Let x = |C^| > K, K the positive root of  x^2 - a x - c,  a = alpha'(1 + 2u),  c = (beta' + max(thr', 0) Dmax)(1 + 5u)
+// (alpha', beta', thr': the stored prefilter constants S_ALPHA_P, S_BETA_P, S_THR_P).  Then
+//   * x^2 - alpha' x - beta' > thr' Dmax >= thr' D^ (D^ >= 0 for thr' < 0): in real arithmetic the correspondence fails
+//     the streaming test, which the prefilter constants make a proof of an fp64 outlier;
+//   * the fp32 evaluation of sampson_maybe fails too:  h = fl(x^2 - beta') >= x^2 (1 - u) - beta' (1 + u),
+//     g = fl(h - alpha' x) >= (x^2 (1 - u) - alpha' x - beta' (1 + u))(1 - u) > thr' Dmax (1 + 3u)(1 - u) >= fl(thr' D^),
+//     which is what 2u on alpha' and 5u on c buy.  So |C^| <= K accepts every correspondence sampson_maybe accepts.
+// K is computed in fp64, widened by 4u for that evaluation and rounded up; a model whose Dmax or K^2 exceeds 2^100 (or is
+// NaN) gets K = +inf, so that every correspondence is recorded and judged by sampson_point.
+SCR_HD void sampson_rows(const double *M, const float *cmax, double *A, double *B) {
+    for (int r = 0; r < 3; ++r) A[r] = fabs(M[3 * r]) * (double)cmax[0] + fabs(M[3 * r + 1]) * (double)cmax[1] + fabs(M[3 * r + 2]);
+    for (int c = 0; c < 2; ++c) B[c] = fabs(M[c]) * (double)cmax[2] + fabs(M[3 + c]) * (double)cmax[3] + fabs(M[6 + c]);
+}
+SCR_HD double sampson_beta_d(const double *A, const double *B) {
+    const double Amax = fmax(fmax(A[0], A[1]), fmax(B[0], B[1]));
+    return 9.0 * Ud * Amax * Amax;
+}
+SCR_HD double sampson_dmax(const double *M, const float *cmax) {
+    double A[3], B[2];
+    sampson_rows(M, cmax, A, B);
+    return (A[0] * A[0] + A[1] * A[1] + B[0] * B[0] + B[1] * B[1] + sampson_beta_d(A, B)) * (1.0 + 16.0 * Ud);
+}
 // M: row-major 3x3 in fp64 (the exact model the fp64 kernels use); cmax: a0max a1max b0max b1max.
 SCR_HD void sampson_setup(const double *M, const float *cmax, double sq_thr, float *ctx) {
-    const double a0 = cmax[0], a1 = cmax[1], b0 = cmax[2], b1 = cmax[3];
+    const double b0 = cmax[2], b1 = cmax[3];
     double A[3], B[2];
-    for (int r = 0; r < 3; ++r) A[r] = fabs(M[3 * r]) * a0 + fabs(M[3 * r + 1]) * a1 + fabs(M[3 * r + 2]);
-    for (int c = 0; c < 2; ++c) B[c] = fabs(M[c]) * b0 + fabs(M[3 + c]) * b1 + fabs(M[6 + c]);
+    sampson_rows(M, cmax, A, B);
     const double S = b0 * A[0] + b1 * A[1] + A[2];
     const double Amax = fmax(fmax(A[0], A[1]), fmax(B[0], B[1]));
     const double eC = 8.0 * Ud * S;
-    const double betaD = 9.0 * Ud * Amax * Amax;
+    const double betaD = sampson_beta_d(A, B);
     const float thr = (float)sq_thr;
     const double thr_hi = (double)thr * (1.0 + 2.0 * Ud) + 1e-300; // >= sq_thr and >= thr^
     const double alpha = 2.0 * eC, beta = eC * eC + thr_hi * betaD * (1.0 + 4.0 * Ud);
@@ -136,6 +162,11 @@ SCR_HD void sampson_setup(const double *M, const float *cmax, double sq_thr, flo
     ctx[S_BETA_P] = f_up(beta * (1.0 + 64.0 * Ud));
     ctx[S_ERR_K] = f_up((4.0 * beta + 2.0 * thr_hi * betaD) * (1.0 + 8.0 * Ud));
     ctx[S_DMIN] = f_up(4.0 * betaD);
+    const double Dmax = sampson_dmax(M, cmax);
+    const double ka = (double)ctx[S_ALPHA_P] * (1.0 + 2.0 * Ud);
+    const double kc = ((double)ctx[S_BETA_P] + fmax((double)ctx[S_THR_P], 0.0) * Dmax) * (1.0 + 5.0 * Ud);
+    const double K = 0.5 * (ka + sqrt(ka * ka + 4.0 * kc)) * (1.0 + 4.0 * Ud);
+    ctx[S_CK] = (Dmax <= SCR_FIT && K * K <= SCR_FIT) ? f_up(K) : INFINITY;
     // |C| <= S, D <= 4 Amax^2, t <= thr D, the model entries themselves (NaN fails every comparison)
     double msum = 0.0;
     for (int k = 0; k < 9; ++k) msum += fabs(M[k]);
@@ -163,6 +194,15 @@ SCR_HD bool sampson_maybe(const float *ctx, float a0, float a1, float b0, float 
     const SampsonTerms T = sampson_terms(ctx, a0, a1, b0, b1);
     const float g = fmaf(-ctx[S_ALPHA_P], fabsf(T.C), fmaf(T.C, T.C, -ctx[S_BETA_P]));
     return g <= ctx[S_THR_P] * T.D;
+}
+// The test k_screen streams with: |C^| <= K (K = ctx[S_CK], derivation at sampson_setup).  It accepts every
+// correspondence sampson_maybe accepts and rejects only provable fp64 outliers.  C^ is the same expression as in
+// sampson_terms, so sampson_point sees the same C^.  Ordered: false for a NaN C^.
+SCR_HD bool sampson_maybe_c(const float *M, float K, float a0, float a1, float b0, float b1) {
+    const float e0 = fmaf(M[0], a0, fmaf(M[1], a1, M[2]));
+    const float e1 = fmaf(M[3], a0, fmaf(M[4], a1, M[5]));
+    const float e2 = fmaf(M[6], a0, fmaf(M[7], a1, M[8]));
+    return fabsf(fmaf(b0, e0, fmaf(b1, e1, e2))) <= K;
 }
 // Full evaluation of one correspondence the streaming pass could not rule out.
 //   plain  : the fp32 decision num < t (what count32 / score32 use)
@@ -344,6 +384,8 @@ SCR_HD void transfer_point(const float *ctx, TransferTerms T, bool &plain, bool 
 // For d u <= 1/16:  gamma_d = d u / (1 - d u) <= 16/15 d u, and a sum of nonnegative terms S computed as S^ satisfies
 // S <= S^ / (1 - gamma_d) = S^ (1 + d u / (1 - 2 d u)) <= S^ (1 + 8/7 d u); 1.25 d u covers both.  Deeper sums (2^20
 // terms per lane: a problem of more than 67 M correspondences) make no claim.
+// The bound holds however many cases the streaming test records (at most RQ_TAKE per lane and pass, at most 32 TM /
+// RQ_TAKE passes per chunk): a looser streaming test sends more cases through the queue, not deeper sums.
 // The NaN padding of the shared-memory path adds no term and no chunk (it pads to a multiple of 4 NTHR).
 // ============================================================================================================
 constexpr int RQ_TAKE = 8; // SCR_RQ_TAKE of k_screen: cases a lane queues per pass
