@@ -204,6 +204,7 @@ struct Engine {
     DevBuf<double> in, soa64, px64, models, lm_in, s5_blk, s5_park, s5_cpoly, s5_roots;
     DevBuf<int> s5_nroots;
     DevBuf<float> soa32, cmax;
+    DevBuf<uint4> qrows; // relpose / fundamental: ProblemDev::q
     DevBuf<uint32_t> samples;
     DevBuf<int> work, slots, subset, act, model_prob, prob_count;
     // round state that stays on the device: sampler states, per-sample / per-model records, candidate lists
@@ -393,6 +394,7 @@ static int usable_cpus() {
 struct Resident {
     DevBuf<double> soa64;
     DevBuf<float> soa32, cmax;
+    DevBuf<uint4> qrows; // relpose / fundamental: ProblemDev::q
     int n = 0, n_pad = 0, kind = 0, device = 0;
 };
 static std::mutex g_res_mtx;
@@ -620,7 +622,7 @@ struct Group {
     std::vector<PState> PS;
     cudaStream_t st = nullptr;
     // device layout of the group (upload)
-    size_t in_doubles = 0, soa_elems = 0, mask_bytes = 0, px_elems = 0;
+    size_t in_doubles = 0, soa_elems = 0, mask_bytes = 0, px_elems = 0, q_rows = 0;
     int max_n = 0, max_n_pad = 0, n_up = 0, n_probdev = 0;
     // Round sizes.  A small group leaves the GPU mostly idle, so speculating further ahead costs little time while every
     // round saved is a whole launch chain of latency: the first round and the per-round cap grow as the group shrinks
@@ -722,6 +724,7 @@ struct Group {
             if (!S.t->res) {
                 in_doubles += (size_t)in_arr * S.n;
                 soa_elems += (size_t)n_arr * S.n_pad;
+                if (kind == KIND_RELPOSE || kind == KIND_FUND) q_rows += (size_t)S.n_pad;
                 ++n_up;
             }
             S.mask_off = (long long)mask_bytes;
@@ -735,7 +738,7 @@ struct Group {
         }
         n_probdev = NP + n_polish;
         if ((rc = E.h_in.ensure(in_doubles)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
-            (rc = E.soa32.ensure(soa_elems)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
+            (rc = E.soa32.ensure(soa_elems)) || (rc = E.qrows.ensure(q_rows)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
             (rc = E.mask_bits.ensure(mask_bytes / 32 + 1)) || (rc = E.h_mask_bits.ensure(mask_bytes / 32 + 1)) ||
             (rc = E.work.ensure(8)) || (rc = E.probs.ensure(n_probdev)) ||
             (rc = E.h_probs.ensure(n_probdev)) || (rc = E.tdesc.ensure(std::max(n_up, 1))) ||
@@ -747,7 +750,7 @@ struct Group {
             size_t bytes;
         };
         std::vector<DirectCopy> direct; // page-locked caller arrays: DMA straight from them (issued below, in one turn)
-        size_t in_off = 0, soa_off = 0, px_off = 0;
+        size_t in_off = 0, soa_off = 0, px_off = 0, q_off = 0;
         std::vector<std::pair<size_t, size_t>> staged; // (offset, doubles) of the inputs that went through the staging buffer
         int iu = 0, ipol = 0;
         for (int i = 0; i < NP; ++i) {
@@ -768,6 +771,7 @@ struct Group {
                     P.f[c] = S.t->res->soa32.p + (size_t)c * S.n_pad;
                 }
                 P.cmax = S.t->res->cmax.p;
+                P.q = S.t->res->qrows.p;
                 assert(!S.t->polish.evaluates_camera()); // plb_resident_create takes no camera
             } else {
                 S.in_off = (long long)in_off;
@@ -795,6 +799,12 @@ struct Group {
                 D.scale = S.t->pre_scale;
                 D.cam_a = S.t->cam_a;
                 D.cam_b = S.t->cam_b;
+                D.q = nullptr;
+                if (kind == KIND_RELPOSE || kind == KIND_FUND) {
+                    D.q = E.qrows.p + q_off;
+                    P.q = D.q;
+                    q_off += (size_t)S.n_pad;
+                }
                 if (kind == KIND_RELPOSE_TS) {
                     P.ts = D.s64;
                 } else {
@@ -891,6 +901,10 @@ struct Group {
             for (int i = 0; i < n_up; ++i) xcam = xcam || cam_is_x(E.h_tdesc.p[i].cam_a.model) || cam_is_x(E.h_tdesc.p[i].cam_b.model);
             launch_transpose(E.tdesc.p, n_up, max_n_pad, xcam, st);
             E.launches++;
+            if (kind == KIND_RELPOSE || kind == KIND_FUND) {
+                launch_qrows(E.tdesc.p, n_up, max_n_pad, st);
+                E.launches++;
+            }
         }
         return PLB_OK;
     }
@@ -2386,7 +2400,9 @@ int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts
     const int n = (int)n_pts, n_pad = (n + 31) & ~31, b_dim = (kind == KIND_PNP) ? 3 : 2, n_arr = 2 + b_dim;
     std::shared_ptr<Resident> R = std::make_shared<Resident>(); // freed on every early return below
     DevBuf<double> da, db;
+    const bool qk = kind == KIND_RELPOSE || kind == KIND_FUND;
     if ((rc = R->soa64.ensure((size_t)n_arr * n_pad)) || (rc = R->soa32.ensure((size_t)n_arr * n_pad)) ||
+        (rc = R->qrows.ensure(qk ? (size_t)n_pad : 0)) ||
         (rc = R->cmax.ensure(8)) || (rc = da.ensure(2 * (size_t)n)) || (rc = db.ensure((size_t)b_dim * n)) ||
         (rc = E.tdesc.ensure(1)) || (rc = E.h_tdesc.ensure(1)))
         return rc;
@@ -2399,6 +2415,7 @@ int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts
     D.s64 = R->soa64.p;
     D.s32 = R->soa32.p;
     D.cmax = R->cmax.p;
+    D.q = qk ? R->qrows.p : nullptr;
     D.n = n;
     D.n_pad = n_pad;
     D.b_dim = b_dim;
@@ -2407,6 +2424,7 @@ int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts
     PLB_CUDA(cudaMemsetAsync(R->cmax.p, 0, sizeof(float) * 8, E.stream));
     PLB_CUDA(cudaMemcpyAsync(E.tdesc.p, E.h_tdesc.p, sizeof(TransposeDesc), cudaMemcpyHostToDevice, E.stream));
     launch_transpose(E.tdesc.p, 1, n_pad, false, E.stream);
+    launch_qrows(E.tdesc.p, 1, n_pad, E.stream);
     PLB_CUDA(cudaStreamSynchronize(E.stream));
     R->n = n;
     R->n_pad = n_pad;

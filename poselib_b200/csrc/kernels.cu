@@ -106,6 +106,23 @@ template <bool X> __global__ void k_transpose(const TransposeDesc *__restrict__ 
         coord_max(d.cmax, 2 + c, v);
     }
 }
+// The integer rows of the Sampson kinds' streaming test (screen_math.cuh), once per problem; zero rows in [n, n_pad).
+__global__ void k_qrows(const TransposeDesc *__restrict__ descs) {
+    const TransposeDesc &d = descs[blockIdx.y];
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (!d.q || k >= d.n_pad) return;
+    uint32_t w[4] = {0u, 0u, 0u, 0u};
+    if (k < d.n) {
+        int e[8];
+        scr::sampson_qscale(d.cmax, e);
+        float f[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] = ldexpf(1.f, 15 - e[j]);
+        const float *s = d.s32;
+        scr::sampson_qrow(s[k], s[(size_t)d.n_pad + k], s[2 * (size_t)d.n_pad + k], s[3 * (size_t)d.n_pad + k], f, w);
+    }
+    d.q[k] = make_uint4(w[0], w[1], w[2], w[3]);
+}
 // normalize_points (robust/utils.cc:584-644, shared scale) of one problem per CTA, in place on the AoS doubles the caller
 // uploaded: optional centroid shift, then division by the mean norm / sqrt(2).  The two reductions run in the order of
 // the reference's loops — one thread adds the terms one after the other (centroid: x1[k], x2[k] for k = 0..n-1 in four
@@ -183,6 +200,10 @@ __global__ void __launch_bounds__(NORM_THREADS) k_normalize(const NormDesc *__re
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream) {
     if (n_desc <= 0) return;
     k_normalize<<<n_desc, NORM_THREADS, 0, stream>>>(descs_dev);
+}
+void launch_qrows(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream) {
+    if (n_desc <= 0) return;
+    k_qrows<<<dim3((max_n_pad + 255) / 256, n_desc, 1), 256, 0, stream>>>(descs_dev);
 }
 void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, bool xcam, cudaStream_t stream) {
     if (n_desc <= 0) return;
@@ -854,6 +875,7 @@ constexpr int SCR_TM = 8;
 constexpr int SCR_RQ_TAKE = 8; // cases a lane may queue per pass of the warp-compacted handling
 constexpr int SCR_PB = 4;      // correspondences per thread and step of the streaming pass
 constexpr int SCR_CTX_THREADS = 128;
+constexpr int QW = 8;          // Sampson kinds: word groups of 8 streaming steps per chunk (hit[] words of a lane)
 static_assert(SCR_RQ_TAKE == scr::RQ_TAKE && SCR_TM == scr::REC_TM, "the depth bound of scr::record_depth");
 
 // The fp32 screening constants of every model of the round (scr::CTX_FLOATS floats per model slot, fctx), one
@@ -884,6 +906,17 @@ __global__ void __launch_bounds__(SCR_CTX_THREADS) k_screen_ctx(const RoundDesc 
     else if (KIND == KIND_HOMOG) scr::transfer_setup<2>(cp, cm, cm + 2, P.sq_thr, c);
     else scr::sampson_setup(cp, cm, P.sq_thr, c);
     if constexpr (KIND == KIND_RELPOSE) scr::cheirality_setup(cp + 9, cp + 13, c);
+    if constexpr (KIND == KIND_RELPOSE || KIND == KIND_FUND) { // the integer streaming test (screen_math.cuh)
+        uint32_t w[4];
+        int qc, qoff;
+        scr::sampson_qmodel(cp, cm, c[scr::S_CK], w, qc, qoff);
+        c[scr::S_QH0] = __uint_as_float(w[0]);
+        c[scr::S_QH1] = __uint_as_float(w[1]);
+        c[scr::S_QL0] = __uint_as_float(w[2]);
+        c[scr::S_QL1] = __uint_as_float(w[3]);
+        c[scr::S_QC] = __int_as_float(qc);
+        c[scr::S_QOFF] = __int_as_float(qoff);
+    }
     float4 *dst = reinterpret_cast<float4 *>(fctx + slot * scr::CTX_FLOATS);
 #pragma unroll
     for (int k = 0; k < scr::CTX_FLOATS / 4; ++k) dst[k] = make_float4(c[4 * k], c[4 * k + 1], c[4 * k + 2], c[4 * k + 3]);
@@ -939,6 +972,19 @@ PLB_DEV float2 lds_f2(const float2 *p) {
     asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)));
     return v;
 }
+// The integer streaming test of the Sampson kinds (screen_math.cuh): the A fragment of 16 staged rows, the s8 MMA with
+// int32 accumulation, and h |= bit if (uint32)v <= lim as one predicated LOP3.
+PLB_DEV void ldsm_x2(uint32_t saddr, uint32_t &r0, uint32_t &r1) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(saddr));
+}
+PLB_DEV void mma_s8(int *d, uint32_t a0, uint32_t a1, uint32_t b, int c0, int c1) {
+    asm("mma.sync.aligned.m16n8k16.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%7,%8,%7,%8};"
+        : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3])
+        : "r"(a0), "r"(a1), "r"(b), "r"(c0), "r"(c1));
+}
+PLB_DEV void or_if_le(uint32_t &h, uint32_t v, uint32_t lim, uint32_t bit) {
+    asm("{\n.reg .pred p;\nsetp.le.u32 p, %1, %2;\n@p or.b32 %0, %0, %3;\n}" : "+r"(h) : "r"(v), "r"(lim), "r"(bit));
+}
 PLB_DEV float warp_sum_f(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -961,11 +1007,18 @@ template <int NTHR> constexpr __host__ __device__ int scr_stage_len(int n) {
 //     and the record writes of tile t are done by threads 0..SCR_TM-1 at the start of tile t+1 (the last tile of a
 //     problem right after its barrier), always in warp order, so the records do not depend on timing;
 //   * on the shared-memory path the staged arrays are padded with NaN to whole streaming steps (scr_stage_len), so there
-//     is no remainder pass; the global-memory path runs one guarded step for the last < SCR_PB correspondences.
+//     is no remainder pass; the global-memory path runs one guarded step for the last < SCR_PB correspondences;
+//   * the Sampson kinds (relpose, fundamental) stream the integer form of |C^| <= K on the int8 tensor cores instead
+//     (screen_math.cuh): the CTA stages the problem's 16 B integer rows (ProblemDev::q, built once per problem by
+//     k_qrows; zero rows up to scr_stage_len), a warp step is one ldmatrix and two mma.m16n8k16.s8 over 16 rows x the
+//     tile's 8 models, and the queue pass reads the fp32 coordinates of a recorded case from global memory.  Unstaged,
+//     the lanes read their fragment words from ProblemDev::q.  A caller that supplies no rows (q null) gets them built
+//     from the fp32 arrays, by the CTA when staged and by every lane for its own words otherwise (the same bits).
 template <int KIND, int NTHR>
 __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const RoundDesc R, HypOut out, const float *__restrict__ fctx, int use_smem) {
     constexpr int SCR_THREADS = NTHR, SCR_WARPS = NTHR / 32; // shadow the file-scope defaults
     constexpr int NARR = (KIND == KIND_PNP) ? 5 : 4;
+    constexpr bool SAMP = KIND == KIND_RELPOSE || KIND == KIND_FUND;
     constexpr int CTX_V4 = scr::CTX_FLOATS / 4;
     extern __shared__ __align__(128) unsigned char scr_smem[];
     __shared__ __align__(8) uint64_t bar;
@@ -974,7 +1027,8 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     __shared__ float red_e[2][SCR_WARPS][SCR_TM];
     __shared__ uint32_t red_c[2][SCR_WARPS][SCR_TM];
     __shared__ uint32_t s_border[2][SCR_TM];
-    __shared__ uint16_t rq[SCR_WARPS][32 * SCR_RQ_TAKE]; // per-warp queue of recorded cases: lane << 8 | bit << 3 | model
+    __shared__ uint16_t rq[SCR_WARPS][32 * SCR_RQ_TAKE]; // per-warp queue of recorded cases: lane << 8 | bit << 3 | hit[] word
+                                                         // (the model; Sampson kinds: the word group)
     // ---- static, cost-balanced partition of the round's (problem, tile) list over the CTAs of the grid ------------
     // cost of a tile = correspondences of its problem; CTA c owns the tiles whose start cost lies in
     // [W c / G, W (c+1) / G).  The grid is ONE wave (resident CTAs x SMs), so there is no tail wave; a CTA touches a
@@ -1107,7 +1161,41 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
     const float *arr[NARR];
     uint32_t sarr[NARR] = {}; // shared-memory addresses of the staged arrays (the streaming pass reads them with LDS)
     int n_str = n; // correspondences the streaming pass runs over (padded on the shared-memory path)
-    if (use_smem) {
+    float qf[8];   // Sampson kinds: 2^(15 - e_j), the column scales of the integer rows (screen_math.cuh)
+    uint32_t srow = 0; // Sampson kinds: shared-memory address of the staged rows
+    if constexpr (SAMP) {
+        int e[8];
+        scr::sampson_qscale(P.cmax, e);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) qf[j] = ldexpf(1.f, 15 - e[j]);
+#pragma unroll
+        for (int c = 0; c < NARR; ++c) arr[c] = P.f[c]; // the queue pass reads the recorded cases from L2
+    }
+    if (use_smem && SAMP) {
+        // the integer rows (16 B each) of the problem's correspondences, zero rows up to whole streaming word groups;
+        // a zero row may be recorded, the queue pass skips it (k >= n).  The rows of P.q (launch_qrows) come in by one
+        // TMA bulk copy; without them the CTA builds the rows from the fp32 arrays.
+        uint4 *rows = reinterpret_cast<uint4 *>(scr_smem);
+        const int n_st = scr_stage_len<NTHR>(n);
+        __syncthreads(); // every thread is done with the previous problem's rows
+        int k_have = 0;
+        if (P.q) {
+            if (tid == 0) {
+                mbar_expect_tx(&bar, (uint32_t)n_pad * 16u);
+                tma_bulk_g2s(rows, P.q, (uint32_t)n_pad * 16u, &bar);
+            }
+            mbar_wait(&bar, phase);
+            phase ^= 1u;
+            k_have = n_pad;
+        }
+        for (int k = k_have + tid; k < n_st; k += SCR_THREADS) {
+            uint32_t w[4] = {0u, 0u, 0u, 0u};
+            if (k < n) scr::sampson_qrow(P.f[0][k], P.f[1][k], P.f[2][k], P.f[3][k], qf, w);
+            rows[k] = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+        srow = smem_u32(rows);
+        n_str = n_st;
+    } else if (use_smem) {
         float *pts = reinterpret_cast<float *>(scr_smem);
         const int n_st = scr_stage_len<NTHR>(n);
         __syncthreads(); // every thread is done with the previous problem's arrays
@@ -1135,7 +1223,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
             sarr[c] = smem_u32(arr[c]);
         }
         n_str = n_st;
-    } else {
+    } else if (!SAMP) {
 #pragma unroll
         for (int c = 0; c < NARR; ++c) arr[c] = P.f[c];
     }
@@ -1169,11 +1257,87 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                 if (KIND == KIND_PNP) return scr::transfer_maybe<true>(M, scr::pnp_terms(M, p[0], p[1], p[2], p[3], p[4]));
                 return scr::transfer_maybe<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]));
             };
+            // Sampson kinds: the lane's B fragments (of model lane >> 2: [e_hi; 0] and [e_lo; e_hi]) and, for the models
+            // 2 (lane & 3) + {0, 1} of its accumulators, init + off and 2 off; a model missing from a partial tile
+            // records nothing (off = QOFF_NONE), so the streaming pass needs no per-model guard
+            uint32_t qbh = 0u, qbl = 0u, qlim[2] = {0u, 0u};
+            int qc[2] = {0, 0};
+            if constexpr (SAMP) {
+                const int t = lane & 3, g = lane >> 2;
+                if (g < tm) {
+                    if (t < 2) qbh = __float_as_uint(cx[g][scr::S_QH0 + t]);
+                    qbl = __float_as_uint(cx[g][t < 2 ? scr::S_QL0 + t : scr::S_QH0 + t - 2]);
+                }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int mi = 2 * t + i;
+                    qc[i] = mi < tm ? __float_as_int(cx[mi][scr::S_QC]) : scr::QOFF_NONE;
+                    qlim[i] = (uint32_t)(mi < tm ? __float_as_int(cx[mi][scr::S_QOFF]) : scr::QOFF_NONE) << 1;
+                }
+            }
+            // one step: 16 rows x 8 models; bit 4 s + j of h: accumulator j of the lane, i.e. row (lane >> 2) + 8 (j >> 1)
+            // of the step and model 2 (lane & 3) + (j & 1)
+            auto qstep = [&](uint32_t &h, uint32_t a0, uint32_t a1, int s) {
+                int d1[4], d2[4];
+                mma_s8(d1, a0, a1, qbh, 0, 0);
+                mma_s8(d2, a0, a1, qbl, qc[0], qc[1]);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) or_if_le(h, (uint32_t)d1[j] * 256u + (uint32_t)d2[j], qlim[j & 1], 1u << (4 * s + j));
+            };
+            // the lane's word of row k for the unstaged path (zero past n, as the staged padding): from P.q, or built
+            const uint32_t *qg = reinterpret_cast<const uint32_t *>(P.q);
+            auto qword_ld = [&](int k) -> uint32_t { return k < n ? qg[4 * (size_t)k + (lane & 3)] : 0u; };
+            auto qword_at = [&](int k) -> uint32_t {
+                return k < n ? scr::sampson_qword(arr[0][k], arr[1][k], arr[2][k], arr[3][k], qf, lane & 3) : 0u;
+            };
             for (int base = 0; base < n_str; base += 32 * SCR_THREADS) {
                 const int lim = min_i(n_str, base + 32 * SCR_THREADS);
                 uint32_t hit[SCR_TM];
 #pragma unroll
                 for (int i = 0; i < SCR_TM; ++i) hit[i] = 0u;
+                if constexpr (SAMP) {
+                    // A chunk is QW word groups of 4 NTHR rows; in group w, step s of a warp covers the 16 rows
+                    // base + 4 NTHR w + 16 (s SCR_WARPS + warp) + 0..15, and its hits go to bits 4 s .. 4 s + 3 of hit[w].
+                    // n_str (or, unstaged, the zero rows past n) fills whole groups.  The words are shifted in, so that
+                    // hit[] is indexed by constants only.
+                    static_assert(QW == SCR_TM && 4 * 8 * QW == 32 * scr::REC_TM, "bits per lane and chunk of scr::record_depth");
+#pragma unroll 1
+                    for (int w = 0; w < QW; ++w) {
+                        const int g0 = base + w * 4 * SCR_THREADS;
+                        uint32_t h = 0u;
+                        if (g0 < n_str) {
+                            if (use_smem) {
+                                const uint32_t a = srow + 16u * (uint32_t)(g0 + 16 * warp + (lane & 15));
+#pragma unroll
+                                for (int s = 0; s < 8; ++s) {
+                                    uint32_t a0, a1;
+                                    ldsm_x2(a + (uint32_t)(s * 256 * SCR_WARPS), a0, a1);
+                                    qstep(h, a0, a1, s);
+                                }
+                            } else if (qg) {
+                                // the group's 16 words first: all loads in flight before the first MMA
+                                uint32_t fa[8][2];
+#pragma unroll
+                                for (int s = 0; s < 8; ++s) {
+                                    const int r = g0 + 16 * (s * SCR_WARPS + warp) + (lane >> 2);
+                                    fa[s][0] = qword_ld(r);
+                                    fa[s][1] = qword_ld(r + 8);
+                                }
+#pragma unroll
+                                for (int s = 0; s < 8; ++s) qstep(h, fa[s][0], fa[s][1], s);
+                            } else {
+#pragma unroll
+                                for (int s = 0; s < 8; ++s) {
+                                    const int r = g0 + 16 * (s * SCR_WARPS + warp) + (lane >> 2);
+                                    qstep(h, qword_at(r), qword_at(r + 8), s);
+                                }
+                            }
+                        }
+#pragma unroll
+                        for (int i = 0; i + 1 < SCR_TM; ++i) hit[i] = hit[i + 1];
+                        hit[SCR_TM - 1] = h;
+                    }
+                } else {
                 int k0 = base + tid;
                 uint32_t qbit = 1u;
                 // GUARDED: correspondences at or past lim read as NaN (never recorded, see the padding above);
@@ -1194,24 +1358,13 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
 #pragma unroll
                     for (int i = 0; i < SCR_TM; ++i) {
                         if (i >= tm) continue;
-                        if constexpr (KIND == KIND_RELPOSE || KIND == KIND_FUND) {
-                            float E[12]; // [0..8] the model; |C^| <= K is all the test reads
-                            lds_v4(cx[i], E);
-                            lds_v4(cx[i] + 4, E + 4);
-                            E[8] = lds_f(smem_u32(cx[i] + 8));
-                            const float K = lds_f(smem_u32(cx[i] + scr::S_CK));
+                        float Mr[20]; // [0..11] model, [16..19] constants of the streaming test
+                        lds_v4(cx[i], Mr);
+                        lds_v4(cx[i] + 4, Mr + 4);
+                        lds_v4(cx[i] + 8, Mr + 8);
+                        lds_v4(cx[i] + 16, Mr + 16);
 #pragma unroll
-                            for (int j = 0; j < SCR_PB; ++j)
-                                or_if(hit[i], scr::sampson_maybe_c(E, K, p[j][0], p[j][1], p[j][2], p[j][3]), bit[j]);
-                        } else {
-                            float Mr[20]; // [0..11] model, [16..19] constants of the streaming test
-                            lds_v4(cx[i], Mr);
-                            lds_v4(cx[i] + 4, Mr + 4);
-                            lds_v4(cx[i] + 8, Mr + 8);
-                            lds_v4(cx[i] + 16, Mr + 16);
-#pragma unroll
-                            for (int j = 0; j < SCR_PB; ++j) or_if(hit[i], transfer_maybe(Mr, p[j]), bit[j]);
-                        }
+                        for (int j = 0; j < SCR_PB; ++j) or_if(hit[i], transfer_maybe(Mr, p[j]), bit[j]);
                     }
                 };
                 auto stream = [&](auto staged) {
@@ -1222,6 +1375,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                 };
                 if (use_smem) stream(std::true_type{});
                 else stream(std::false_type{});
+                }
                 // Handling of the recorded cases, compacted across the WARP: the lanes list their cases (model, bit, lane)
                 // in a per-warp queue in shared memory — at most SCR_RQ_TAKE per lane and pass, so the queue cannot
                 // overflow — and the warp then works through the queue 32 entries at a time.  A case is evaluated by
@@ -1261,8 +1415,17 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                     __syncwarp();
                     for (int eidx = lane; eidx < total; eidx += 32) {
                         const uint32_t ent = rq[warp][eidx];
-                        const int mi = (int)(ent & 7u), q = (int)((ent >> 3) & 31u), otid = warp * 32 + (int)(ent >> 8);
-                        const int k = base + otid + q * SCR_THREADS;
+                        const int q = (int)((ent >> 3) & 31u), ol = (int)(ent >> 8);
+                        int mi, k;
+                        if constexpr (SAMP) { // (word group, bit) -> (row, model), see the streaming pass
+                            const int s = 8 * (int)(ent & 7u) + (q >> 2), j = q & 3;
+                            k = base + 16 * (s * SCR_WARPS + warp) + (ol >> 2) + 8 * (j >> 1);
+                            mi = 2 * (ol & 3) + (j & 1);
+                            if (k >= n) continue; // a zero row of the padding
+                        } else {
+                            mi = (int)(ent & 7u);
+                            k = base + warp * 32 + ol + q * SCR_THREADS;
+                        }
                         float p[NARR];
 #pragma unroll
                         for (int c = 0; c < NARR; ++c) p[c] = arr[c][k];
@@ -1274,7 +1437,7 @@ __global__ void __launch_bounds__(NTHR, NTHR >= 512 ? 1 : 4) k_screen(const Roun
                         } else if (KIND == KIND_HOMOG) {
                             scr::transfer_point<false>(M, scr::homography_terms(M, p[0], p[1], p[2], p[3]), plain, border, v, e);
                         } else {
-                            scr::sampson_point(M, p[0], p[1], p[2], p[3], plain, border, v, e);
+                            scr::sampson_point(M, thr, p[0], p[1], p[2], p[3], plain, border, v, e);
                             if (KIND == KIND_RELPOSE && (plain || border)) {
                                 bool ok, cb;
                                 scr::cheirality_point(M + 9, M[scr::S_EH], p[0], p[1], p[2], p[3], ok, cb);

@@ -26,6 +26,9 @@ struct ProblemDev {
     int n_pad;      // array stride of ts
     const double *ts;
     const float *cmax; // max |coordinate| of every SoA array (fp64 values rounded up): error bounds of the fp32 screening
+    // Relpose / fundamental: the integer rows of k_screen's streaming test (screen_math.cuh, 16 B per correspondence, n_pad
+    // rows, zero past n), built once per problem by launch_qrows.  Null: k_screen builds them from f[] itself.
+    const uint4 *q;
     // The cameras k_lm evaluates, cam[0 .. kind_cam_count(kind)); CAMM_NULL for a problem whose jobs use no camera.
     // Only the polish problem of a task whose final bundle evaluates a camera has them: a copy of the task's problem
     // whose p[0 .. 2 * kind_cam_count(kind)) are the pixels in the units of these cameras (PnP: x.x x.y; RELPOSE_TS:
@@ -202,6 +205,7 @@ struct TransposeDesc {
     CamDev cam_a, cam_b;
     double *px;
     double px_scale;
+    uint4 *q; // relpose / fundamental: n_pad integer rows of the streaming test (launch_qrows), or null
 };
 // normalize_points of one problem (robust/utils.cc:584-644, shared scale), in place on the uploaded AoS doubles.
 struct NormDesc {
@@ -223,6 +227,9 @@ void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream
 // AoS (caller layout) -> SoA fp64 + fp32 for n_desc problems (descriptors in device memory), camera pre-step fused.
 // xcam: some camera of the descriptors is a fisheye or division model (the kernel's instantiation that evaluates them)
 void launch_transpose(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, bool xcam, cudaStream_t stream);
+// The integer rows of the relpose / fundamental streaming test (TransposeDesc::q, where set) from the fp32 arrays and the
+// coordinate maxima that launch_transpose left: after it on the same stream.
+void launch_qrows(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cudaStream_t stream);
 // Solve + score kernels of one round (kind = kind of every problem of the group); *out.overflow must be zeroed.
 // mode 0: exact fp64 scoring of every model; mode 1: fp32 screening of every model (the candidates k_select lists are
 // rescored exactly by launch_confirm).  fctx (mode 1): scratch of scr::CTX_FLOATS floats per model slot for the

@@ -212,10 +212,10 @@ SCR_HD bool sampson_maybe_c(const float *M, float K, float a0, float a1, float b
 //            (r^2 - thr) = f / D;  | f/D - f~/D^ | <= 2 E_f / D^ + 2 thr (16u + beta_D / D^)  for D^ > 4 beta_D; a
 //            misclassified borderline point contributes at most |f| / D <= 4 E_f / D^.  Rounding of the division and of
 //            the subtraction: 4u (num/D^ + thr) <= 8u thr.   =>  e = rD (4 E_f + 2 thr beta_D) + 40u thr
-SCR_HD void sampson_point(const float *ctx, float a0, float a1, float b0, float b1, bool &plain, bool &border, float &v,
-                          float &e) {
+// thr: thr^ = fl32(sq_thr), what sampson_setup stores in ctx[S_THR] (k_screen passes it from the problem).
+SCR_HD void sampson_point(const float *ctx, float thr, float a0, float a1, float b0, float b1, bool &plain, bool &border,
+                          float &v, float &e) {
     const SampsonTerms T = sampson_terms(ctx, a0, a1, b0, b1);
-    const float thr = ctx[S_THR];
     const float num = T.C * T.C, t = thr * T.D;
     plain = num < t;
     const float Ef = fmaf(ctx[S_ALPHA], fabsf(T.C), fmaf(24.f * U, num + t, ctx[S_BETA]));
@@ -224,6 +224,153 @@ SCR_HD void sampson_point(const float *ctx, float a0, float a1, float b0, float 
     v = fmaf(num, rD, -thr);
     e = fmaf(rD, fmaf(4.f, Ef, ctx[S_ERR_K]), 40.f * U * thr);
     if (!(T.D > ctx[S_DMIN])) e = INFINITY;
+}
+SCR_HD void sampson_point(const float *ctx, float a0, float a1, float b0, float b1, bool &plain, bool &border, float &v,
+                          float &e) {
+    sampson_point(ctx, ctx[S_THR], a0, a1, b0, b1, plain, border, v, e);
+}
+
+// ============================================================================================================
+// The streaming test of the Sampson kinds as an exact integer contraction (k_screen, int8 tensor cores).
+//   C = x2^T E x1 = sum_j E_j p_j + E_8,   p = (b0 a0, b0 a1, b0, b1 a0, b1 a1, b1, a0, a1)  (j = 3r + c: b_r a_c).
+// Correspondence side (k_screen, when it stages a problem): p^_j = fl32(b^_r a^_c) from the fp32 coordinates, scaled by
+// the per-problem column scale s_j = 2^e_j >= (32768 / QMAX) Bnd_j, Bnd_j = cmax_b[r] cmax_a[c] (cmax_2 = 1), so the
+// product with 2^(15 - e_j) is exact and at most QMAX in magnitude:  qp_j = rn(p^_j 2^15 / s_j),
+//   |qp_j - 2^15 p_j / s_j| <= 1/2 + 2^15 3.0001u Bnd_j / s_j <= 1/2 + 0.0059 =: dp    (p: the product of the fp64 data).
+// Model side (sampson_qmodel, fp64): with m = max_j |E_j s_j| (s_8 = 1),  qe_j = rn(QMAX E_j s_j / m)  (dq <= 1/2 + 1e-11)
+// and the constant term  init = rn(128 QMAX E_8 / m).  Every q (|q| <= QMAX = 127 * 256) is split exactly into
+// q = 256 hi + lo, hi in [-127, 127], lo in [-128, 127], and the row of a correspondence is [hi_0..7, lo_0..7]: one
+// A-fragment row of mma.m16n8k16.s8.  The kernel computes, exactly in int32,
+//   acc1 = sum hp he,  acc2 = sum (hp le + lp he) + init,  v = 256 acc1 + acc2 = (sum qp qe - sum lp le) / 256 + init,
+// and with lambda = 128 QMAX / m the exact  V = lambda C  satisfies
+//   |v - V| <= sigma = (sum_j (dp |qe_j| + QMAX dq + 128 |le_j|)) / 256 + 1/2 + 1e-8
+// (|qp qe - ab| <= |qe| |qp - b| + |b| |qe - a| with |b| = 2^15 |p_j| / s_j <= QMAX; the dropped lo lo term).
+// The fp32 test accepts only |C^| <= K, and |C^ - C| <= eC = 8u S (sampson_setup), so it accepts only |C| <= K + eC and
+//   K_int = ceil(lambda (K + eC) + sigma)  (outward rounded)  gives  |v| <= K_int  for every pair it accepts.
+// Encoding (off: one int per model): the kernel starts acc2 at init + off and records iff (uint32)(v + off) <= 2 off, i.e.
+// |v| <= off for off >= 0.  |v| <= 8 (127^2 256 + 2 128 127) + 128 QMAX < 2^26, so off = 2^26 records every pair
+// (K = inf, bounds that do not fit, a zero model) and off = -2^26 none (a NaN model, which the fp32 test rejects
+// everywhere; the missing models of a partial tile).  The queue pass then decides every recorded pair exactly as before.
+// ============================================================================================================
+constexpr int QMAX = 32512; // 127 * 256
+constexpr int QOFF_ALL = 1 << 26, QOFF_NONE = -(1 << 26);
+// Where k_screen_ctx keeps the integer test in a Sampson model's constants.  They replace constants the device does not
+// read: the full prefilter's (the setup derives K from them), K itself and thr^ (k_screen takes it from the problem).
+enum {
+    S_QH0 = S_THR_P, // packed int8 he_0..3
+    S_QH1 = S_ALPHA_P, //        he_4..7
+    S_QL0 = S_BETA_P, //         le_0..3
+    S_QL1 = S_THR,    //         le_4..7
+    S_QC = S_CK,      // init + off
+    S_QOFF = 27       // off
+};
+// k_screen reads the four B-fragment words as S_QH0 + 0..3 (the e_hi words again as S_QH0 + t - 2)
+static_assert(S_QH1 == S_QH0 + 1 && S_QL0 == S_QH0 + 2 && S_QL1 == S_QH0 + 3 && S_QC < CTX_FLOATS && S_QOFF < CTX_FLOATS,
+              "the integer test's slots in a Sampson model's constants");
+// Exponents of the column scales from the coordinate maxima; false if a bound is not finite or exceeds 2^100 (the rows
+// then make no claim: every model records every pair).
+SCR_HD bool sampson_qscale(const float *cmax, int *e) {
+    bool ok = true;
+    for (int j = 0; j < 8; ++j) {
+        const int r = j / 3, c = j % 3;
+        const double bnd = (double)(c < 2 ? cmax[c] : 1.f) * (double)(r < 2 ? cmax[2 + r] : 1.f); // exact
+        const double x = bnd * (32768.0 / (double)QMAX) * (1.0 + 1e-15);
+        int ex = -100;
+        if (!(x <= 1.2676506002282294e30)) ok = false, ex = 0;
+        else if (x > 0.0) frexp(x, &ex); // 2^ex > x
+        e[j] = ex < -100 ? -100 : ex;
+    }
+    return ok;
+}
+SCR_HD int q_round(float x) {
+    x = fminf(fmaxf(x, -(float)QMAX), (float)QMAX); // also maps NaN to a fixed value
+#if defined(__CUDA_ARCH__)
+    return __float2int_rn(x);
+#else
+    return (int)rintf(x);
+#endif
+}
+SCR_HD uint32_t q_pack(const int *h) {
+    return (uint32_t)(h[0] & 255) | (uint32_t)(h[1] & 255) << 8 | (uint32_t)(h[2] & 255) << 16 | (uint32_t)(h[3] & 255) << 24;
+}
+// hi and lo bytes of q (|q| <= QMAX)
+SCR_HD void q_split(int q, int &hi, int &lo) {
+    hi = (q + 128) >> 8;
+    lo = q - 256 * hi;
+}
+// The row of a correspondence (the words [hi_0..3], [hi_4..7], [lo_0..3], [lo_4..7]); f_j = 2^(15 - e_j).
+SCR_HD void sampson_qrow(float a0, float a1, float b0, float b1, const float *f, uint32_t *row) {
+    const float p[8] = {b0 * a0, b0 * a1, b0, b1 * a0, b1 * a1, b1, a0, a1};
+    int hi[8], lo[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) q_split(q_round(p[j] * f[j]), hi[j], lo[j]);
+    row[0] = q_pack(hi);
+    row[1] = q_pack(hi + 4);
+    row[2] = q_pack(lo);
+    row[3] = q_pack(lo + 4);
+}
+// Word `word` of the same row alone (the same products, so the same bits), for a lane that builds its A fragment itself.
+SCR_HD uint32_t sampson_qword(float a0, float a1, float b0, float b1, const float *f, int word) {
+    const bool h = word & 1, low = word >> 1;
+    const float p[4] = {h ? b1 * a1 : b0 * a0, h ? b1 : b0 * a1, h ? a0 : b0, h ? a1 : b1 * a0};
+    int o[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        int hi, lo;
+        q_split(q_round(p[i] * (h ? f[4 + i] : f[i])), hi, lo);
+        o[i] = low ? lo : hi;
+    }
+    return q_pack(o);
+}
+// The four words of one model's B fragments (S_QH0, S_QH1, S_QL0, S_QL1) and init + off, off; M: the fp64 model (row
+// major), K: ctx[S_CK] as sampson_setup left it.
+SCR_HD void sampson_qmodel(const double *M, const float *cmax, float K, uint32_t *w, int &c, int &off) {
+    for (int k = 0; k < 4; ++k) w[k] = 0u;
+    c = off = QOFF_NONE;
+    double msum = 0.0;
+    for (int k = 0; k < 9; ++k) msum += fabs(M[k]);
+    if (msum != msum) return; // NaN model: the fp32 test rejects every pair
+    c = off = QOFF_ALL;
+    int e[8];
+    if (!sampson_qscale(cmax, e) || !(K < INFINITY)) return;
+    double m = fabs(M[8]);
+    for (int j = 0; j < 8; ++j) m = fmax(m, fabs(ldexp(M[j], e[j])));
+    if (!(m >= 1e-270 && m <= 1e270)) return; // also a zero model: C = 0 everywhere
+    const double rq = (double)QMAX / m, lambda = 128.0 * (double)QMAX / m;
+    int hi[8], lo[8];
+    double sig = 0.0;
+    for (int j = 0; j < 8; ++j) {
+        double x = ldexp(M[j], e[j]) * rq;
+        x = fmin(fmax(x, -(double)QMAX), (double)QMAX);
+        const int q = (int)rint(x);
+        q_split(q, hi[j], lo[j]);
+        sig += 0.5059 * fabs((double)q) + (double)QMAX * (0.5 + 1e-11) + 128.0 * fabs((double)lo[j]);
+    }
+    sig = sig / 256.0 + 0.5 + 1e-8;
+    const int init = (int)rint(M[8] * lambda);
+    double A[3], B[2];
+    sampson_rows(M, cmax, A, B);
+    const double eC = 8.0 * Ud * ((double)cmax[2] * A[0] + (double)cmax[3] * A[1] + A[2]);
+    const double kk = (lambda * ((double)K + eC) + sig) * (1.0 + 16.0 * Ud * Ud) + 1.0;
+    if (!(kk < (double)QOFF_ALL)) return;
+    off = (int)ceil(kk);
+    c = init + off;
+    w[0] = q_pack(hi);
+    w[1] = q_pack(hi + 4);
+    w[2] = q_pack(lo);
+    w[3] = q_pack(lo + 4);
+}
+// The integer test of one pair as the kernel evaluates it (the host restatement of the two MMAs); i: the model's row of
+// the fragments, row: the four words of the correspondence.
+SCR_HD bool sampson_qtest(const uint32_t *w, int c, int off, const uint32_t *row) {
+    int acc1 = 0, acc2 = c;
+    for (int i = 0; i < 8; ++i) {
+        const int hp = (int8_t)(row[i >> 2] >> (8 * (i & 3))), lp = (int8_t)(row[2 + (i >> 2)] >> (8 * (i & 3)));
+        const int he = (int8_t)(w[i >> 2] >> (8 * (i & 3))), le = (int8_t)(w[2 + (i >> 2)] >> (8 * (i & 3)));
+        acc1 += hp * he;
+        acc2 += hp * le + lp * he;
+    }
+    return (uint32_t)(256 * acc1 + acc2) <= (uint32_t)off << 1;
 }
 
 // ============================================================================================================
@@ -377,7 +524,8 @@ SCR_HD void transfer_point(const float *ctx, TransferTerms T, bool &plain, bool 
 //     not to the lane that owns the correspondence, so a lane's share is NOT n / NTHR: per pass of the queue a lane
 //     handles at most RQ_TAKE entries (the queue holds at most 32 RQ_TAKE), and a chunk of 32 NTHR correspondences needs
 //     at most 32 TM / RQ_TAKE passes (a lane has at most TM models x 32 bits of cases, and it queues min(its cases,
-//     RQ_TAKE) per pass), so a lane adds at most 32 TM = 256 terms per chunk to any one sum.  Neither can it add more
+//     RQ_TAKE) per pass), so a lane adds at most 32 TM = 256 terms per chunk to any one sum.  The Sampson kinds' integer
+//     pass holds the same 256 bits per lane and chunk (8 word groups of 8 steps x 4 accumulators), mapped differently.  Neither can it add more
 //     terms than the sum has: count32 for the score, count32 + border for the error bound (plain or border cases);
 //   * the warp butterfly (5 levels), the cross-warp sum (NTHR / 32 additions) and the final + n thr (1).
 //   depth = min(terms, 256 chunks) + 5 + NTHR / 32 + 1.

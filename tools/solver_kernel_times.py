@@ -6,7 +6,7 @@ with a kernel of another group.  After --warmup untimed runs, --steps runs are t
 activities) and the kernels are listed with their launches, total device time per step and share of the traced kernel
 time.  Prints the table, then one JSON line with the card's name, power limit and max SM clock beside the numbers.
 
-    python tools/solver_kernel_times.py [--pairs 256] [--steps 1] [--warmup 1]
+    python tools/solver_kernel_times.py [--pairs 256] [--n 10000] [--steps 1] [--warmup 1]
 """
 import argparse
 import json
@@ -46,6 +46,7 @@ def short_name(name):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pairs", type=int, default=256)
+    ap.add_argument("--n", type=int, default=10000, help="correspondences per pair (above 12 288 k_screen does not stage)")
     ap.add_argument("--steps", type=int, default=1)
     ap.add_argument("--warmup", type=int, default=1)
     a = ap.parse_args()
@@ -58,7 +59,7 @@ def main():
     ropt = dict(max_iterations=100000, min_iterations=1000, seed=0)
     handles, probs = [], []
     for i in range(a.pairs):
-        p = G.config_c2(i)
+        p = G.config_c2(i, n=a.n)
         h = cabi.resident_create("relpose", p["x1"] / G.FOCAL, p["x2"] / G.FOCAL)
         handles.append(h)
         probs.append(dict(kind="relpose", resident=h, n=len(p["x1"]), ransac=cabi.RansacOpt(**ropt),
@@ -88,7 +89,7 @@ def main():
     solver = sum(us[k] for k in rows if k == "k_sample" or k.startswith("k5_"))
     print(f"{'all kernels':<40} {sum(launches.values()) / a.steps:>14.1f} {total / 1e3 / a.steps:>10.3f}")
     print(f"{'5-point solver chain':<40} {'':>14} {solver / 1e3 / a.steps:>10.3f} {100 * solver / total:>6.1f}%")
-    out = dict(card(), pairs=a.pairs, steps=a.steps, streams=1,
+    out = dict(card(), pairs=a.pairs, n=a.n, steps=a.steps, streams=1,
                kernels={k: dict(launches_per_step=launches[k] / a.steps, ms_per_step=us[k] / 1e3 / a.steps)
                         for k in rows},
                total_ms_per_step=total / 1e3 / a.steps, solver_5pt_ms_per_step=solver / 1e3 / a.steps)
