@@ -244,7 +244,16 @@ int plb_relpose_8pt_batch(size_t count, size_t n, const double *x1, const double
 
 /* ---- PoseLib/robust/bundle.h: bundle_adjust (calibrated, :41-43), refine_relpose (:84-86), refine_fundamental
  * (:132-134), refine_homography (:148-150) — the LM refiners the LO step and the final polish are built from.
- * Uniform weights.  bundle_stats_out (may be NULL): {iterations, initial_cost, cost}. ------------------------- */
+ * bundle_stats_out (may be NULL): {iterations, initial_cost, cost}.
+ * Weights: every refiner below but plb_bundle_adjust has a *_weighted twin that takes PoseLib's per-residual weights,
+ * `weights` = n doubles in point order, or NULL for uniform weights (the twin is then the unweighted call).  Point k's
+ * residuals enter the cost as weights[k] * loss and the normal equations with weights[k] * loss weight
+ * (jacobian_accumulator.h:65-133); a residual with weight 0 still counts in the 1 / max(1, count) scale of the cost, so a
+ * zero weight is not the same as dropping the point.  The homography refiner applies a point's weight to both its
+ * forward and its backward residual.  Weights are not checked, as in the reference.  The reference uses the weights
+ * only when weights.size() == n (bundle.cc:107-111 etc.); the adapter passes NULL otherwise.  There is no weighted
+ * plb_bundle_adjust: the reference's calibrated bundle_adjust(x, X, CameraPose*, opt, weights) drops its weights
+ * (bundle.cc:84-92). ------------------------------------------------------------------------------------------ */
 int plb_bundle_adjust(const double *x_xy, const double *X_xyz, size_t n, double pose_inout[7],
                       const plb_bundle_opt *opt, double bundle_stats_out[3]);
 /* bundle.h:47 bundle_adjust(x, X, Image*, opt) (bundle.cc:95-112): the pose and the camera parameters opt->refine_intrinsics
@@ -269,6 +278,21 @@ int plb_refine_fundamental(const double *x1_xy, const double *x2_xy, size_t n, d
                            const plb_bundle_opt *opt, double bundle_stats_out[3]);
 int plb_refine_homography(const double *x1_xy, const double *x2_xy, size_t n, double H_inout[9],
                           const plb_bundle_opt *opt, double bundle_stats_out[3]);
+int plb_bundle_adjust_image_weighted(const double *x_px, const double *X_xyz, size_t n, double pose_inout[7],
+                                     plb_camera *camera_inout, const plb_bundle_opt *opt, double bundle_stats_out[3],
+                                     const double *weights);
+int plb_refine_relpose_weighted(const double *x1_xy, const double *x2_xy, size_t n, double pose_inout[7],
+                                const plb_bundle_opt *opt, double bundle_stats_out[3], const double *weights);
+int plb_refine_relpose_cameras_weighted(const double *x1_px, const double *x2_px, size_t n, const plb_camera *camera1,
+                                        const plb_camera *camera2, double pose_inout[7], const plb_bundle_opt *opt,
+                                        double bundle_stats_out[3], const double *weights);
+int plb_refine_relpose_pair_weighted(const double *x1_px, const double *x2_px, size_t n, plb_camera *camera1_inout,
+                                     plb_camera *camera2_inout, double pose_inout[7], const plb_bundle_opt *opt,
+                                     double bundle_stats_out[3], const double *weights);
+int plb_refine_fundamental_weighted(const double *x1_xy, const double *x2_xy, size_t n, double F_inout[9],
+                                    const plb_bundle_opt *opt, double bundle_stats_out[3], const double *weights);
+int plb_refine_homography_weighted(const double *x1_xy, const double *x2_xy, size_t n, double H_inout[9],
+                                   const plb_bundle_opt *opt, double bundle_stats_out[3], const double *weights);
 
 /* ---- batch of independent problems (BASELINE config 5); sharded by the caller across GPUs ---------- */
 enum { PLB_KIND_PNP = 0, PLB_KIND_RELPOSE = 1, PLB_KIND_FUNDAMENTAL = 2, PLB_KIND_HOMOGRAPHY = 3 };

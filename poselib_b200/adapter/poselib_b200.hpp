@@ -251,8 +251,10 @@ RansacStats estimate_homography(const std::vector<P2> &x1, const std::vector<P2>
     return detail::from_c<RansacStats>(st);
 }
 
-// ---- robust/bundle.h: the LM refiners (uniform weights; the reference's optional per-residual weights are NYI) -----
+// ---- robust/bundle.h: the LM refiners, with the reference's optional per-residual weights ---------------------------
 // BundleStats carries iterations, initial_cost and cost; lambda / step_norm / grad_norm stay at their defaults.
+// Weights are used when weights.size() == n and otherwise mean uniform weights, as in the reference (bundle.cc:107-111,
+// 217-221, 261-265, 272-276, 328-332, 406-410).
 namespace detail {
 template <typename BundleStats> inline BundleStats bundle_from_c(const double s[3]) {
     BundleStats b = BundleStats();
@@ -261,15 +263,17 @@ template <typename BundleStats> inline BundleStats bundle_from_c(const double s[
     b.cost = s[2];
     return b;
 }
-inline void no_weights(const std::vector<double> &weights) {
-    if (!weights.empty()) throw std::runtime_error("poselib_b200: NYI (per-residual weights in the LM refiners)");
+// the weights the *_weighted entry points take: the caller's when there is one per point, else null (uniform)
+inline const double *weights_of(const std::vector<double> &weights, size_t n) {
+    return weights.size() == n ? weights.data() : nullptr;
 }
 } // namespace detail
-// bundle_adjust(x, X, CameraPose*, BundleOptions, weights)   robust/bundle.h:41-43
+// bundle_adjust(x, X, CameraPose*, BundleOptions, weights)   robust/bundle.h:41-43.  The weights are ignored: the
+// reference calls the Image* overload without them (bundle.cc:84-92).
 template <typename BundleStats, typename P2, typename P3, typename Pose, typename BOpt>
 BundleStats bundle_adjust(const std::vector<P2> &x, const std::vector<P3> &X, Pose *pose, const BOpt &opt,
                           const std::vector<double> &weights = std::vector<double>()) {
-    detail::no_weights(weights);
+    (void)weights;
     double m[7], st[3];
     detail::pose_to(*pose, m);
     plb_bundle_opt bo = detail::bundle_to_c(opt);
@@ -282,12 +286,12 @@ BundleStats bundle_adjust(const std::vector<P2> &x, const std::vector<P3> &X, Po
 template <typename BundleStats, typename P2, typename P3, typename Image, typename BOpt>
 BundleStats bundle_adjust_image(const std::vector<P2> &x, const std::vector<P3> &X, Image *image, const BOpt &opt,
                                 const std::vector<double> &weights = std::vector<double>()) {
-    detail::no_weights(weights);
     double m[7], st[3];
     detail::pose_to(image->pose, m);
     plb_bundle_opt bo = detail::bundle_to_c(opt);
     plb_camera cam = detail::camera_to_c(image->camera);
-    detail::check(plb_bundle_adjust_image(detail::raw(x), detail::raw(X), x.size(), m, &cam, &bo, st));
+    detail::check(plb_bundle_adjust_image_weighted(detail::raw(x), detail::raw(X), x.size(), m, &cam, &bo, st,
+                                                   detail::weights_of(weights, x.size())));
     detail::pose_from(m, &image->pose);
     detail::camera_from_c(cam, &image->camera);
     return detail::bundle_from_c<BundleStats>(st);
@@ -296,11 +300,11 @@ BundleStats bundle_adjust_image(const std::vector<P2> &x, const std::vector<P3> 
 template <typename BundleStats, typename P2, typename Pose, typename BOpt>
 BundleStats refine_relpose(const std::vector<P2> &x1, const std::vector<P2> &x2, Pose *pose, const BOpt &opt,
                            const std::vector<double> &weights = std::vector<double>()) {
-    detail::no_weights(weights);
     double m[7], st[3];
     detail::pose_to(*pose, m);
     plb_bundle_opt bo = detail::bundle_to_c(opt);
-    detail::check(plb_refine_relpose(detail::raw(x1), detail::raw(x2), x1.size(), m, &bo, st));
+    detail::check(plb_refine_relpose_weighted(detail::raw(x1), detail::raw(x2), x1.size(), m, &bo, st,
+                                              detail::weights_of(weights, x1.size())));
     detail::pose_from(m, pose);
     return detail::bundle_from_c<BundleStats>(st);
 }
@@ -309,12 +313,12 @@ BundleStats refine_relpose(const std::vector<P2> &x1, const std::vector<P2> &x2,
 template <typename BundleStats, typename P2, typename ImagePair, typename BOpt>
 BundleStats refine_relpose_pair(const std::vector<P2> &x1, const std::vector<P2> &x2, ImagePair *pair, const BOpt &opt,
                                 const std::vector<double> &weights = std::vector<double>()) {
-    detail::no_weights(weights);
     double m[7], st[3];
     detail::pose_to(pair->pose, m);
     plb_bundle_opt bo = detail::bundle_to_c(opt);
     plb_camera c1 = detail::camera_to_c(pair->camera1), c2 = detail::camera_to_c(pair->camera2);
-    detail::check(plb_refine_relpose_pair(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, m, &bo, st));
+    detail::check(plb_refine_relpose_pair_weighted(detail::raw(x1), detail::raw(x2), x1.size(), &c1, &c2, m, &bo, st,
+                                                   detail::weights_of(weights, x1.size())));
     detail::pose_from(m, &pair->pose);
     detail::camera_from_c(c1, &pair->camera1);
     detail::camera_from_c(c2, &pair->camera2);
@@ -325,10 +329,10 @@ template <typename BundleStats, typename P2, typename Mat3, typename BOpt>
 BundleStats refine_fundamental(const std::vector<P2> &x1, const std::vector<P2> &x2, Mat3 *F, const BOpt &opt,
                                const std::vector<double> &weights = std::vector<double>()) {
     static_assert(sizeof(Mat3) == 9 * sizeof(double), "column-major 3x3 of doubles required");
-    detail::no_weights(weights);
     double st[3];
     plb_bundle_opt bo = detail::bundle_to_c(opt);
-    detail::check(plb_refine_fundamental(detail::raw(x1), detail::raw(x2), x1.size(), reinterpret_cast<double *>(F), &bo, st));
+    detail::check(plb_refine_fundamental_weighted(detail::raw(x1), detail::raw(x2), x1.size(), reinterpret_cast<double *>(F),
+                                                  &bo, st, detail::weights_of(weights, x1.size())));
     return detail::bundle_from_c<BundleStats>(st);
 }
 // refine_homography(x1, x2, Matrix3d*, BundleOptions, weights)   robust/bundle.h:148-150
@@ -336,10 +340,10 @@ template <typename BundleStats, typename P2, typename Mat3, typename BOpt>
 BundleStats refine_homography(const std::vector<P2> &x1, const std::vector<P2> &x2, Mat3 *H, const BOpt &opt,
                               const std::vector<double> &weights = std::vector<double>()) {
     static_assert(sizeof(Mat3) == 9 * sizeof(double), "column-major 3x3 of doubles required");
-    detail::no_weights(weights);
     double st[3];
     plb_bundle_opt bo = detail::bundle_to_c(opt);
-    detail::check(plb_refine_homography(detail::raw(x1), detail::raw(x2), x1.size(), reinterpret_cast<double *>(H), &bo, st));
+    detail::check(plb_refine_homography_weighted(detail::raw(x1), detail::raw(x2), x1.size(), reinterpret_cast<double *>(H),
+                                                 &bo, st, detail::weights_of(weights, x1.size())));
     return detail::bundle_from_c<BundleStats>(st);
 }
 

@@ -102,7 +102,9 @@ EXPORTS = [
     "plb_estimate_homography", "plb_p3p_batch", "plb_p3p_lambdatwist_batch", "plb_relpose_5pt_batch", "plb_relpose_5pt_poses_batch",
     "plb_relpose_7pt_batch", "plb_homography_4pt_batch", "plb_essential_matrix_8pt_batch", "plb_relpose_8pt_batch", "plb_ransac_batch", "plb_ransac_batch_multi", "plb_estimate_batch", "plb_bundle_adjust",
     "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_relpose_pair", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
-    "plb_resident_free",
+    "plb_resident_free", "plb_bundle_adjust_image_weighted", "plb_refine_relpose_weighted",
+    "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
+    "plb_refine_homography_weighted",
 ]
 
 class EstimateProblem(C.Structure):
@@ -173,6 +175,15 @@ def _d(a):
     return a, a.ctypes.data_as(_P)
 
 
+def _w(weights, n):
+    """PoseLib's per-residual weights for n points: used when there is one per point, else uniform (None), as in the
+    reference (bundle.cc:107-111 etc.).  Returns (array kept alive by the caller, pointer or None)."""
+    if weights is None:
+        return None, None
+    w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+    return (w, w.ctypes.data_as(_P)) if len(w) == n else (None, None)
+
+
 def _init_model(kind, init):
     if kind in ("pnp", "relpose"):
         m = np.array([1, 0, 0, 0, 0, 0, 0] if init is None else init, dtype=np.float64)
@@ -227,15 +238,17 @@ def ransac_relpose_cameras(x1, x2, cam1, cam2, ropt, max_error):
     return {"model": _model_out("relpose", m), "inliers": mask[:n], "stats": st.as_dict(), "counters": cn.as_dict()}
 
 
-def refine_relpose_cameras(pose, x1, x2, cam1, cam2, bopt):
-    """refine_relpose(x1, x2, ImagePair*, opt) with fixed intrinsics (bundle.cc:237-247)."""
+def refine_relpose_cameras(pose, x1, x2, cam1, cam2, bopt, weights=None):
+    """refine_relpose(x1, x2, ImagePair*, opt) with fixed intrinsics (bundle.cc:237-247); weights: one per point, or
+    None (uniform)."""
     n = len(x1)
     aa, ap = _d(x1)
     ba, bp = _d(x2)
+    wa, wp = _w(weights, n)
     m = _init_model("relpose", pose)
     bs = np.zeros(3)
-    _check(_lib.plb_refine_relpose_cameras(ap, bp, C.c_size_t(n), C.byref(cam1), C.byref(cam2),
-                                           m.ctypes.data_as(_P), C.byref(bopt), bs.ctypes.data_as(_P)))
+    _check(_lib.plb_refine_relpose_cameras_weighted(ap, bp, C.c_size_t(n), C.byref(cam1), C.byref(cam2),
+                                                    m.ctypes.data_as(_P), C.byref(bopt), bs.ctypes.data_as(_P), wp))
     return _model_out("relpose", m), bs
 
 
@@ -313,47 +326,55 @@ def estimate_relative_pose_pair(x1, x2, cam1, cam2, ropt, bopt, max_error, tange
             "stats": st.as_dict(), "counters": cn.as_dict()}
 
 
-def refine_image(pose, x, X, cam, bopt):
-    """bundle_adjust(x, X, Image*, opt) (robust/bundle.h:47): points in the camera's pixel units, bopt.refine_intrinsics
-    selects the camera parameters refined with the pose.  Returns (pose, camera parameters, [iterations, initial_cost,
-    cost]); `cam` is not modified."""
+def refine_image(pose, x, X, cam, bopt, weights=None):
+    """bundle_adjust(x, X, Image*, opt, weights) (robust/bundle.h:47): points in the camera's pixel units,
+    bopt.refine_intrinsics selects the camera parameters refined with the pose; weights: one per point, or None
+    (uniform).  Returns (pose, camera parameters, [iterations, initial_cost, cost]); `cam` is not modified."""
     n = len(x)
     aa, ap = _d(x)
     ba, bp = _d(X)
+    wa, wp = _w(weights, n)
     m = _init_model("pnp", pose)
     c = _copy_camera(cam)
     bs = np.zeros(3)
-    _check(_lib.plb_bundle_adjust_image(ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(c), C.byref(bopt),
-                                        bs.ctypes.data_as(_P)))
+    _check(_lib.plb_bundle_adjust_image_weighted(ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(c),
+                                                 C.byref(bopt), bs.ctypes.data_as(_P), wp))
     return m, _camera_params(c), bs
 
 
-def refine_relpose_pair(pose, x1, x2, cam1, cam2, bopt):
-    """refine_relpose(x1, x2, ImagePair*, opt) (bundle.cc:237-256): pixels as given, bopt.refine_intrinsics selects the
-    parameters of each camera refined with the pose.  Returns (pose, camera 1 parameters, camera 2 parameters,
-    [iterations, initial_cost, cost]); cam1 / cam2 are not modified."""
+def refine_relpose_pair(pose, x1, x2, cam1, cam2, bopt, weights=None):
+    """refine_relpose(x1, x2, ImagePair*, opt, weights) (bundle.cc:237-256): pixels as given, bopt.refine_intrinsics
+    selects the parameters of each camera refined with the pose; weights: one per point, or None (uniform).  Returns
+    (pose, camera 1 parameters, camera 2 parameters, [iterations, initial_cost, cost]); cam1 / cam2 are not modified."""
     n = len(x1)
     aa, ap = _d(x1)
     ba, bp = _d(x2)
+    wa, wp = _w(weights, n)
     m = _init_model("relpose", pose)
     c1, c2 = _copy_camera(cam1), _copy_camera(cam2)
     bs = np.zeros(3)
-    _check(_lib.plb_refine_relpose_pair(ap, bp, C.c_size_t(n), C.byref(c1), C.byref(c2), m.ctypes.data_as(_P),
-                                        C.byref(bopt), bs.ctypes.data_as(_P)))
+    _check(_lib.plb_refine_relpose_pair_weighted(ap, bp, C.c_size_t(n), C.byref(c1), C.byref(c2), m.ctypes.data_as(_P),
+                                                 C.byref(bopt), bs.ctypes.data_as(_P), wp))
     return m, _camera_params(c1), _camera_params(c2), bs
 
 
-def refine(kind, model, a, b, bopt):
-    """bundle_adjust / refine_relpose / refine_fundamental / refine_homography (robust/bundle.h), uniform weights.
+def refine(kind, model, a, b, bopt, weights=None):
+    """bundle_adjust / refine_relpose / refine_fundamental / refine_homography (robust/bundle.h); weights: one per point,
+    or None (uniform).  "pnp" ignores the weights, as the reference's calibrated bundle_adjust does (bundle.cc:84-92).
     Returns (model, [iterations, initial_cost, cost])."""
     n = len(a)
     aa, ap = _d(a)
     ba, bp = _d(b)
     m = _init_model(kind, model)
     bs = np.zeros(3)
-    fn = {"pnp": _lib.plb_bundle_adjust, "relpose": _lib.plb_refine_relpose,
-          "fundamental": _lib.plb_refine_fundamental, "homography": _lib.plb_refine_homography}[kind]
-    _check(fn(ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(bopt), bs.ctypes.data_as(_P)))
+    args = [ap, bp, C.c_size_t(n), m.ctypes.data_as(_P), C.byref(bopt), bs.ctypes.data_as(_P)]
+    if kind == "pnp":
+        _check(_lib.plb_bundle_adjust(*args))
+    else:
+        wa, wp = _w(weights, n)
+        fn = {"relpose": _lib.plb_refine_relpose_weighted, "fundamental": _lib.plb_refine_fundamental_weighted,
+              "homography": _lib.plb_refine_homography_weighted}[kind]
+        _check(fn(*args, wp))
     return _model_out(kind, m), bs
 
 

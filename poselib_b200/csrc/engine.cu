@@ -232,6 +232,7 @@ struct Engine {
     MapBuf<double> h_norm;
     DevBuf<MaskDesc> mdesc;
     DevBuf<LmJob> jobs;
+    DevBuf<double> wts; // per-residual weights of a refiner call (LmJob::w)
     PinBuf<double> h_in, h_lm_in;
     PinBuf<int> h_slots, h_act, h_work;
     PinBuf<ProblemDev> h_probs;
@@ -595,6 +596,7 @@ static LmJob lm_job(int pidx, long long mask_off, const LmParams &prm) {
     J.mask_off = mask_off;
     J.scratch_off = 0;
     J.prm = prm;
+    J.w = nullptr;
     return J;
 }
 
@@ -948,9 +950,12 @@ struct Group {
         for (int cam = 0; cam < 2; ++cam) {
             const int j0 = cam ? n_fixed : 0, n = cam ? nj - n_fixed : n_fixed;
             if (n == 0) continue;
-            bool xcam = false;
-            for (int j = j0; j < j0 + n; ++j) xcam = xcam || uses_x_camera(batch[j].job);
-            launch_lm(kind, cam, xcam, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
+            bool xcam = false, weighted = false;
+            for (int j = j0; j < j0 + n; ++j) {
+                xcam = xcam || uses_x_camera(batch[j].job);
+                weighted = weighted || batch[j].job.w;
+            }
+            launch_lm(kind, cam, xcam, weighted, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, n, max_n, E.mask.p, E.subset.p,
                       max_n_pad, E.h_lm_out.d + j0, cam ? E.h_cam_out.d + (size_t)j0 * nc * CAM_MAX_PARAMS : nullptr, st);
             E.launches++;
         }
@@ -1545,9 +1550,11 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
 // the fixed-camera refiner.
 // No points is not special: the job runs with empty slices and reports what lm_impl reports for an empty problem
 // (iterations 0, costs 0; the fundamental refiner returns the matrix its factorisation reconstructs).
+// weights (or null: uniform): n_pts doubles, one per correspondence, in the caller's point order, which the layout keeps
+// for every kind; they go up with the points and the job runs k_lm's weighted instantiation.
 static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
                       const plb_bundle_opt &bopt, double *bstats, const CamDev *cams = nullptr, int cam_refine = 0,
-                      double *const *params_out = nullptr) {
+                      double *const *params_out = nullptr, const double *weights = nullptr) {
     Task t;
     t.kind = kind;
     t.a = a;
@@ -1570,6 +1577,11 @@ static int run_refine(int kind, const double *a, const double *b, size_t n_pts, 
     lm_set_sm_share(100);
     LmJob J = lm_job(G.PS[0].polish_pidx >= 0 ? G.PS[0].polish_pidx : 0, -1, prm);
     J.cam_refine = cam_refine;
+    if (weights && n_pts > 0) {
+        if ((rc = G.E.wts.ensure(n_pts))) return rc;
+        PLB_CUDA(cudaMemcpyAsync(G.E.wts.p, weights, sizeof(double) * n_pts, cudaMemcpyHostToDevice, G.st));
+        J.w = G.E.wts.p;
+    }
     if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
     PLB_CUDA(cudaGetLastError());
     const LmJobOut &o = G.E.h_lm_out.p[0];
@@ -2003,13 +2015,16 @@ int plb_estimate_homography(const double *x1, const double *x2, size_t n, const 
 }
 
 // ---- robust/bundle.h refiners -------------------------------------------------------------------------------
+// Every refiner has a _weighted twin that takes PoseLib's per-residual weights (n doubles, null: uniform); the
+// unweighted entry point is the twin with null weights.  The weights are not checked, as in the reference: zero and
+// negative values enter the sums as they are.
 static int refine_entry(int kind, const double *a, const double *b, size_t n, double *model, const plb_bundle_opt *opt,
-                        double *bs) {
+                        double *bs, const double *weights = nullptr) {
     if (!opt || !model || (n > 0 && (!a || !b))) {
         g_err = "null argument";
         return PLB_ERR_ARG;
     }
-    return run_refine(kind, a, b, n, model, *opt, bs);
+    return run_refine(kind, a, b, n, model, *opt, bs, nullptr, 0, nullptr, weights);
 }
 int plb_bundle_adjust(const double *x, const double *X, size_t n, double pose[7], const plb_bundle_opt *opt,
                       double bs[3]) {
@@ -2019,9 +2034,14 @@ int plb_refine_relpose(const double *x1, const double *x2, size_t n, double pose
                        double bs[3]) {
     return refine_entry(KIND_RELPOSE, x1, x2, n, pose, opt, bs);
 }
+int plb_refine_relpose_weighted(const double *x1, const double *x2, size_t n, double pose[7], const plb_bundle_opt *opt,
+                                double bs[3], const double *weights) {
+    return refine_entry(KIND_RELPOSE, x1, x2, n, pose, opt, bs, weights);
+}
 // robust/bundle.cc:237-266 with fixed intrinsics: unproject_with_jac of both images, then the tangent-Sampson refiner
-int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
-                               const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
+static int refine_relpose_cameras(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
+                                  const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt, double bs[3],
+                                  const double *weights) {
     if (!opt || !pose || (n > 0 && (!x1 || !x2))) {
         g_err = "null argument";
         return PLB_ERR_ARG;
@@ -2033,11 +2053,20 @@ int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, con
         g_err = "NYI: camera refinement needs cameras to return: use plb_refine_relpose_pair";
         return PLB_ERR_NYI;
     }
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams);
+    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, 0, nullptr, weights);
+}
+int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
+                               const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
+    return refine_relpose_cameras(x1, x2, n, camera1, camera2, pose, opt, bs, nullptr);
+}
+int plb_refine_relpose_cameras_weighted(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
+                                        const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt,
+                                        double bs[3], const double *weights) {
+    return refine_relpose_cameras(x1, x2, n, camera1, camera2, pose, opt, bs, weights);
 }
 // robust/bundle.cc:95-112: AbsolutePoseRefiner on an Image, camera_refine_idx from the flags; points in camera units
-int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
-                            const plb_bundle_opt *opt, double bs[3]) {
+static int bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
+                               const plb_bundle_opt *opt, double bs[3], const double *weights) {
     if (!opt || !pose || !camera_inout || (n > 0 && (!x || !X))) {
         g_err = "null argument";
         return PLB_ERR_ARG;
@@ -2045,12 +2074,22 @@ int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double p
     CamDev cam;
     if (int r = camera_dev(camera_inout, &cam)) return r;
     double *out[1] = {camera_inout->params};
-    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, &cam, refine_flags(opt), out);
+    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, &cam, refine_flags(opt), out, weights);
+}
+int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
+                            const plb_bundle_opt *opt, double bs[3]) {
+    return bundle_adjust_image(x, X, n, pose, camera_inout, opt, bs, nullptr);
+}
+int plb_bundle_adjust_image_weighted(const double *x, const double *X, size_t n, double pose[7],
+                                     plb_camera *camera_inout, const plb_bundle_opt *opt, double bs[3],
+                                     const double *weights) {
+    return bundle_adjust_image(x, X, n, pose, camera_inout, opt, bs, weights);
 }
 // robust/bundle.cc:237-256: refine_relpose(x1, x2, ImagePair*, opt), CameraRelativePoseRefiner with the parameters the
 // flags select in either camera (shared_camera false); pixels as given, only the refined parameters written
-int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
-                            plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
+static int refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                               plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3],
+                               const double *weights) {
     if (!opt || !pose || !camera1_inout || !camera2_inout || (n > 0 && (!x1 || !x2))) {
         g_err = "null argument";
         return PLB_ERR_ARG;
@@ -2059,15 +2098,32 @@ int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_ca
     if (int r = camera_dev(camera1_inout, &cams[0])) return r;
     if (int r = camera_dev(camera2_inout, &cams[1])) return r;
     double *out[2] = {camera1_inout->params, camera2_inout->params};
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, refine_flags(opt), out);
+    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, refine_flags(opt), out, weights);
+}
+int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                            plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
+    return refine_relpose_pair(x1, x2, n, camera1_inout, camera2_inout, pose, opt, bs, nullptr);
+}
+int plb_refine_relpose_pair_weighted(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
+                                     plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3],
+                                     const double *weights) {
+    return refine_relpose_pair(x1, x2, n, camera1_inout, camera2_inout, pose, opt, bs, weights);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {
     return refine_entry(KIND_FUND, x1, x2, n, F, opt, bs);
 }
+int plb_refine_fundamental_weighted(const double *x1, const double *x2, size_t n, double F[9],
+                                    const plb_bundle_opt *opt, double bs[3], const double *weights) {
+    return refine_entry(KIND_FUND, x1, x2, n, F, opt, bs, weights);
+}
 int plb_refine_homography(const double *x1, const double *x2, size_t n, double H[9], const plb_bundle_opt *opt,
                           double bs[3]) {
     return refine_entry(KIND_HOMOG, x1, x2, n, H, opt, bs);
+}
+int plb_refine_homography_weighted(const double *x1, const double *x2, size_t n, double H[9],
+                                   const plb_bundle_opt *opt, double bs[3], const double *weights) {
+    return refine_entry(KIND_HOMOG, x1, x2, n, H, opt, bs, weights);
 }
 
 // ---- solvers ------------------------------------------------------------------------------------------------

@@ -1965,9 +1965,9 @@ template <int NP> struct JacAcc {
         for (int i = 0; i < NP; ++i) jtr[i] = 0.0;
         cnt = 0.0;
     }
-    // 1-dim residual (jacobian_accumulator.h:125-141)
-    PLB_DEV void add1(const LossFn &L, double res, const double *J) {
-        const double w = L.weight(res * res);
+    // 1-dim residual (jacobian_accumulator.h:125-141); W: the residual's weight wk, w = wk * loss weight (:122)
+    template <bool W = false> PLB_DEV void add1(const LossFn &L, double res, const double *J, double wk = 1.0) {
+        const double w = W ? wk * L.weight(res * res) : L.weight(res * res);
         if (w == 0) return;
         int t = 0;
 #pragma unroll
@@ -1979,9 +1979,10 @@ template <int NP> struct JacAcc {
         for (int i = 0; i < NP; ++i) jtr[i] += wr * J[i];
         cnt += 1.0;
     }
-    // 2-dim residual (jacobian_accumulator.h:87-104)
-    PLB_DEV void add2(const LossFn &L, double r0, double r1, const double *J0, const double *J1) {
-        const double w = L.weight(r0 * r0 + r1 * r1);
+    // 2-dim residual (jacobian_accumulator.h:87-104); W as in add1 (:86)
+    template <bool W = false>
+    PLB_DEV void add2(const LossFn &L, double r0, double r1, const double *J0, const double *J1, double wk = 1.0) {
+        const double w = W ? wk * L.weight(r0 * r0 + r1 * r1) : L.weight(r0 * r0 + r1 * r1);
         if (w == 0) return;
         int t = 0;
 #pragma unroll
@@ -2094,12 +2095,24 @@ template <class Shared> PLB_DEV int block_bcast(Shared *S, int v) {
     return r;
 }
 
+// The weight of point k's residuals: wt[k] (W, uniform where wt is null), 1 otherwise; wmul<W>(wk, v) is wk * v (W) or v
+template <bool W> PLB_DEV double lm_weight(const double *wt, int k) {
+    if constexpr (W) return wt ? wt[k] : 1.0;
+    else return 1.0;
+}
+template <bool W> PLB_DEV double wmul(double wk, double v) {
+    if constexpr (W) return wk * v;
+    else return v;
+}
+
 // One evaluation pass at the parameters whose context is in S->ctx: robust cost + row count (compute_residual of the
 // refiners) AND the normal equations JtJ (lower triangle, packed row-major), Jtr + count of non-zero-weight rows
 // (compute_jacobian), accumulated separately exactly as two passes of the reference would.
 // Output layout in S->tot: [0] loss sum, [1] residual rows, [2..2+NT) JtJ, [2+NT..2+NT+NP) Jtr, [2+NT+NP] jac rows.
-template <int KIND, bool X = false>
-PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list, int lo, int na,
+// W: point k's residuals carry the weight wt[k] (uniform where wt is null): its loss terms are wt[k] * loss and its
+// Jacobian weight wt[k] * loss weight (jacobian_accumulator.h:65-74,83-133); every residual still counts as a row.
+template <int KIND, bool X = false, bool W = false>
+PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const double *wt, const int *list, int lo, int na,
                           LmShared<LmDims<KIND>::NP> *S, int &buf, int csize) {
     constexpr int NP = LmDims<KIND>::NP;
     constexpr int NT = NP * (NP + 1) / 2;
@@ -2115,6 +2128,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
             const double Z1 = ctx[3] * X0 + ctx[4] * X1 + ctx[5] * X2 + ctx[10];
             const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
             if (Z2 < 0) continue; // optim/absolute.h:57-58,93-94
+            const double wk = lm_weight<W>(wt, k);
             double zp0, zp1, xr0, xr1, Jp[2][3];
             if (P.cam[0].model != CAMM_NULL) { // <Model>::project for the residual, ::project_with_jac for the Jacobian pass
                 cam_project<X>(P.cam[0], Z0, Z1, Z2, xr0, xr1); // (optim/absolute.h:59-61,97-104)
@@ -2131,7 +2145,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
             const double x0 = P.p[0][k], x1 = P.p[1][k];
             {
                 const double q0 = xr0 - x0, q1 = xr1 - x1;
-                lsum += L.loss(q0 * q0 + q1 * q1);
+                lsum += wmul<W>(wk, L.loss(q0 * q0 + q1 * q1));
                 rows += 1.0;
             }
             const double r0 = zp0 - x0, r1 = zp1 - x1;
@@ -2146,9 +2160,10 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
                 J[a][2] = -X1 * dZ[0] + X0 * dZ[1];
                 J[a][3] = dZ[0]; J[a][4] = dZ[1]; J[a][5] = dZ[2];
             }
-            A.add2(L, r0, r1, J[0], J[1]);
+            A.template add2<W>(L, r0, r1, J[0], J[1], wk);
         } else if (KIND == KIND_HOMOG) {
             const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
+            const double wk = lm_weight<W>(wt, k); // one weight for both transfers (optim/homography.h:75,84,121,147)
             const double *H = ctx, *G = ctx + 9;
             // forward transfer (optim/homography.h:63-71,107-123); parameters = H00,H10,H20,H01,H11,H21,H02,H12
             const double Hx0 = H[0] * a0 + H[1] * a1 + H[2];
@@ -2156,7 +2171,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
             const double iw = 1.0 / (H[6] * a0 + H[7] * a1 + H[8]);
             const double z0 = Hx0 * iw, z1 = Hx1 * iw;
             const double r0 = z0 - b0, r1 = z1 - b1;
-            lsum += L.loss(r0 * r0 + r1 * r1);
+            lsum += wmul<W>(wk, L.loss(r0 * r0 + r1 * r1));
             double J0[8] = {a0, 0.0, -a0 * z0, a1, 0.0, -a1 * z0, 1.0, 0.0};
             double J1[8] = {0.0, a0, -a0 * z1, 0.0, a1, -a1 * z1, 0.0, 1.0};
 #pragma unroll
@@ -2164,7 +2179,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
                 J0[m] = J0[m] * iw;
                 J1[m] = J1[m] * iw;
             }
-            A.add2(L, r0, r1, J0, J1);
+            A.template add2<W>(L, r0, r1, J0, J1, wk);
             // backward transfer through adj(H) (optim/homography.h:73-81,125-152):  y = pi(G x2),
             // dy_i/dH_k = ( (dG/dH_k x2)_i - y_i (dG/dH_k x2)_2 ) / (G x2)_2
             const double Gx0 = G[0] * b0 + G[1] * b1 + G[2];
@@ -2172,7 +2187,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
             const double iv = 1.0 / (G[6] * b0 + G[7] * b1 + G[8]);
             const double y0 = Gx0 * iv, y1 = Gx1 * iv;
             const double s0 = y0 - a0, s1 = y1 - a1;
-            lsum += L.loss(s0 * s0 + s1 * s1);
+            lsum += wmul<W>(wk, L.loss(s0 * s0 + s1 * s1));
             rows += 2.0;
             const double y0b1 = y0 * b1, y0b0 = y0 * b0, y1b1 = y1 * b1, y1b0 = y1 * b0;
             const double H00 = H[0], H01 = H[1], H02 = H[2], H10 = H[3], H11 = H[4], H12 = H[5], H20 = H[6],
@@ -2199,17 +2214,18 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
                 K0[m] = K0[m] * iv;
                 K1[m] = K1[m] * iv;
             }
-            A.add2(L, s0, s1, K0, K1);
+            A.template add2<W>(L, s0, s1, K0, K1, wk);
         } else if (KIND == KIND_RELPOSE_TS) {
             // FixCameraRelativePoseRefiner (optim/relative.h:181-249)
             double v[TS_ARRAYS];
             load_ts(P, k, v);
+            const double wk = lm_weight<W>(wt, k);
             double C, JC[4];
             tangent_terms(ctx, v, v + 3, v + 6, v + 12, C, JC);
             {
                 const double nJc_sq = (JC[2] * JC[2] + JC[3] * JC[3]) + (JC[0] * JC[0] + JC[1] * JC[1]);
                 const double rr = C / sqrt(nJc_sq);
-                lsum += L.loss(rr * rr);
+                lsum += wmul<W>(wk, L.loss(rr * rr));
                 rows += 1.0;
             }
             const double nJ_C = sqrt((JC[0] * JC[0] + JC[2] * JC[2]) + (JC[1] * JC[1] + JC[3] * JC[3]));
@@ -2235,12 +2251,13 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
                 for (int m = 0; m < 9; ++m) t += dF[m] * D[NP * m + p];
                 J[p] = t;
             }
-            A.add1(L, r, J);
+            A.template add1<W>(L, r, J, wk);
         } else {
             const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
+            const double wk = lm_weight<W>(wt, k);
             {
                 const double rr = sampson_res(ctx, a0, a1, b0, b1);
-                lsum += L.loss(rr * rr);
+                lsum += wmul<W>(wk, L.loss(rr * rr));
                 rows += 1.0;
             }
             double r, dF[9], J[NP];
@@ -2253,7 +2270,7 @@ PLB_DEV void lm_eval_pass(const ProblemDev &P, const LossFn &L, const int *list,
                 for (int m = 0; m < 9; ++m) s += dF[m] * D[NP * m + p];
                 J[p] = s;
             }
-            A.add1(L, r, J);
+            A.template add1<W>(L, r, J, wk);
         }
     }
     constexpr int NV = 2 + NT + NP + 1;
@@ -2373,10 +2390,11 @@ PLB_DEV void ts_cam_row(const double *E, const double *D, const CamDev &c1, cons
 //         the fixed-camera refiner and the camera columns of ts_cam_row (optim/relative.h:289-441)
 // Every 256 points each thread writes its point's row of the tile; thread e < NV then adds value e of every row in point
 // order.  Order of the sums: points in order inside a CTA, CTAs in rank order (deterministic for a given cluster size).
-template <int KIND, bool X = false>
-PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *cams, const double (*cp)[CAM_MAX_PARAMS],
-                           const int *m, const int (*idx)[CAM_MAX_PARAMS], const int *list, int lo, int na,
-                           LmCamShared<KIND> *S, double *tile, int &buf, int csize) {
+// W: the residual weights of lm_eval_pass, folded into the row's loss and w columns.
+template <int KIND, bool X = false, bool W = false>
+PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const double *wt, const CamDev *cams,
+                           const double (*cp)[CAM_MAX_PARAMS], const int *m, const int (*idx)[CAM_MAX_PARAMS],
+                           const int *list, int lo, int na, LmCamShared<KIND> *S, double *tile, int &buf, int csize) {
     using Y = LmCamLayout<KIND>;
     constexpr int NP = Y::NP, NC = Y::NCAM;
     const double *ctx = S->ctx;
@@ -2425,15 +2443,16 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                 const double Z1 = ctx[3] * X0 + ctx[4] * X1 + ctx[5] * X2 + ctx[10];
                 const double Z2 = ctx[6] * X0 + ctx[7] * X1 + ctx[8] * X2 + ctx[11];
                 if (!(Z2 < 0)) { // optim/absolute.h:57-58,93-94
+                    const double wk = lm_weight<W>(wt, k);
                     double xr0, xr1, zp0, zp1, Jp[2][3];
                     cam_project<X>(cam[0], Z0, Z1, Z2, xr0, xr1);
                     cam_project_with_jac<X>(cam[0], Z0, Z1, Z2, zp0, zp1, &Jp[0][0]);
                     const double x0 = P.p[0][k], x1 = P.p[1][k];
                     const double q0 = xr0 - x0, q1 = xr1 - x1;
-                    tr[Y::LOSS] = L.loss(q0 * q0 + q1 * q1);
+                    tr[Y::LOSS] = wmul<W>(wk, L.loss(q0 * q0 + q1 * q1));
                     tr[Y::ROW] = 1.0;
                     const double r0 = zp0 - x0, r1 = zp1 - x1;
-                    const double w = L.weight(r0 * r0 + r1 * r1);
+                    const double w = wmul<W>(wk, L.weight(r0 * r0 + r1 * r1));
                     if (w != 0) { // jacobian_accumulator.h:87-104
                         filled = true;
                         tr[Y::JROW] = 1.0;
@@ -2463,6 +2482,7 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                 }
             } else { // KIND_RELPOSE_TS
                 const double a0 = P.p[0][k], a1 = P.p[1][k], b0 = P.p[2][k], b1 = P.p[3][k];
+                const double wk = lm_weight<W>(wt, k);
                 double d1[3], d2[3], M1[6], M2[6];
                 cam_unproject_with_jac_params<X>(cam[0], a0, a1, d1, M1, tr + Y::JP);
                 cam_unproject_with_jac_params<X>(cam[1], b0, b1, d2, M2, tr + Y::JP + 3 * CAM_MAX_PARAMS);
@@ -2471,12 +2491,12 @@ PLB_DEV void lmi_eval_pass(const ProblemDev &P, const LossFn &L, const CamDev *c
                 {
                     const double nJc_sq = (JC[2] * JC[2] + JC[3] * JC[3]) + (JC[0] * JC[0] + JC[1] * JC[1]);
                     const double rr = C / sqrt(nJc_sq);
-                    tr[Y::LOSS] = L.loss(rr * rr);
+                    tr[Y::LOSS] = wmul<W>(wk, L.loss(rr * rr));
                     tr[Y::ROW] = 1.0;
                 }
                 const double nJ_C = sqrt((JC[0] * JC[0] + JC[2] * JC[2]) + (JC[1] * JC[1] + JC[3] * JC[3]));
                 const double r = C * (1.0 / nJ_C);
-                const double w = L.weight(r * r);
+                const double w = wmul<W>(wk, L.weight(r * r));
                 if (w != 0) { // jacobian_accumulator.h:125-141
                     filled = true;
                     tr[Y::JROW] = 1.0;
@@ -2585,7 +2605,7 @@ template <class Shared, class Keep> PLB_DEV int lm_compact(Shared *S, int lo, in
 // CAM writes camera i of job j to cam_outs[(j * kind_cam_count(KIND) + i) * CAM_MAX_PARAMS ..].
 template <int KIND, bool CAM> struct LmNP { static constexpr int v = LmDims<KIND>::NP; };
 template <int KIND> struct LmNP<KIND, true> { static constexpr int v = LmCamLayout<KIND>::NP; };
-template <int KIND, bool CAM, bool X = false>
+template <int KIND, bool CAM, bool X = false, bool W = false>
 __global__ void __launch_bounds__(LM_THREADS, 1)
     k_lm(const ProblemDev *__restrict__ probs, const LmJob *__restrict__ jobs, const LoJobSrc *__restrict__ job_src,
          const double *__restrict__ models_in, const int *__restrict__ n_jobs_dev, int n_jobs, const char *mask_base,
@@ -2695,11 +2715,13 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
         }
     }
     // one evaluation pass at par (trial: par_new), totals in S.tot
+    const double *wt = W ? J.w : nullptr;
     auto eval = [&](bool trial) {
         if constexpr (CAM)
-            lmi_eval_pass<KIND, X>(P, L, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf, csize);
+            lmi_eval_pass<KIND, X, W>(P, L, wt, cams, trial ? S.cam_new : S.cam, m, idx, list, lo, na, &S, lmi_tile, buf,
+                                      csize);
         else
-            lm_eval_pass<KIND, X>(P, L, list, lo, na, &S, buf, csize);
+            lm_eval_pass<KIND, X, W>(P, L, wt, list, lo, na, &S, buf, csize);
     };
 
     int iterations = 0;
@@ -2867,10 +2889,11 @@ static int lm_cluster_size(int n_jobs, int max_n) {
 }
 // A grid of n_clusters clusters of csize CTAs over a job list: k_lm<kind> of the fixed-camera refiner, or with
 // refine_camera the refiner with camera parameters of the kind (KIND_PNP or KIND_RELPOSE_TS).
+// weighted: the W instantiation (LmJob::w); the LO launches of the rounds have no weights.
 static void launch_lm_any(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs,
                           const LoJobSrc *job_src, const double *models_in, const int *n_jobs_dev, int n_jobs,
                           int n_clusters, int csize, const char *mask_base, int *idx_scratch, int scratch_stride,
-                          LmJobOut *out, double *cam_out, cudaStream_t stream) {
+                          LmJobOut *out, double *cam_out, cudaStream_t stream, bool weighted = false) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)(n_clusters * csize), 1, 1);
@@ -2896,21 +2919,25 @@ static void launch_lm_any(int kind, bool refine_camera, bool xcam, const Problem
     if (refine_camera) {
         auto cam_kernel = kind == KIND_RELPOSE_TS ? (xcam ? k_lm<KIND_RELPOSE_TS, true, true> : k_lm<KIND_RELPOSE_TS, true>)
                                                   : (xcam ? k_lm<KIND_PNP, true, true> : k_lm<KIND_PNP, true>);
+        if (weighted)
+            cam_kernel = kind == KIND_RELPOSE_TS
+                             ? (xcam ? k_lm<KIND_RELPOSE_TS, true, true, true> : k_lm<KIND_RELPOSE_TS, true, false, true>)
+                             : (xcam ? k_lm<KIND_PNP, true, true, true> : k_lm<KIND_PNP, true, false, true>);
         cudaFuncSetAttribute(cam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile);
         launch(cam_kernel);
     } else if (xcam && kind == KIND_PNP) {
-        launch(k_lm<KIND_PNP, false, true>);
+        launch(weighted ? k_lm<KIND_PNP, false, true, true> : k_lm<KIND_PNP, false, true>);
     } else {
-        with_kind(kind, [&](auto K) { launch(k_lm<K, false>); });
+        with_kind(kind, [&](auto K) { launch(weighted ? k_lm<K, false, false, true> : k_lm<K, false>); });
     }
 }
-void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs_dev,
+void launch_lm(int kind, bool refine_camera, bool xcam, bool weighted, const ProblemDev *probs, const LmJob *jobs_dev,
                const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
                int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream) {
     if (n_jobs <= 0) return;
     const int csize = lm_cluster_size(n_jobs, max_n);
     launch_lm_any(kind, refine_camera, xcam, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base,
-                  idx_scratch, scratch_stride, out, cam_out, stream);
+                  idx_scratch, scratch_stride, out, cam_out, stream, weighted);
 }
 // Clusters of a round's LO launch: at most one wave (a k_lm CTA owns an SM), at most the estimated number of jobs.
 int lm_round_max_clusters(int kind, int est_jobs, int max_n) {

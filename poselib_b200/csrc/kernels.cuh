@@ -180,6 +180,8 @@ struct LmJob {
     long long mask_off;     // offset into the mask buffer (subset_mode 2), else -1
     long long scratch_off;  // offset (ints) into idx_scratch for the active-point list (subset modes 1, 2)
     LmParams prm;
+    const double *w;        // per-residual weights of the problem's n points, in point order (device), or null: uniform.
+                            // Read only by the W instantiations of k_lm, which launch_lm runs when some job has them
 };
 struct LmJobOut {
     double model[9];
@@ -243,8 +245,9 @@ void launch_score_models(int kind, const ProblemDev *probs, const double *models
 // KIND_RELPOSE_TS): every job refines camera parameters with the pose (LmJob::cam_refine) and writes its
 // kind_cam_count(kind) cameras to cam_out[(j * kind_cam_count(kind) + i) * CAM_MAX_PARAMS ..].
 constexpr __host__ __device__ int kind_cam_count(int kind) { return kind == KIND_RELPOSE_TS ? 2 : 1; }
-// xcam: some camera of the jobs' problems (ProblemDev::cam) is a fisheye or division model
-void launch_lm(int kind, bool refine_camera, bool xcam, const ProblemDev *probs, const LmJob *jobs_dev,
+// xcam: some camera of the jobs' problems (ProblemDev::cam) is a fisheye or division model.  weighted: some job has
+// per-residual weights (LmJob::w); the jobs without them then run with uniform weights in the same launch.
+void launch_lm(int kind, bool refine_camera, bool xcam, bool weighted, const ProblemDev *probs, const LmJob *jobs_dev,
                const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
                int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream);
 // LO jobs of a round, listed on the device by k_pass1: job j refines model slot job_src[j].slot of the round's model
