@@ -345,6 +345,22 @@ typedef struct plb_estimate_problem {
 } plb_estimate_problem;
 /* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device). */
 int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
+/* plb_estimate_batch(problems, count, -1, streams) with the correspondences and masks in device memory, for callers whose
+ * matches are already on the GPU.  Everything else (kinds, cameras, options, model, stats, counters, status, camera1)
+ * is as in plb_estimate_batch; only where the data lives differs:
+ *  - a, b: device (or managed) memory of the calling thread's device (plb_set_device), contiguous row-major [n,2] /
+ *    [n,3] arrays of `dtype`, aligned to it.  With PLB_DTYPE_F32 they are `const float *` cast into the `const double *`
+ *    fields.  They are only read: the engine works on its own fp64 copy, and fp32 -> fp64 is exact, so a float call gives
+ *    the results of the double call on the widened values.
+ *  - inliers: NULL or n bytes of device memory on the same device; receives 0 / 1 as the host call writes them.
+ *  - stream: a cudaStream_t of that device (NULL = the legacy default stream).  No input is read before the work queued
+ *    on `stream` ahead of the call has finished; when the call returns, every device write it made is complete.
+ * Checked before any copy or launch, with every status set and nothing else written on failure: NULL problems or an
+ * unknown dtype -> PLB_ERR_ARG (before the device check); no device -> PLB_ERR_CUDA; a / b / inliers of a problem with
+ * n > 0 that are not device memory of the current device (pageable or page-locked host memory, another GPU), or a / b
+ * misaligned for the dtype -> PLB_ERR_ARG.  counters.h2d_bytes holds no correspondences and d2h_bytes no masks. */
+enum { PLB_DTYPE_F64 = 0, PLB_DTYPE_F32 = 1 };
+int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams);
 
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers
  * that run several estimations on the same matches).  kind: PLB_KIND_*; returns a handle > 0 or an error < 0. */

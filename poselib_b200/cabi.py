@@ -104,8 +104,9 @@ EXPORTS = [
     "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_relpose_pair", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
     "plb_resident_free", "plb_bundle_adjust_image_weighted", "plb_refine_relpose_weighted",
     "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
-    "plb_refine_homography_weighted",
+    "plb_refine_homography_weighted", "plb_estimate_batch_device",
 ]
+DTYPE_F64, DTYPE_F32 = 0, 1
 
 class EstimateProblem(C.Structure):
     _fields_ = [("kind", C.c_int32), ("real_focal_check", C.c_int32), ("tangent_sampson", C.c_int32), ("reserved", C.c_int32),
@@ -563,26 +564,83 @@ def estimate_batch(problems, streams=8, n_gpus=-1):
         npts = len(aa)
         mask = np.zeros(max(npts, 1), dtype=np.int8)
         keep.append((aa, ba, mask))
-        q.kind = KIND[p["kind"]]
-        q.real_focal_check = int(p.get("rfc", False))
-        q.tangent_sampson = int(p.get("tangent_sampson", False))
-        q.n = npts
+        _fill_estimate_problem(q, p, npts)
         q.a, q.b = ap, bp
-        q.camera1 = p.get("cam1") or Camera("NULL", ())
-        q.camera2 = p.get("cam2") or Camera("NULL", ())
-        q.ransac = p["ransac"]
-        q.bundle = p["bundle"]
-        q.max_error = p["max_error"]
-        m = _init_model(p["kind"], p.get("init"))
-        for k in range(len(m)):
-            q.model[k] = m[k]
         q.inliers = C.cast(mask.ctypes.data_as(C.POINTER(C.c_char)), C.c_char_p)
     _check(_lib.plb_estimate_batch(arr, C.c_size_t(count), int(n_gpus), int(streams)))
+    return _estimate_results(arr, problems, [k[2][:q.n].copy() for k, q in zip(keep, arr)])
+
+
+def _fill_estimate_problem(q, p, npts):
+    """Everything of one plb_estimate_problem but its point and mask pointers."""
+    q.kind = KIND[p["kind"]]
+    q.real_focal_check = int(p.get("rfc", False))
+    q.tangent_sampson = int(p.get("tangent_sampson", False))
+    q.n = npts
+    q.camera1 = p.get("cam1") or Camera("NULL", ())
+    q.camera2 = p.get("cam2") or Camera("NULL", ())
+    q.ransac = p["ransac"]
+    q.bundle = p["bundle"]
+    q.max_error = p["max_error"]
+    m = _init_model(p["kind"], p.get("init"))
+    for k in range(len(m)):
+        q.model[k] = m[k]
+
+
+def _estimate_results(arr, problems, masks):
     out = []
     for i, p in enumerate(problems):
         q = arr[i]
         kind = p["kind"]
         m = np.array(q.model[:7] if kind in ("pnp", "relpose") else q.model[:9], dtype=np.float64)
-        out.append({"model": _model_out(kind, m), "inliers": keep[i][2][:q.n].copy(), "stats": q.stats.as_dict(),
+        out.append({"model": _model_out(kind, m), "inliers": masks[i], "stats": q.stats.as_dict(),
                     "counters": q.counters.as_dict(), "status": q.status, "camera1": _camera_params(q.camera1)})
     return out
+
+
+def estimate_batch_device(problems, streams=8, stream=None):
+    """estimate_batch (n_gpus=-1) on correspondences that are already on the GPU (plb_estimate_batch_device).
+    problems: the dicts estimate_batch takes, with a / b as CUDA torch tensors [n,2] / [n,3] ([n,2] for the 2D-2D kinds),
+    all on one device and of one dtype, float32 or float64.  The call runs on that device and reads the inputs after the
+    work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle; default: the device's current stream).
+    Returns the dicts of estimate_batch, with `inliers` a CUDA torch.bool tensor of length n (the masks of one call are
+    views of one allocation)."""
+    import torch
+    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
+    tensors = [t for p in problems for t in (p["a"], p["b"])]
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
+        raise TypeError("estimate_batch_device: a and b must be CUDA torch tensors")
+    if not tensors:
+        return []
+    dev, dt = tensors[0].device, tensors[0].dtype
+    if any(t.device != dev for t in tensors):
+        raise ValueError(f"estimate_batch_device: every tensor must be on {dev} (shard the batch by device)")
+    if dt not in dtypes or any(t.dtype != dt for t in tensors):
+        raise TypeError("estimate_batch_device: a and b must share one dtype, torch.float32 or torch.float64")
+    set_device(dev.index)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev)
+    elif not isinstance(stream, torch.cuda.Stream):
+        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    count = len(problems)
+    arr = (EstimateProblem * count)()
+    keep = []
+    sizes = [p["a"].shape[0] for p in problems]
+    with torch.cuda.stream(stream):  # the copies and masks below are ordered before the call's reads and writes
+        # one zeroed allocation for the whole batch (one launch, not one per problem); problem i's mask is a view of it
+        masks = list(torch.zeros(sum(sizes), dtype=torch.bool, device=dev).split(sizes))
+        for i, p in enumerate(problems):
+            q = arr[i]
+            a, b = p["a"].contiguous(), p["b"].contiguous()
+            npts = sizes[i]
+            b_dim = 3 if p["kind"] == "pnp" else 2
+            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
+                raise ValueError(f"estimate_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
+                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
+            keep.append((a, b))
+            _fill_estimate_problem(q, p, npts)
+            q.a, q.b = C.cast(C.c_void_p(a.data_ptr()), _P), C.cast(C.c_void_p(b.data_ptr()), _P)
+            q.inliers = C.cast(C.c_void_p(masks[i].data_ptr() if npts else None), C.c_char_p)
+    _check(_lib.plb_estimate_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+                                          int(streams)))
+    return _estimate_results(arr, problems, masks)

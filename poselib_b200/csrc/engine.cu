@@ -199,6 +199,7 @@ struct Engine {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev4 = nullptr;
     cudaEvent_t ev_block = nullptr; // cudaEventBlockingSync: the waiting thread sleeps instead of spinning
+    cudaEvent_t ev_in = nullptr;    // plb_estimate_batch_device: recorded in the caller's stream, waited on by every group
     bool ready = false;
     int device = -1;
     DevBuf<double> in, soa64, px64, models, lm_in, s5_blk, s5_park, s5_cpoly, s5_roots;
@@ -231,6 +232,10 @@ struct Engine {
     PinBuf<NormDesc> h_ndesc;
     MapBuf<double> h_norm;
     DevBuf<MaskDesc> mdesc;
+    DevBuf<IngestDesc> idesc; // device-resident inputs and masks (plb_estimate_batch_device)
+    PinBuf<IngestDesc> h_idesc;
+    DevBuf<ScatterDesc> sdesc;
+    PinBuf<ScatterDesc> h_sdesc;
     DevBuf<LmJob> jobs;
     DevBuf<double> wts; // per-residual weights of a refiner call (LmJob::w)
     PinBuf<double> h_in, h_lm_in;
@@ -274,6 +279,7 @@ struct Engine {
         if (!ev3) PLB_CUDA(cudaEventCreate(&ev3));
         if (!ev4) PLB_CUDA(cudaEventCreate(&ev4));
         if (!ev_block) PLB_CUDA(cudaEventCreateWithFlags(&ev_block, cudaEventBlockingSync | cudaEventDisableTiming));
+        if (!ev_in) PLB_CUDA(cudaEventCreateWithFlags(&ev_in, cudaEventDisableTiming));
         {
             int r = h_work.ensure(8);
             if (r) return r;
@@ -293,6 +299,16 @@ static bool host_pinned(const void *p) {
         return false;
     }
     return at.type == cudaMemoryTypeHost;
+}
+// Is p device or managed memory of `device` (plb_estimate_batch_device)?  Pageable and page-locked host memory are not.
+// Needs a current context.
+static bool device_memory(const void *p, int device) {
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == device;
 }
 
 // Batch workers of an oversubscribed process (more lock-step groups in flight than cores this process may use: several
@@ -549,6 +565,10 @@ struct Task {
     int pre_mode = 0;
     double pre_scale = 1.0;
     CamDev cam_a{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}}, cam_b{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
+    // plb_estimate_batch_device: a, b (float when f32) and inliers are device memory of the group's device, read and
+    // written only after `ready` (recorded in the caller's stream) has completed
+    bool dev_io = false, f32 = false;
+    cudaEvent_t ready = nullptr;
 };
 
 // per-problem serial state of the reference loop (ransac_impl.h:99-104,157-201)
@@ -717,13 +737,21 @@ struct Group {
     }
 
     // ---- device layout of the group: SoA arrays of every non-resident problem, masks, ProblemDev table -------------
-    // Stages the caller's arrays and issues their host -> device copies; the layout kernel runs in transpose().
+    // Stages the caller's arrays and issues their host -> device copies (device-resident arrays: k_ingest); the layout
+    // kernel runs in transpose().
     int upload() {
-        int rc, n_polish = 0;
+        int rc, n_polish = 0, n_ingest = 0;
+        size_t host_doubles = 0, max_ingest = 0; // inputs staged on the host / gathered on the device (k_ingest)
         const int nc = kind_cam_count(kind);
         for (PState &S : PS) {
             if (S.n == 0) continue;
             if (!S.t->res) {
+                if (S.t->dev_io) {
+                    ++n_ingest;
+                    max_ingest = std::max(max_ingest, (size_t)in_arr * S.n);
+                } else {
+                    host_doubles += (size_t)in_arr * S.n;
+                }
                 in_doubles += (size_t)in_arr * S.n;
                 soa_elems += (size_t)n_arr * S.n_pad;
                 if (kind == KIND_RELPOSE || kind == KIND_FUND) q_rows += (size_t)S.n_pad;
@@ -739,12 +767,14 @@ struct Group {
             }
         }
         n_probdev = NP + n_polish;
-        if ((rc = E.h_in.ensure(in_doubles)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
+        // the staging buffer mirrors E.in's offsets; a group of device-resident inputs needs none
+        if ((rc = E.h_in.ensure(host_doubles ? in_doubles : 0)) || (rc = E.in.ensure(in_doubles)) || (rc = E.soa64.ensure(soa_elems)) ||
             (rc = E.soa32.ensure(soa_elems)) || (rc = E.qrows.ensure(q_rows)) || (rc = E.cmax.ensure(5 * (size_t)NP)) || (rc = E.px64.ensure(px_elems)) || (rc = E.mask.ensure(mask_bytes)) ||
             (rc = E.mask_bits.ensure(mask_bytes / 32 + 1)) || (rc = E.h_mask_bits.ensure(mask_bytes / 32 + 1)) ||
             (rc = E.work.ensure(8)) || (rc = E.probs.ensure(n_probdev)) ||
             (rc = E.h_probs.ensure(n_probdev)) || (rc = E.tdesc.ensure(std::max(n_up, 1))) ||
-            (rc = E.h_tdesc.ensure(std::max(n_up, 1))))
+            (rc = E.h_tdesc.ensure(std::max(n_up, 1))) ||
+            (n_ingest && ((rc = E.idesc.ensure(n_ingest)) || (rc = E.h_idesc.ensure(n_ingest)))))
             return rc;
         struct DirectCopy {
             double *dst;
@@ -754,7 +784,8 @@ struct Group {
         std::vector<DirectCopy> direct; // page-locked caller arrays: DMA straight from them (issued below, in one turn)
         size_t in_off = 0, soa_off = 0, px_off = 0, q_off = 0;
         std::vector<std::pair<size_t, size_t>> staged; // (offset, doubles) of the inputs that went through the staging buffer
-        int iu = 0, ipol = 0;
+        int iu = 0, ipol = 0, ii = 0;
+        cudaEvent_t ready = nullptr; // the one event of the device call the group's tasks come from
         for (int i = 0; i < NP; ++i) {
             PState &S = PS[i];
             ProblemDev &P = E.h_probs.p[i];
@@ -777,7 +808,16 @@ struct Group {
                 assert(!S.t->polish.evaluates_camera()); // plb_resident_create takes no camera
             } else {
                 S.in_off = (long long)in_off;
-                if (host_pinned(S.t->a) && host_pinned(S.t->b)) {
+                if (S.t->dev_io) { // gathered on the device by k_ingest (below): nothing crosses PCIe
+                    IngestDesc &I = E.h_idesc.p[ii++];
+                    I.a = S.t->a;
+                    I.b = S.t->b;
+                    I.dst = E.in.p + in_off;
+                    I.n = S.n;
+                    I.b_dim = b_dim;
+                    I.f32 = S.t->f32 ? 1 : 0;
+                    ready = S.t->ready;
+                } else if (host_pinned(S.t->a) && host_pinned(S.t->b)) {
                     // the caller's arrays are page-locked: DMA straight from them, no staging copy on the host
                     direct.push_back({E.in.p + in_off, S.t->a, sizeof(double) * 2 * S.n});
                     direct.push_back({E.in.p + in_off + 2 * (size_t)S.n, S.t->b, sizeof(double) * (size_t)b_dim * S.n});
@@ -844,6 +884,13 @@ struct Group {
             PLB_CUDA(cudaMemcpyAsync(E.in.p + off, E.h_in.p + off, sizeof(double) * len, cudaMemcpyHostToDevice, st));
             h2d += sizeof(double) * len;
             i = j;
+        }
+        if (n_ingest) {
+            PLB_CUDA(cudaMemcpyAsync(E.idesc.p, E.h_idesc.p, sizeof(IngestDesc) * n_ingest, cudaMemcpyHostToDevice, st));
+            // the caller's arrays are read after the work it queued on its stream before the call
+            PLB_CUDA(cudaStreamWaitEvent(st, ready, 0));
+            launch_ingest(E.idesc.p, n_ingest, max_ingest, st);
+            E.launches++;
         }
         return PLB_OK;
     }
@@ -1429,10 +1476,31 @@ struct Group {
                 pol_of.push_back(&S);
             }
         if (!pol.empty() && (rc = lm_batch(pol))) return rc;
-        // the masks cross PCIe as bits (1/8 of the bytes) and are expanded into the caller's char[n] below
-        launch_pack_mask(E.mask.p, E.mask_bits.p, mask_bytes, st);
-        E.launches++;
-        PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
+        // host callers: the masks cross PCIe as bits (1/8 of the bytes) and are expanded into the caller's char[n] below;
+        // device callers (plb_estimate_batch_device): k_scatter_masks writes them into the caller's buffers
+        bool host_out = false;
+        int n_scatter = 0, max_scatter = 0;
+        for (const PState &S : PS) {
+            host_out = host_out || !S.t->dev_io;
+            if (S.t->dev_io && S.t->inliers && S.n > 0) {
+                ++n_scatter;
+                max_scatter = std::max(max_scatter, S.n);
+            }
+        }
+        if (host_out) {
+            launch_pack_mask(E.mask.p, E.mask_bits.p, mask_bytes, st);
+            E.launches++;
+            PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, sizeof(uint32_t) * (mask_bytes / 32), cudaMemcpyDeviceToHost, st));
+        }
+        if (n_scatter) {
+            if ((rc = E.sdesc.ensure(n_scatter)) || (rc = E.h_sdesc.ensure(n_scatter))) return rc;
+            int j = 0;
+            for (const PState &S : PS)
+                if (S.t->dev_io && S.t->inliers && S.n > 0) E.h_sdesc.p[j++] = {S.t->inliers, S.mask_off, S.n};
+            PLB_CUDA(cudaMemcpyAsync(E.sdesc.p, E.h_sdesc.p, sizeof(ScatterDesc) * n_scatter, cudaMemcpyHostToDevice, st));
+            launch_scatter_masks(E.mask.p, E.sdesc.p, n_scatter, max_scatter, st);
+            E.launches++;
+        }
         if ((rc = sync())) return rc;
         for (size_t j = 0; j < pol.size(); ++j) {
             const FinalPolish &fp = pol_of[j]->t->polish;
@@ -1445,13 +1513,15 @@ struct Group {
                                       fp.cam_out[i]);
         }
         for (PState &S : PS) {
-            if (S.t->inliers && S.n > 0) {
-                const uint32_t *w = E.h_mask_bits.p + (S.mask_off >> 5); // mask_off is a multiple of 32
-                char *dst = S.t->inliers;
-                for (int k = 0; k < S.n; ++k) dst[k] = (char)((w[k >> 5] >> (k & 31)) & 1u);
+            if (!S.t->dev_io) {
+                if (S.t->inliers && S.n > 0) {
+                    const uint32_t *w = E.h_mask_bits.p + (S.mask_off >> 5); // mask_off is a multiple of 32
+                    char *dst = S.t->inliers;
+                    for (int k = 0; k < S.n; ++k) dst[k] = (char)((w[k >> 5] >> (k & 31)) & 1u);
+                }
+                d2h += (size_t)S.n_pad / 8;
             }
             std::copy(S.best_model, S.best_model + MSZ, S.t->model);
-            d2h += (size_t)S.n_pad / 8;
         }
         PLB_CUDA(cudaGetLastError());
         return PLB_OK;
@@ -2402,6 +2472,36 @@ int plb_ransac_batch_multi(plb_problem *problems, size_t count, int n_gpus, int 
     return batch_impl(problems, count, devs.data(), n_gpus, streams_per_gpu);
 }
 
+// The body of the two estimate batch calls: the pre-step of every problem, LO-RANSAC of the tasks over `devs`, the
+// post-step.  dev_io: a / b (float when f32) and inliers are device memory, read after `ready` has completed.
+static int estimate_batch_run(plb_estimate_problem *problems, size_t count, const std::vector<int> &devs, int streams,
+                              bool dev_io, bool f32, cudaEvent_t ready) {
+    std::vector<EstimateJob> jobs(count);
+    for (size_t i = 0; i < count; ++i) {
+        plb_estimate_problem &p = problems[i];
+        if (int r = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
+                                     p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
+                                     &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED)) {
+            for (size_t j = 0; j < count; ++j) problems[j].status = r;
+            return r;
+        }
+    }
+    std::vector<Task> tasks(count);
+    std::vector<int> dev_of(count, -1);
+    for (size_t i = 0; i < count; ++i) {
+        tasks[i] = jobs[i].t;
+        tasks[i].dev_io = dev_io;
+        tasks[i].f32 = f32;
+        tasks[i].ready = ready;
+    }
+    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
+    for (size_t i = 0; i < count; ++i) {
+        problems[i].status = rc;
+        if (rc == PLB_OK) estimate_finish(jobs[i], tasks[i]);
+    }
+    return rc;
+}
+
 // Batch form of the four estimate_* entry points (robust.h:45-46,68-70,112-113,133-134): pixels + cameras in, the
 // pre-step of every problem (threshold scaling, camera unprojection and normalize_points on the device), LO-RANSAC in
 // lock-step groups per kind (tangent-Sampson problems form their own groups), final bundle and un-normalisation.  n_gpus: 0 = all devices of the process, k = the first k, -1 = the calling thread's device only.
@@ -2424,25 +2524,42 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
     if (n_gpus == -1) devs.push_back(g_device);
     else
         for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
-    std::vector<EstimateJob> jobs(count);
+    return estimate_batch_run(problems, count, devs, streams_per_gpu, false, false, nullptr);
+}
+// The same on the calling thread's device with device-resident inputs and masks: the inputs are gathered into the engine's
+// own buffer by k_ingest (F / H normalisation then works in place on that copy, the caller's arrays are only read) and
+// the masks are written by k_scatter_masks, so what runs between is the host path's work on the same doubles.
+int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    if (count == 0) return PLB_OK;
+    if (!problems) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    auto fail_all = [&](int rc, const std::string &msg) {
+        g_err = msg;
+        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
+        return rc;
+    };
+    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
+    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    Engine &E = *engine();
+    if (int rc = E.init()) return fail_all(rc, g_err);
+    const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
     for (size_t i = 0; i < count; ++i) {
-        plb_estimate_problem &p = problems[i];
-        if (int r = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
-                                     p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
-                                     &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED)) {
-            for (size_t j = 0; j < count; ++j) problems[j].status = r;
-            return r;
+        const plb_estimate_problem &p = problems[i];
+        if (p.n == 0) continue;
+        auto bad = [&](const char *what) { return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": " + what); };
+        for (const void *q : {(const void *)p.a, (const void *)p.b}) {
+            if (!device_memory(q, E.device)) return bad("a / b must be device memory of the current device");
+            if ((uintptr_t)q % elem) return bad("a / b are not aligned to the dtype");
         }
+        if (p.inliers && !device_memory(p.inliers, E.device))
+            return bad("inliers must be NULL or device memory of the current device");
     }
-    std::vector<Task> tasks(count);
-    std::vector<int> dev_of(count, -1);
-    for (size_t i = 0; i < count; ++i) tasks[i] = jobs[i].t;
-    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams_per_gpu);
-    for (size_t i = 0; i < count; ++i) {
-        problems[i].status = rc;
-        if (rc == PLB_OK) estimate_finish(jobs[i], tasks[i]);
-    }
-    return rc;
+    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
+    const std::vector<int> devs{E.device};
+    return estimate_batch_run(problems, count, devs, streams, true, dtype == PLB_DTYPE_F32, E.ev_in);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {

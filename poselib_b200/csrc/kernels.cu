@@ -1,5 +1,6 @@
 // poselib_b200 — CUDA kernels of the LO-RANSAC hot path for sm_90a (H100).
 //
+//   k_ingest           device-resident caller arrays (fp32 / fp64) -> the engine's fp64 AoS input buffer
 //   k_transpose        caller AoS doubles -> SoA fp64 (+ fp32 copy) in HBM, coalesced both ways
 //   k_solve_lane<KIND> / k7_solve_lane / k5_gather -> k5_null -> k5_elim -> k5_roots -> k5_back
 //                      minimal solvers of a round, one thread per minimal sample (the 5-point solver in phases)
@@ -9,7 +10,7 @@
 //   k_confirm          exact rescoring of the fast-mode candidates of a round
 //   k_lm<KIND, CAM>    Levenberg-Marquardt refit (LO step + final polish): one cluster per job, cluster-wide reductions
 //                      of the normal equations, scalar LM logic on thread 0; CAM refines PnP camera parameters too
-//   k_inlier_mask      final inlier masks
+//   k_inlier_mask      final inlier masks (k_scatter_masks: into the callers' device buffers)
 //   Every exact score (k_score_tiled, k_score, k_confirm, the rescoring in k_lm) comes from one routine, msac_score,
 //   and every fp64 inlier decision (those, k_inlier_mask, the LO subset in k_lm) from one test per kind, under_thr
 //   (+ cheirality for the relpose kinds); the PnP mask alone keeps the reference's own formula.
@@ -196,6 +197,39 @@ __global__ void __launch_bounds__(NORM_THREADS) k_normalize(const NormDesc *__re
         d.a[i] = d.a[i] / scale;
         d.b[i] = d.b[i] / scale;
     }
+}
+// Device-resident inputs (plb_estimate_batch_device) -> the fp64 AoS the host path would have uploaded, one problem per
+// blockIdx.y.  fp32 -> fp64 is exact, so everything downstream sees the values the host path sees for the widened input.
+// The copy also keeps the caller's arrays read-only: k_normalize works in place on the engine's buffer.
+constexpr int INGEST_THREADS = 256, INGEST_MAX_BLOCKS = 512;
+__global__ void __launch_bounds__(INGEST_THREADS) k_ingest(const IngestDesc *__restrict__ descs) {
+    const IngestDesc d = descs[blockIdx.y];
+    const size_t na = 2 * (size_t)d.n, total = na + (size_t)d.b_dim * d.n;
+    for (size_t i = (size_t)blockIdx.x * INGEST_THREADS + threadIdx.x; i < total; i += (size_t)gridDim.x * INGEST_THREADS) {
+        const bool in_a = i < na;
+        const size_t j = in_a ? i : i - na;
+        const void *src = in_a ? d.a : d.b;
+        d.dst[i] = d.f32 ? (double)static_cast<const float *>(src)[j] : static_cast<const double *>(src)[j];
+    }
+}
+void launch_ingest(const IngestDesc *descs_dev, int n_desc, size_t max_vals, cudaStream_t stream) {
+    if (n_desc <= 0 || max_vals == 0) return;
+    const unsigned bx = (unsigned)std::min<size_t>((max_vals + INGEST_THREADS - 1) / INGEST_THREADS, INGEST_MAX_BLOCKS);
+    k_ingest<<<dim3(bx, n_desc, 1), INGEST_THREADS, 0, stream>>>(descs_dev);
+}
+// Final masks into the callers' device buffers (plb_estimate_batch_device), one problem per blockIdx.y: the 0 / 1 bytes
+// the host path expands from the packed bits.
+__global__ void __launch_bounds__(INGEST_THREADS) k_scatter_masks(const char *__restrict__ mask,
+                                                                  const ScatterDesc *__restrict__ descs) {
+    const ScatterDesc d = descs[blockIdx.y];
+    const char *src = mask + d.mask_off;
+    for (int k = blockIdx.x * INGEST_THREADS + threadIdx.x; k < d.n; k += gridDim.x * INGEST_THREADS)
+        d.dst[k] = src[k] != 0 ? 1 : 0;
+}
+void launch_scatter_masks(const char *mask, const ScatterDesc *descs_dev, int n_desc, int max_n, cudaStream_t stream) {
+    if (n_desc <= 0 || max_n <= 0) return;
+    const unsigned bx = (unsigned)std::min((max_n + INGEST_THREADS - 1) / INGEST_THREADS, INGEST_MAX_BLOCKS);
+    k_scatter_masks<<<dim3(bx, n_desc, 1), INGEST_THREADS, 0, stream>>>(mask, descs_dev);
 }
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream) {
     if (n_desc <= 0) return;

@@ -222,6 +222,19 @@ struct MaskDesc {
     long long mask_off;
     double model[9];
 };
+// Correspondences of one problem already in device memory (plb_estimate_batch_device): the caller's contiguous AoS arrays,
+// read only, gathered into the engine's own input buffer as fp64 (a then b, the layout the host path uploads).
+struct IngestDesc {
+    const void *a, *b; // 2n and b_dim*n values: float (f32) or double
+    double *dst;       // (2 + b_dim) * n doubles
+    int n, b_dim, f32;
+};
+// One final inlier mask for a caller's device buffer: n bytes 0 / 1 from the mask buffer at mask_off.
+struct ScatterDesc {
+    char *dst;
+    long long mask_off;
+    int n;
+};
 
 // ---- launchers (all asynchronous on `stream`) --------------------------------------------------------------
 // normalize_points for n_desc problems (descriptors in device memory), one CTA each.
@@ -276,6 +289,11 @@ void launch_inlier_masks(int kind, const ProblemDev *probs, const MaskDesc *desc
                          char *mask_base, cudaStream_t stream);
 // Inlier masks as bits (bit k & 31 of word k >> 5) for the device -> host copy; n_bytes is a multiple of 32.
 void launch_pack_mask(const char *mask, uint32_t *bits, size_t n_bytes, cudaStream_t stream);
+// Device-resident inputs -> fp64 AoS for n_desc problems (descriptors in device memory); max_vals: the largest
+// (2 + b_dim) * n of the descriptors.
+void launch_ingest(const IngestDesc *descs_dev, int n_desc, size_t max_vals, cudaStream_t stream);
+// Final masks straight into the callers' device buffers for n_desc problems; max_n: the largest n of the descriptors.
+void launch_scatter_masks(const char *mask, const ScatterDesc *descs_dev, int n_desc, int max_n, cudaStream_t stream);
 // Batched direct solver calls (solvers/*.h surface): one thread per instance.  kind KIND_RELPOSE also needs the s5_*
 // phase buffers of s5 for `count` instances (the other fields are unused).  Returns the number of kernels launched.
 int launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out, int *n_out,
