@@ -362,6 +362,61 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
 enum { PLB_DTYPE_F64 = 0, PLB_DTYPE_F32 = 1 };
 int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams);
 
+/* Batch form of the robust/bundle.h refiners above (bundle.cc:84-112,206-222,237-256,313-333,394-411), for callers that
+ * refine many independent problems at once: every two-view geometry of a matching graph, every query of a localisation
+ * run.  Each problem carries what its single entry point takes and receives what that call writes; the single entry
+ * points are the one-problem case of this call.  Each problem's model, bundle_stats and camera parameters are bit for bit
+ * what its single call returns on the same inputs, whatever else is in the batch and for any n_gpus / streams.
+ *   refiner                          single entry point                           cameras read / written
+ *   PLB_REFINER_BUNDLE               plb_bundle_adjust (weights ignored, as the reference drops them, bundle.cc:84-92)
+ *   PLB_REFINER_BUNDLE_IMAGE         plb_bundle_adjust_image[_weighted]           camera1 / its refined parameters
+ *   PLB_REFINER_RELPOSE              plb_refine_relpose[_weighted]
+ *   PLB_REFINER_RELPOSE_CAMERAS      plb_refine_relpose_cameras[_weighted]        camera1, camera2 / none
+ *   PLB_REFINER_RELPOSE_PAIR         plb_refine_relpose_pair[_weighted]           camera1, camera2 / their refined parameters
+ *   PLB_REFINER_FUNDAMENTAL          plb_refine_fundamental[_weighted]
+ *   PLB_REFINER_HOMOGRAPHY           plb_refine_homography[_weighted]
+ * Cameras a refiner does not read are ignored, and parameters the single call leaves alone stay untouched.
+ * Every problem is checked before any device call, by its single entry point's rules; on failure every status gets the
+ * code and nothing else is written: NULL problems, an unknown refiner, or a / b NULL with n > 0 -> PLB_ERR_ARG; a camera
+ * the refiner reads outside the ten models -> PLB_ERR_NYI; PLB_REFINER_RELPOSE_CAMERAS with a non-empty refine_intrinsics
+ * selection -> PLB_ERR_NYI; n_gpus < -1 -> PLB_ERR_ARG; no device -> PLB_ERR_CUDA; n_gpus above the device count ->
+ * PLB_ERR_ARG. */
+enum {
+    PLB_REFINER_BUNDLE = 0,
+    PLB_REFINER_BUNDLE_IMAGE = 1,
+    PLB_REFINER_RELPOSE = 2,
+    PLB_REFINER_RELPOSE_CAMERAS = 3,
+    PLB_REFINER_RELPOSE_PAIR = 4,
+    PLB_REFINER_FUNDAMENTAL = 5,
+    PLB_REFINER_HOMOGRAPHY = 6
+};
+typedef struct plb_refine_problem {
+    int32_t refiner;          /* PLB_REFINER_* */
+    int32_t reserved;
+    uint64_t n;
+    const double *a;          /* x (2n doubles) or x1 (2n) */
+    const double *b;          /* X (3n doubles) or x2 (2n) */
+    const double *weights;    /* n per-residual weights, or NULL (uniform) */
+    plb_camera camera1;       /* in; the refined parameters written back as the single call writes them */
+    plb_camera camera2;
+    plb_bundle_opt bundle;
+    double model[9];          /* in/out: pose (7) or matrix (9, column-major) */
+    double bundle_stats[3];   /* out: iterations, initial_cost, cost */
+    int32_t status;           /* out */
+    int32_t reserved2;
+} plb_refine_problem;
+/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device);
+ * streams_per_gpu groups of problems are in flight on each device. */
+int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
+/* plb_refine_batch(problems, count, -1, streams) with a, b and weights in device memory, as plb_estimate_batch_device
+ * takes them: device (or managed) memory of the calling thread's device, contiguous arrays of `dtype` aligned to it
+ * (PLB_DTYPE_F32: `const float *` cast into the `const double *` fields).  They are only read, after the work queued on
+ * `stream` ahead of the call has finished; fp32 values are widened exactly, so a float call gives the results of the
+ * double call on the widened values.  Models, stats and cameras come back in the host array.  An unknown dtype ->
+ * PLB_ERR_ARG; a / b / weights of a problem with n > 0 that are not device memory of the current device, or misaligned
+ * for the dtype -> PLB_ERR_ARG, with every status set and nothing else written. */
+int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams);
+
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers
  * that run several estimations on the same matches).  kind: PLB_KIND_*; returns a handle > 0 or an error < 0. */
 int plb_resident_create(int kind, const double *a, const double *b, size_t n);

@@ -473,5 +473,71 @@ std::vector<RansacStats> estimate_relative_pose_batch(const std::vector<std::vec
     }
     return out;
 }
+// Many refine_relpose(x1, x2, CameraPose*, opt, weights) (robust/bundle.h:84-86) in one call (plb_refine_batch): element
+// i refines (*poses)[i] on x1[i], x2[i] with weights[i], and returns what the single call returns, bit for bit.
+// weights[i] is used when it has one weight per point; a missing or wrongly sized entry means uniform weights.
+template <typename BundleStats, typename P2, typename Pose, typename BOpt>
+std::vector<BundleStats> refine_relpose_batch(const std::vector<std::vector<P2>> &x1, const std::vector<std::vector<P2>> &x2,
+                                              std::vector<Pose> *poses, const BOpt &opt,
+                                              const std::vector<std::vector<double>> &weights = {}, int n_gpus = 0,
+                                              int streams = 8) {
+    const size_t count = x1.size();
+    if (x2.size() != count || poses->size() != count)
+        throw std::invalid_argument("poselib_b200::refine_relpose_batch: x1, x2 and poses differ in size");
+    std::vector<plb_refine_problem> P(count);
+    for (size_t i = 0; i < count; ++i) {
+        plb_refine_problem &q = P[i];
+        q = plb_refine_problem();
+        q.refiner = PLB_REFINER_RELPOSE;
+        q.n = x1[i].size();
+        q.a = detail::raw(x1[i]);
+        q.b = detail::raw(x2[i]);
+        q.weights = i < weights.size() ? detail::weights_of(weights[i], x1[i].size()) : nullptr;
+        q.camera1.model_id = q.camera2.model_id = PLB_CAMERA_NULL;
+        q.bundle = detail::bundle_to_c(opt);
+        detail::pose_to((*poses)[i], q.model);
+    }
+    detail::check(plb_refine_batch(P.data(), count, n_gpus, streams));
+    std::vector<BundleStats> out(count);
+    for (size_t i = 0; i < count; ++i) {
+        detail::pose_from(P[i].model, &(*poses)[i]);
+        out[i] = detail::bundle_from_c<BundleStats>(P[i].bundle_stats);
+    }
+    return out;
+}
+// Many bundle_adjust(x, X, Image*, opt, weights) (robust/bundle.h:47) in one call (plb_refine_batch): element i refines
+// the pose and the selected camera parameters of (*images)[i], as the single call does, bit for bit.  Weights as in
+// refine_relpose_batch.
+template <typename BundleStats, typename P2, typename P3, typename Image, typename BOpt>
+std::vector<BundleStats> bundle_adjust_image_batch(const std::vector<std::vector<P2>> &x, const std::vector<std::vector<P3>> &X,
+                                                   std::vector<Image> *images, const BOpt &opt,
+                                                   const std::vector<std::vector<double>> &weights = {}, int n_gpus = 0,
+                                                   int streams = 8) {
+    const size_t count = x.size();
+    if (X.size() != count || images->size() != count)
+        throw std::invalid_argument("poselib_b200::bundle_adjust_image_batch: x, X and images differ in size");
+    std::vector<plb_refine_problem> P(count);
+    for (size_t i = 0; i < count; ++i) {
+        plb_refine_problem &q = P[i];
+        q = plb_refine_problem();
+        q.refiner = PLB_REFINER_BUNDLE_IMAGE;
+        q.n = x[i].size();
+        q.a = detail::raw(x[i]);
+        q.b = detail::raw(X[i]);
+        q.weights = i < weights.size() ? detail::weights_of(weights[i], x[i].size()) : nullptr;
+        q.camera1 = detail::camera_to_c((*images)[i].camera);
+        q.camera2.model_id = PLB_CAMERA_NULL;
+        q.bundle = detail::bundle_to_c(opt);
+        detail::pose_to((*images)[i].pose, q.model);
+    }
+    detail::check(plb_refine_batch(P.data(), count, n_gpus, streams));
+    std::vector<BundleStats> out(count);
+    for (size_t i = 0; i < count; ++i) {
+        detail::pose_from(P[i].model, &(*images)[i].pose);
+        detail::camera_from_c(P[i].camera1, &(*images)[i].camera);
+        out[i] = detail::bundle_from_c<BundleStats>(P[i].bundle_stats);
+    }
+    return out;
+}
 
 } // namespace poselib_b200

@@ -104,7 +104,7 @@ EXPORTS = [
     "plb_bundle_adjust_image", "plb_estimate_absolute_pose_image", "plb_refine_relpose", "plb_refine_relpose_cameras", "plb_refine_relpose_pair", "plb_refine_fundamental", "plb_refine_homography", "plb_resident_create",
     "plb_resident_free", "plb_bundle_adjust_image_weighted", "plb_refine_relpose_weighted",
     "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
-    "plb_refine_homography_weighted", "plb_estimate_batch_device",
+    "plb_refine_homography_weighted", "plb_estimate_batch_device", "plb_refine_batch", "plb_refine_batch_device",
 ]
 DTYPE_F64, DTYPE_F32 = 0, 1
 
@@ -114,6 +114,18 @@ class EstimateProblem(C.Structure):
                 ("camera1", Camera), ("camera2", Camera), ("ransac", RansacOpt), ("bundle", BundleOpt),
                 ("max_error", C.c_double), ("model", C.c_double * 9), ("inliers", C.c_char_p),
                 ("stats", RansacStats), ("counters", Counters), ("status", C.c_int32), ("reserved2", C.c_int32)]
+
+
+# plb_refine_problem::refiner: the robust/bundle.h refiner of each single entry point
+REFINER = {"bundle": 0, "bundle_image": 1, "relpose": 2, "relpose_cameras": 3, "relpose_pair": 4, "fundamental": 5,
+           "homography": 6}
+
+
+class RefineProblem(C.Structure):
+    _fields_ = [("refiner", C.c_int32), ("reserved", C.c_int32), ("n", C.c_uint64), ("a", C.POINTER(C.c_double)),
+                ("b", C.POINTER(C.c_double)), ("weights", C.POINTER(C.c_double)), ("camera1", Camera),
+                ("camera2", Camera), ("bundle", BundleOpt), ("model", C.c_double * 9), ("bundle_stats", C.c_double * 3),
+                ("status", C.c_int32), ("reserved2", C.c_int32)]
 
 
 if not os.path.exists(LIB_PATH):
@@ -644,3 +656,99 @@ def estimate_batch_device(problems, streams=8, stream=None):
     _check(_lib.plb_estimate_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
                                           int(streams)))
     return _estimate_results(arr, problems, masks)
+
+
+# ---- batch of refiner problems (plb_refine_batch) ------------------------------------------------------------
+def _refine_kind(refiner):
+    """The model layout of a refiner: a pose, or a 3x3 matrix for "fundamental" / "homography"."""
+    return refiner if refiner in ("fundamental", "homography") else "pnp"
+
+
+def _fill_refine_problem(q, p, npts):
+    """Everything of one plb_refine_problem but its point and weight pointers."""
+    q.refiner = REFINER[p["refiner"]]
+    q.n = npts
+    q.camera1 = p.get("cam1") or Camera("NULL", ())
+    q.camera2 = p.get("cam2") or Camera("NULL", ())
+    q.bundle = p["bundle"]
+    m = _init_model(_refine_kind(p["refiner"]), p.get("model"))
+    for k in range(len(m)):
+        q.model[k] = m[k]
+
+
+def _refine_results(arr, problems):
+    out = []
+    for i, p in enumerate(problems):
+        q = arr[i]
+        kind = _refine_kind(p["refiner"])
+        m = np.array(q.model[:7] if kind == "pnp" else q.model[:9], dtype=np.float64)
+        out.append({"model": _model_out(kind, m), "bundle_stats": np.array(q.bundle_stats[:3]), "status": q.status,
+                    "camera1": _camera_params(q.camera1), "camera2": _camera_params(q.camera2)})
+    return out
+
+
+def refine_batch(problems, n_gpus=-1, streams=8):
+    """Batch form of refine / refine_image / refine_relpose_cameras / refine_relpose_pair (plb_refine_batch): each result
+    equals its single call bit for bit.  problems: list of dict(refiner [a REFINER key], a, b, bundle=BundleOpt,
+    model=None [start pose, or 3x3 matrix [r,c]], weights=None [one per point, else uniform], cam1=None, cam2=None).
+    n_gpus: -1 current device, 0 all devices, k the first k.  Returns list of dict(model, bundle_stats [iterations,
+    initial_cost, cost], camera1, camera2 [the models' parameters], status); the given cameras are not modified."""
+    count = len(problems)
+    arr = (RefineProblem * count)()
+    keep = []
+    for i, p in enumerate(problems):
+        q = arr[i]
+        aa, ap = _d(p["a"])
+        ba, bp = _d(p["b"])
+        wa, wp = _w(p.get("weights"), len(aa))
+        keep.append((aa, ba, wa))
+        _fill_refine_problem(q, p, len(aa))
+        q.a, q.b, q.weights = ap, bp, wp
+    _check(_lib.plb_refine_batch(arr, C.c_size_t(count), int(n_gpus), int(streams)))
+    return _refine_results(arr, problems)
+
+
+def refine_batch_device(problems, stream=None, streams=8):
+    """refine_batch (n_gpus=-1) on points and weights that are already on the GPU (plb_refine_batch_device).
+    problems: the dicts refine_batch takes, with a / b / weights as CUDA torch tensors ([n,2] / [n,3] / [n]), all on one
+    device and of one dtype, float32 or float64; weights with other than n elements mean uniform weights.  The call runs
+    on that device and reads the inputs after the work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle;
+    default: the device's current stream).  Returns the dicts of refine_batch."""
+    import torch
+    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
+    tensors = [t for p in problems for t in (p["a"], p["b"], p.get("weights")) if t is not None]
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
+        raise TypeError("refine_batch_device: a, b and weights must be CUDA torch tensors")
+    if not tensors:
+        return []
+    dev, dt = tensors[0].device, tensors[0].dtype
+    if any(t.device != dev for t in tensors):
+        raise ValueError(f"refine_batch_device: every tensor must be on {dev} (shard the batch by device)")
+    if dt not in dtypes or any(t.dtype != dt for t in tensors):
+        raise TypeError("refine_batch_device: a, b and weights must share one dtype, torch.float32 or torch.float64")
+    set_device(dev.index)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev)
+    elif not isinstance(stream, torch.cuda.Stream):
+        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    count = len(problems)
+    arr = (RefineProblem * count)()
+    keep = []
+    ptr = lambda t: C.cast(C.c_void_p(t.data_ptr() if t is not None else None), _P)
+    with torch.cuda.stream(stream):  # any copy .contiguous() makes is ordered before the call's reads
+        for i, p in enumerate(problems):
+            q = arr[i]
+            a, b = p["a"].contiguous(), p["b"].contiguous()
+            npts = a.shape[0]
+            b_dim = 3 if p["refiner"] in ("bundle", "bundle_image") else 2
+            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
+                raise ValueError(f"refine_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
+                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
+            w = p.get("weights")
+            w = w.contiguous().reshape(-1) if w is not None and w.numel() == npts else None
+            keep.append((a, b, w))
+            _fill_refine_problem(q, p, npts)
+            q.a, q.b, q.weights = ptr(a), ptr(b), ptr(w)
+    _check(_lib.plb_refine_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+                                        int(streams)))
+    return _refine_results(arr, problems)

@@ -32,6 +32,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <vector>
 
 namespace plb {
@@ -232,12 +233,11 @@ struct Engine {
     PinBuf<NormDesc> h_ndesc;
     MapBuf<double> h_norm;
     DevBuf<MaskDesc> mdesc;
-    DevBuf<IngestDesc> idesc; // device-resident inputs and masks (plb_estimate_batch_device)
+    DevBuf<IngestDesc> idesc; // device-resident inputs (plb_estimate_batch_device, plb_refine_batch_device)
     PinBuf<IngestDesc> h_idesc;
     DevBuf<ScatterDesc> sdesc;
     PinBuf<ScatterDesc> h_sdesc;
     DevBuf<LmJob> jobs;
-    DevBuf<double> wts; // per-residual weights of a refiner call (LmJob::w)
     PinBuf<double> h_in, h_lm_in;
     PinBuf<int> h_slots, h_act, h_work;
     PinBuf<ProblemDev> h_probs;
@@ -565,10 +565,18 @@ struct Task {
     int pre_mode = 0;
     double pre_scale = 1.0;
     CamDev cam_a{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}}, cam_b{CAMM_NULL, 0, {0, 0, 0, 0, 0, 0, 0, 0}};
-    // plb_estimate_batch_device: a, b (float when f32) and inliers are device memory of the group's device, read and
-    // written only after `ready` (recorded in the caller's stream) has completed
+    // plb_estimate_batch_device / plb_refine_batch_device: a, b, weights (float when f32) and inliers are device memory
+    // of the group's device, read and written only after `ready` (recorded in the caller's stream) has completed
     bool dev_io = false, f32 = false;
     cudaEvent_t ready = nullptr;
+    // A robust/bundle.h refiner call instead of LO-RANSAC (run_refine_group): one LM job over all n points with
+    // polish.bundle, polish.cam_refine and the cameras polish.cam; the refined model goes to `model`, {iterations,
+    // initial_cost, cost} to bstats (or nowhere), the refined parameters of camera i to polish.cam_out[i].
+    bool refine = false;
+    const void *weights = nullptr; // refine: n per-residual weights in point order (float when f32), or null: uniform
+    double *bstats = nullptr;
+    // doubles per correspondence the group uploads: the caller layout, then the weight
+    size_t in_per_point(int in_arr) const { return (size_t)in_arr + (weights ? 1 : 0); }
 };
 
 // per-problem serial state of the reference loop (ransac_impl.h:99-104,157-201)
@@ -746,13 +754,14 @@ struct Group {
         for (PState &S : PS) {
             if (S.n == 0) continue;
             if (!S.t->res) {
+                const size_t vals = S.t->in_per_point(in_arr) * S.n;
                 if (S.t->dev_io) {
                     ++n_ingest;
-                    max_ingest = std::max(max_ingest, (size_t)in_arr * S.n);
+                    max_ingest = std::max(max_ingest, vals);
                 } else {
-                    host_doubles += (size_t)in_arr * S.n;
+                    host_doubles += vals;
                 }
-                in_doubles += (size_t)in_arr * S.n;
+                in_doubles += vals;
                 soa_elems += (size_t)n_arr * S.n_pad;
                 if (kind == KIND_RELPOSE || kind == KIND_FUND) q_rows += (size_t)S.n_pad;
                 ++n_up;
@@ -808,25 +817,29 @@ struct Group {
                 assert(!S.t->polish.evaluates_camera()); // plb_resident_create takes no camera
             } else {
                 S.in_off = (long long)in_off;
+                const size_t nw = S.t->weights ? (size_t)S.n : 0; // the weights follow b
                 if (S.t->dev_io) { // gathered on the device by k_ingest (below): nothing crosses PCIe
                     IngestDesc &I = E.h_idesc.p[ii++];
                     I.a = S.t->a;
                     I.b = S.t->b;
+                    I.w = S.t->weights;
                     I.dst = E.in.p + in_off;
                     I.n = S.n;
                     I.b_dim = b_dim;
                     I.f32 = S.t->f32 ? 1 : 0;
                     ready = S.t->ready;
-                } else if (host_pinned(S.t->a) && host_pinned(S.t->b)) {
+                } else if (host_pinned(S.t->a) && host_pinned(S.t->b) && (!nw || host_pinned(S.t->weights))) {
                     // the caller's arrays are page-locked: DMA straight from them, no staging copy on the host
                     direct.push_back({E.in.p + in_off, S.t->a, sizeof(double) * 2 * S.n});
                     direct.push_back({E.in.p + in_off + 2 * (size_t)S.n, S.t->b, sizeof(double) * (size_t)b_dim * S.n});
-                    h2d += sizeof(double) * (size_t)in_arr * S.n;
+                    if (nw) direct.push_back({E.in.p + in_off + (size_t)in_arr * S.n, (const double *)S.t->weights, sizeof(double) * nw});
+                    h2d += sizeof(double) * ((size_t)in_arr * S.n + nw);
                 } else {
-                    staged.emplace_back(in_off, (size_t)in_arr * S.n);
+                    staged.emplace_back(in_off, (size_t)in_arr * S.n + nw);
                     double *ha = E.h_in.p + in_off, *hb = ha + 2 * (size_t)S.n;
                     std::memcpy(ha, S.t->a, sizeof(double) * 2 * S.n);
                     std::memcpy(hb, S.t->b, sizeof(double) * (size_t)b_dim * S.n);
+                    if (nw) std::memcpy(hb + (size_t)b_dim * S.n, S.t->weights, sizeof(double) * nw);
                 }
                 TransposeDesc &D = E.h_tdesc.p[iu++];
                 D.a = E.in.p + in_off;
@@ -866,7 +879,7 @@ struct Group {
                     for (int c = 0; c < nc; ++c) PP.cam[c] = fp.cam[c];
                     px_off += 2 * (size_t)nc * S.n_pad;
                 }
-                in_off += (size_t)in_arr * S.n;
+                in_off += (size_t)in_arr * S.n + nw;
                 soa_off += (size_t)n_arr * S.n_pad;
             }
         }
@@ -945,11 +958,18 @@ struct Group {
         PLB_CUDA(cudaMemcpyAsync(E.probs.p, E.h_probs.p, sizeof(ProblemDev) * n_probdev, cudaMemcpyHostToDevice, st));
         if (n_up) {
             PLB_CUDA(cudaMemsetAsync(E.cmax.p, 0, sizeof(float) * 5 * (size_t)NP, st));
+            // Problems with a fisheye or division camera go to the layout kernel's instantiation that evaluates them, the
+            // others to the one without: each problem is laid out by the instantiation its lone call uses.
+            auto xcam = [](const TransposeDesc &D) { return cam_is_x(D.cam_a.model) || cam_is_x(D.cam_b.model); };
+            const int n_plain = (int)(std::stable_partition(E.h_tdesc.p, E.h_tdesc.p + n_up, [&](const TransposeDesc &D) { return !xcam(D); }) -
+                                      E.h_tdesc.p);
             PLB_CUDA(cudaMemcpyAsync(E.tdesc.p, E.h_tdesc.p, sizeof(TransposeDesc) * n_up, cudaMemcpyHostToDevice, st));
-            bool xcam = false;
-            for (int i = 0; i < n_up; ++i) xcam = xcam || cam_is_x(E.h_tdesc.p[i].cam_a.model) || cam_is_x(E.h_tdesc.p[i].cam_b.model);
-            launch_transpose(E.tdesc.p, n_up, max_n_pad, xcam, st);
-            E.launches++;
+            for (int x = 0; x < 2; ++x) {
+                const int d0 = x ? n_plain : 0, nd = x ? n_up - n_plain : n_plain;
+                if (nd == 0) continue;
+                launch_transpose(E.tdesc.p + d0, nd, max_n_pad, x == 1, st);
+                E.launches++;
+            }
             if (kind == KIND_RELPOSE || kind == KIND_FUND) {
                 launch_qrows(E.tdesc.p, n_up, max_n_pad, st);
                 E.launches++;
@@ -973,27 +993,36 @@ struct Group {
             if (cam_is_x(E.h_probs.p[J.pidx].cam[i].model)) return true;
         return false;
     }
-    int lm_batch(const std::vector<LmTask> &batch) {
+    // Stages the jobs and their start models and sizes the result rows.  scratch: the jobs select their points
+    // (subset modes 1, 2) and need a max_n_pad slice of E.subset each.
+    int lm_stage(const std::vector<LmTask> &batch, bool scratch) {
         const int nj = (int)batch.size(), nc = kind_cam_count(kind);
-        const int n_fixed = (int)(std::partition_point(batch.begin(), batch.end(),
-                                                       [&](const LmTask &t) { return !refines_camera(t.job); }) -
-                                  batch.begin());
+        const bool any_cam = std::any_of(batch.begin(), batch.end(), [&](const LmTask &t) { return refines_camera(t.job); });
         int rc;
         if ((rc = E.h_lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_jobs.ensure(nj)) || (rc = E.jobs.ensure(nj)) ||
             (rc = E.lm_in.ensure(9 * (size_t)nj)) || (rc = E.h_lm_out.ensure(nj)) ||
-            (rc = E.subset.ensure((size_t)nj * max_n_pad)) ||
-            (n_fixed < nj && (rc = E.h_cam_out.ensure((size_t)nj * nc * CAM_MAX_PARAMS))))
+            (scratch && (rc = E.subset.ensure((size_t)nj * max_n_pad))) ||
+            (any_cam && (rc = E.h_cam_out.ensure((size_t)nj * nc * CAM_MAX_PARAMS))))
             return rc;
         for (int j = 0; j < nj; ++j) {
             double *row = E.h_lm_in.p + 9 * (size_t)j;
             std::fill(row, row + 9, 0.0);
             std::copy(batch[j].model, batch[j].model + MSZ, row);
             E.h_jobs.p[j] = batch[j].job;
-            E.h_jobs.p[j].scratch_off = (long long)j * max_n_pad;
+            E.h_jobs.p[j].scratch_off = scratch ? (long long)j * max_n_pad : 0;
         }
         PLB_CUDA(cudaMemcpyAsync(E.jobs.p, E.h_jobs.p, sizeof(LmJob) * nj, cudaMemcpyHostToDevice, st));
         PLB_CUDA(cudaMemcpyAsync(E.lm_in.p, E.h_lm_in.p, sizeof(double) * 9 * nj, cudaMemcpyHostToDevice, st));
         h2d += (sizeof(LmJob) + sizeof(double) * 9) * nj;
+        return PLB_OK;
+    }
+    int lm_batch(const std::vector<LmTask> &batch) {
+        const int nj = (int)batch.size(), nc = kind_cam_count(kind);
+        const int n_fixed = (int)(std::partition_point(batch.begin(), batch.end(),
+                                                       [&](const LmTask &t) { return !refines_camera(t.job); }) -
+                                  batch.begin());
+        int rc;
+        if ((rc = lm_stage(batch, true))) return rc;
         for (int cam = 0; cam < 2; ++cam) {
             const int j0 = cam ? n_fixed : 0, n = cam ? nj - n_fixed : n_fixed;
             if (n == 0) continue;
@@ -1007,6 +1036,68 @@ struct Group {
             E.launches++;
         }
         d2h += sizeof(LmJobOut) * nj + sizeof(double) * nc * CAM_MAX_PARAMS * (nj - n_fixed);
+        return PLB_OK;
+    }
+    // ---- the robust/bundle.h refiners (bundle.cc:84-112,206-222,237-256,313-333,394-411): one LM job per problem over
+    // all its points.  A job's bits depend on the k_lm instantiation and on the cluster width, which fixes the order of
+    // its reductions, and on nothing else in the launch.  So every job runs at the width a lone call of its size takes
+    // (lm_lone_width), in one launch per class of (camera refinement, fisheye / division camera, weights, width): each
+    // problem gets the bits of its single call whatever else is in the batch.
+    // No points is not special: the job runs with empty slices and reports what lm_impl reports for an empty problem
+    // (iterations 0, costs 0; the fundamental refiner returns the matrix its factorisation reconstructs).
+    int refine() {
+        const int nc = kind_cam_count(kind);
+        struct Item {
+            int i, cam, xcam, w, width;
+            LmJob job;
+            bool operator<(const Item &o) const {
+                return std::tie(cam, xcam, w, width) < std::tie(o.cam, o.xcam, o.w, o.width);
+            }
+        };
+        std::vector<Item> items(NP);
+        for (int i = 0; i < NP; ++i) {
+            const PState &S = PS[i];
+            LmParams prm = bundle_params(S.t->polish.bundle);
+            prm.subset_mode = 0;
+            LmJob J = lm_job(S.polish_pidx >= 0 ? S.polish_pidx : i, -1, prm);
+            J.cam_refine = S.t->polish.cam_refine;
+            // the weights follow the problem's points in E.in (upload)
+            if (S.t->weights && S.n > 0) J.w = E.in.p + S.in_off + (size_t)in_arr * S.n;
+            items[i] = {i, refines_camera(J), uses_x_camera(J), J.w != nullptr, lm_lone_width(S.n), J};
+        }
+        std::stable_sort(items.begin(), items.end());
+        std::vector<LmTask> batch(NP);
+        for (int j = 0; j < NP; ++j) batch[j] = {PS[items[j].i].t->model, items[j].job};
+        int rc;
+        if ((rc = lm_stage(batch, false))) return rc;
+        for (int j0 = 0, j1; j0 < NP; j0 = j1) { // one launch per class: a run of equal keys of the sorted items
+            j1 = j0 + 1;
+            while (j1 < NP && !(items[j0] < items[j1])) ++j1;
+            const Item &c = items[j0];
+            launch_lm_width(kind, c.cam, c.xcam, c.w, E.probs.p, E.jobs.p + j0, E.lm_in.p + 9 * (size_t)j0, j1 - j0,
+                            c.width, E.h_lm_out.d + j0, c.cam ? E.h_cam_out.d + (size_t)j0 * nc * CAM_MAX_PARAMS : nullptr,
+                            st);
+            E.launches++;
+        }
+        if ((rc = sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        for (int j = 0; j < NP; ++j) {
+            Task &t = *PS[items[j].i].t;
+            const LmJobOut &o = E.h_lm_out.p[j];
+            std::copy(o.model, o.model + MSZ, t.model);
+            if (items[j].cam) // only the parameters the flags select
+                for (int i = 0; i < nc; ++i) {
+                    int idx[CAM_MAX_PARAMS];
+                    const int m = cam_refine_idx(t.polish.cam[i].model, t.polish.cam_refine, idx);
+                    for (int c = 0; c < m; ++c)
+                        t.polish.cam_out[i]->params[idx[c]] = E.h_cam_out.p[((size_t)j * nc + i) * CAM_MAX_PARAMS + idx[c]];
+                }
+            if (t.bstats) {
+                t.bstats[0] = o.iterations;
+                t.bstats[1] = o.initial_cost;
+                t.bstats[2] = o.cost;
+            }
+        }
         return PLB_OK;
     }
     LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
@@ -1611,62 +1702,12 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
     return run_group(kind, v);
 }
 
-// One LM refinement over all n points (robust/bundle.cc:84-112,206-222,313-333,394-411): the upload of a one-problem
-// group (sq_thr 0, no normalisation, no pre-step beyond the tangent-Sampson one), then one LM job over every point.
-// cams (or null): the kind_cam_count(kind) cameras of the points, in their units (scale 1); the parameters the flags
-// cam_refine select are refined with the pose and written to params_out[i].
-// PnP on an Image (bundle.cc:95-112): the points are projected with cams[0].
-// Tangent Sampson on an ImagePair (bundle.cc:237-256): cams[0] / cams[1] unproject the points; without a selection it is
-// the fixed-camera refiner.
-// No points is not special: the job runs with empty slices and reports what lm_impl reports for an empty problem
-// (iterations 0, costs 0; the fundamental refiner returns the matrix its factorisation reconstructs).
-// weights (or null: uniform): n_pts doubles, one per correspondence, in the caller's point order, which the layout keeps
-// for every kind; they go up with the points and the job runs k_lm's weighted instantiation.
-static int run_refine(int kind, const double *a, const double *b, size_t n_pts, double *model,
-                      const plb_bundle_opt &bopt, double *bstats, const CamDev *cams = nullptr, int cam_refine = 0,
-                      double *const *params_out = nullptr, const double *weights = nullptr) {
-    Task t;
-    t.kind = kind;
-    t.a = a;
-    t.b = b;
-    t.n = n_pts;
-    const int nc = kind_cam_count(kind);
-    if (kind == KIND_RELPOSE_TS) { // the cameras of the pre-step
-        t.cam_a = cams[0];
-        t.cam_b = cams[1];
-    }
-    // the bundle evaluates the cameras: PnP always, tangent Sampson only to refine them (else ts carries them)
-    if (cams && (kind == KIND_PNP || refines_camera(cams[0], cam_refine) || refines_camera(cams[1], cam_refine)))
-        std::copy(cams, cams + nc, t.polish.cam);
-    std::vector<Task *> v{&t};
-    Group G(kind, v);
+// Runs a group of refiner tasks of the same kind (Task::refine): the upload of the group (sq_thr 0, no normalisation,
+// no pre-step beyond the tangent-Sampson one), then one LM job per problem (Group::refine).
+static int run_refine_group(int kind, std::vector<Task *> &tasks) {
+    Group G(kind, tasks);
     int rc;
-    if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose())) return rc;
-    LmParams prm = bundle_params(bopt);
-    prm.subset_mode = 0;
-    lm_set_sm_share(100);
-    LmJob J = lm_job(G.PS[0].polish_pidx >= 0 ? G.PS[0].polish_pidx : 0, -1, prm);
-    J.cam_refine = cam_refine;
-    if (weights && n_pts > 0) {
-        if ((rc = G.E.wts.ensure(n_pts))) return rc;
-        PLB_CUDA(cudaMemcpyAsync(G.E.wts.p, weights, sizeof(double) * n_pts, cudaMemcpyHostToDevice, G.st));
-        J.w = G.E.wts.p;
-    }
-    if ((rc = G.lm_batch({{model, J}})) || (rc = G.sync())) return rc;
-    PLB_CUDA(cudaGetLastError());
-    const LmJobOut &o = G.E.h_lm_out.p[0];
-    std::copy(o.model, o.model + G.MSZ, model);
-    if (G.refines_camera(J))
-        for (int i = 0; i < nc; ++i) {
-            int idx[CAM_MAX_PARAMS];
-            const int m = cam_refine_idx(cams[i].model, cam_refine, idx);
-            for (int c = 0; c < m; ++c) params_out[i][idx[c]] = G.E.h_cam_out.p[i * CAM_MAX_PARAMS + idx[c]];
-        }
-    if (bstats) {
-        bstats[0] = o.iterations;
-        bstats[1] = o.initial_cost;
-        bstats[2] = o.cost;
-    }
+    if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose()) || (rc = G.refine())) return rc;
     return PLB_OK;
 }
 
@@ -2087,113 +2128,129 @@ int plb_estimate_homography(const double *x1, const double *x2, size_t n, const 
 // ---- robust/bundle.h refiners -------------------------------------------------------------------------------
 // Every refiner has a _weighted twin that takes PoseLib's per-residual weights (n doubles, null: uniform); the
 // unweighted entry point is the twin with null weights.  The weights are not checked, as in the reference: zero and
-// negative values enter the sums as they are.
-static int refine_entry(int kind, const double *a, const double *b, size_t n, double *model, const plb_bundle_opt *opt,
-                        double *bs, const double *weights = nullptr) {
-    if (!opt || !model || (n > 0 && (!a || !b))) {
+// negative values enter the sums as they are.  Each entry point is the one-problem case of plb_refine_batch.
+// One refiner call, checked and turned into the Task of run_refine_group, by the rules of the single entry points:
+// null options, model or camera (where the refiner takes one), or null points with n > 0 -> PLB_ERR_ARG; a camera
+// outside the ten models -> PLB_ERR_NYI; PLB_REFINER_RELPOSE_CAMERAS with a non-empty refine_intrinsics selection ->
+// PLB_ERR_NYI, as it cannot return the cameras.  cam1 / cam2 are read; out1 / out2 (the Image* / ImagePair* forms)
+// receive the refined parameters, and only those.  Nothing is written here.
+//   PLB_REFINER_BUNDLE: bundle.cc:84-92, the calibrated AbsolutePoseRefiner; the reference drops the weights.
+//   PLB_REFINER_BUNDLE_IMAGE: bundle.cc:95-112, camera_refine_idx from the flags, points in the camera's pixel units.
+//   PLB_REFINER_RELPOSE: bundle.cc:206-222.  PLB_REFINER_FUNDAMENTAL: :313-333.  PLB_REFINER_HOMOGRAPHY: :394-411.
+//   PLB_REFINER_RELPOSE_CAMERAS: bundle.cc:237-247 with fixed intrinsics, the tangent-Sampson refiner on the
+//   unproject_with_jac of both images (the layout kernel's pre-step).
+//   PLB_REFINER_RELPOSE_PAIR: bundle.cc:237-256, CameraRelativePoseRefiner with the parameters the flags select in
+//   either camera (shared_camera false), pixels as given; without a selection it is PLB_REFINER_RELPOSE_CAMERAS.
+static int refine_prepare(int refiner, const double *a, const double *b, size_t n, const double *weights,
+                          const plb_camera *cam1, const plb_camera *cam2, plb_camera *out1, plb_camera *out2,
+                          const plb_bundle_opt *opt, double *model, double *bstats, Task &t) {
+    if (refiner < PLB_REFINER_BUNDLE || refiner > PLB_REFINER_HOMOGRAPHY) {
+        g_err = "unknown refiner";
+        return PLB_ERR_ARG;
+    }
+    const bool image = refiner == PLB_REFINER_BUNDLE_IMAGE, pair = refiner == PLB_REFINER_RELPOSE_PAIR;
+    if (!opt || !model || (image && !out1) || (pair && (!out1 || !out2)) || (n > 0 && (!a || !b))) {
         g_err = "null argument";
         return PLB_ERR_ARG;
     }
-    return run_refine(kind, a, b, n, model, *opt, bs, nullptr, 0, nullptr, weights);
-}
-int plb_bundle_adjust(const double *x, const double *X, size_t n, double pose[7], const plb_bundle_opt *opt,
-                      double bs[3]) {
-    return refine_entry(KIND_PNP, x, X, n, pose, opt, bs);
-}
-int plb_refine_relpose(const double *x1, const double *x2, size_t n, double pose[7], const plb_bundle_opt *opt,
-                       double bs[3]) {
-    return refine_entry(KIND_RELPOSE, x1, x2, n, pose, opt, bs);
-}
-int plb_refine_relpose_weighted(const double *x1, const double *x2, size_t n, double pose[7], const plb_bundle_opt *opt,
-                                double bs[3], const double *weights) {
-    return refine_entry(KIND_RELPOSE, x1, x2, n, pose, opt, bs, weights);
-}
-// robust/bundle.cc:237-266 with fixed intrinsics: unproject_with_jac of both images, then the tangent-Sampson refiner
-static int refine_relpose_cameras(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
-                                  const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt, double bs[3],
-                                  const double *weights) {
-    if (!opt || !pose || (n > 0 && (!x1 || !x2))) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    CamDev cams[2];
-    if (int r = camera_dev(camera1, &cams[0])) return r;
-    if (int r = camera_dev(camera2, &cams[1])) return r;
-    if (refines_camera(cams[0], refine_flags(opt)) || refines_camera(cams[1], refine_flags(opt))) {
+    static const int kinds[] = {KIND_PNP, KIND_PNP, KIND_RELPOSE, KIND_RELPOSE_TS, KIND_RELPOSE_TS, KIND_FUND, KIND_HOMOG};
+    t.kind = kinds[refiner];
+    t.refine = true;
+    t.a = a;
+    t.b = b;
+    t.n = n;
+    t.weights = refiner == PLB_REFINER_BUNDLE ? nullptr : weights;
+    t.model = model;
+    t.bstats = bstats;
+    FinalPolish &fp = t.polish;
+    fp.bundle = *opt;
+    const int nc = image ? 1 : t.kind == KIND_RELPOSE_TS ? 2 : 0;
+    const plb_camera *in[2] = {cam1, cam2};
+    CamDev cams[2] = {fp.cam[0], fp.cam[1]};
+    for (int i = 0; i < nc; ++i)
+        if (int r = camera_dev(in[i], &cams[i])) return r;
+    if (!nc) return PLB_OK;
+    const int flags = (image || pair) ? refine_flags(opt) : 0;
+    const bool refined = refines_camera(cams[0], refine_flags(opt)) || refines_camera(cams[1], refine_flags(opt));
+    if (refiner == PLB_REFINER_RELPOSE_CAMERAS && refined) {
         g_err = "NYI: camera refinement needs cameras to return: use plb_refine_relpose_pair";
         return PLB_ERR_NYI;
     }
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, 0, nullptr, weights);
+    if (t.kind == KIND_RELPOSE_TS) { // the cameras of the pre-step
+        t.cam_a = cams[0];
+        t.cam_b = cams[1];
+    }
+    // the bundle evaluates the cameras: PnP always, tangent Sampson only to refine them (else ts carries them)
+    if (image || refined) std::copy(cams, cams + nc, fp.cam);
+    fp.cam_refine = flags;
+    fp.cam_out[0] = out1;
+    fp.cam_out[1] = out2;
+    return PLB_OK;
+}
+static int refine_single(int refiner, const double *a, const double *b, size_t n, const double *weights,
+                         const plb_camera *cam1, const plb_camera *cam2, plb_camera *out1, plb_camera *out2,
+                         const plb_bundle_opt *opt, double *model, double *bstats) {
+    Task t;
+    if (int r = refine_prepare(refiner, a, b, n, weights, cam1, cam2, out1, out2, opt, model, bstats, t)) return r;
+    std::vector<Task *> v{&t};
+    return run_refine_group(t.kind, v);
+}
+int plb_bundle_adjust(const double *x, const double *X, size_t n, double pose[7], const plb_bundle_opt *opt,
+                      double bs[3]) {
+    return refine_single(PLB_REFINER_BUNDLE, x, X, n, nullptr, nullptr, nullptr, nullptr, nullptr, opt, pose, bs);
+}
+int plb_refine_relpose(const double *x1, const double *x2, size_t n, double pose[7], const plb_bundle_opt *opt,
+                       double bs[3]) {
+    return plb_refine_relpose_weighted(x1, x2, n, pose, opt, bs, nullptr);
+}
+int plb_refine_relpose_weighted(const double *x1, const double *x2, size_t n, double pose[7], const plb_bundle_opt *opt,
+                                double bs[3], const double *weights) {
+    return refine_single(PLB_REFINER_RELPOSE, x1, x2, n, weights, nullptr, nullptr, nullptr, nullptr, opt, pose, bs);
 }
 int plb_refine_relpose_cameras(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                                const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
-    return refine_relpose_cameras(x1, x2, n, camera1, camera2, pose, opt, bs, nullptr);
+    return plb_refine_relpose_cameras_weighted(x1, x2, n, camera1, camera2, pose, opt, bs, nullptr);
 }
 int plb_refine_relpose_cameras_weighted(const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                                         const plb_camera *camera2, double pose[7], const plb_bundle_opt *opt,
                                         double bs[3], const double *weights) {
-    return refine_relpose_cameras(x1, x2, n, camera1, camera2, pose, opt, bs, weights);
-}
-// robust/bundle.cc:95-112: AbsolutePoseRefiner on an Image, camera_refine_idx from the flags; points in camera units
-static int bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
-                               const plb_bundle_opt *opt, double bs[3], const double *weights) {
-    if (!opt || !pose || !camera_inout || (n > 0 && (!x || !X))) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    CamDev cam;
-    if (int r = camera_dev(camera_inout, &cam)) return r;
-    double *out[1] = {camera_inout->params};
-    return run_refine(KIND_PNP, x, X, n, pose, *opt, bs, &cam, refine_flags(opt), out, weights);
+    return refine_single(PLB_REFINER_RELPOSE_CAMERAS, x1, x2, n, weights, camera1, camera2, nullptr, nullptr, opt, pose, bs);
 }
 int plb_bundle_adjust_image(const double *x, const double *X, size_t n, double pose[7], plb_camera *camera_inout,
                             const plb_bundle_opt *opt, double bs[3]) {
-    return bundle_adjust_image(x, X, n, pose, camera_inout, opt, bs, nullptr);
+    return plb_bundle_adjust_image_weighted(x, X, n, pose, camera_inout, opt, bs, nullptr);
 }
 int plb_bundle_adjust_image_weighted(const double *x, const double *X, size_t n, double pose[7],
                                      plb_camera *camera_inout, const plb_bundle_opt *opt, double bs[3],
                                      const double *weights) {
-    return bundle_adjust_image(x, X, n, pose, camera_inout, opt, bs, weights);
-}
-// robust/bundle.cc:237-256: refine_relpose(x1, x2, ImagePair*, opt), CameraRelativePoseRefiner with the parameters the
-// flags select in either camera (shared_camera false); pixels as given, only the refined parameters written
-static int refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
-                               plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3],
-                               const double *weights) {
-    if (!opt || !pose || !camera1_inout || !camera2_inout || (n > 0 && (!x1 || !x2))) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    CamDev cams[2];
-    if (int r = camera_dev(camera1_inout, &cams[0])) return r;
-    if (int r = camera_dev(camera2_inout, &cams[1])) return r;
-    double *out[2] = {camera1_inout->params, camera2_inout->params};
-    return run_refine(KIND_RELPOSE_TS, x1, x2, n, pose, *opt, bs, cams, refine_flags(opt), out, weights);
+    return refine_single(PLB_REFINER_BUNDLE_IMAGE, x, X, n, weights, camera_inout, nullptr, camera_inout, nullptr, opt,
+                         pose, bs);
 }
 int plb_refine_relpose_pair(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
                             plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3]) {
-    return refine_relpose_pair(x1, x2, n, camera1_inout, camera2_inout, pose, opt, bs, nullptr);
+    return plb_refine_relpose_pair_weighted(x1, x2, n, camera1_inout, camera2_inout, pose, opt, bs, nullptr);
 }
 int plb_refine_relpose_pair_weighted(const double *x1, const double *x2, size_t n, plb_camera *camera1_inout,
                                      plb_camera *camera2_inout, double pose[7], const plb_bundle_opt *opt, double bs[3],
                                      const double *weights) {
-    return refine_relpose_pair(x1, x2, n, camera1_inout, camera2_inout, pose, opt, bs, weights);
+    return refine_single(PLB_REFINER_RELPOSE_PAIR, x1, x2, n, weights, camera1_inout, camera2_inout, camera1_inout,
+                         camera2_inout, opt, pose, bs);
 }
 int plb_refine_fundamental(const double *x1, const double *x2, size_t n, double F[9], const plb_bundle_opt *opt,
                            double bs[3]) {
-    return refine_entry(KIND_FUND, x1, x2, n, F, opt, bs);
+    return plb_refine_fundamental_weighted(x1, x2, n, F, opt, bs, nullptr);
 }
 int plb_refine_fundamental_weighted(const double *x1, const double *x2, size_t n, double F[9],
                                     const plb_bundle_opt *opt, double bs[3], const double *weights) {
-    return refine_entry(KIND_FUND, x1, x2, n, F, opt, bs, weights);
+    return refine_single(PLB_REFINER_FUNDAMENTAL, x1, x2, n, weights, nullptr, nullptr, nullptr, nullptr, opt, F, bs);
 }
 int plb_refine_homography(const double *x1, const double *x2, size_t n, double H[9], const plb_bundle_opt *opt,
                           double bs[3]) {
-    return refine_entry(KIND_HOMOG, x1, x2, n, H, opt, bs);
+    return plb_refine_homography_weighted(x1, x2, n, H, opt, bs, nullptr);
 }
 int plb_refine_homography_weighted(const double *x1, const double *x2, size_t n, double H[9],
                                    const plb_bundle_opt *opt, double bs[3], const double *weights) {
-    return refine_entry(KIND_HOMOG, x1, x2, n, H, opt, bs, weights);
+    return refine_single(PLB_REFINER_HOMOGRAPHY, x1, x2, n, weights, nullptr, nullptr, nullptr, nullptr, opt, H, bs);
 }
 
 // ---- solvers ------------------------------------------------------------------------------------------------
@@ -2294,6 +2351,7 @@ int plb_relpose_8pt_batch(size_t count, size_t n, const double *x1, const double
 // are assigned to devices by longest-processing-time-first on (correspondences x expected iterations), problems whose
 // correspondences are resident stay on the device that holds them.
 static double task_cost(const Task &t) {
+    if (t.refine) return (double)std::max<size_t>(t.n, 1) * (double)std::max<uint64_t>(t.polish.bundle.max_iterations, 1);
     static const double its[5] = {4.0 * 1000, 0.5 * 14000, 2.0 * 30000, 1.0 * 1000, 0.5 * 14000}; // models x iterations, typical
     const double cap = (double)std::max<uint64_t>(t.opt.max_iterations, 1) * 4.0;
     return (double)std::max<size_t>(t.n, 1) * std::min(its[t.kind], cap);
@@ -2327,7 +2385,7 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
             }
         }
     }
-    // groups per device: tasks of the same engine kind run in lock-step
+    // groups per device: tasks of the same engine kind run in lock-step (refiner tasks: in one LM phase)
     const int nthreads_req = std::max(1, streams);
     struct Job {
         int device;
@@ -2367,7 +2425,7 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
         t_blocking_sync = oversubscribed;
         t_batch_worker = jobs.size() > 1;
         for (auto &grp : jobs[w].groups) {
-            const int rc = run_group(grp[0]->kind, grp);
+            const int rc = grp[0]->refine ? run_refine_group(grp[0]->kind, grp) : run_group(grp[0]->kind, grp);
             if (rc != PLB_OK) {
                 int exp = PLB_OK;
                 if (first_err.compare_exchange_strong(exp, rc)) {
@@ -2472,6 +2530,15 @@ int plb_ransac_batch_multi(plb_problem *problems, size_t count, int n_gpus, int 
     return batch_impl(problems, count, devs.data(), n_gpus, streams_per_gpu);
 }
 
+// The devices of a batch call: n_gpus -1 the calling thread's device, 0 all `have` devices, k the first k.
+static std::vector<int> batch_devices(int n_gpus, int have) {
+    std::vector<int> devs;
+    if (n_gpus == -1) devs.push_back(g_device);
+    else
+        for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
+    return devs;
+}
+
 // The body of the two estimate batch calls: the pre-step of every problem, LO-RANSAC of the tasks over `devs`, the
 // post-step.  dev_io: a / b (float when f32) and inliers are device memory, read after `ready` has completed.
 static int estimate_batch_run(plb_estimate_problem *problems, size_t count, const std::vector<int> &devs, int streams,
@@ -2520,11 +2587,7 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
         g_err = "n_gpus out of range";
         return PLB_ERR_ARG;
     }
-    std::vector<int> devs;
-    if (n_gpus == -1) devs.push_back(g_device);
-    else
-        for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
-    return estimate_batch_run(problems, count, devs, streams_per_gpu, false, false, nullptr);
+    return estimate_batch_run(problems, count, batch_devices(n_gpus, have), streams_per_gpu, false, false, nullptr);
 }
 // The same on the calling thread's device with device-resident inputs and masks: the inputs are gathered into the engine's
 // own buffer by k_ingest (F / H normalisation then works in place on that copy, the caller's arrays are only read) and
@@ -2560,6 +2623,87 @@ int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int 
     if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
     const std::vector<int> devs{E.device};
     return estimate_batch_run(problems, count, devs, streams, true, dtype == PLB_DTYPE_F32, E.ev_in);
+}
+
+// ---- batch form of the robust/bundle.h refiners ----------------------------------------------------------------
+// Every problem checked by its single entry point's rules (refine_prepare), before any device call; on failure every
+// status gets the code and nothing else is written.
+static int refine_batch_prepare(plb_refine_problem *problems, size_t count, std::vector<Task> &tasks) {
+    tasks.assign(count, Task());
+    for (size_t i = 0; i < count; ++i) {
+        plb_refine_problem &p = problems[i];
+        if (int r = refine_prepare(p.refiner, p.a, p.b, (size_t)p.n, p.weights, &p.camera1, &p.camera2, &p.camera1,
+                                   &p.camera2, &p.bundle, p.model, p.bundle_stats, tasks[i])) {
+            for (size_t j = 0; j < count; ++j) problems[j].status = r;
+            return r;
+        }
+    }
+    return PLB_OK;
+}
+static int refine_batch_run(plb_refine_problem *problems, std::vector<Task> &tasks, const std::vector<int> &devs,
+                            int streams) {
+    std::vector<int> dev_of(tasks.size(), -1);
+    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
+    for (size_t i = 0; i < tasks.size(); ++i) problems[i].status = rc;
+    return rc;
+}
+int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    if (count == 0) return PLB_OK;
+    if (!problems) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    std::vector<Task> tasks;
+    if (int r = refine_batch_prepare(problems, count, tasks)) return r;
+    auto fail_all = [&](int rc, const char *msg) {
+        g_err = msg;
+        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
+        return rc;
+    };
+    if (n_gpus < -1) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    const int have = plb_device_count();
+    if (have == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    if (n_gpus > have) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    return refine_batch_run(problems, tasks, batch_devices(n_gpus, have), streams_per_gpu);
+}
+// The same on the calling thread's device with a / b / weights in its memory: k_ingest gathers them into the engine's
+// own input buffer, where the host path's upload puts them, so what runs after is the host path's work on the same doubles.
+int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    if (count == 0) return PLB_OK;
+    if (!problems) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    auto fail_all = [&](int rc, const std::string &msg) {
+        g_err = msg;
+        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
+        return rc;
+    };
+    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
+    std::vector<Task> tasks;
+    if (int r = refine_batch_prepare(problems, count, tasks)) return r;
+    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    Engine &E = *engine();
+    if (int rc = E.init()) return fail_all(rc, g_err);
+    const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
+    for (size_t i = 0; i < count; ++i) {
+        const Task &t = tasks[i];
+        if (t.n == 0) continue;
+        for (const void *q : {(const void *)t.a, (const void *)t.b, t.weights}) {
+            if (!q) continue; // only the weights may be null
+            if (!device_memory(q, E.device))
+                return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": a / b / weights must be device memory of the current device");
+            if ((uintptr_t)q % elem) return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": a / b / weights are not aligned to the dtype");
+        }
+    }
+    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
+    for (Task &t : tasks) {
+        t.dev_io = true;
+        t.f32 = dtype == PLB_DTYPE_F32;
+        t.ready = E.ev_in;
+    }
+    return refine_batch_run(problems, tasks, {E.device}, streams);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {

@@ -198,17 +198,17 @@ __global__ void __launch_bounds__(NORM_THREADS) k_normalize(const NormDesc *__re
         d.b[i] = d.b[i] / scale;
     }
 }
-// Device-resident inputs (plb_estimate_batch_device) -> the fp64 AoS the host path would have uploaded, one problem per
-// blockIdx.y.  fp32 -> fp64 is exact, so everything downstream sees the values the host path sees for the widened input.
-// The copy also keeps the caller's arrays read-only: k_normalize works in place on the engine's buffer.
+// Device-resident inputs (plb_estimate_batch_device, plb_refine_batch_device) -> the fp64 AoS the host path would have
+// uploaded (a, b, then the weights), one problem per blockIdx.y.  fp32 -> fp64 is exact, so everything downstream sees
+// the values the host path sees for the widened input.  The copy also keeps the caller's arrays read-only: k_normalize
+// works in place on the engine's buffer.
 constexpr int INGEST_THREADS = 256, INGEST_MAX_BLOCKS = 512;
 __global__ void __launch_bounds__(INGEST_THREADS) k_ingest(const IngestDesc *__restrict__ descs) {
     const IngestDesc d = descs[blockIdx.y];
-    const size_t na = 2 * (size_t)d.n, total = na + (size_t)d.b_dim * d.n;
+    const size_t na = 2 * (size_t)d.n, nb = na + (size_t)d.b_dim * d.n, total = nb + (d.w ? (size_t)d.n : 0);
     for (size_t i = (size_t)blockIdx.x * INGEST_THREADS + threadIdx.x; i < total; i += (size_t)gridDim.x * INGEST_THREADS) {
-        const bool in_a = i < na;
-        const size_t j = in_a ? i : i - na;
-        const void *src = in_a ? d.a : d.b;
+        const size_t j = i < na ? i : i < nb ? i - na : i - nb;
+        const void *src = i < na ? d.a : i < nb ? d.b : d.w;
         d.dst[i] = d.f32 ? (double)static_cast<const float *>(src)[j] : static_cast<const double *>(src)[j];
     }
 }
@@ -2896,7 +2896,7 @@ __global__ void __launch_bounds__(LM_THREADS, 1)
 // k_lm needs ~255 registers per thread: one 256-thread CTA (one job, or one slice of a job's cluster) per SM.
 static thread_local int t_lm_sm_share = 50;
 void lm_set_sm_share(int pct) { t_lm_sm_share = (pct > 0 && pct <= 100) ? pct : 50; }
-static int lm_cluster_size(int n_jobs, int max_n) {
+static int lm_cluster_size(int n_jobs, int max_n, int share = t_lm_sm_share) {
     static const int per_cta = [] { // correspondences per CTA before another CTA of the cluster pays off
         const char *e = std::getenv("PLB_LM_PER_CTA");
         const int v = e ? std::atoi(e) : 0;
@@ -2917,7 +2917,7 @@ static int lm_cluster_size(int n_jobs, int max_n) {
         const int v = e ? std::atoi(e) : 0;
         return (v > 0 && v <= 100) ? v : 0;
     }();
-    const int sm_share = forced ? forced : t_lm_sm_share;
+    const int sm_share = forced ? forced : share;
     while (csize > 1 && n_jobs * csize > sm_count() * sm_share / 100) csize /= 2;
     return csize;
 }
@@ -2972,6 +2972,15 @@ void launch_lm(int kind, bool refine_camera, bool xcam, bool weighted, const Pro
     const int csize = lm_cluster_size(n_jobs, max_n);
     launch_lm_any(kind, refine_camera, xcam, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, n_jobs, csize, mask_base,
                   idx_scratch, scratch_stride, out, cam_out, stream, weighted);
+}
+int lm_lone_width(int n) { return lm_cluster_size(1, n, 100); }
+void launch_lm_width(int kind, bool refine_camera, bool xcam, bool weighted, const ProblemDev *probs,
+                     const LmJob *jobs_dev, const double *models_in, int n_jobs, int csize, LmJobOut *out,
+                     double *cam_out, cudaStream_t stream) {
+    if (n_jobs <= 0) return;
+    const int nc = std::max(1, std::min(n_jobs, sm_count() / csize));
+    launch_lm_any(kind, refine_camera, xcam, probs, jobs_dev, nullptr, models_in, nullptr, n_jobs, nc, csize, nullptr,
+                  nullptr, 0, out, cam_out, stream, weighted);
 }
 // Clusters of a round's LO launch: at most one wave (a k_lm CTA owns an SM), at most the estimated number of jobs.
 int lm_round_max_clusters(int kind, int est_jobs, int max_n) {

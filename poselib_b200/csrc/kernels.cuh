@@ -222,11 +222,13 @@ struct MaskDesc {
     long long mask_off;
     double model[9];
 };
-// Correspondences of one problem already in device memory (plb_estimate_batch_device): the caller's contiguous AoS arrays,
-// read only, gathered into the engine's own input buffer as fp64 (a then b, the layout the host path uploads).
+// Correspondences of one problem already in device memory (plb_estimate_batch_device, plb_refine_batch_device): the
+// caller's contiguous AoS arrays, read only, gathered into the engine's own input buffer as fp64 (a, b, then w: the
+// layout the host path uploads).
 struct IngestDesc {
     const void *a, *b; // 2n and b_dim*n values: float (f32) or double
-    double *dst;       // (2 + b_dim) * n doubles
+    const void *w;     // n per-residual weights of the same dtype, or null
+    double *dst;       // (2 + b_dim + (w ? 1 : 0)) * n doubles
     int n, b_dim, f32;
 };
 // One final inlier mask for a caller's device buffer: n bytes 0 / 1 from the mask buffer at mask_off.
@@ -263,6 +265,15 @@ constexpr __host__ __device__ int kind_cam_count(int kind) { return kind == KIND
 void launch_lm(int kind, bool refine_camera, bool xcam, bool weighted, const ProblemDev *probs, const LmJob *jobs_dev,
                const double *models_in, int n_jobs, int max_n, const char *mask_base, int *idx_scratch,
                int scratch_stride, LmJobOut *out, double *cam_out, cudaStream_t stream);
+// The cluster width a launch of one job over n correspondences takes with every SM to itself (lm_set_sm_share(100);
+// PLB_LM_PER_CTA and PLB_LM_SM_PCT apply).  The width fixes a job's reduction order, so a job run at this width gives the
+// bits of a lone call.
+int lm_lone_width(int n);
+// launch_lm with the cluster width fixed (lm_lone_width of every job) on a persistent grid of at most sm_count / csize
+// clusters, for jobs with subset_mode 0 (no mask, no index scratch).
+void launch_lm_width(int kind, bool refine_camera, bool xcam, bool weighted, const ProblemDev *probs,
+                     const LmJob *jobs_dev, const double *models_in, int n_jobs, int csize, LmJobOut *out,
+                     double *cam_out, cudaStream_t stream);
 // LO jobs of a round, listed on the device by k_pass1: job j refines model slot job_src[j].slot of the round's model
 // list (stride MSZ) with the template tmpl[job_src[j].pidx]; *n_jobs_dev jobs.  n_jobs_dev is &ctl[CTL_JOB_TOTAL] of the
 // round's control words: when the round's CTL_FLAGS word is set no job runs and no job_src entry is read (k_pass1
@@ -290,7 +301,7 @@ void launch_inlier_masks(int kind, const ProblemDev *probs, const MaskDesc *desc
 // Inlier masks as bits (bit k & 31 of word k >> 5) for the device -> host copy; n_bytes is a multiple of 32.
 void launch_pack_mask(const char *mask, uint32_t *bits, size_t n_bytes, cudaStream_t stream);
 // Device-resident inputs -> fp64 AoS for n_desc problems (descriptors in device memory); max_vals: the largest
-// (2 + b_dim) * n of the descriptors.
+// (2 + b_dim + (w ? 1 : 0)) * n of the descriptors.
 void launch_ingest(const IngestDesc *descs_dev, int n_desc, size_t max_vals, cudaStream_t stream);
 // Final masks straight into the callers' device buffers for n_desc problems; max_n: the largest n of the descriptors.
 void launch_scatter_masks(const char *mask, const ScatterDesc *descs_dev, int n_desc, int max_n, cudaStream_t stream);
