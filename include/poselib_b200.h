@@ -417,6 +417,58 @@ int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int
  * for the dtype -> PLB_ERR_ARG, with every status set and nothing else written. */
 int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams);
 
+/* Scores and inlier masks of given models (robust/utils.h:40-87), for callers that check matches against models they
+ * already have: a pose prior, guided matching against verified F / H, E / F / H inlier counts on the same matches, or
+ * hypotheses made outside the library.  One record per (problem, model), at the ransac_* level: points as plb_ransac_*
+ * and plb_ransac_relpose_cameras take them, no normalisation, sq_threshold the squared threshold in their units (tangent
+ * Sampson: pixels^2).
+ *   kind (+ option)                      model       score / num_inliers                   inliers (get_inliers)
+ *   PLB_KIND_PNP                         pose (7)    compute_msac_score, utils.cc:36-63    utils.cc:374-383
+ *   PLB_KIND_RELPOSE                     pose        compute_sampson_msac_score :158-201   get_inliers :434-476
+ *   PLB_KIND_RELPOSE + tangent_sampson   pose        compute_tangent_sampson_msac_score    get_tangent_sampson_inliers
+ *     (x1 / x2 pixels of camera1 / camera2, unprojected as ransac.cc:155-168 does)  :269-298   :541-569
+ *   PLB_KIND_FUNDAMENTAL (F or E)        3x3 (9)     compute_sampson_msac_score :204-239   get_inliers :479-513
+ *   PLB_KIND_HOMOGRAPHY                  3x3         compute_homography_msac_score :300-329  get_homography_inliers :331-351
+ * num_inliers and the mask are exactly the reference's; for PnP the count comes from the scorer and the mask from
+ * get_inliers, whose formulas can disagree at the last bit, as in the reference.  A score is the fp64 sum of the device's
+ * scorer: the same terms as the reference's in a fixed order, the outliers added as one product (n - count) * sq_threshold,
+ * so it equals the reference's up to summation order and, bit for bit, the score the RANSAC path records for the same
+ * model.  n = 0 gives score 0 and count 0; m = 0 writes nothing.  Camera1 / camera2 are read only with tangent_sampson. */
+typedef struct plb_score_problem {
+    int32_t kind;             /* PLB_KIND_* */
+    int32_t tangent_sampson;  /* relative pose only */
+    uint64_t n;
+    const double *a;          /* x (pnp) or x1: 2n doubles */
+    const double *b;          /* X (pnp): 3n doubles; else x2: 2n doubles */
+    plb_camera camera1;
+    plb_camera camera2;
+    uint64_t m;               /* models */
+    const double *models;     /* m x 7 (poses) or m x 9 (column-major matrices) doubles */
+    double sq_threshold;
+    double *scores;           /* out: m (required when m > 0) */
+    int64_t *num_inliers;     /* out: m (required when m > 0) */
+    char *inliers;            /* out: NULL, or m x n bytes 0 / 1, model-major */
+    int32_t status;           /* out */
+    int32_t reserved;
+} plb_score_problem;
+/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device);
+ * streams_per_gpu groups of problems are in flight on each device.  Every pointer is host memory.  Each problem's
+ * outputs are the same bits whatever else is in the batch and for any n_gpus / streams.
+ * Checked before any device call; on failure every status gets the code and nothing else is written: NULL problems, an
+ * unknown kind, tangent_sampson on another kind, a / b NULL with n > 0, models / scores / num_inliers NULL with m > 0, a
+ * non-finite sq_threshold, m >= 2^31, n > 2^26 or m * n overflowing -> PLB_ERR_ARG; a camera (tangent_sampson) outside
+ * the ten models -> PLB_ERR_NYI; n_gpus < -1 -> PLB_ERR_ARG; no device -> PLB_ERR_CUDA; n_gpus above the device count ->
+ * PLB_ERR_ARG. */
+int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
+/* plb_score_batch(problems, count, -1, streams) with a, b, models, scores, num_inliers and inliers in device (or managed)
+ * memory of the calling thread's device: a / b contiguous arrays of `dtype` aligned to it (PLB_DTYPE_F32: `const float *`
+ * cast into the `const double *` fields; widened exactly, so a float call gives the double call's results on the widened
+ * values), models fp64.  Nothing sized by n or m crosses PCIe.  Inputs are read after the work queued on `stream` ahead of
+ * the call; when the call returns, every device write it made is complete.  Besides the checks above: an unknown dtype, or
+ * a pointer of a problem that is not device memory of the current device or is misaligned (a / b: the dtype; models,
+ * scores, num_inliers: 8 bytes) -> PLB_ERR_ARG, checked as plb_estimate_batch_device checks its pointers. */
+int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams);
+
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers
  * that run several estimations on the same matches).  kind: PLB_KIND_*; returns a handle > 0 or an error < 0. */
 int plb_resident_create(int kind, const double *a, const double *b, size_t n);

@@ -18,6 +18,7 @@
 #pragma once
 #include "../../include/poselib_b200.h"
 
+#include <cstdint>
 #include <limits>
 #include <stdexcept>
 #include <string>
@@ -538,6 +539,107 @@ std::vector<BundleStats> bundle_adjust_image_batch(const std::vector<std::vector
         out[i] = detail::bundle_from_c<BundleStats>(P[i].bundle_stats);
     }
     return out;
+}
+
+// ---- robust/utils.h scorers and get_inliers on given models (plb_score_batch) ----------------------------------------
+// compute_msac_score / compute_sampson_msac_score / compute_tangent_sampson_msac_score / compute_homography_msac_score
+// with get_inliers / get_tangent_sampson_inliers / get_homography_inliers (robust/utils.h:40-87) for many models of one
+// problem in one call: scores[i], num_inliers[i] and, when asked for, inliers[i] (n chars) of model i.  sq_threshold is
+// squared, in the points' units (pixels^2 for the tangent-Sampson form).  These are separate names on purpose: the
+// drop-in does not redefine utils.h, whose functions PoseLib's own CPU estimators call once per hypothesis.
+struct ScoreResult {
+    std::vector<double> scores;
+    std::vector<int64_t> num_inliers;
+    std::vector<std::vector<char>> inliers; // empty unless asked for
+};
+namespace detail {
+inline ScoreResult score_models(plb_score_problem q, const std::vector<double> &rows, bool want_inliers) {
+    const size_t m = q.m, n = q.n;
+    ScoreResult r;
+    r.scores.assign(m, 0.0);
+    r.num_inliers.assign(m, 0);
+    std::vector<char> flat(want_inliers ? m * n : 0);
+    q.models = rows.empty() ? nullptr : rows.data();
+    q.scores = r.scores.empty() ? nullptr : r.scores.data();
+    q.num_inliers = r.num_inliers.empty() ? nullptr : r.num_inliers.data();
+    q.inliers = flat.empty() ? nullptr : flat.data();
+    check(plb_score_batch(&q, 1, -1, 1));
+    if (want_inliers)
+        for (size_t i = 0; i < m; ++i) r.inliers.emplace_back(flat.begin() + i * n, flat.begin() + (i + 1) * n);
+    return r;
+}
+inline plb_score_problem score_problem(int kind, size_t n, const double *a, const double *b, double sq_threshold) {
+    plb_score_problem q = plb_score_problem();
+    q.kind = kind;
+    q.n = n;
+    q.a = a;
+    q.b = b;
+    q.camera1.model_id = q.camera2.model_id = PLB_CAMERA_NULL;
+    q.sq_threshold = sq_threshold;
+    return q;
+}
+template <typename Pose> inline std::vector<double> pose_rows(const std::vector<Pose> &poses) {
+    std::vector<double> rows(7 * poses.size());
+    for (size_t i = 0; i < poses.size(); ++i) pose_to(poses[i], rows.data() + 7 * i);
+    return rows;
+}
+template <typename Mat3> inline std::vector<double> matrix_rows(const std::vector<Mat3> &ms) {
+    static_assert(sizeof(Mat3) == 9 * sizeof(double), "column-major 3x3 of doubles required");
+    std::vector<double> rows(9 * ms.size());
+    for (size_t i = 0; i < ms.size(); ++i)
+        for (int k = 0; k < 9; ++k) rows[9 * i + k] = reinterpret_cast<const double *>(&ms[i])[k];
+    return rows;
+}
+} // namespace detail
+// compute_msac_score(pose, x, X) (utils.cc:36-63) and get_inliers(pose, x, X) (:374-383)
+template <typename P2, typename P3, typename Pose>
+ScoreResult score_absolute_poses(const std::vector<P2> &x, const std::vector<P3> &X, const std::vector<Pose> &poses,
+                                 double sq_threshold, bool want_inliers = false) {
+    static_assert(sizeof(P2) == 2 * sizeof(double) && sizeof(P3) == 3 * sizeof(double), "dense point layout required");
+    plb_score_problem q = detail::score_problem(PLB_KIND_PNP, x.size(), detail::raw(x), detail::raw(X), sq_threshold);
+    q.m = poses.size();
+    return detail::score_models(q, detail::pose_rows(poses), want_inliers);
+}
+// compute_sampson_msac_score(pose, x1, x2) (utils.cc:158-201) and get_inliers(pose, x1, x2) (:434-476)
+template <typename P2, typename Pose>
+ScoreResult score_relative_poses(const std::vector<P2> &x1, const std::vector<P2> &x2, const std::vector<Pose> &poses,
+                                 double sq_threshold, bool want_inliers = false) {
+    static_assert(sizeof(P2) == 2 * sizeof(double), "dense point layout required");
+    plb_score_problem q = detail::score_problem(PLB_KIND_RELPOSE, x1.size(), detail::raw(x1), detail::raw(x2), sq_threshold);
+    q.m = poses.size();
+    return detail::score_models(q, detail::pose_rows(poses), want_inliers);
+}
+// compute_tangent_sampson_msac_score / get_tangent_sampson_inliers (utils.cc:269-298,541-569) on the pixels x1, x2 of
+// camera1, camera2, unprojected as ransac_relpose(x1, x2, camera1, camera2) does (ransac.cc:155-168)
+template <typename P2, typename Camera, typename Pose>
+ScoreResult score_relative_poses(const std::vector<P2> &x1, const std::vector<P2> &x2, const Camera &camera1,
+                                 const Camera &camera2, const std::vector<Pose> &poses, double sq_threshold,
+                                 bool want_inliers = false) {
+    static_assert(sizeof(P2) == 2 * sizeof(double), "dense point layout required");
+    plb_score_problem q = detail::score_problem(PLB_KIND_RELPOSE, x1.size(), detail::raw(x1), detail::raw(x2), sq_threshold);
+    q.tangent_sampson = 1;
+    q.camera1 = detail::camera_to_c(camera1);
+    q.camera2 = detail::camera_to_c(camera2);
+    q.m = poses.size();
+    return detail::score_models(q, detail::pose_rows(poses), want_inliers);
+}
+// compute_sampson_msac_score(F, x1, x2) (utils.cc:204-239) and get_inliers(E, x1, x2) (:479-513)
+template <typename P2, typename Mat3>
+ScoreResult score_fundamentals(const std::vector<P2> &x1, const std::vector<P2> &x2, const std::vector<Mat3> &F,
+                               double sq_threshold, bool want_inliers = false) {
+    static_assert(sizeof(P2) == 2 * sizeof(double), "dense point layout required");
+    plb_score_problem q = detail::score_problem(PLB_KIND_FUNDAMENTAL, x1.size(), detail::raw(x1), detail::raw(x2), sq_threshold);
+    q.m = F.size();
+    return detail::score_models(q, detail::matrix_rows(F), want_inliers);
+}
+// compute_homography_msac_score (utils.cc:300-329) and get_homography_inliers (:331-351)
+template <typename P2, typename Mat3>
+ScoreResult score_homographies(const std::vector<P2> &x1, const std::vector<P2> &x2, const std::vector<Mat3> &H,
+                               double sq_threshold, bool want_inliers = false) {
+    static_assert(sizeof(P2) == 2 * sizeof(double), "dense point layout required");
+    plb_score_problem q = detail::score_problem(PLB_KIND_HOMOGRAPHY, x1.size(), detail::raw(x1), detail::raw(x2), sq_threshold);
+    q.m = H.size();
+    return detail::score_models(q, detail::matrix_rows(H), want_inliers);
 }
 
 } // namespace poselib_b200

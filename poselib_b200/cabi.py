@@ -105,6 +105,7 @@ EXPORTS = [
     "plb_resident_free", "plb_bundle_adjust_image_weighted", "plb_refine_relpose_weighted",
     "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
     "plb_refine_homography_weighted", "plb_estimate_batch_device", "plb_refine_batch", "plb_refine_batch_device",
+    "plb_score_batch", "plb_score_batch_device",
 ]
 DTYPE_F64, DTYPE_F32 = 0, 1
 
@@ -126,6 +127,14 @@ class RefineProblem(C.Structure):
                 ("b", C.POINTER(C.c_double)), ("weights", C.POINTER(C.c_double)), ("camera1", Camera),
                 ("camera2", Camera), ("bundle", BundleOpt), ("model", C.c_double * 9), ("bundle_stats", C.c_double * 3),
                 ("status", C.c_int32), ("reserved2", C.c_int32)]
+
+
+class ScoreProblem(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("tangent_sampson", C.c_int32), ("n", C.c_uint64), ("a", C.POINTER(C.c_double)),
+                ("b", C.POINTER(C.c_double)), ("camera1", Camera), ("camera2", Camera), ("m", C.c_uint64),
+                ("models", C.POINTER(C.c_double)), ("sq_threshold", C.c_double), ("scores", C.POINTER(C.c_double)),
+                ("num_inliers", C.POINTER(C.c_int64)), ("inliers", C.c_char_p), ("status", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 if not os.path.exists(LIB_PATH):
@@ -752,3 +761,122 @@ def refine_batch_device(problems, stream=None, streams=8):
     _check(_lib.plb_refine_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
                                         int(streams)))
     return _refine_results(arr, problems)
+
+
+# ---- scores and inlier masks of given models (plb_score_batch) -------------------------------------------------
+def _score_models(kind, models):
+    """Models of one problem as the C-ABI reads them: [m,7] poses, or [m,3,3] matrices [r,c] -> column-major rows."""
+    m = np.asarray(models, dtype=np.float64)
+    if kind in ("pnp", "relpose"):
+        return np.ascontiguousarray(m.reshape(-1, 7))
+    return np.ascontiguousarray(m.reshape(-1, 3, 3).transpose(0, 2, 1).reshape(-1, 9))
+
+
+def _fill_score_problem(q, p, npts, m):
+    """Everything of one plb_score_problem but its pointers."""
+    q.kind = KIND[p["kind"]]
+    q.tangent_sampson = int(p.get("tangent_sampson", False))
+    q.n = npts
+    q.m = m
+    q.camera1 = p.get("cam1") or Camera("NULL", ())
+    q.camera2 = p.get("cam2") or Camera("NULL", ())
+    q.sq_threshold = p["sq_threshold"]
+
+
+def score_batch(problems, n_gpus=-1, streams=8):
+    """MSAC scores, inlier counts and (optionally) inlier masks of given models (plb_score_batch; robust/utils.h).
+    problems: list of dict(kind, a, b, models [[m,7] poses or [m,3,3] matrices [r,c]], sq_threshold [squared, in the
+    points' units], tangent_sampson=False with cam1 / cam2 [pixels], inliers=False [True: return the masks]).
+    n_gpus: -1 current device, 0 all devices, k the first k.  Returns list of dict(scores [m] float64, num_inliers [m]
+    int64, inliers [m,n] bool or None, status)."""
+    count = len(problems)
+    arr = (ScoreProblem * count)()
+    out = []
+    keep = []
+    for i, p in enumerate(problems):
+        q = arr[i]
+        aa, ap = _d(p["a"])
+        ba, bp = _d(p["b"])
+        mo = _score_models(p["kind"], p["models"])
+        m, npts = len(mo), len(aa)
+        r = {"scores": np.zeros(m), "num_inliers": np.zeros(m, dtype=np.int64),
+             "inliers": np.zeros((m, npts), dtype=np.bool_) if p.get("inliers") else None}
+        keep.append((aa, ba, mo))
+        out.append(r)
+        _fill_score_problem(q, p, npts, m)
+        q.a, q.b, q.models = ap, bp, mo.ctypes.data_as(_P)
+        q.scores = r["scores"].ctypes.data_as(_P)
+        q.num_inliers = r["num_inliers"].ctypes.data_as(C.POINTER(C.c_int64))
+        if r["inliers"] is not None:
+            q.inliers = C.cast(r["inliers"].ctypes.data_as(C.POINTER(C.c_char)), C.c_char_p)
+    _check(_lib.plb_score_batch(arr, C.c_size_t(count), int(n_gpus), int(streams)))
+    for r, q in zip(out, arr):
+        r["status"] = q.status
+    return out
+
+
+def score_batch_device(problems, stream=None, streams=8):
+    """score_batch (n_gpus=-1) with everything on the GPU (plb_score_batch_device).  problems: the dicts score_batch
+    takes, with a / b as CUDA torch tensors ([n,2] / [n,3] or [n,2]) of one device and one dtype, float32 or float64, and
+    models a CUDA float64 tensor [m,7] or [m,3,3] ([r,c]).  The call runs on that device and reads the inputs after the
+    work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle; default: the device's current stream).
+    Returns the dicts of score_batch with CUDA tensors: scores (float64), num_inliers (int64) and inliers (bool [m,n] or
+    None; the masks of one call are views of one zeroed allocation)."""
+    import torch
+    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
+    tensors = [t for p in problems for t in (p["a"], p["b"])]
+    models = [p["models"] for p in problems]
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors + models):
+        raise TypeError("score_batch_device: a, b and models must be CUDA torch tensors")
+    if not tensors:
+        return []
+    dev, dt = tensors[0].device, tensors[0].dtype
+    if any(t.device != dev for t in tensors + models):
+        raise ValueError(f"score_batch_device: every tensor must be on {dev} (shard the batch by device)")
+    if dt not in dtypes or any(t.dtype != dt for t in tensors):
+        raise TypeError("score_batch_device: a and b must share one dtype, torch.float32 or torch.float64")
+    if any(t.dtype != torch.float64 for t in models):
+        raise TypeError("score_batch_device: models must be torch.float64")
+    set_device(dev.index)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev)
+    elif not isinstance(stream, torch.cuda.Stream):
+        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    count = len(problems)
+    arr = (ScoreProblem * count)()
+    keep = []
+    out = []
+    ptr = lambda t: C.cast(C.c_void_p(t.data_ptr() if t is not None and t.numel() else None), _P)
+    with torch.cuda.stream(stream):  # the copies and outputs below are ordered before the call's reads and writes
+        mods = []
+        for i, p in enumerate(problems):
+            msz = 7 if p["kind"] in ("pnp", "relpose") else 9
+            mo = p["models"].reshape(-1, msz) if msz == 7 else p["models"].reshape(-1, 3, 3).transpose(1, 2).reshape(-1, 9)
+            mods.append(mo.contiguous())
+        ms = [len(mo) for mo in mods]
+        ns = [p["a"].shape[0] for p in problems]
+        scores = list(torch.zeros(sum(ms), dtype=torch.float64, device=dev).split(ms))
+        counts = list(torch.zeros(sum(ms), dtype=torch.int64, device=dev).split(ms))
+        want = [bool(p.get("inliers")) for p in problems]
+        sizes = [ms[i] * ns[i] if want[i] else 0 for i in range(count)]
+        flat = torch.zeros(sum(sizes), dtype=torch.bool, device=dev).split(sizes)
+        for i, p in enumerate(problems):
+            q = arr[i]
+            a, b = p["a"].contiguous(), p["b"].contiguous()
+            npts = ns[i]
+            b_dim = 3 if p["kind"] == "pnp" else 2
+            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
+                raise ValueError(f"score_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
+                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
+            mask = flat[i].view(ms[i], npts) if want[i] else None
+            keep.append((a, b))
+            _fill_score_problem(q, p, npts, ms[i])
+            q.a, q.b, q.models, q.scores = ptr(a), ptr(b), ptr(mods[i]), ptr(scores[i])
+            q.num_inliers = C.cast(C.c_void_p(counts[i].data_ptr() if ms[i] else None), C.POINTER(C.c_int64))
+            q.inliers = C.cast(C.c_void_p(mask.data_ptr() if mask is not None and mask.numel() else None), C.c_char_p)
+            out.append({"scores": scores[i], "num_inliers": counts[i], "inliers": mask})
+    _check(_lib.plb_score_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+                                       int(streams)))
+    for r, q in zip(out, arr):
+        r["status"] = q.status
+    return out

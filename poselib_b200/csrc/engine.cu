@@ -208,7 +208,7 @@ struct Engine {
     DevBuf<float> soa32, cmax;
     DevBuf<uint4> qrows; // relpose / fundamental: ProblemDev::q
     DevBuf<uint32_t> samples;
-    DevBuf<int> work, slots, subset, act, model_prob, prob_count;
+    DevBuf<int> work, subset, act, model_prob, prob_count;
     // round state that stays on the device: sampler states, per-sample / per-model records, candidate lists
     DevBuf<SamplerDev> smp;
     DevBuf<uint64_t> growth;
@@ -237,9 +237,12 @@ struct Engine {
     PinBuf<IngestDesc> h_idesc;
     DevBuf<ScatterDesc> sdesc;
     PinBuf<ScatterDesc> h_sdesc;
+    DevBuf<ScoreDesc> scdesc; // explicit models (initial models, plb_score_batch)
+    PinBuf<ScoreDesc> h_scdesc;
+    PinBuf<double> h_models;
     DevBuf<LmJob> jobs;
     PinBuf<double> h_in, h_lm_in;
-    PinBuf<int> h_slots, h_act, h_work;
+    PinBuf<int> h_act, h_work;
     PinBuf<ProblemDev> h_probs;
     PinBuf<TransposeDesc> h_tdesc;
     PinBuf<MaskDesc> h_mdesc;
@@ -247,7 +250,7 @@ struct Engine {
     // result records written by the kernels directly into mapped pinned memory (no explicit D2H copies): per round and
     // problem one header, the models that improved the best-minimal state and the LO results
     MapBuf<double> h_scores;
-    MapBuf<uint32_t> h_counts;
+    MapBuf<long long> h_counts;
     MapBuf<SelHeader> h_hdr;
     MapBuf<ImpRec> h_imp;
     MapBuf<LmJobOut> h_lm_out;
@@ -575,6 +578,14 @@ struct Task {
     bool refine = false;
     const void *weights = nullptr; // refine: n per-residual weights in point order (float when f32), or null: uniform
     double *bstats = nullptr;
+    // Scoring given models instead of LO-RANSAC (run_score_group): m models (MSZ doubles each; device memory with
+    // dev_io), threshold sq_thr; records to scores / counts, and with `inliers` m x n mask bytes, model-major.
+    bool score = false;
+    size_t m = 0;
+    const double *models = nullptr;
+    double sq_thr = 0;
+    double *scores = nullptr;
+    int64_t *counts = nullptr;
     // doubles per correspondence the group uploads: the caller layout, then the weight
     size_t in_per_point(int in_arr) const { return (size_t)in_arr + (weights ? 1 : 0); }
 };
@@ -802,7 +813,7 @@ struct Group {
             P.cam[0].model = P.cam[1].model = CAMM_NULL;
             P.n = S.n;
             P.kind = kind;
-            P.sq_thr = S.t->max_error * S.t->max_error;
+            P.sq_thr = S.t->score ? S.t->sq_thr : S.t->max_error * S.t->max_error;
             P.rfc = S.t->rfc;
             P.n_pad = S.n_pad;
             if (S.n == 0) continue;
@@ -1100,6 +1111,106 @@ struct Group {
         }
         return PLB_OK;
     }
+    // ---- given models (plb_score_batch): one k_score pass over the group's (problem, tile) list, one wait --------------
+    // The problems that want masks are scored by the mask instantiation, the others by the plain one.  Host tasks: the
+    // models go up through a pinned staging buffer, the records come back through mapped memory and the masks as bits
+    // (k_pack_mask), from the engine's mask buffer (n_pad bytes per model).  Device tasks: k_score reads the caller's
+    // models and writes records and mask bytes (stride n) into the caller's buffers.
+    int score() {
+        const int TMX = score_tile_models(kind);
+        const bool host = !PS[0].t->dev_io; // a call's tasks are all host or all device tasks
+        std::vector<int> order;
+        for (int pass = 0; pass < 2; ++pass)
+            for (int i = 0; i < NP; ++i)
+                if (PS[i].t->m > 0 && (PS[i].t->inliers != nullptr) == (pass == 1)) order.push_back(i);
+        const int nd = (int)order.size();
+        if (!nd) return PLB_OK;
+        size_t n_models = 0, mask_total = 0;
+        for (int i : order) {
+            n_models += PS[i].t->m;
+            if (PS[i].t->inliers) mask_total += PS[i].t->m * (size_t)PS[i].n_pad;
+        }
+        int rc;
+        if ((rc = E.scdesc.ensure(nd)) || (rc = E.h_scdesc.ensure(nd))) return rc;
+        if (host && ((rc = E.models.ensure(n_models * MSZ)) || (rc = E.h_models.ensure(n_models * MSZ)) ||
+                     (rc = E.h_counts.ensure(n_models)) || (rc = E.h_scores.ensure(n_models)) ||
+                     (rc = E.mask.ensure(mask_total)) || (rc = E.mask_bits.ensure(mask_total / 32 + 1)) ||
+                     (rc = E.h_mask_bits.ensure(mask_total / 32 + 1))))
+            return rc;
+        size_t moff = 0, maskoff = 0;
+        long long tiles = 0, tiles_plain = 0;
+        int nd_plain = 0;
+        for (int j = 0; j < nd; ++j) {
+            const PState &S = PS[order[j]];
+            const Task &t = *S.t;
+            ScoreDesc &D = E.h_scdesc.p[j];
+            D.pidx = S.pidx;
+            D.reserved = 0;
+            D.counts32 = nullptr;
+            D.m = (long long)t.m;
+            D.tile0 = tiles;
+            if (host) {
+                std::memcpy(E.h_models.p + moff * MSZ, t.models, sizeof(double) * MSZ * t.m);
+                D.models = E.models.p + moff * MSZ;
+                D.counts = E.h_counts.d + moff;
+                D.scores = E.h_scores.d + moff;
+                D.mask = t.inliers ? E.mask.p + maskoff : nullptr;
+                D.mask_stride = S.n_pad;
+                if (t.inliers) maskoff += t.m * (size_t)S.n_pad;
+            } else {
+                D.models = t.models;
+                D.counts = reinterpret_cast<long long *>(t.counts);
+                D.scores = t.scores;
+                D.mask = t.inliers;
+                D.mask_stride = S.n;
+            }
+            moff += t.m;
+            tiles += (long long)((t.m + TMX - 1) / TMX);
+            if (!t.inliers) {
+                tiles_plain = tiles;
+                nd_plain = j + 1;
+            }
+        }
+        if (host) {
+            PLB_CUDA(cudaMemcpyAsync(E.models.p, E.h_models.p, sizeof(double) * MSZ * n_models, cudaMemcpyHostToDevice, st));
+            h2d += sizeof(double) * MSZ * n_models;
+        } else { // the caller's models are read after its queued work (a group without points has no k_ingest to wait)
+            PLB_CUDA(cudaStreamWaitEvent(st, PS[0].t->ready, 0));
+        }
+        // the mask descriptors count their tiles from 0 in their own launch
+        for (int j = nd_plain; j < nd; ++j) E.h_scdesc.p[j].tile0 -= tiles_plain;
+        PLB_CUDA(cudaMemcpyAsync(E.scdesc.p, E.h_scdesc.p, sizeof(ScoreDesc) * nd, cudaMemcpyHostToDevice, st));
+        h2d += sizeof(ScoreDesc) * nd;
+        launch_score_models(kind, false, E.probs.p, E.scdesc.p, nd_plain, tiles_plain, TMX, st);
+        launch_score_models(kind, true, E.probs.p, E.scdesc.p + nd_plain, nd - nd_plain, tiles - tiles_plain, TMX, st);
+        E.launches += (nd_plain > 0) + (nd > nd_plain);
+        if (host && mask_total) {
+            launch_pack_mask(E.mask.p, E.mask_bits.p, mask_total, st);
+            E.launches++;
+            PLB_CUDA(cudaMemcpyAsync(E.h_mask_bits.p, E.mask_bits.p, mask_total / 8, cudaMemcpyDeviceToHost, st));
+            d2h += mask_total / 8;
+        }
+        if ((rc = sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        if (!host) return PLB_OK;
+        moff = maskoff = 0;
+        for (int i : order) {
+            const PState &S = PS[i];
+            const Task &t = *S.t;
+            std::copy(E.h_scores.p + moff, E.h_scores.p + moff + t.m, t.scores);
+            for (size_t j = 0; j < t.m; ++j) t.counts[j] = (int64_t)E.h_counts.p[moff + j];
+            moff += t.m;
+            d2h += (sizeof(double) + sizeof(long long)) * t.m;
+            if (!t.inliers) continue;
+            for (size_t j = 0; j < t.m; ++j) {
+                const uint32_t *w = E.h_mask_bits.p + ((maskoff + j * S.n_pad) >> 5); // n_pad is a multiple of 32
+                char *dst = t.inliers + j * (size_t)S.n;
+                for (int k = 0; k < S.n; ++k) dst[k] = (char)((w[k >> 5] >> (k & 31)) & 1u);
+            }
+            maskoff += t.m * (size_t)S.n_pad;
+        }
+        return PLB_OK;
+    }
     LmJob lo_job(const PState &S) const { return lm_job(S.pidx, -1, lo_params(kind, S.t->max_error)); }
     // one LO call of the serial loop and its result (ransac_impl.h:135-153)
     void apply_lo(PState &S, const LmJobOut &o) const {
@@ -1122,17 +1233,17 @@ struct Group {
         const int nw = (int)who.size();
         if (!nw) return PLB_OK;
         int rc;
-        if ((rc = E.h_slots.ensure(nw)) || (rc = E.slots.ensure(nw)) || (rc = E.h_counts.ensure(nw)) ||
+        if ((rc = E.h_scdesc.ensure(nw)) || (rc = E.scdesc.ensure(nw)) || (rc = E.h_counts.ensure(nw)) ||
             (rc = E.h_scores.ensure(nw)) || (rc = E.models.ensure((size_t)nw * MSZ)))
             return rc;
         std::vector<double> packed((size_t)nw * MSZ); // the MSZ-strided model list k_score reads
         for (int j = 0; j < nw; ++j) {
             std::copy(PS[who[j]].t->model, PS[who[j]].t->model + MSZ, packed.data() + (size_t)j * MSZ);
-            E.h_slots.p[j] = who[j];
+            E.h_scdesc.p[j] = {E.models.p + (size_t)j * MSZ, E.h_counts.d + j, E.h_scores.d + j, nullptr, 0, j, 1, who[j], 0};
         }
         PLB_CUDA(cudaMemcpyAsync(E.models.p, packed.data(), sizeof(double) * nw * MSZ, cudaMemcpyHostToDevice, st));
-        PLB_CUDA(cudaMemcpyAsync(E.slots.p, E.h_slots.p, sizeof(int) * nw, cudaMemcpyHostToDevice, st));
-        launch_score_models(kind, E.probs.p, E.models.p, E.slots.p, nw, E.h_counts.d, E.h_scores.d, st);
+        PLB_CUDA(cudaMemcpyAsync(E.scdesc.p, E.h_scdesc.p, sizeof(ScoreDesc) * nw, cudaMemcpyHostToDevice, st));
+        launch_score_models(kind, false, E.probs.p, E.scdesc.p, nw, nw, 1, st); // one-model tiles
         E.launches++;
         if ((rc = sync())) return rc;
         std::vector<LmTask> lo;
@@ -1708,6 +1819,15 @@ static int run_refine_group(int kind, std::vector<Task *> &tasks) {
     Group G(kind, tasks);
     int rc;
     if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose()) || (rc = G.refine())) return rc;
+    return PLB_OK;
+}
+
+// Runs a group of score tasks of the same kind (Task::score): the upload of the group (tangent Sampson: the camera
+// pre-step), then one scoring pass over every given model (Group::score).
+static int run_score_group(int kind, std::vector<Task *> &tasks) {
+    Group G(kind, tasks);
+    int rc;
+    if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose()) || (rc = G.score())) return rc;
     return PLB_OK;
 }
 
@@ -2352,6 +2472,7 @@ int plb_relpose_8pt_batch(size_t count, size_t n, const double *x1, const double
 // correspondences are resident stay on the device that holds them.
 static double task_cost(const Task &t) {
     if (t.refine) return (double)std::max<size_t>(t.n, 1) * (double)std::max<uint64_t>(t.polish.bundle.max_iterations, 1);
+    if (t.score) return (double)std::max<size_t>(t.n, 1) * (double)std::max<size_t>(t.m, 1);
     static const double its[5] = {4.0 * 1000, 0.5 * 14000, 2.0 * 30000, 1.0 * 1000, 0.5 * 14000}; // models x iterations, typical
     const double cap = (double)std::max<uint64_t>(t.opt.max_iterations, 1) * 4.0;
     return (double)std::max<size_t>(t.n, 1) * std::min(its[t.kind], cap);
@@ -2425,7 +2546,9 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
         t_blocking_sync = oversubscribed;
         t_batch_worker = jobs.size() > 1;
         for (auto &grp : jobs[w].groups) {
-            const int rc = grp[0]->refine ? run_refine_group(grp[0]->kind, grp) : run_group(grp[0]->kind, grp);
+            const int rc = grp[0]->refine  ? run_refine_group(grp[0]->kind, grp)
+                           : grp[0]->score ? run_score_group(grp[0]->kind, grp)
+                                           : run_group(grp[0]->kind, grp);
             if (rc != PLB_OK) {
                 int exp = PLB_OK;
                 if (first_err.compare_exchange_strong(exp, rc)) {
@@ -2704,6 +2827,139 @@ int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtyp
         t.ready = E.ev_in;
     }
     return refine_batch_run(problems, tasks, {E.device}, streams);
+}
+
+// ---- given models: the robust/utils.h scorers and get_inliers (plb_score_batch) ------------------------------------
+// One problem checked and turned into the Task of run_score_group: sq_thr is the caller's squared threshold, no
+// normalisation and no threshold scaling (the ransac_* level); tangent Sampson unprojects the pixels with the cameras as
+// ransac_relpose(x1, x2, camera1, camera2) does (ransac.cc:155-168).  Nothing is written here.
+static int score_prepare(const plb_score_problem &p, Task &t) {
+    if (p.kind < PLB_KIND_PNP || p.kind > PLB_KIND_HOMOGRAPHY) {
+        g_err = "unknown problem kind";
+        return PLB_ERR_ARG;
+    }
+    if (p.tangent_sampson && p.kind != PLB_KIND_RELPOSE) {
+        g_err = "tangent_sampson is a relative-pose option";
+        return PLB_ERR_ARG;
+    }
+    if ((p.n > 0 && (!p.a || !p.b)) || (p.m > 0 && (!p.models || !p.scores || !p.num_inliers))) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    if (!std::isfinite(p.sq_threshold)) {
+        g_err = "sq_threshold must be finite";
+        return PLB_ERR_ARG;
+    }
+    uint64_t mn = 0;
+    if (p.m >= (1ull << 31) || __builtin_mul_overflow(p.m, p.n, &mn) || mn > SIZE_MAX) {
+        g_err = "too many models";
+        return PLB_ERR_ARG;
+    }
+    if (p.n > (1u << 26)) {
+        g_err = "too many correspondences";
+        return PLB_ERR_ARG;
+    }
+    t.kind = p.kind == PLB_KIND_PNP ? KIND_PNP : p.kind == PLB_KIND_RELPOSE ? KIND_RELPOSE
+                                              : p.kind == PLB_KIND_FUNDAMENTAL ? KIND_FUND : KIND_HOMOG;
+    if (p.tangent_sampson) {
+        if (int r = camera_dev(&p.camera1, &t.cam_a)) return r;
+        if (int r = camera_dev(&p.camera2, &t.cam_b)) return r;
+        t.kind = KIND_RELPOSE_TS;
+        t.pre_mode = 2;
+    }
+    t.score = true;
+    t.a = p.a;
+    t.b = p.b;
+    t.n = (size_t)p.n;
+    t.m = (size_t)p.m;
+    t.models = p.models;
+    t.sq_thr = p.sq_threshold;
+    t.scores = p.scores;
+    t.counts = p.num_inliers;
+    t.inliers = p.m > 0 && p.n > 0 ? p.inliers : nullptr;
+    return PLB_OK;
+}
+// Every problem checked before any device call; on failure every status gets the code and nothing else is written.
+static int score_batch_prepare(plb_score_problem *problems, size_t count, std::vector<Task> &tasks) {
+    tasks.assign(count, Task());
+    for (size_t i = 0; i < count; ++i)
+        if (int r = score_prepare(problems[i], tasks[i])) {
+            for (size_t j = 0; j < count; ++j) problems[j].status = r;
+            return r;
+        }
+    return PLB_OK;
+}
+static int score_batch_run(plb_score_problem *problems, std::vector<Task> &tasks, const std::vector<int> &devs,
+                           int streams) {
+    std::vector<int> dev_of(tasks.size(), -1);
+    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
+    for (size_t i = 0; i < tasks.size(); ++i) problems[i].status = rc;
+    return rc;
+}
+int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    if (count == 0) return PLB_OK;
+    if (!problems) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    std::vector<Task> tasks;
+    if (int r = score_batch_prepare(problems, count, tasks)) return r;
+    auto fail_all = [&](int rc, const char *msg) {
+        g_err = msg;
+        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
+        return rc;
+    };
+    if (n_gpus < -1) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    const int have = plb_device_count();
+    if (have == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    if (n_gpus > have) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    return score_batch_run(problems, tasks, batch_devices(n_gpus, have), streams_per_gpu);
+}
+// The same on the calling thread's device with everything sized by n or m in its memory: k_ingest gathers a / b into the
+// engine's input buffer, k_score reads the caller's models and writes the caller's records and masks.
+int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    if (count == 0) return PLB_OK;
+    if (!problems) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    auto fail_all = [&](int rc, const std::string &msg) {
+        g_err = msg;
+        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
+        return rc;
+    };
+    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
+    std::vector<Task> tasks;
+    if (int r = score_batch_prepare(problems, count, tasks)) return r;
+    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    Engine &E = *engine();
+    if (int rc = E.init()) return fail_all(rc, g_err);
+    const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
+    for (size_t i = 0; i < count; ++i) {
+        const Task &t = tasks[i];
+        auto bad = [&](const char *what) { return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": " + what); };
+        if (t.n > 0)
+            for (const void *q : {(const void *)t.a, (const void *)t.b}) {
+                if (!device_memory(q, E.device)) return bad("a / b must be device memory of the current device");
+                if ((uintptr_t)q % elem) return bad("a / b are not aligned to the dtype");
+            }
+        if (t.m > 0)
+            for (const void *q : {(const void *)t.models, (const void *)t.scores, (const void *)t.counts}) {
+                if (!device_memory(q, E.device))
+                    return bad("models / scores / num_inliers must be device memory of the current device");
+                if ((uintptr_t)q % sizeof(double)) return bad("models / scores / num_inliers are not 8-byte aligned");
+            }
+        if (t.inliers && !device_memory(t.inliers, E.device))
+            return bad("inliers must be NULL or device memory of the current device");
+    }
+    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
+    for (Task &t : tasks) {
+        t.dev_io = true;
+        t.f32 = dtype == PLB_DTYPE_F32;
+        t.ready = E.ev_in;
+    }
+    return score_batch_run(problems, tasks, {E.device}, streams);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {

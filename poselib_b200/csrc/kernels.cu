@@ -6,7 +6,7 @@
 //                      minimal solvers of a round, one thread per minimal sample (the 5-point solver in phases)
 //   k_score_tiled / k_screen
 //                      MSAC scoring of every model of a round over all correspondences (exact fp64 / fp32 screening)
-//   k_score            exact scoring of explicit models (initial models)
+//   k_score            exact scoring (and masks) of explicit models: initial models, plb_score_batch
 //   k_confirm          exact rescoring of the fast-mode candidates of a round
 //   k_lm<KIND, CAM>    Levenberg-Marquardt refit (LO step + final polish): one cluster per job, cluster-wide reductions
 //                      of the normal equations, scalar LM logic on thread 0; CAM refines PnP camera parameters too
@@ -376,6 +376,19 @@ template <int KIND> PLB_DEV void corr_bearings(const double *v, d3 &b1, d3 &b2) 
     }
 }
 PLB_DEV bool cheirality_ctx(const double *C, d3 b1, d3 b2) { return cheirality_ok(C + 9, C + 13, b1, b2, 0.01); }
+// The PnP mask keeps its own formula on purpose (DESIGN.md §3): the reference's get_inliers (robust/utils.cc:374-383)
+// divides, r2 = |Z.hnormalized() - x|^2 with Z = R*X + t, and tests Z(2) > 0 after the threshold, while its scorer
+// (under_thr) multiplies by 1/z2 and skips z2 <= 0 first.  The two give different bits.  C: the PnP model context;
+// v(j): value j of the correspondence as load_corr lays it out (x.x x.y X.x X.y X.z).
+template <class V> PLB_DEV bool pnp_get_inlier(const double *C, V v, double sq_thr) {
+    const double X0 = v(2), X1 = v(3), X2 = v(4);
+    const double z0 = C[0] * X0 + C[1] * X1 + C[2] * X2 + C[3];
+    const double z1 = C[4] * X0 + C[5] * X1 + C[6] * X2 + C[7];
+    const double z2 = C[8] * X0 + C[9] * X1 + C[10] * X2 + C[11];
+    const double d0 = z0 / z2 - v(0), d1 = z1 / z2 - v(1);
+    const double r2 = d0 * d0 + d1 * d1;
+    return r2 < sq_thr && z2 > 0.0;
+}
 template <int KIND> PLB_DEV bool is_inlier(const double *C, const double *v, double sq_thr) {
     double r2;
     if (!under_thr<KIND>(C, v, sq_thr, r2)) return false;
@@ -400,9 +413,11 @@ template <int TM> struct ScoreRed {
     double s[SCORE_WARPS][TM];
     uint32_t c[SCORE_WARPS][TM];
 };
-template <int KIND, int TM>
+// MASK: also write model i's decision on correspondence k to mask[i * mask_stride + k] (get_inliers: is_inlier, and
+// pnp_get_inlier for PnP), from the correspondence loaded for the score.
+template <int KIND, int TM, bool MASK = false>
 PLB_DEV void msac_score(const ProblemDev &P, const double (&ctx)[TM][CTX_MAX], int tm, ScoreRed<TM> &red,
-                        uint32_t *counts, double *scores) {
+                        uint32_t *counts, double *scores, char *mask = nullptr, long long mask_stride = 0) {
     const int tid = threadIdx.x, lane = tid & 31;
     const int n = P.n;
     const double sq_thr = P.sq_thr;
@@ -422,7 +437,7 @@ PLB_DEV void msac_score(const ProblemDev &P, const double (&ctx)[TM][CTX_MAX], i
         // Without cheirality a model under the threshold is an inlier and is accumulated at once; the relpose kinds
         // collect the models under the threshold first, so that the bearings are computed once for the tile.
         double r2u[TM];
-        unsigned under = 0;
+        unsigned under = 0, dec = 0;
 #pragma unroll
         for (int i = 0; i < TM; ++i) {
             double r2;
@@ -433,6 +448,7 @@ PLB_DEV void msac_score(const ProblemDev &P, const double (&ctx)[TM][CTX_MAX], i
                 } else {
                     ++cnt[i];
                     sc[i] += r2;
+                    dec |= 1u << i;
                 }
             }
         }
@@ -448,6 +464,16 @@ PLB_DEV void msac_score(const ProblemDev &P, const double (&ctx)[TM][CTX_MAX], i
                     ++cnt[i];
                     sc[i] += r2u[i];
                 }
+            }
+        }
+        if constexpr (MASK) {
+            if constexpr (kind_is_relpose(KIND)) dec = under;
+#pragma unroll
+            for (int i = 0; i < TM; ++i) {
+                if (i >= tm) break;
+                bool in = (dec >> i) & 1u;
+                if constexpr (KIND == KIND_PNP) in = pnp_get_inlier(ctx[i], [&](int j) { return v[j]; }, sq_thr);
+                mask[i * mask_stride + k] = in ? 1 : 0;
             }
         }
     }
@@ -847,28 +873,68 @@ __device__ __forceinline__ int seg_models(const HypOut &out, int a) {
     return c < cap ? c : cap;
 }
 
-// Score kernel: persistent grid of 256-thread CTAs, one CTA scores one model at a time over all correspondences of
-// the model's problem.
-template <int KIND>
-__global__ void __launch_bounds__(SCORE_THREADS, 4)
-    k_score(const ProblemDev *__restrict__ probs, const double *__restrict__ models, const int *__restrict__ model_prob,
-            int n_models, uint32_t *counts, double *scores) {
-    constexpr int MSZ = kind_model_size(KIND);
-    __shared__ ScoreRed<1> red;
-    for (int m = blockIdx.x; m < n_models; m += gridDim.x) {
-        const ProblemDev P = probs[model_prob[m]];
-        double mdl[MSZ];
-#pragma unroll
-        for (int k = 0; k < MSZ; ++k) mdl[k] = models[(size_t)m * MSZ + k];
-        cta_score<KIND>(P, mdl, red, counts + m, scores + m);
-    }
-}
-
 // Tiled score kernel of the round path: CTA (x, a) scores tiles of SCORE_TM models of active problem a (model constants
 // are broadcast reads from shared memory), which divides the L2 -> SM traffic of one CTA per model by the tile size.
 constexpr int SCORE_TM = 4;
 // the tangent-Sampson kind carries 18 values per correspondence: two models per tile keep it inside 128 registers
 template <int KIND> constexpr __host__ __device__ int score_tm() { return KIND == KIND_RELPOSE_TS ? 2 : SCORE_TM; }
+
+// Explicit-model scorer: a persistent 1D grid of 256-thread CTAs walks the (problem, first model, tile size) items of
+// the descriptors — descriptor d owns tiles [tile0, tile0 + ceil(m / tm_max)), tile j of it models j*tm_max .. — and
+// scores each tile with msac_score, every correspondence loaded once per tile.  tm_max is score_tm<KIND>() or 1 (the
+// initial models); a record's bits depend on neither.  MASK: the descriptors' masks are written in the same pass.
+template <int KIND, bool MASK>
+__global__ void __launch_bounds__(SCORE_THREADS, 2)
+    k_score(const ProblemDev *__restrict__ probs, const ScoreDesc *__restrict__ descs, int n_desc, long long n_tiles,
+            int tm_max) {
+    constexpr int MSZ = kind_model_size(KIND);
+    constexpr int TM = score_tm<KIND>();
+    __shared__ double ctx[TM][CTX_MAX];
+    __shared__ ScoreRed<TM> red;
+    __shared__ uint32_t cnt[TM];
+    __shared__ double sc[TM];
+    // the tile's item, read back from shared memory after the scoring pass rather than kept live through it (the
+    // 128-register budget of the pass has no room for it)
+    __shared__ const ScoreDesc *item;
+    __shared__ long long item_m0;
+    __shared__ int item_tm;
+    const int tid = threadIdx.x;
+    for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        if (tid == 0) {
+            int lo = 0, hi = n_desc - 1; // the last descriptor with tile0 <= t
+            while (lo < hi) {
+                const int mid = (lo + hi + 1) >> 1;
+                if (descs[mid].tile0 <= t) lo = mid;
+                else hi = mid - 1;
+            }
+            const long long m0 = (t - descs[lo].tile0) * tm_max;
+            item = descs + lo;
+            item_m0 = m0;
+            item_tm = (int)(descs[lo].m - m0 < tm_max ? descs[lo].m - m0 : tm_max);
+        }
+        __syncthreads();
+        {
+            const ScoreDesc &D = *item;
+            const long long m0 = item_m0;
+            const int tm = item_tm;
+            if (tid < tm) {
+                double mdl[MSZ];
+#pragma unroll
+                for (int k = 0; k < MSZ; ++k) mdl[k] = D.models[(size_t)(m0 + tid) * MSZ + k];
+                model_ctx<KIND>(mdl, ctx[tid]);
+            }
+            __syncthreads();
+            msac_score<KIND, TM, MASK>(probs[D.pidx], ctx, tm, red, cnt, sc,
+                                       MASK ? D.mask + m0 * D.mask_stride : nullptr, D.mask_stride);
+        }
+        if (tid < item_tm) { // msac_score ends with a barrier; thread tid wrote cnt[tid], sc[tid]
+            if (item->counts) item->counts[item_m0 + tid] = cnt[tid];
+            else item->counts32[item_m0 + tid] = cnt[tid];
+            item->scores[item_m0 + tid] = sc[tid];
+        }
+        __syncthreads(); // item is rewritten for the next tile
+    }
+}
 template <int KIND>
 __global__ void __launch_bounds__(SCORE_THREADS, 2)
     k_score_tiled(const RoundDesc R, HypOut out) {
@@ -1657,14 +1723,38 @@ void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, cons
 // ============================================================================================================
 // explicit model scoring
 // ============================================================================================================
+int score_tile_models(int kind) {
+    int tm = 0;
+    with_kind(kind, [&](auto K) { tm = score_tm<K>(); });
+    return tm;
+}
+void launch_score_models(int kind, bool mask, const ProblemDev *probs, const ScoreDesc *descs_dev, int n_desc,
+                         long long n_tiles, int tm_max, cudaStream_t stream) {
+    if (n_desc <= 0 || n_tiles <= 0) return;
+    const long long blocks = n_tiles < 8LL * sm_count() ? n_tiles : 8LL * sm_count();
+    with_kind(kind, [&](auto K) {
+        if (mask)
+            k_score<K, true><<<(unsigned)blocks, SCORE_THREADS, 0, stream>>>(probs, descs_dev, n_desc, n_tiles, tm_max);
+        else
+            k_score<K, false><<<(unsigned)blocks, SCORE_THREADS, 0, stream>>>(probs, descs_dev, n_desc, n_tiles, tm_max);
+    });
+}
+// One-model descriptors of a device list of (model, problem index) pairs.
+__global__ void k_score_list(const double *models, const int *model_prob, int n_models, int msz, uint32_t *counts,
+                             double *scores, ScoreDesc *descs) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= n_models) return;
+    descs[m] = {models + (size_t)m * msz, nullptr, scores + m, nullptr, 0, m, 1, model_prob[m], 0, counts + m};
+}
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
                          uint32_t *counts, double *scores, cudaStream_t stream) {
     if (n_models <= 0) return;
-    int blocks = n_models;
-    if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
-    with_kind(kind, [&](auto K) {
-        k_score<K><<<blocks, SCORE_THREADS, 0, stream>>>(probs, models, model_prob, n_models, counts, scores);
-    });
+    ScoreDesc *descs = nullptr;
+    if (cudaMallocAsync(&descs, sizeof(ScoreDesc) * n_models, stream) != cudaSuccess) return;
+    k_score_list<<<(n_models + 255) / 256, 256, 0, stream>>>(models, model_prob, n_models, kind_model_size(kind), counts,
+                                                              scores, descs);
+    launch_score_models(kind, false, probs, descs, n_models, n_models, 1, stream);
+    cudaFreeAsync(descs, stream);
 }
 
 // ============================================================================================================
@@ -1682,18 +1772,12 @@ __global__ void k_inlier_mask(const ProblemDev *__restrict__ probs, const MaskDe
     for (int k = 0; k < MSZ; ++k) mdl[k] = D.model[k];
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= P.n) return;
+    double C[kind_ctx_size(KIND)];
+    model_ctx<KIND>(mdl, C);
     if constexpr (KIND == KIND_PNP) {
-        // The PnP mask keeps its own formula on purpose (DESIGN.md §3): the reference's mask (robust/utils.cc:374-383)
-        // divides, r2 = |Z.hnormalized() - x|^2 with Z = R*X + t, and tests Z(2) > 0 after the threshold, while its
-        // scorer (under_thr) multiplies by 1/z2 and skips z2 <= 0 first.  The two give different bits.
-        const m3 R = quat_to_rot(mdl);
-        const d3 Z = mvec(R, mk(P.p[2][k], P.p[3][k], P.p[4][k])) + mk(mdl[4], mdl[5], mdl[6]);
-        const double d0 = Z.x / Z.z - P.p[0][k], d1 = Z.y / Z.z - P.p[1][k];
-        const double r2 = d0 * d0 + d1 * d1;
-        mask[k] = (r2 < sq_thr && Z.z > 0.0) ? 1 : 0;
+        mask[k] = pnp_get_inlier(C, [&](int j) { return P.p[j][k]; }, sq_thr) ? 1 : 0;
     } else { // the scorer's test (tangent Sampson: robust/utils.cc:541-569)
-        double C[kind_ctx_size(KIND)], v[kind_corr_size(KIND)];
-        model_ctx<KIND>(mdl, C);
+        double v[kind_corr_size(KIND)];
         load_corr<KIND>(P, k, v);
         mask[k] = is_inlier<KIND>(C, v, sq_thr) ? 1 : 0;
     }

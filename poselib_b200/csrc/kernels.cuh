@@ -238,6 +238,22 @@ struct ScatterDesc {
     int n;
 };
 
+// Explicit models of one problem for k_score: m models (stride kind_model_size), records to counts[0..m) / scores[0..m),
+// and with masks model i's decision on correspondence k to mask[i * mask_stride + k].  The descriptors of a launch are
+// ordered by tile0, the first of their ceil(m / tm_max) tiles in the launch's tile list.
+struct ScoreDesc {
+    const double *models;
+    long long *counts;
+    double *scores;
+    char *mask;
+    long long mask_stride;
+    long long tile0;
+    long long m;
+    int pidx;
+    int reserved;
+    uint32_t *counts32; // when counts is null: the counts as uint32 (the round's record layout)
+};
+
 // ---- launchers (all asynchronous on `stream`) --------------------------------------------------------------
 // normalize_points for n_desc problems (descriptors in device memory), one CTA each.
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream);
@@ -253,7 +269,13 @@ void launch_qrows(const TransposeDesc *descs_dev, int n_desc, int max_n_pad, cud
 // screening constants of the round's models.
 void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode, int max_n_pad, float *fctx,
                        cudaStream_t stream, cudaEvent_t ev_between = nullptr);
-// Exact fp64 scoring of an explicit list of n_models models (stride MSZ) with problem indices.
+// Exact fp64 scoring of explicit models: the n_tiles tiles of tm_max (score_tile_models(kind) or 1) models of the n_desc
+// descriptors (device memory); mask: every descriptor has a mask, written in the same pass.
+int score_tile_models(int kind);
+void launch_score_models(int kind, bool mask, const ProblemDev *probs, const ScoreDesc *descs_dev, int n_desc,
+                         long long n_tiles, int tm_max, cudaStream_t stream);
+// The same over a device list of n_models models (stride kind_model_size) with their problem indices, records in the
+// round's layout (uint32 counts), in one-model tiles.
 void launch_score_models(int kind, const ProblemDev *probs, const double *models, const int *model_prob, int n_models,
                          uint32_t *counts, double *scores, cudaStream_t stream);
 // LM refinement: one thread-block cluster per job.  models_in: n_jobs * 9 doubles.  refine_camera (KIND_PNP,
