@@ -295,6 +295,19 @@ int plb_refine_homography_weighted(const double *x1_xy, const double *x2_xy, siz
                                    const plb_bundle_opt *opt, double bundle_stats_out[3], const double *weights);
 
 /* ---- batch of independent problems (BASELINE config 5); sharded by the caller across GPUs ---------- */
+/* Every batch call below (plb_ransac_batch[_multi], plb_estimate_batch[_device], plb_refine_batch[_device],
+ * plb_score_batch[_device]) checks its arguments in one order, before any copy or launch:
+ *   1. count 0 -> PLB_OK, nothing written;
+ *   2. problems NULL -> PLB_ERR_ARG, nothing written;
+ *   3. device forms: a dtype other than PLB_DTYPE_F64 / PLB_DTYPE_F32 -> PLB_ERR_ARG;
+ *   4. every problem in order, by the rules its call lists; the first failure's code;
+ *   5. n_gpus < -1 -> PLB_ERR_ARG (plb_ransac_batch_multi: n_gpus < 0);
+ *   6. no device -> PLB_ERR_CUDA;
+ *   7. n_gpus above the device count -> PLB_ERR_ARG;
+ *   8. resident correspondences on a device the call does not use -> PLB_ERR_ARG; device forms: a pointer of a problem
+ *      that is not device (or managed) memory of the calling thread's device, or is misaligned -> PLB_ERR_ARG.
+ * A failure in steps 3-8 writes its code into every status and nothing else: no model, stats, counters, camera, mask,
+ * score or count changes.  After the checks, every status receives the call's result. */
 enum { PLB_KIND_PNP = 0, PLB_KIND_RELPOSE = 1, PLB_KIND_FUNDAMENTAL = 2, PLB_KIND_HOMOGRAPHY = 3 };
 typedef struct plb_problem {
     int32_t kind;             /* PLB_KIND_* */
@@ -312,7 +325,8 @@ typedef struct plb_problem {
     int32_t resident;         /* > 0: handle from plb_resident_create, a/b are ignored (points already in HBM) */
 } plb_problem;
 /* Runs ransac_{pnp,relpose,fundamental,homography} on every problem on the calling thread's device; `streams` lock-step
- * groups of problems are in flight at once. */
+ * groups of problems are in flight at once.  An unknown kind, a / b NULL with n > 0 (and no resident handle), or a
+ * resident handle that is not one of plb_resident_create's for the problem's kind -> PLB_ERR_ARG. */
 int plb_ransac_batch(plb_problem *problems, size_t count, int streams);
 /* The same over the first n_gpus CUDA devices of the process (0 = all of them), in one call from one host thread:
  * problems are partitioned by size x expected iterations, every device runs streams_per_gpu groups at once, results
@@ -343,7 +357,11 @@ typedef struct plb_estimate_problem {
     int32_t status;           /* out */
     int32_t reserved2;
 } plb_estimate_problem;
-/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device). */
+/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device).
+ * Each problem is checked by its single entry point's rules: an unknown kind, or a / b NULL with n > 0 -> PLB_ERR_ARG;
+ * a camera the kind reads (camera1 for PnP, both for relative pose) outside the ten models -> PLB_ERR_NYI;
+ * tangent_sampson with a non-empty refine_intrinsics selection in either camera -> PLB_ERR_NYI, as the batch returns no
+ * relative-pose cameras. */
 int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
 /* plb_estimate_batch(problems, count, -1, streams) with the correspondences and masks in device memory, for callers whose
  * matches are already on the GPU.  Everything else (kinds, cameras, options, model, stats, counters, status, camera1)
@@ -355,10 +373,9 @@ int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus,
  *  - inliers: NULL or n bytes of device memory on the same device; receives 0 / 1 as the host call writes them.
  *  - stream: a cudaStream_t of that device (NULL = the legacy default stream).  No input is read before the work queued
  *    on `stream` ahead of the call has finished; when the call returns, every device write it made is complete.
- * Checked before any copy or launch, with every status set and nothing else written on failure: NULL problems or an
- * unknown dtype -> PLB_ERR_ARG (before the device check); no device -> PLB_ERR_CUDA; a / b / inliers of a problem with
- * n > 0 that are not device memory of the current device (pageable or page-locked host memory, another GPU), or a / b
- * misaligned for the dtype -> PLB_ERR_ARG.  counters.h2d_bytes holds no correspondences and d2h_bytes no masks. */
+ * Pointers are checked for a problem with n > 0: a / b / inliers that are not device memory of the current device
+ * (pageable or page-locked host memory, another GPU), or a / b misaligned for the dtype -> PLB_ERR_ARG.
+ * counters.h2d_bytes holds no correspondences and d2h_bytes no masks. */
 enum { PLB_DTYPE_F64 = 0, PLB_DTYPE_F32 = 1 };
 int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams);
 
@@ -376,11 +393,9 @@ int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int 
  *   PLB_REFINER_FUNDAMENTAL          plb_refine_fundamental[_weighted]
  *   PLB_REFINER_HOMOGRAPHY           plb_refine_homography[_weighted]
  * Cameras a refiner does not read are ignored, and parameters the single call leaves alone stay untouched.
- * Every problem is checked before any device call, by its single entry point's rules; on failure every status gets the
- * code and nothing else is written: NULL problems, an unknown refiner, or a / b NULL with n > 0 -> PLB_ERR_ARG; a camera
- * the refiner reads outside the ten models -> PLB_ERR_NYI; PLB_REFINER_RELPOSE_CAMERAS with a non-empty refine_intrinsics
- * selection -> PLB_ERR_NYI; n_gpus < -1 -> PLB_ERR_ARG; no device -> PLB_ERR_CUDA; n_gpus above the device count ->
- * PLB_ERR_ARG. */
+ * Every problem is checked by its single entry point's rules: an unknown refiner, or a / b NULL with n > 0 ->
+ * PLB_ERR_ARG; a camera the refiner reads outside the ten models -> PLB_ERR_NYI; PLB_REFINER_RELPOSE_CAMERAS with a
+ * non-empty refine_intrinsics selection -> PLB_ERR_NYI. */
 enum {
     PLB_REFINER_BUNDLE = 0,
     PLB_REFINER_BUNDLE_IMAGE = 1,
@@ -412,9 +427,8 @@ int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int
  * takes them: device (or managed) memory of the calling thread's device, contiguous arrays of `dtype` aligned to it
  * (PLB_DTYPE_F32: `const float *` cast into the `const double *` fields).  They are only read, after the work queued on
  * `stream` ahead of the call has finished; fp32 values are widened exactly, so a float call gives the results of the
- * double call on the widened values.  Models, stats and cameras come back in the host array.  An unknown dtype ->
- * PLB_ERR_ARG; a / b / weights of a problem with n > 0 that are not device memory of the current device, or misaligned
- * for the dtype -> PLB_ERR_ARG, with every status set and nothing else written. */
+ * double call on the widened values.  Models, stats and cameras come back in the host array.  A / b / weights of a
+ * problem with n > 0 that are not device memory of the current device, or misaligned for the dtype -> PLB_ERR_ARG. */
 int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams);
 
 /* Scores and inlier masks of given models (robust/utils.h:40-87), for callers that check matches against models they
@@ -454,19 +468,17 @@ typedef struct plb_score_problem {
 /* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device);
  * streams_per_gpu groups of problems are in flight on each device.  Every pointer is host memory.  Each problem's
  * outputs are the same bits whatever else is in the batch and for any n_gpus / streams.
- * Checked before any device call; on failure every status gets the code and nothing else is written: NULL problems, an
- * unknown kind, tangent_sampson on another kind, a / b NULL with n > 0, models / scores / num_inliers NULL with m > 0, a
- * non-finite sq_threshold, m >= 2^31, n > 2^26 or m * n overflowing -> PLB_ERR_ARG; a camera (tangent_sampson) outside
- * the ten models -> PLB_ERR_NYI; n_gpus < -1 -> PLB_ERR_ARG; no device -> PLB_ERR_CUDA; n_gpus above the device count ->
- * PLB_ERR_ARG. */
+ * Each problem is checked: an unknown kind, tangent_sampson on another kind, a / b NULL with n > 0, models / scores /
+ * num_inliers NULL with m > 0, a non-finite sq_threshold, m >= 2^31, n > 2^26 or m * n overflowing -> PLB_ERR_ARG; a
+ * camera (tangent_sampson) outside the ten models -> PLB_ERR_NYI. */
 int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
 /* plb_score_batch(problems, count, -1, streams) with a, b, models, scores, num_inliers and inliers in device (or managed)
  * memory of the calling thread's device: a / b contiguous arrays of `dtype` aligned to it (PLB_DTYPE_F32: `const float *`
  * cast into the `const double *` fields; widened exactly, so a float call gives the double call's results on the widened
  * values), models fp64.  Nothing sized by n or m crosses PCIe.  Inputs are read after the work queued on `stream` ahead of
- * the call; when the call returns, every device write it made is complete.  Besides the checks above: an unknown dtype, or
- * a pointer of a problem that is not device memory of the current device or is misaligned (a / b: the dtype; models,
- * scores, num_inliers: 8 bytes) -> PLB_ERR_ARG, checked as plb_estimate_batch_device checks its pointers. */
+ * the call; when the call returns, every device write it made is complete.  A pointer of a problem that is not device
+ * memory of the current device or is misaligned (a / b: the dtype; models, scores, num_inliers: 8 bytes) ->
+ * PLB_ERR_ARG. */
 int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams);
 
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers

@@ -619,6 +619,42 @@ def _estimate_results(arr, problems, masks):
     return out
 
 
+def _device_form(fn, what, points, models=(), stream=None):
+    """The checks and set-up of a device form: `points` (a, b and weights, named `what`) must be CUDA torch tensors of
+    one device and one dtype, float32 or float64, and `models` CUDA float64 tensors on the same device.  Selects that
+    device and returns (device, PLB_DTYPE_*, `stream` as a torch.cuda.Stream [None: the device's current stream]), or
+    None when there are no points."""
+    import torch
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in [*points, *models]):
+        raise TypeError(f"{fn}: {what}{' and models' if models else ''} must be CUDA torch tensors")
+    if not points:
+        return None
+    dev, dt = points[0].device, points[0].dtype
+    if any(t.device != dev for t in [*points, *models]):
+        raise ValueError(f"{fn}: every tensor must be on {dev} (shard the batch by device)")
+    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
+    if dt not in dtypes or any(t.dtype != dt for t in points):
+        raise TypeError(f"{fn}: {what} must share one dtype, torch.float32 or torch.float64")
+    if any(t.dtype != torch.float64 for t in models):
+        raise TypeError(f"{fn}: models must be torch.float64")
+    set_device(dev.index)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev)
+    elif not isinstance(stream, torch.cuda.Stream):
+        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    return dev, dtypes[dt], stream
+
+
+def _device_points(fn, i, p, b_dim):
+    """Problem i's a [n,2] and b [n,b_dim] as contiguous tensors."""
+    a, b = p["a"].contiguous(), p["b"].contiguous()
+    n = a.shape[0]
+    if tuple(a.shape) != (n, 2) or tuple(b.shape) != (n, b_dim):
+        raise ValueError(f"{fn}: problem {i}: a must be [n,2] and b [n,{b_dim}], got {tuple(a.shape)} and "
+                         f"{tuple(b.shape)}")
+    return a, b
+
+
 def estimate_batch_device(problems, streams=8, stream=None):
     """estimate_batch (n_gpus=-1) on correspondences that are already on the GPU (plb_estimate_batch_device).
     problems: the dicts estimate_batch takes, with a / b as CUDA torch tensors [n,2] / [n,3] ([n,2] for the 2D-2D kinds),
@@ -627,22 +663,11 @@ def estimate_batch_device(problems, streams=8, stream=None):
     Returns the dicts of estimate_batch, with `inliers` a CUDA torch.bool tensor of length n (the masks of one call are
     views of one allocation)."""
     import torch
-    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
-    tensors = [t for p in problems for t in (p["a"], p["b"])]
-    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
-        raise TypeError("estimate_batch_device: a and b must be CUDA torch tensors")
-    if not tensors:
+    form = _device_form("estimate_batch_device", "a and b", [t for p in problems for t in (p["a"], p["b"])],
+                        stream=stream)
+    if form is None:
         return []
-    dev, dt = tensors[0].device, tensors[0].dtype
-    if any(t.device != dev for t in tensors):
-        raise ValueError(f"estimate_batch_device: every tensor must be on {dev} (shard the batch by device)")
-    if dt not in dtypes or any(t.dtype != dt for t in tensors):
-        raise TypeError("estimate_batch_device: a and b must share one dtype, torch.float32 or torch.float64")
-    set_device(dev.index)
-    if stream is None:
-        stream = torch.cuda.current_stream(dev)
-    elif not isinstance(stream, torch.cuda.Stream):
-        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    dev, dtype, stream = form
     count = len(problems)
     arr = (EstimateProblem * count)()
     keep = []
@@ -652,17 +677,13 @@ def estimate_batch_device(problems, streams=8, stream=None):
         masks = list(torch.zeros(sum(sizes), dtype=torch.bool, device=dev).split(sizes))
         for i, p in enumerate(problems):
             q = arr[i]
-            a, b = p["a"].contiguous(), p["b"].contiguous()
+            a, b = _device_points("estimate_batch_device", i, p, 3 if p["kind"] == "pnp" else 2)
             npts = sizes[i]
-            b_dim = 3 if p["kind"] == "pnp" else 2
-            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
-                raise ValueError(f"estimate_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
-                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
             keep.append((a, b))
             _fill_estimate_problem(q, p, npts)
             q.a, q.b = C.cast(C.c_void_p(a.data_ptr()), _P), C.cast(C.c_void_p(b.data_ptr()), _P)
             q.inliers = C.cast(C.c_void_p(masks[i].data_ptr() if npts else None), C.c_char_p)
-    _check(_lib.plb_estimate_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+    _check(_lib.plb_estimate_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
                                           int(streams)))
     return _estimate_results(arr, problems, masks)
 
@@ -724,22 +745,11 @@ def refine_batch_device(problems, stream=None, streams=8):
     on that device and reads the inputs after the work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle;
     default: the device's current stream).  Returns the dicts of refine_batch."""
     import torch
-    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
-    tensors = [t for p in problems for t in (p["a"], p["b"], p.get("weights")) if t is not None]
-    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
-        raise TypeError("refine_batch_device: a, b and weights must be CUDA torch tensors")
-    if not tensors:
+    form = _device_form("refine_batch_device", "a, b and weights",
+                        [t for p in problems for t in (p["a"], p["b"], p.get("weights")) if t is not None], stream=stream)
+    if form is None:
         return []
-    dev, dt = tensors[0].device, tensors[0].dtype
-    if any(t.device != dev for t in tensors):
-        raise ValueError(f"refine_batch_device: every tensor must be on {dev} (shard the batch by device)")
-    if dt not in dtypes or any(t.dtype != dt for t in tensors):
-        raise TypeError("refine_batch_device: a, b and weights must share one dtype, torch.float32 or torch.float64")
-    set_device(dev.index)
-    if stream is None:
-        stream = torch.cuda.current_stream(dev)
-    elif not isinstance(stream, torch.cuda.Stream):
-        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    _, dtype, stream = form
     count = len(problems)
     arr = (RefineProblem * count)()
     keep = []
@@ -747,18 +757,14 @@ def refine_batch_device(problems, stream=None, streams=8):
     with torch.cuda.stream(stream):  # any copy .contiguous() makes is ordered before the call's reads
         for i, p in enumerate(problems):
             q = arr[i]
-            a, b = p["a"].contiguous(), p["b"].contiguous()
+            a, b = _device_points("refine_batch_device", i, p, 3 if p["refiner"] in ("bundle", "bundle_image") else 2)
             npts = a.shape[0]
-            b_dim = 3 if p["refiner"] in ("bundle", "bundle_image") else 2
-            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
-                raise ValueError(f"refine_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
-                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
             w = p.get("weights")
             w = w.contiguous().reshape(-1) if w is not None and w.numel() == npts else None
             keep.append((a, b, w))
             _fill_refine_problem(q, p, npts)
             q.a, q.b, q.weights = ptr(a), ptr(b), ptr(w)
-    _check(_lib.plb_refine_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+    _check(_lib.plb_refine_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
                                         int(streams)))
     return _refine_results(arr, problems)
 
@@ -823,25 +829,11 @@ def score_batch_device(problems, stream=None, streams=8):
     Returns the dicts of score_batch with CUDA tensors: scores (float64), num_inliers (int64) and inliers (bool [m,n] or
     None; the masks of one call are views of one zeroed allocation)."""
     import torch
-    dtypes = {torch.float64: DTYPE_F64, torch.float32: DTYPE_F32}
-    tensors = [t for p in problems for t in (p["a"], p["b"])]
-    models = [p["models"] for p in problems]
-    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors + models):
-        raise TypeError("score_batch_device: a, b and models must be CUDA torch tensors")
-    if not tensors:
+    form = _device_form("score_batch_device", "a and b", [t for p in problems for t in (p["a"], p["b"])],
+                        [p["models"] for p in problems], stream)
+    if form is None:
         return []
-    dev, dt = tensors[0].device, tensors[0].dtype
-    if any(t.device != dev for t in tensors + models):
-        raise ValueError(f"score_batch_device: every tensor must be on {dev} (shard the batch by device)")
-    if dt not in dtypes or any(t.dtype != dt for t in tensors):
-        raise TypeError("score_batch_device: a and b must share one dtype, torch.float32 or torch.float64")
-    if any(t.dtype != torch.float64 for t in models):
-        raise TypeError("score_batch_device: models must be torch.float64")
-    set_device(dev.index)
-    if stream is None:
-        stream = torch.cuda.current_stream(dev)
-    elif not isinstance(stream, torch.cuda.Stream):
-        stream = torch.cuda.ExternalStream(int(stream), device=dev)
+    dev, dtype, stream = form
     count = len(problems)
     arr = (ScoreProblem * count)()
     keep = []
@@ -862,12 +854,8 @@ def score_batch_device(problems, stream=None, streams=8):
         flat = torch.zeros(sum(sizes), dtype=torch.bool, device=dev).split(sizes)
         for i, p in enumerate(problems):
             q = arr[i]
-            a, b = p["a"].contiguous(), p["b"].contiguous()
+            a, b = _device_points("score_batch_device", i, p, 3 if p["kind"] == "pnp" else 2)
             npts = ns[i]
-            b_dim = 3 if p["kind"] == "pnp" else 2
-            if tuple(a.shape) != (npts, 2) or tuple(b.shape) != (npts, b_dim):
-                raise ValueError(f"score_batch_device: problem {i}: a must be [n,2] and b [n,{b_dim}], got "
-                                 f"{tuple(a.shape)} and {tuple(b.shape)}")
             mask = flat[i].view(ms[i], npts) if want[i] else None
             keep.append((a, b))
             _fill_score_problem(q, p, npts, ms[i])
@@ -875,7 +863,7 @@ def score_batch_device(problems, stream=None, streams=8):
             q.num_inliers = C.cast(C.c_void_p(counts[i].data_ptr() if ms[i] else None), C.POINTER(C.c_int64))
             q.inliers = C.cast(C.c_void_p(mask.data_ptr() if mask is not None and mask.numel() else None), C.c_char_p)
             out.append({"scores": scores[i], "num_inliers": counts[i], "inliers": mask})
-    _check(_lib.plb_score_batch_device(arr, C.c_size_t(count), dtypes[dt], C.c_void_p(stream.cuda_stream or None),
+    _check(_lib.plb_score_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
                                        int(streams)))
     for r, q in zip(out, arr):
         r["status"] = q.status

@@ -556,8 +556,11 @@ struct Task {
     plb_ransac_stats *stats_out = nullptr;
     plb_counters *cnt_out = nullptr;
     FinalPolish polish;
-    const Resident *res = nullptr;
-    bool skip = false; // nothing to run (estimate_* with too few points): the batch runner leaves it alone
+    std::shared_ptr<const Resident> res; // resident correspondences, held for the duration of the call
+    // Written by commit_task once the whole call has passed its checks (estimate_* only): `skip`, nothing to run (too
+    // few points), gets the default stats and counters; `reset_pose` resets the start pose to the identity (tangent
+    // Sampson, ransac.cc:159-160, even when score_initial_model is set).
+    bool skip = false, reset_pose = false;
     // normalize_points on the device before anything else (estimate_fundamental / estimate_homography, robust.cc:561,724):
     // 0 none, 1 scale only (real_focal_check keeps the principal point at the origin), 2 centroid + scale.  max_error and
     // the polish loss scale are then given in the units of the raw points and divided by the scale once it is known
@@ -1788,9 +1791,8 @@ static int run_group(int kind, std::vector<Task *> &tasks) {
 // Single-problem convenience used by the plb_ransac_* / plb_estimate_* entry points.
 static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, const plb_ransac_opt &opt,
                       double max_error, int rfc, double *model, char *inliers, plb_ransac_stats *stats_out,
-                      plb_counters *cnt_out, const FinalPolish &polish, const Resident *res = nullptr,
-                      int pre_mode = 0, const CamDev *cam_a = nullptr, const CamDev *cam_b = nullptr,
-                      double pre_scale = 1.0) {
+                      plb_counters *cnt_out, const FinalPolish &polish, int pre_mode = 0,
+                      const CamDev *cam_a = nullptr, const CamDev *cam_b = nullptr, double pre_scale = 1.0) {
     Task t;
     t.pre_mode = pre_mode;
     t.pre_scale = pre_scale;
@@ -1808,7 +1810,6 @@ static int run_ransac(int kind, const double *a, const double *b, size_t n_pts, 
     t.stats_out = stats_out;
     t.cnt_out = cnt_out;
     t.polish = polish;
-    t.res = res;
     std::vector<Task *> v{&t};
     return run_group(kind, v);
 }
@@ -2013,8 +2014,8 @@ int plb_ransac_relpose_cameras(const double *x1, const double *x2, size_t n, con
     if (int r = camera_dev(camera2, &c2)) return r;
     pose[0] = 1.0; // :159-160
     for (int i = 1; i < 7; ++i) pose[i] = 0.0;
-    return run_ransac(KIND_RELPOSE_TS, x1, x2, n, *opt, max_error, 0, pose, inliers, stats, counters, FinalPolish(),
-                      nullptr, 2, &c1, &c2, 1.0);
+    return run_ransac(KIND_RELPOSE_TS, x1, x2, n, *opt, max_error, 0, pose, inliers, stats, counters, FinalPolish(), 2,
+                      &c1, &c2, 1.0);
 }
 int plb_ransac_fundamental(const double *x1, const double *x2, size_t n, const plb_ransac_opt *opt, double max_error,
                            int real_focal_check, double F[9], char *inliers, plb_ransac_stats *stats,
@@ -2030,23 +2031,8 @@ int plb_ransac_homography(const double *x1, const double *x2, size_t n, const pl
 }
 
 // ---- PoseLib/robust.cc estimate_* : pre-step -> Task for the group engine -> post-step -------------------------------
-// One estimate_* call, prepared: the Task (points, scaled threshold, camera pre-step mode, final polish) plus what the
-// post-step needs (normalising transforms of F / H).  Used by the four single entry points and by plb_estimate_batch.
-struct EstimateJob {
-    Task t;
-    int api_kind = 0; // PLB_KIND_*
-    HM3 T1, T2;
-    bool normalised = false;
-    double *model = nullptr;
-};
-static void default_stats(plb_ransac_stats *stats, plb_counters *counters) {
-    if (stats) {
-        stats->refinements = stats->iterations = stats->num_inliers = 0;
-        stats->inlier_ratio = 0;
-        stats->model_score = std::numeric_limits<double>::max();
-    }
-    if (counters) std::memset(counters, 0, sizeof(*counters));
-}
+// One estimate_* call is prepared into a Task (points, scaled threshold, camera pre-step mode, final polish), committed,
+// run and finished.  Used by the four single entry points and by plb_estimate_batch[_device].
 // robust.cc:36-126 (absolute pose, no focal estimation), :242-314 (relative pose; tangent_sampson keeps the scaled pixels
 // and runs the tangent-Sampson estimator with the cameras), :544-594 (fundamental), :712-757 (homography).
 // The camera pre-step (Camera::unproject / unproject_with_jac of every point) and the scaling of the polish pixels run on
@@ -2056,10 +2042,11 @@ static void default_stats(plb_ransac_stats *stats, plb_counters *counters) {
 // BundleOptions::refine_focal_length / refine_principal_point / refine_extra_params as a bit set
 static int refine_flags(const plb_bundle_opt *b) { return b->refine_intrinsics & (CAM_REFINE_FOCAL | CAM_REFINE_PP | CAM_REFINE_EXTRA); }
 enum { CAM_RET_NONE = 0, CAM_RET_ALWAYS = 1, CAM_RET_REFINED = 2 };
+// Checks one call and fills its Task; nothing is written (commit_task writes what the Task asks for).
 static int estimate_prepare(int kind, const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                             const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                             double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
-                            plb_ransac_stats *stats, plb_counters *counters, EstimateJob &J,
+                            plb_ransac_stats *stats, plb_counters *counters, Task &t,
                             plb_camera *camera_out = nullptr, int cam_ret = CAM_RET_NONE,
                             plb_camera *camera2_out = nullptr) {
     if (int r = check_ptrs(x1, x2, ransac, model, n)) return r;
@@ -2071,9 +2058,6 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         g_err = "unknown problem kind";
         return PLB_ERR_ARG;
     }
-    J.api_kind = kind;
-    J.model = model;
-    Task &t = J.t;
     t.a = x1;
     t.b = x2;
     t.n = n;
@@ -2125,8 +2109,7 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
         if (tangent_sampson) {
             cam_rescale(c1, scale);
             cam_rescale(c2, scale);
-            model[0] = 1.0; // ransac.cc:159-160: the start pose is reset even when score_initial_model is set
-            for (int i = 1; i < 7; ++i) model[i] = 0.0;
+            t.reset_pose = true;
             t.kind = KIND_RELPOSE_TS;
             t.pre_mode = 2;
             t.pre_scale = scale;
@@ -2148,14 +2131,12 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
     }
     const size_t min_pts = (kind == PLB_KIND_FUNDAMENTAL) ? 7 : 4; // robust.cc:548-550,716-718
     if (n < min_pts) {
-        default_stats(stats, counters);
         t.skip = true;
         return PLB_OK;
     }
     // normalize_points(scale = true, centroid = !real_focal_check | true, shared = true) runs on the device (k_normalize);
     // the engine divides max_error and the polish loss scale by the scale it finds (robust.cc:561-564,724-727)
     const bool fund = kind == PLB_KIND_FUNDAMENTAL;
-    J.normalised = true;
     fp.bundle.loss_scale = bundle->loss_scale;
     fp.min_inliers = min_pts;
     t.kind = fund ? KIND_FUND : KIND_HOMOG;
@@ -2164,31 +2145,49 @@ static int estimate_prepare(int kind, const double *x1, const double *x2, size_t
     t.rfc = fund ? real_focal_check : 0;
     return PLB_OK;
 }
-static void estimate_finish(EstimateJob &J, const Task &t) {
-    if (!J.normalised || t.skip) return;
-    // robust.cc:590-591: F = T2^T F T1 ; :753-754: H = T2^-1 H T1 ; both renormalised
-    norm_transforms(t.norm_out, J.T1, J.T2);
-    HM3 M = (J.api_kind == PLB_KIND_FUNDAMENTAL) ? hm_mul(hm_mul(hm_T(J.T2), hm_from_cm(J.model)), J.T1)
-                                                 : hm_mul(hm_mul(hm_inv(J.T2), hm_from_cm(J.model)), J.T1);
+// The writes a prepared Task asks for before it runs (Task::skip, Task::reset_pose); none for tasks of other calls.
+static void commit_task(Task &t) {
+    if (t.skip) {
+        if (t.stats_out) {
+            plb_ransac_stats &s = *t.stats_out;
+            s.refinements = s.iterations = s.num_inliers = 0;
+            s.inlier_ratio = 0;
+            s.model_score = std::numeric_limits<double>::max();
+        }
+        if (t.cnt_out) std::memset(t.cnt_out, 0, sizeof(*t.cnt_out));
+    }
+    if (t.reset_pose) {
+        t.model[0] = 1.0;
+        for (int i = 1; i < 7; ++i) t.model[i] = 0.0;
+    }
+}
+// The post-step of a normalised F / H task after a successful run; none for other tasks.
+// robust.cc:590-591: F = T2^T F T1 ; :753-754: H = T2^-1 H T1 ; both renormalised
+static void finish_task(Task &t) {
+    if (!t.norm_mode) return;
+    HM3 T1, T2;
+    norm_transforms(t.norm_out, T1, T2);
+    HM3 M = (t.kind == KIND_FUND) ? hm_mul(hm_mul(hm_T(T2), hm_from_cm(t.model)), T1)
+                                  : hm_mul(hm_mul(hm_inv(T2), hm_from_cm(t.model)), T1);
     const double nm = hm_norm(M);
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) M.m[i][j] /= nm;
-    hm_to_cm(M, J.model);
+    hm_to_cm(M, t.model);
 }
 static int estimate_single(int kind, const double *x1, const double *x2, size_t n, const plb_camera *camera1,
                            const plb_camera *camera2, const plb_ransac_opt *ransac, const plb_bundle_opt *bundle,
                            double max_error, int real_focal_check, int tangent_sampson, double *model, char *inliers,
                            plb_ransac_stats *stats, plb_counters *counters, plb_camera *camera_out = nullptr,
                            int cam_ret = CAM_RET_NONE, plb_camera *camera2_out = nullptr) {
-    EstimateJob J;
+    Task t;
     if (int r = estimate_prepare(kind, x1, x2, n, camera1, camera2, ransac, bundle, max_error, real_focal_check,
-                                 tangent_sampson, model, inliers, stats, counters, J, camera_out, cam_ret, camera2_out))
+                                 tangent_sampson, model, inliers, stats, counters, t, camera_out, cam_ret, camera2_out))
         return r;
-    if (J.t.skip) return PLB_OK;
-    std::vector<Task *> v{&J.t};
-    const int rc = run_group(J.t.kind, v);
-    if (rc != PLB_OK) return rc;
-    estimate_finish(J, J.t);
+    commit_task(t);
+    if (t.skip) return PLB_OK;
+    std::vector<Task *> v{&t};
+    if (int rc = run_group(t.kind, v)) return rc;
+    finish_task(t);
     return PLB_OK;
 }
 int plb_estimate_absolute_pose(const double *points2D, const double *points3D, size_t n, const plb_ransac_opt *ransac,
@@ -2567,266 +2566,53 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
     if (first_err.load() != PLB_OK) g_err = err_msg;
     return first_err.load();
 }
-static int batch_impl(plb_problem *problems, size_t count, const int *devices, int n_dev, int streams) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
-        g_err = "null argument";
+// ---- the batch entry points -----------------------------------------------------------------------------------------
+// Each family turns one problem into its Task with a prepare function that checks the problem by its single call's rules
+// and writes nothing; run_batch below does everything else.
+
+// ransac_* of one plb_problem, on its points or on resident correspondences, whose handle the Task holds for the call.
+static int ransac_prepare(plb_problem &p, Task &t) {
+    if (p.kind < 0 || p.kind > 3) {
+        g_err = "unknown problem kind";
         return PLB_ERR_ARG;
     }
-    if (plb_device_count() == 0) {
-        g_err = "no usable CUDA device";
-        return PLB_ERR_CUDA;
-    }
-    for (size_t i = 0; i < count; ++i) {
-        problems[i].status = PLB_OK;
-        if (problems[i].kind < 0 || problems[i].kind > 3) {
-            g_err = "unknown problem kind";
-            for (size_t j = 0; j < count; ++j) problems[j].status = PLB_ERR_ARG;
+    t.kind = p.kind;
+    t.a = p.a;
+    t.b = p.b;
+    t.n = (size_t)p.n;
+    t.opt = p.opt;
+    t.max_error = p.max_error;
+    t.rfc = p.real_focal_check;
+    t.model = p.model;
+    t.inliers = p.inliers;
+    t.stats_out = &p.stats;
+    t.cnt_out = &p.counters;
+    if (p.resident > 0) {
+        {
+            std::lock_guard<std::mutex> lk(g_res_mtx);
+            if ((size_t)p.resident <= g_resident.size()) t.res = g_resident[p.resident - 1];
+        }
+        if (!t.res || t.res->kind != p.kind) {
+            g_err = "invalid resident handle";
             return PLB_ERR_ARG;
         }
-    }
-    std::vector<Task> tasks(count);
-    std::vector<int> dev_of(count, -1);
-    std::vector<std::shared_ptr<Resident>> held; // resident inputs stay alive for the duration of the call
-    auto fail_all = [&](int rc, const char *msg) {
-        g_err = msg;
-        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
-        return rc;
-    };
-    for (size_t i = 0; i < count; ++i) {
-        plb_problem &p = problems[i];
-        Task &t = tasks[i];
-        t.kind = p.kind;
-        t.a = p.a;
-        t.b = p.b;
-        t.n = (size_t)p.n;
-        t.opt = p.opt;
-        t.max_error = p.max_error;
-        t.rfc = p.real_focal_check;
-        t.model = p.model;
-        t.inliers = p.inliers;
-        t.stats_out = &p.stats;
-        t.cnt_out = &p.counters;
-        if (p.resident > 0) {
-            std::shared_ptr<Resident> res;
-            {
-                std::lock_guard<std::mutex> lk(g_res_mtx);
-                if ((size_t)p.resident <= g_resident.size()) res = g_resident[p.resident - 1];
-            }
-            if (!res || res->kind != p.kind) return fail_all(PLB_ERR_ARG, "invalid resident handle");
-            bool ok = false;
-            for (int d = 0; d < n_dev; ++d) ok |= (devices[d] == res->device);
-            if (!ok) return fail_all(PLB_ERR_ARG, "resident correspondences live on a device this call does not use");
-            t.res = res.get();
-            t.n = (size_t)res->n;
-            dev_of[i] = res->device;
-            held.push_back(std::move(res));
-        } else if (t.n > 0 && (!p.a || !p.b)) {
-            return fail_all(PLB_ERR_ARG, "null argument");
-        }
-    }
-    const int rc = run_tasks(tasks, dev_of, devices, n_dev, streams);
-    if (rc != PLB_OK)
-        for (size_t i = 0; i < count; ++i) problems[i].status = rc;
-    return rc;
-}
-int plb_ransac_batch(plb_problem *problems, size_t count, int streams) {
-    const int dev = g_device;
-    return batch_impl(problems, count, &dev, 1, streams);
-}
-// The same over the first n_gpus CUDA devices of this process (0 = all): in-process multi-GPU, no collective — image
-// pairs are independent (robust/ransac.cc:144-148 builds one estimator per call).  Results (stats, models, inlier
-// masks) land in the caller's plb_problem array exactly as with plb_ransac_batch.
-int plb_ransac_batch_multi(plb_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
-    const int have = plb_device_count();
-    if (have == 0) {
-        g_err = "no usable CUDA device";
-        return PLB_ERR_CUDA;
-    }
-    if (n_gpus < 0 || n_gpus > have) {
-        g_err = "n_gpus out of range";
-        return PLB_ERR_ARG;
-    }
-    if (n_gpus == 0) n_gpus = have;
-    std::vector<int> devs(n_gpus);
-    for (int d = 0; d < n_gpus; ++d) devs[d] = d;
-    return batch_impl(problems, count, devs.data(), n_gpus, streams_per_gpu);
-}
-
-// The devices of a batch call: n_gpus -1 the calling thread's device, 0 all `have` devices, k the first k.
-static std::vector<int> batch_devices(int n_gpus, int have) {
-    std::vector<int> devs;
-    if (n_gpus == -1) devs.push_back(g_device);
-    else
-        for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
-    return devs;
-}
-
-// The body of the two estimate batch calls: the pre-step of every problem, LO-RANSAC of the tasks over `devs`, the
-// post-step.  dev_io: a / b (float when f32) and inliers are device memory, read after `ready` has completed.
-static int estimate_batch_run(plb_estimate_problem *problems, size_t count, const std::vector<int> &devs, int streams,
-                              bool dev_io, bool f32, cudaEvent_t ready) {
-    std::vector<EstimateJob> jobs(count);
-    for (size_t i = 0; i < count; ++i) {
-        plb_estimate_problem &p = problems[i];
-        if (int r = estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle,
-                                     p.max_error, p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats,
-                                     &p.counters, jobs[i], &p.camera1, CAM_RET_REFINED)) {
-            for (size_t j = 0; j < count; ++j) problems[j].status = r;
-            return r;
-        }
-    }
-    std::vector<Task> tasks(count);
-    std::vector<int> dev_of(count, -1);
-    for (size_t i = 0; i < count; ++i) {
-        tasks[i] = jobs[i].t;
-        tasks[i].dev_io = dev_io;
-        tasks[i].f32 = f32;
-        tasks[i].ready = ready;
-    }
-    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
-    for (size_t i = 0; i < count; ++i) {
-        problems[i].status = rc;
-        if (rc == PLB_OK) estimate_finish(jobs[i], tasks[i]);
-    }
-    return rc;
-}
-
-// Batch form of the four estimate_* entry points (robust.h:45-46,68-70,112-113,133-134): pixels + cameras in, the
-// pre-step of every problem (threshold scaling, camera unprojection and normalize_points on the device), LO-RANSAC in
-// lock-step groups per kind (tangent-Sampson problems form their own groups), final bundle and un-normalisation.  n_gpus: 0 = all devices of the process, k = the first k, -1 = the calling thread's device only.
-int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
+        t.n = (size_t)t.res->n;
+    } else if (t.n > 0 && (!p.a || !p.b)) {
         g_err = "null argument";
         return PLB_ERR_ARG;
-    }
-    const int have = plb_device_count();
-    if (have == 0) {
-        g_err = "no usable CUDA device";
-        return PLB_ERR_CUDA;
-    }
-    if (n_gpus < -1 || n_gpus > have) {
-        g_err = "n_gpus out of range";
-        return PLB_ERR_ARG;
-    }
-    return estimate_batch_run(problems, count, batch_devices(n_gpus, have), streams_per_gpu, false, false, nullptr);
-}
-// The same on the calling thread's device with device-resident inputs and masks: the inputs are gathered into the engine's
-// own buffer by k_ingest (F / H normalisation then works in place on that copy, the caller's arrays are only read) and
-// the masks are written by k_scatter_masks, so what runs between is the host path's work on the same doubles.
-int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    auto fail_all = [&](int rc, const std::string &msg) {
-        g_err = msg;
-        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
-        return rc;
-    };
-    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
-    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
-    Engine &E = *engine();
-    if (int rc = E.init()) return fail_all(rc, g_err);
-    const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
-    for (size_t i = 0; i < count; ++i) {
-        const plb_estimate_problem &p = problems[i];
-        if (p.n == 0) continue;
-        auto bad = [&](const char *what) { return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": " + what); };
-        for (const void *q : {(const void *)p.a, (const void *)p.b}) {
-            if (!device_memory(q, E.device)) return bad("a / b must be device memory of the current device");
-            if ((uintptr_t)q % elem) return bad("a / b are not aligned to the dtype");
-        }
-        if (p.inliers && !device_memory(p.inliers, E.device))
-            return bad("inliers must be NULL or device memory of the current device");
-    }
-    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
-    const std::vector<int> devs{E.device};
-    return estimate_batch_run(problems, count, devs, streams, true, dtype == PLB_DTYPE_F32, E.ev_in);
-}
-
-// ---- batch form of the robust/bundle.h refiners ----------------------------------------------------------------
-// Every problem checked by its single entry point's rules (refine_prepare), before any device call; on failure every
-// status gets the code and nothing else is written.
-static int refine_batch_prepare(plb_refine_problem *problems, size_t count, std::vector<Task> &tasks) {
-    tasks.assign(count, Task());
-    for (size_t i = 0; i < count; ++i) {
-        plb_refine_problem &p = problems[i];
-        if (int r = refine_prepare(p.refiner, p.a, p.b, (size_t)p.n, p.weights, &p.camera1, &p.camera2, &p.camera1,
-                                   &p.camera2, &p.bundle, p.model, p.bundle_stats, tasks[i])) {
-            for (size_t j = 0; j < count; ++j) problems[j].status = r;
-            return r;
-        }
     }
     return PLB_OK;
 }
-static int refine_batch_run(plb_refine_problem *problems, std::vector<Task> &tasks, const std::vector<int> &devs,
-                            int streams) {
-    std::vector<int> dev_of(tasks.size(), -1);
-    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
-    for (size_t i = 0; i < tasks.size(); ++i) problems[i].status = rc;
-    return rc;
+// estimate_* of one plb_estimate_problem: camera1 receives the refined camera of a PnP problem; relative pose returns
+// no cameras, so tangent-Sampson camera refinement is PLB_ERR_NYI.
+static int estimate_problem_prepare(plb_estimate_problem &p, Task &t) {
+    return estimate_prepare(p.kind, p.a, p.b, (size_t)p.n, &p.camera1, &p.camera2, &p.ransac, &p.bundle, p.max_error,
+                            p.real_focal_check, p.tangent_sampson, p.model, p.inliers, &p.stats, &p.counters, t,
+                            &p.camera1, CAM_RET_REFINED);
 }
-int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    std::vector<Task> tasks;
-    if (int r = refine_batch_prepare(problems, count, tasks)) return r;
-    auto fail_all = [&](int rc, const char *msg) {
-        g_err = msg;
-        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
-        return rc;
-    };
-    if (n_gpus < -1) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
-    const int have = plb_device_count();
-    if (have == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
-    if (n_gpus > have) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
-    return refine_batch_run(problems, tasks, batch_devices(n_gpus, have), streams_per_gpu);
-}
-// The same on the calling thread's device with a / b / weights in its memory: k_ingest gathers them into the engine's
-// own input buffer, where the host path's upload puts them, so what runs after is the host path's work on the same doubles.
-int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    auto fail_all = [&](int rc, const std::string &msg) {
-        g_err = msg;
-        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
-        return rc;
-    };
-    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
-    std::vector<Task> tasks;
-    if (int r = refine_batch_prepare(problems, count, tasks)) return r;
-    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
-    Engine &E = *engine();
-    if (int rc = E.init()) return fail_all(rc, g_err);
-    const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
-    for (size_t i = 0; i < count; ++i) {
-        const Task &t = tasks[i];
-        if (t.n == 0) continue;
-        for (const void *q : {(const void *)t.a, (const void *)t.b, t.weights}) {
-            if (!q) continue; // only the weights may be null
-            if (!device_memory(q, E.device))
-                return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": a / b / weights must be device memory of the current device");
-            if ((uintptr_t)q % elem) return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": a / b / weights are not aligned to the dtype");
-        }
-    }
-    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
-    for (Task &t : tasks) {
-        t.dev_io = true;
-        t.f32 = dtype == PLB_DTYPE_F32;
-        t.ready = E.ev_in;
-    }
-    return refine_batch_run(problems, tasks, {E.device}, streams);
+static int refine_problem_prepare(plb_refine_problem &p, Task &t) {
+    return refine_prepare(p.refiner, p.a, p.b, (size_t)p.n, p.weights, &p.camera1, &p.camera2, &p.camera1, &p.camera2,
+                          &p.bundle, p.model, p.bundle_stats, t);
 }
 
 // ---- given models: the robust/utils.h scorers and get_inliers (plb_score_batch) ------------------------------------
@@ -2879,45 +2665,42 @@ static int score_prepare(const plb_score_problem &p, Task &t) {
     t.inliers = p.m > 0 && p.n > 0 ? p.inliers : nullptr;
     return PLB_OK;
 }
-// Every problem checked before any device call; on failure every status gets the code and nothing else is written.
-static int score_batch_prepare(plb_score_problem *problems, size_t count, std::vector<Task> &tasks) {
-    tasks.assign(count, Task());
-    for (size_t i = 0; i < count; ++i)
-        if (int r = score_prepare(problems[i], tasks[i])) {
-            for (size_t j = 0; j < count; ++j) problems[j].status = r;
-            return r;
+
+// What is wrong with the memory of a device-form task, or null.  Sized by n (n > 0): a, b and the weights, when given,
+// must be device (or managed) memory of `device` aligned to the dtype's `elem` bytes; sized by m (m > 0): models, scores
+// and counts, 8-byte aligned; the inliers the task writes must be device memory.
+static const char *device_io_error(const Task &t, int device, size_t elem) {
+    if (t.n > 0)
+        for (const void *q : {(const void *)t.a, (const void *)t.b, t.weights}) {
+            if (!q) continue; // only the weights may be null
+            if (!device_memory(q, device)) return "a / b / weights must be device memory of the current device";
+            if ((uintptr_t)q % elem) return "a / b / weights are not aligned to the dtype";
         }
-    return PLB_OK;
+    if (t.m > 0)
+        for (const void *q : {(const void *)t.models, (const void *)t.scores, (const void *)t.counts}) {
+            if (!device_memory(q, device))
+                return "models / scores / num_inliers must be device memory of the current device";
+            if ((uintptr_t)q % sizeof(double)) return "models / scores / num_inliers are not 8-byte aligned";
+        }
+    if (t.n > 0 && t.inliers && !device_memory(t.inliers, device))
+        return "inliers must be NULL or device memory of the current device";
+    return nullptr;
 }
-static int score_batch_run(plb_score_problem *problems, std::vector<Task> &tasks, const std::vector<int> &devs,
-                           int streams) {
-    std::vector<int> dev_of(tasks.size(), -1);
-    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
-    for (size_t i = 0; i < tasks.size(); ++i) problems[i].status = rc;
-    return rc;
-}
-int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
-    if (count == 0) return PLB_OK;
-    if (!problems) {
-        g_err = "null argument";
-        return PLB_ERR_ARG;
-    }
-    std::vector<Task> tasks;
-    if (int r = score_batch_prepare(problems, count, tasks)) return r;
-    auto fail_all = [&](int rc, const char *msg) {
-        g_err = msg;
-        for (size_t j = 0; j < count; ++j) problems[j].status = rc;
-        return rc;
-    };
-    if (n_gpus < -1) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
-    const int have = plb_device_count();
-    if (have == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
-    if (n_gpus > have) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
-    return score_batch_run(problems, tasks, batch_devices(n_gpus, have), streams_per_gpu);
-}
-// The same on the calling thread's device with everything sized by n or m in its memory: k_ingest gathers a / b into the
-// engine's input buffer, k_score reads the caller's models and writes the caller's records and masks.
-int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams) {
+
+// Every batch entry point, in the order include/poselib_b200.h states: count 0 -> PLB_OK and problems NULL ->
+// PLB_ERR_ARG, writing nothing; then each failure writes its code into every status and nothing else:
+//   an unknown dtype (device forms); prepare() of each problem in order, the first failure's code; n_gpus < min_gpus;
+//   no device (PLB_ERR_CUDA); n_gpus above the device count; resident correspondences on a device the call does not
+//   use; device forms: device_io_error of each task.
+// Then the caller's stream gets the event the groups wait on (device forms), the tasks' writes are committed, the tasks
+// run, every status gets the result, and on success every task gets its post-step.
+// n_gpus: -1 the calling thread's device, 0 every device of the process, k the first k.  dtype: PLB_DTYPE_* of a device
+// form, whose inputs and outputs are memory of the calling thread's device (n_gpus -1); HOST_IO for the host forms.
+enum { HOST_IO = -1 };
+} // extern "C": a template has C++ linkage
+template <typename P, typename Prepare>
+static int run_batch(P *problems, size_t count, Prepare prepare, int n_gpus, int min_gpus, int streams,
+                     int dtype = HOST_IO, void *stream = nullptr) {
     if (count == 0) return PLB_OK;
     if (!problems) {
         g_err = "null argument";
@@ -2928,38 +2711,90 @@ int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype,
         for (size_t j = 0; j < count; ++j) problems[j].status = rc;
         return rc;
     };
-    if (dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
-    std::vector<Task> tasks;
-    if (int r = score_batch_prepare(problems, count, tasks)) return r;
-    if (plb_device_count() == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
-    Engine &E = *engine();
-    if (int rc = E.init()) return fail_all(rc, g_err);
+    const bool dev_io = dtype != HOST_IO;
+    if (dev_io && dtype != PLB_DTYPE_F64 && dtype != PLB_DTYPE_F32) return fail_all(PLB_ERR_ARG, "unknown dtype");
+    std::vector<Task> tasks(count);
+    for (size_t i = 0; i < count; ++i)
+        if (int r = prepare(problems[i], tasks[i])) return fail_all(r, g_err);
+    if (n_gpus < min_gpus) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    const int have = plb_device_count();
+    if (have == 0) return fail_all(PLB_ERR_CUDA, "no usable CUDA device");
+    if (n_gpus > have) return fail_all(PLB_ERR_ARG, "n_gpus out of range");
+    std::vector<int> devs;
+    if (n_gpus == -1) devs.push_back(g_device);
+    else
+        for (int d = 0; d < (n_gpus == 0 ? have : n_gpus); ++d) devs.push_back(d);
+    Engine *E = dev_io ? engine() : nullptr;
+    if (E)
+        if (int rc = E->init()) return fail_all(rc, g_err);
     const size_t elem = dtype == PLB_DTYPE_F32 ? sizeof(float) : sizeof(double);
+    std::vector<int> dev_of(count, -1); // resident inputs stay on the device that holds them
     for (size_t i = 0; i < count; ++i) {
         const Task &t = tasks[i];
-        auto bad = [&](const char *what) { return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": " + what); };
-        if (t.n > 0)
-            for (const void *q : {(const void *)t.a, (const void *)t.b}) {
-                if (!device_memory(q, E.device)) return bad("a / b must be device memory of the current device");
-                if ((uintptr_t)q % elem) return bad("a / b are not aligned to the dtype");
-            }
-        if (t.m > 0)
-            for (const void *q : {(const void *)t.models, (const void *)t.scores, (const void *)t.counts}) {
-                if (!device_memory(q, E.device))
-                    return bad("models / scores / num_inliers must be device memory of the current device");
-                if ((uintptr_t)q % sizeof(double)) return bad("models / scores / num_inliers are not 8-byte aligned");
-            }
-        if (t.inliers && !device_memory(t.inliers, E.device))
-            return bad("inliers must be NULL or device memory of the current device");
+        if (t.res) {
+            if (std::find(devs.begin(), devs.end(), t.res->device) == devs.end())
+                return fail_all(PLB_ERR_ARG, "resident correspondences live on a device this call does not use");
+            dev_of[i] = t.res->device;
+        }
+        if (const char *what = E ? device_io_error(t, E->device, elem) : nullptr)
+            return fail_all(PLB_ERR_ARG, "problem " + std::to_string(i) + ": " + what);
     }
-    cudaError_t e = cudaEventRecord(E.ev_in, (cudaStream_t)stream);
-    if (e != cudaSuccess) return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
-    for (Task &t : tasks) {
-        t.dev_io = true;
-        t.f32 = dtype == PLB_DTYPE_F32;
-        t.ready = E.ev_in;
+    if (E) {
+        cudaError_t e = cudaEventRecord(E->ev_in, (cudaStream_t)stream);
+        if (e != cudaSuccess)
+            return fail_all(PLB_ERR_CUDA, std::string("cudaEventRecord on the caller's stream: ") + cudaGetErrorString(e));
+        for (Task &t : tasks) {
+            t.dev_io = true;
+            t.f32 = dtype == PLB_DTYPE_F32;
+            t.ready = E->ev_in;
+        }
     }
-    return score_batch_run(problems, tasks, {E.device}, streams);
+    for (Task &t : tasks) commit_task(t);
+    const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
+    for (size_t i = 0; i < count; ++i) {
+        problems[i].status = rc;
+        if (rc == PLB_OK) finish_task(tasks[i]);
+    }
+    return rc;
+}
+extern "C" {
+
+int plb_ransac_batch(plb_problem *problems, size_t count, int streams) {
+    return run_batch(problems, count, ransac_prepare, -1, -1, streams);
+}
+// The same over the first n_gpus CUDA devices of this process (0 = all): in-process multi-GPU, no collective — image
+// pairs are independent (robust/ransac.cc:144-148 builds one estimator per call).  Results (stats, models, inlier
+// masks) land in the caller's plb_problem array exactly as with plb_ransac_batch.
+int plb_ransac_batch_multi(plb_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, ransac_prepare, n_gpus, 0, streams_per_gpu);
+}
+// Batch form of the four estimate_* entry points (robust.h:45-46,68-70,112-113,133-134): pixels + cameras in, the
+// pre-step of every problem (threshold scaling, camera unprojection and normalize_points on the device), LO-RANSAC in
+// lock-step groups per kind (tangent-Sampson problems form their own groups), final bundle and un-normalisation.
+int plb_estimate_batch(plb_estimate_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, estimate_problem_prepare, n_gpus, -1, streams_per_gpu);
+}
+// The same on the calling thread's device with device-resident inputs and masks: the inputs are gathered into the engine's
+// own buffer by k_ingest (F / H normalisation then works in place on that copy, the caller's arrays are only read) and
+// the masks are written by k_scatter_masks, so what runs between is the host path's work on the same doubles.
+int plb_estimate_batch_device(plb_estimate_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    return run_batch(problems, count, estimate_problem_prepare, -1, -1, streams, dtype, stream);
+}
+int plb_refine_batch(plb_refine_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, refine_problem_prepare, n_gpus, -1, streams_per_gpu);
+}
+// The same on the calling thread's device with a / b / weights in its memory: k_ingest gathers them into the engine's
+// own input buffer, where the host path's upload puts them, so what runs after is the host path's work on the same doubles.
+int plb_refine_batch_device(plb_refine_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    return run_batch(problems, count, refine_problem_prepare, -1, -1, streams, dtype, stream);
+}
+int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, score_prepare, n_gpus, -1, streams_per_gpu);
+}
+// The same on the calling thread's device with everything sized by n or m in its memory: k_ingest gathers a / b into the
+// engine's input buffer, k_score reads the caller's models and writes the caller's records and masks.
+int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    return run_batch(problems, count, score_prepare, -1, -1, streams, dtype, stream);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {
