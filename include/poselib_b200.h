@@ -296,7 +296,7 @@ int plb_refine_homography_weighted(const double *x1_xy, const double *x2_xy, siz
 
 /* ---- batch of independent problems (BASELINE config 5); sharded by the caller across GPUs ---------- */
 /* Every batch call below (plb_ransac_batch[_multi], plb_estimate_batch[_device], plb_refine_batch[_device],
- * plb_score_batch[_device]) checks its arguments in one order, before any copy or launch:
+ * plb_score_batch[_device], plb_generate_batch[_device]) checks its arguments in one order, before any copy or launch:
  *   1. count 0 -> PLB_OK, nothing written;
  *   2. problems NULL -> PLB_ERR_ARG, nothing written;
  *   3. device forms: a dtype other than PLB_DTYPE_F64 / PLB_DTYPE_F32 -> PLB_ERR_ARG;
@@ -305,8 +305,11 @@ int plb_refine_homography_weighted(const double *x1_xy, const double *x2_xy, siz
  *   6. no device -> PLB_ERR_CUDA;
  *   7. n_gpus above the device count -> PLB_ERR_ARG;
  *   8. resident correspondences on a device the call does not use -> PLB_ERR_ARG; device forms: a pointer of a problem
- *      that is not device (or managed) memory of the calling thread's device, or is misaligned -> PLB_ERR_ARG.
- * A failure in steps 3-8 writes its code into every status and nothing else: no model, stats, counters, camera, mask,
+ *      that is not device (or managed) memory of the calling thread's device, or is misaligned -> PLB_ERR_ARG;
+ *   9. plb_generate_batch_device: a sample index outside [0, n) -> PLB_ERR_ARG, found by one reduction kernel over every
+ *      problem's samples and one synchronisation, after the work queued on the caller's stream and before any other
+ *      kernel reads a sample.
+ * A failure in steps 3-9 writes its code into every status and nothing else: no model, stats, counters, camera, mask,
  * score or count changes.  After the checks, every status receives the call's result. */
 enum { PLB_KIND_PNP = 0, PLB_KIND_RELPOSE = 1, PLB_KIND_FUNDAMENTAL = 2, PLB_KIND_HOMOGRAPHY = 3 };
 typedef struct plb_problem {
@@ -480,6 +483,60 @@ int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int s
  * memory of the current device or is misaligned (a / b: the dtype; models, scores, num_inliers: 8 bytes) ->
  * PLB_ERR_ARG. */
 int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams);
+
+/* Hypotheses of caller-drawn minimal samples: the estimators' generate_models followed by score_model for every model,
+ * for callers that draw their own samples (learned or guided sampling, RANSAC variants of their own) or study the
+ * hypotheses of a scene.  At the ransac_* level, as plb_score_batch: no normalisation, sq_threshold squared in the points'
+ * units (tangent Sampson: pixels^2).
+ *   kind (+ option)                      k   M   solver and estimator
+ *   PLB_KIND_PNP                         3   4   p3p on x.homogeneous().normalized(), X (estimators/absolute_pose.cc:46-58)
+ *   PLB_KIND_RELPOSE                     5  40   relpose_5pt on the normalised homogeneous points (relative_pose.cc:48-60)
+ *   PLB_KIND_RELPOSE + tangent_sampson   5  40   relpose_5pt on the bearings of camera1 / camera2 (relative_pose.cc:88-99)
+ *   PLB_KIND_FUNDAMENTAL                 7   3   relpose_7pt; with real_focal_check the models failing calculate_RFC are
+ *                                                erased, the rest keep their order (relative_pose.cc:384-403)
+ *   PLB_KIND_HOMOGRAPHY                  4   1   homography_4pt with check_cheirality (homography.cc:36-52)
+ * Sample j (row j of `samples`, k indices into [0, n), duplicates go to the solver as given) gives n_models[j] models in
+ * the solver's order in slots [0, n_models[j]) of row j of `models` (M slots of 7 or 9 doubles: poses, or column-major
+ * matrices), each with the fp64 score_model record in `scores` / `num_inliers` (fp64 whatever plb_set_mode says).  Slots
+ * past n_models[j] are not written.  num_inliers is exactly the reference's count; a score equals, bit for bit, what
+ * plb_score_batch returns for the same model; a model is, bit for bit, what the RANSAC path's solver kernels produce for
+ * the sample.  None of the outputs depends on the rest of the batch, n_gpus, streams, the mode or the form of the call. */
+typedef struct plb_generate_problem {
+    int32_t kind;             /* PLB_KIND_* */
+    int32_t tangent_sampson;  /* relative pose only: camera1 / camera2 read, a / b in their pixels */
+    int32_t real_focal_check; /* fundamental only */
+    int32_t reserved;
+    uint64_t n;
+    const double *a;          /* x (pnp) or x1: 2n doubles */
+    const double *b;          /* X (pnp): 3n doubles; else x2: 2n doubles */
+    plb_camera camera1;
+    plb_camera camera2;
+    uint64_t s;               /* samples */
+    const int32_t *samples;   /* s x k indices into [0, n), row-major */
+    double sq_threshold;
+    int32_t *n_models;        /* out: s */
+    double *models;           /* out: s x M x (7 | 9) */
+    double *scores;           /* out: s x M */
+    int64_t *num_inliers;     /* out: s x M */
+    int32_t status;           /* out */
+    int32_t reserved2;
+} plb_generate_problem;
+/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device);
+ * streams_per_gpu groups of problems are in flight on each device.  Every pointer is host memory.
+ * Each problem is checked: an unknown kind, tangent_sampson on another kind than relative pose, real_focal_check on another
+ * kind than fundamental, a / b NULL with n > 0, samples / n_models / models / scores / num_inliers NULL with s > 0, a
+ * non-finite sq_threshold, s >= 2^31, s * M * (7 | 9) doubles overflowing, or n > 2^26 -> PLB_ERR_ARG; a camera
+ * (tangent_sampson) outside the ten models -> PLB_ERR_NYI; then a sample index outside [0, n) -> PLB_ERR_ARG (every index
+ * is checked on the host, before any device call).  s = 0 writes nothing. */
+int plb_generate_batch(plb_generate_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
+/* plb_generate_batch(problems, count, -1, streams) with a, b, samples and every output in device (or managed) memory of the
+ * calling thread's device: a / b contiguous arrays of `dtype` aligned to it (PLB_DTYPE_F32: `const float *` cast into the
+ * `const double *` fields; widened exactly, so a float call gives the double call's results on the widened values),
+ * samples, n_models aligned to 4 bytes, models, scores, num_inliers to 8.  Nothing sized by n or s crosses PCIe.  Inputs
+ * are read after the work queued on `stream` ahead of the call; when the call returns, every device write it made is
+ * complete.  A pointer that is not device memory of the current device or is misaligned -> PLB_ERR_ARG (step 8); the
+ * sample indices are range-checked on the device (step 9). */
+int plb_generate_batch_device(plb_generate_problem *problems, size_t count, int dtype, void *stream, int streams);
 
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers
  * that run several estimations on the same matches).  kind: PLB_KIND_*; returns a handle > 0 or an error < 0. */

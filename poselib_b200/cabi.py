@@ -105,7 +105,7 @@ EXPORTS = [
     "plb_resident_free", "plb_bundle_adjust_image_weighted", "plb_refine_relpose_weighted",
     "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
     "plb_refine_homography_weighted", "plb_estimate_batch_device", "plb_refine_batch", "plb_refine_batch_device",
-    "plb_score_batch", "plb_score_batch_device",
+    "plb_score_batch", "plb_score_batch_device", "plb_generate_batch", "plb_generate_batch_device",
 ]
 DTYPE_F64, DTYPE_F32 = 0, 1
 
@@ -135,6 +135,20 @@ class ScoreProblem(C.Structure):
                 ("models", C.POINTER(C.c_double)), ("sq_threshold", C.c_double), ("scores", C.POINTER(C.c_double)),
                 ("num_inliers", C.POINTER(C.c_int64)), ("inliers", C.c_char_p), ("status", C.c_int32),
                 ("reserved", C.c_int32)]
+
+
+class GenerateProblem(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("tangent_sampson", C.c_int32), ("real_focal_check", C.c_int32),
+                ("reserved", C.c_int32), ("n", C.c_uint64), ("a", C.POINTER(C.c_double)), ("b", C.POINTER(C.c_double)),
+                ("camera1", Camera), ("camera2", Camera), ("s", C.c_uint64), ("samples", C.POINTER(C.c_int32)),
+                ("sq_threshold", C.c_double), ("n_models", C.POINTER(C.c_int32)), ("models", C.POINTER(C.c_double)),
+                ("scores", C.POINTER(C.c_double)), ("num_inliers", C.POINTER(C.c_int64)), ("status", C.c_int32),
+                ("reserved2", C.c_int32)]
+
+
+# plb_generate_problem: indices per sample (k) and model slots per sample (M) of each kind
+GENERATE_K = {"pnp": 3, "relpose": 5, "fundamental": 7, "homography": 4}
+GENERATE_M = {"pnp": 4, "relpose": 40, "fundamental": 3, "homography": 1}
 
 
 if not os.path.exists(LIB_PATH):
@@ -865,6 +879,111 @@ def score_batch_device(problems, stream=None, streams=8):
             out.append({"scores": scores[i], "num_inliers": counts[i], "inliers": mask})
     _check(_lib.plb_score_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
                                        int(streams)))
+    for r, q in zip(out, arr):
+        r["status"] = q.status
+    return out
+
+
+# ---- hypotheses of caller-drawn minimal samples (plb_generate_batch) ---------------------------------------------
+def _fill_generate_problem(q, p, npts, s):
+    """Everything of one plb_generate_problem but its pointers."""
+    q.kind = KIND[p["kind"]]
+    q.tangent_sampson = int(p.get("tangent_sampson", False))
+    q.real_focal_check = int(p.get("rfc", False))
+    q.n = npts
+    q.s = s
+    q.camera1 = p.get("cam1") or Camera("NULL", ())
+    q.camera2 = p.get("cam2") or Camera("NULL", ())
+    q.sq_threshold = p["sq_threshold"]
+
+
+def _generate_models_out(kind, models):
+    """[s, M, 7] poses as they are; [s, M, 9] column-major matrices -> [s, M, 3, 3] [r,c] (a view for torch tensors)."""
+    if kind in ("pnp", "relpose"):
+        return models
+    return models.reshape(*models.shape[:2], 3, 3).swapaxes(-1, -2)
+
+
+def generate_batch(problems, n_gpus=-1, streams=8):
+    """Models and MSAC records of caller-drawn minimal samples (plb_generate_batch): each estimator's generate_models,
+    then score_model of every model.  problems: list of dict(kind, a, b, samples [s,k] int indices into [0, n),
+    sq_threshold [squared, in the points' units], rfc=False [fundamental], tangent_sampson=False with cam1 / cam2
+    [pixels]).  n_gpus: -1 current device, 0 all devices, k the first k.  Returns list of dict(n_models [s] int32,
+    models [s,M,7] poses or [s,M,3,3] matrices [r,c], scores [s,M] float64, num_inliers [s,M] int64, status); slots past
+    n_models[j] keep the NaN / -1 they start with."""
+    count = len(problems)
+    arr = (GenerateProblem * count)()
+    out = []
+    keep = []
+    for i, p in enumerate(problems):
+        q = arr[i]
+        kind, k, M = p["kind"], GENERATE_K[p["kind"]], GENERATE_M[p["kind"]]
+        aa, ap = _d(p["a"])
+        ba, bp = _d(p["b"])
+        smp = np.ascontiguousarray(np.asarray(p["samples"], dtype=np.int32).reshape(-1, k))
+        s = len(smp)
+        msz = 7 if kind in ("pnp", "relpose") else 9
+        r = {"n_models": np.zeros(s, dtype=np.int32), "models": np.full((s, M, msz), np.nan),
+             "scores": np.full((s, M), np.nan), "num_inliers": np.full((s, M), -1, dtype=np.int64)}
+        keep.append((aa, ba, smp))
+        out.append(r)
+        _fill_generate_problem(q, p, len(aa), s)
+        q.a, q.b, q.samples = ap, bp, smp.ctypes.data_as(C.POINTER(C.c_int32))
+        q.n_models = r["n_models"].ctypes.data_as(C.POINTER(C.c_int32))
+        q.models, q.scores = r["models"].ctypes.data_as(_P), r["scores"].ctypes.data_as(_P)
+        q.num_inliers = r["num_inliers"].ctypes.data_as(C.POINTER(C.c_int64))
+    _check(_lib.plb_generate_batch(arr, C.c_size_t(count), int(n_gpus), int(streams)))
+    for p, r, q in zip(problems, out, arr):
+        r["models"] = _generate_models_out(p["kind"], r["models"])
+        r["status"] = q.status
+    return out
+
+
+def generate_batch_device(problems, stream=None, streams=8):
+    """generate_batch (n_gpus=-1) with everything on the GPU (plb_generate_batch_device).  problems: the dicts
+    generate_batch takes, with a / b as CUDA torch tensors ([n,2] / [n,3] or [n,2]) of one device and one dtype, float32
+    or float64, and samples a CUDA torch.int32 tensor [s,k] on the same device.  The call runs on that device and reads
+    the inputs after the work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle; default: the device's
+    current stream).  Returns the dicts of generate_batch with CUDA tensors (models a view [s,M,3,3] [r,c] for the
+    matrix kinds); the outputs of one call are views of one allocation per field."""
+    import torch
+    form = _device_form("generate_batch_device", "a and b", [t for p in problems for t in (p["a"], p["b"])],
+                        stream=stream)
+    if form is None:
+        return []
+    dev, dtype, stream = form
+    for i, p in enumerate(problems):
+        smp = p["samples"]
+        if not (isinstance(smp, torch.Tensor) and smp.is_cuda and smp.device == dev and smp.dtype == torch.int32):
+            raise TypeError(f"generate_batch_device: problem {i}: samples must be a torch.int32 tensor on {dev}")
+    count = len(problems)
+    arr = (GenerateProblem * count)()
+    keep = []
+    out = []
+    ptr = lambda t, ct=_P: C.cast(C.c_void_p(t.data_ptr() if t.numel() else None), ct)
+    with torch.cuda.stream(stream):  # the copies and outputs below are ordered before the call's reads and writes
+        smps = [p["samples"].reshape(-1, GENERATE_K[p["kind"]]).contiguous() for p in problems]
+        ss = [len(t) for t in smps]
+        Ms = [GENERATE_M[p["kind"]] for p in problems]
+        mszs = [7 if p["kind"] in ("pnp", "relpose") else 9 for p in problems]
+        slots = [s * M for s, M in zip(ss, Ms)]
+        n_models = torch.zeros(sum(ss), dtype=torch.int32, device=dev).split(ss)
+        models = torch.full((sum(sl * m for sl, m in zip(slots, mszs)),), float("nan"), dtype=torch.float64,
+                            device=dev).split([sl * m for sl, m in zip(slots, mszs)])
+        scores = torch.full((sum(slots),), float("nan"), dtype=torch.float64, device=dev).split(slots)
+        counts = torch.full((sum(slots),), -1, dtype=torch.int64, device=dev).split(slots)
+        for i, p in enumerate(problems):
+            q = arr[i]
+            a, b = _device_points("generate_batch_device", i, p, 3 if p["kind"] == "pnp" else 2)
+            keep.append((a, b, smps[i]))
+            _fill_generate_problem(q, p, a.shape[0], ss[i])
+            q.a, q.b, q.samples = ptr(a), ptr(b), ptr(smps[i], C.POINTER(C.c_int32))
+            q.n_models, q.models = ptr(n_models[i], C.POINTER(C.c_int32)), ptr(models[i])
+            q.scores, q.num_inliers = ptr(scores[i]), ptr(counts[i], C.POINTER(C.c_int64))
+            out.append({"n_models": n_models[i], "models": _generate_models_out(p["kind"], models[i].view(ss[i], Ms[i], mszs[i])),
+                        "scores": scores[i].view(ss[i], Ms[i]), "num_inliers": counts[i].view(ss[i], Ms[i])})
+    _check(_lib.plb_generate_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
+                                          int(streams)))
     for r, q in zip(out, arr):
         r["status"] = q.status
     return out

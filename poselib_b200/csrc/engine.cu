@@ -240,6 +240,17 @@ struct Engine {
     DevBuf<ScoreDesc> scdesc; // explicit models (initial models, plb_score_batch)
     PinBuf<ScoreDesc> h_scdesc;
     PinBuf<double> h_models;
+    // caller-drawn samples (plb_generate_batch): the callers' sample tables (host form: staged here; device form: taken
+    // by k_take_samples), the record descriptors, and the host form's packed records (device staging, per-sample count
+    // and offset in mapped memory, the copy the host expands)
+    PinBuf<uint32_t> h_samples;
+    DevBuf<TakeDesc> tkdesc;
+    PinBuf<TakeDesc> h_tkdesc;
+    DevBuf<PutDesc> pdesc;
+    PinBuf<PutDesc> h_pdesc;
+    DevBuf<double> gen_stage;
+    PinBuf<double> h_gen_stage;
+    MapBuf<int> h_gen;
     DevBuf<LmJob> jobs;
     PinBuf<double> h_in, h_lm_in;
     PinBuf<int> h_act, h_work;
@@ -589,6 +600,14 @@ struct Task {
     double sq_thr = 0;
     double *scores = nullptr;
     int64_t *counts = nullptr;
+    // Hypotheses of caller-drawn samples instead of LO-RANSAC (run_generate_group): s samples of K indices (device memory
+    // with dev_io), sample j's n_models[j] models with their records (threshold sq_thr) in row j of gen_models / scores /
+    // counts, kind_max_models slots per row.
+    bool generate = false;
+    size_t s = 0;
+    const int32_t *samples = nullptr;
+    int32_t *n_models = nullptr;
+    double *gen_models = nullptr;
     // doubles per correspondence the group uploads: the caller layout, then the weight
     size_t in_per_point(int in_arr) const { return (size_t)in_arr + (weights ? 1 : 0); }
 };
@@ -679,6 +698,7 @@ struct Group {
     const int mode;
     int cap_factor;
     bool big_caps = false;
+    size_t gen_rows = 0; // generate(): samples of the largest chunk (the stride of E.h_gen's two per-sample arrays)
     int smp_cur = 0; // sampler states of the current round: E.smp[smp_cur * NP ..]; the advanced ones land in the other half
     std::vector<int> act; // active problems of the current round
     std::vector<uint8_t> first_round;
@@ -816,7 +836,7 @@ struct Group {
             P.cam[0].model = P.cam[1].model = CAMM_NULL;
             P.n = S.n;
             P.kind = kind;
-            P.sq_thr = S.t->score ? S.t->sq_thr : S.t->max_error * S.t->max_error;
+            P.sq_thr = (S.t->score || S.t->generate) ? S.t->sq_thr : S.t->max_error * S.t->max_error;
             P.rfc = S.t->rfc;
             P.n_pad = S.n_pad;
             if (S.n == 0) continue;
@@ -1211,6 +1231,158 @@ struct Group {
                 for (int k = 0; k < S.n; ++k) dst[k] = (char)((w[k >> 5] >> (k & 31)) & 1u);
             }
             maskoff += t.m * (size_t)S.n_pad;
+        }
+        return PLB_OK;
+    }
+    // ---- caller-drawn samples (plb_generate_batch): the round's solve kernels and its exact scoring on given samples ---
+    // Chunks of at most ROUND_MAX samples, taken from the problems in order.  A problem's segment holds B x MAXM slots,
+    // the worst case, so no chunk overflows or is redone.  Per chunk: the sample table (host form: staged and uploaded;
+    // device form: k_take_samples from the callers' tables), launch_hypotheses in mode 0 (fp64 records of every model),
+    // then k_put_hyps into the callers' rows (device form) or packed into a staging buffer the host expands (host form),
+    // so the padding of the rows does not cross PCIe.  A model's bits depend only on its sample and a record's only on its
+    // model and problem, so the chunking changes no output.
+    int generate() {
+        const bool host = !PS[0].t->dev_io; // a call's tasks are all host or all device tasks
+        size_t all = 0;
+        for (const PState &S : PS) all += S.t->s;
+        if (!all) return PLB_OK;
+        const size_t max_total = std::min(all, ROUND_MAX), cap = max_total * (size_t)MAXM;
+        gen_rows = max_total;
+        int rc;
+        // sized once for the largest chunk: a reallocation would synchronise the device
+        if ((rc = E.samples.ensure(max_total * K)) || (rc = E.n_models.ensure(max_total)) ||
+            (rc = E.first_slot.ensure(max_total)) || (rc = E.counts.ensure(cap)) || (rc = E.scores.ensure(cap)) ||
+            (rc = E.models.ensure(cap * MSZ)) || (rc = E.model_prob.ensure(cap)) || (rc = E.h_act.ensure(4 * (size_t)NP + 2)) ||
+            (rc = E.act.ensure(4 * (size_t)NP + 2)) || (rc = E.prob_count.ensure(NP)) || (rc = E.work.ensure(CTL_WORDS)) ||
+            (rc = E.pdesc.ensure(NP)) || (rc = E.h_pdesc.ensure(NP)))
+            return rc;
+        if (kind_is_relpose(kind) && ((rc = E.s5_blk.ensure(max_total * 105)) || (rc = E.s5_park.ensure(max_total * 100)) ||
+                                      (rc = E.s5_cpoly.ensure(max_total * 11)) || (rc = E.s5_roots.ensure(max_total * 10)) ||
+                                      (rc = E.s5_nroots.ensure(max_total))))
+            return rc;
+        if (host ? ((rc = E.h_samples.ensure(max_total * K)) || (rc = E.h_gen.ensure(2 * max_total)) ||
+                    (rc = E.gen_stage.ensure(cap * (MSZ + 2))))
+                 : ((rc = E.tkdesc.ensure(NP)) || (rc = E.h_tkdesc.ensure(NP))))
+            return rc;
+        PLB_CUDA(cudaMemsetAsync(E.work.p, 0, CTL_WORDS * sizeof(int), st));
+        if (!host) PLB_CUDA(cudaStreamWaitEvent(st, PS[0].t->ready, 0)); // the callers' tables after their queued work
+        std::vector<size_t> done(NP, 0);
+        for (;;) {
+            act.clear();
+            size_t total = 0;
+            for (int i = 0; i < NP && total < ROUND_MAX; ++i) {
+                PState &S = PS[i];
+                if (S.t->s == done[i]) continue;
+                S.B = std::min(S.t->s - done[i], ROUND_MAX - total);
+                S.g0 = total;
+                total += S.B;
+                act.push_back(i);
+            }
+            if (act.empty()) return PLB_OK;
+            if ((rc = generate_chunk(total, done, host))) return rc;
+            for (int i : act) done[i] += PS[i].B;
+        }
+    }
+    int generate_chunk(size_t total, const std::vector<size_t> &done, bool host) {
+        const int na = (int)act.size();
+        const size_t cap = total * (size_t)MAXM;
+        int rc;
+        size_t seg = 0; // h_act layout as in launch_round: active[na] | g_off[na+1] | seg_base[na] | seg_cap[na]
+        for (int a = 0; a < na; ++a) {
+            const PState &S = PS[act[a]];
+            const Task &t = *S.t;
+            E.h_act.p[a] = act[a];
+            E.h_act.p[na + a] = (int)S.g0;
+            E.h_act.p[2 * na + 1 + a] = (int)seg;
+            E.h_act.p[3 * na + 1 + a] = (int)(S.B * MAXM);
+            seg += S.B * MAXM;
+            const int32_t *src = t.samples + done[act[a]] * K;
+            PutDesc &D = E.h_pdesc.p[a];
+            if (host) {
+                std::copy(src, src + S.B * K, E.h_samples.p + S.g0 * K); // int32 -> uint32, all checked to be in [0, n)
+                D = {E.h_gen.d + S.g0, E.h_gen.d + gen_rows + S.g0, E.gen_stage.p, E.gen_stage.p + cap * MSZ,
+                     reinterpret_cast<long long *>(E.gen_stage.p + cap * (MSZ + 1))};
+            } else {
+                E.h_tkdesc.p[a] = {src, E.samples.p + S.g0 * K, (long long)(S.B * K), S.n, 0};
+                const size_t row = done[act[a]];
+                D = {t.n_models + row, nullptr, t.gen_models + row * MAXM * MSZ, t.scores + row * MAXM,
+                     reinterpret_cast<long long *>(t.counts) + row * MAXM};
+            }
+        }
+        E.h_act.p[2 * na] = (int)total;
+        PLB_CUDA(cudaMemcpyAsync(E.act.p, E.h_act.p, sizeof(int) * (4 * na + 1), cudaMemcpyHostToDevice, st));
+        PLB_CUDA(cudaMemcpyAsync(E.pdesc.p, E.h_pdesc.p, sizeof(PutDesc) * na, cudaMemcpyHostToDevice, st));
+        if (host) {
+            PLB_CUDA(cudaMemcpyAsync(E.samples.p, E.h_samples.p, sizeof(uint32_t) * total * K, cudaMemcpyHostToDevice, st));
+            h2d += sizeof(uint32_t) * total * K;
+        } else {
+            long long max_count = 0;
+            for (int a = 0; a < na; ++a) max_count = std::max(max_count, E.h_tkdesc.p[a].count);
+            PLB_CUDA(cudaMemcpyAsync(E.tkdesc.p, E.h_tkdesc.p, sizeof(TakeDesc) * na, cudaMemcpyHostToDevice, st));
+            launch_take_samples(E.tkdesc.p, na, max_count, nullptr, st);
+            E.launches++;
+        }
+        RoundDesc R;
+        R.probs = E.probs.p;
+        R.active = E.act.p;
+        R.g_off = E.act.p + na;
+        R.n_active = na;
+        R.samples = E.samples.p;
+        R.n_total = (int)total;
+        HypOut out{};
+        out.n_models = E.n_models.p;
+        out.first_slot = E.first_slot.p;
+        out.seg_base = E.act.p + 2 * na + 1;
+        out.seg_cap = E.act.p + 3 * na + 1;
+        out.prob_count = E.prob_count.p;
+        out.max_seg_cap = 0;
+        for (int a = 0; a < na; ++a) out.max_seg_cap = std::max(out.max_seg_cap, E.h_act.p[3 * na + 1 + a]);
+        out.overflow = E.work.p + CTL_OVERFLOW; // cannot be set: every segment has the worst-case capacity
+        out.counts = E.counts.p;
+        out.scores = E.scores.p;
+        out.models = E.models.p;
+        out.model_prob = E.model_prob.p;
+        if (kind_is_relpose(kind)) {
+            out.s5_blk = E.s5_blk.p;
+            out.s5_park = E.s5_park.p;
+            out.s5_cpoly = E.s5_cpoly.p;
+            out.s5_roots = E.s5_roots.p;
+            out.s5_nroots = E.s5_nroots.p;
+        }
+        launch_hypotheses(kind, R, out, 0, max_n_pad, nullptr, st);
+        launch_put_hyps(R, out, E.pdesc.p, MSZ, MAXM, host, st);
+        E.launches += (kind_is_relpose(kind) ? 6 : 2) + 1;
+        // the staging buffers of the next chunk are rewritten once this one's copies and kernels are done
+        if ((rc = sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        if (!host) return PLB_OK;
+        const int *nm = E.h_gen.p, *off = E.h_gen.p + gen_rows;
+        size_t n_out = 0;
+        for (size_t g = 0; g < total; ++g) n_out += (size_t)nm[g];
+        d2h += sizeof(int) * 2 * total;
+        if (n_out) {
+            if ((rc = E.h_gen_stage.ensure(n_out * (MSZ + 2)))) return rc;
+            double *hm = E.h_gen_stage.p, *hs = hm + n_out * MSZ, *hc = hs + n_out;
+            PLB_CUDA(cudaMemcpyAsync(hm, E.gen_stage.p, sizeof(double) * n_out * MSZ, cudaMemcpyDeviceToHost, st));
+            PLB_CUDA(cudaMemcpyAsync(hs, E.gen_stage.p + cap * MSZ, sizeof(double) * n_out, cudaMemcpyDeviceToHost, st));
+            PLB_CUDA(cudaMemcpyAsync(hc, E.gen_stage.p + cap * (MSZ + 1), sizeof(double) * n_out, cudaMemcpyDeviceToHost, st));
+            d2h += sizeof(double) * n_out * (MSZ + 2);
+            if ((rc = sync())) return rc;
+        }
+        const double *hm = E.h_gen_stage.p, *hs = hm + n_out * MSZ;
+        const long long *hc = reinterpret_cast<const long long *>(hs + n_out);
+        for (int a = 0; a < na; ++a) {
+            const PState &S = PS[act[a]];
+            const Task &t = *S.t;
+            for (size_t j = 0; j < S.B; ++j) {
+                const size_t row = done[act[a]] + j, g = S.g0 + j;
+                const int c = nm[g];
+                const size_t o = (size_t)off[g];
+                t.n_models[row] = c;
+                std::copy(hm + o * MSZ, hm + (o + c) * MSZ, t.gen_models + row * MAXM * MSZ);
+                std::copy(hs + o, hs + o + c, t.scores + row * MAXM);
+                for (int m = 0; m < c; ++m) t.counts[row * MAXM + m] = (int64_t)hc[o + m];
+            }
         }
         return PLB_OK;
     }
@@ -1829,6 +2001,15 @@ static int run_score_group(int kind, std::vector<Task *> &tasks) {
     Group G(kind, tasks);
     int rc;
     if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose()) || (rc = G.score())) return rc;
+    return PLB_OK;
+}
+
+// Runs a group of generate tasks of the same kind (Task::generate): the upload of the group (tangent Sampson: the camera
+// pre-step), then the solve kernels and exact scoring of every caller-drawn sample (Group::generate).
+static int run_generate_group(int kind, std::vector<Task *> &tasks) {
+    Group G(kind, tasks);
+    int rc;
+    if ((rc = G.init()) || (rc = G.upload()) || (rc = G.transpose()) || (rc = G.generate())) return rc;
     return PLB_OK;
 }
 
@@ -2472,6 +2653,7 @@ int plb_relpose_8pt_batch(size_t count, size_t n, const double *x1, const double
 static double task_cost(const Task &t) {
     if (t.refine) return (double)std::max<size_t>(t.n, 1) * (double)std::max<uint64_t>(t.polish.bundle.max_iterations, 1);
     if (t.score) return (double)std::max<size_t>(t.n, 1) * (double)std::max<size_t>(t.m, 1);
+    if (t.generate) return (double)std::max<size_t>(t.n, 1) * (double)std::max<size_t>(t.s, 1) * kind_max_models(t.kind);
     static const double its[5] = {4.0 * 1000, 0.5 * 14000, 2.0 * 30000, 1.0 * 1000, 0.5 * 14000}; // models x iterations, typical
     const double cap = (double)std::max<uint64_t>(t.opt.max_iterations, 1) * 4.0;
     return (double)std::max<size_t>(t.n, 1) * std::min(its[t.kind], cap);
@@ -2545,9 +2727,10 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
         t_blocking_sync = oversubscribed;
         t_batch_worker = jobs.size() > 1;
         for (auto &grp : jobs[w].groups) {
-            const int rc = grp[0]->refine  ? run_refine_group(grp[0]->kind, grp)
-                           : grp[0]->score ? run_score_group(grp[0]->kind, grp)
-                                           : run_group(grp[0]->kind, grp);
+            const int rc = grp[0]->refine     ? run_refine_group(grp[0]->kind, grp)
+                           : grp[0]->score    ? run_score_group(grp[0]->kind, grp)
+                           : grp[0]->generate ? run_generate_group(grp[0]->kind, grp)
+                                              : run_group(grp[0]->kind, grp);
             if (rc != PLB_OK) {
                 int exp = PLB_OK;
                 if (first_err.compare_exchange_strong(exp, rc)) {
@@ -2666,9 +2849,112 @@ static int score_prepare(const plb_score_problem &p, Task &t) {
     return PLB_OK;
 }
 
+// ---- caller-drawn samples: the estimators' generate_models + score_model (plb_generate_batch) ------------------------
+// One problem checked and turned into the Task of run_generate_group, at the ransac_* level as score_prepare; the
+// sample indices are left to the caller of this function (host form: generate_host_prepare; device form: the device
+// check of run_batch).  Nothing is written here.
+static int generate_prepare(const plb_generate_problem &p, Task &t) {
+    if (p.kind < PLB_KIND_PNP || p.kind > PLB_KIND_HOMOGRAPHY) {
+        g_err = "unknown problem kind";
+        return PLB_ERR_ARG;
+    }
+    if (p.tangent_sampson && p.kind != PLB_KIND_RELPOSE) {
+        g_err = "tangent_sampson is a relative-pose option";
+        return PLB_ERR_ARG;
+    }
+    if (p.real_focal_check && p.kind != PLB_KIND_FUNDAMENTAL) {
+        g_err = "real_focal_check is a fundamental-matrix option";
+        return PLB_ERR_ARG;
+    }
+    if ((p.n > 0 && (!p.a || !p.b)) ||
+        (p.s > 0 && (!p.samples || !p.n_models || !p.models || !p.scores || !p.num_inliers))) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    if (!std::isfinite(p.sq_threshold)) {
+        g_err = "sq_threshold must be finite";
+        return PLB_ERR_ARG;
+    }
+    int kind = p.kind == PLB_KIND_PNP ? KIND_PNP : p.kind == PLB_KIND_RELPOSE ? KIND_RELPOSE
+                                      : p.kind == PLB_KIND_FUNDAMENTAL ? KIND_FUND : KIND_HOMOG;
+    uint64_t sm = 0;
+    if (p.s >= (1ull << 31) || __builtin_mul_overflow(p.s, (uint64_t)kind_max_models(kind) * kind_model_size(kind), &sm) ||
+        sm > SIZE_MAX / sizeof(double)) {
+        g_err = "too many samples";
+        return PLB_ERR_ARG;
+    }
+    if (p.n > (1u << 26)) {
+        g_err = "too many correspondences";
+        return PLB_ERR_ARG;
+    }
+    if (p.tangent_sampson) {
+        if (int r = camera_dev(&p.camera1, &t.cam_a)) return r;
+        if (int r = camera_dev(&p.camera2, &t.cam_b)) return r;
+        kind = KIND_RELPOSE_TS;
+        t.pre_mode = 2;
+    }
+    t.kind = kind;
+    t.generate = true;
+    t.rfc = p.real_focal_check ? 1 : 0;
+    t.a = p.a;
+    t.b = p.b;
+    t.n = (size_t)p.n;
+    t.s = (size_t)p.s;
+    t.samples = p.samples;
+    t.sq_thr = p.sq_threshold;
+    t.n_models = p.n_models;
+    t.gen_models = p.models;
+    t.scores = p.scores;
+    t.counts = p.num_inliers;
+    return PLB_OK;
+}
+// The host form: every index of the host table in [0, n), checked before any device call.
+static int generate_host_prepare(plb_generate_problem &p, Task &t) {
+    if (int r = generate_prepare(p, t)) return r;
+    const size_t cnt = t.s * (size_t)kind_sample_size(t.kind);
+    for (size_t i = 0; i < cnt; ++i)
+        if (t.samples[i] < 0 || (uint64_t)t.samples[i] >= p.n) {
+            g_err = "sample index outside [0, n)";
+            return PLB_ERR_ARG;
+        }
+    return PLB_OK;
+}
+static int generate_device_prepare(plb_generate_problem &p, Task &t) { return generate_prepare(p, t); }
+
+// Step 9 of the device forms: every sample index of the generate tasks in [0, n), by one reduction kernel over all of
+// them, after the work queued on the caller's stream (E.ev_in), and one synchronisation.  The kernels that gather with
+// the indices run only after this has passed.
+static int check_device_samples(const std::vector<Task> &tasks, Engine &E) {
+    int nd = 0;
+    for (const Task &t : tasks) nd += t.generate && t.s > 0;
+    if (!nd) return PLB_OK;
+    int rc;
+    if ((rc = E.tkdesc.ensure(nd)) || (rc = E.h_tkdesc.ensure(nd)) || (rc = E.work.ensure(CTL_WORDS))) return rc;
+    long long max_count = 0;
+    int j = 0;
+    for (const Task &t : tasks)
+        if (t.generate && t.s > 0) {
+            E.h_tkdesc.p[j++] = {t.samples, nullptr, (long long)(t.s * kind_sample_size(t.kind)), (int)t.n, 0};
+            max_count = std::max(max_count, E.h_tkdesc.p[j - 1].count);
+        }
+    PLB_CUDA(cudaMemcpyAsync(E.tkdesc.p, E.h_tkdesc.p, sizeof(TakeDesc) * nd, cudaMemcpyHostToDevice, E.stream));
+    PLB_CUDA(cudaMemsetAsync(E.work.p, 0, sizeof(int), E.stream));
+    PLB_CUDA(cudaStreamWaitEvent(E.stream, E.ev_in, 0));
+    launch_take_samples(E.tkdesc.p, nd, max_count, E.work.p, E.stream);
+    PLB_CUDA(cudaMemcpyAsync(E.h_work.p, E.work.p, sizeof(int), cudaMemcpyDeviceToHost, E.stream));
+    PLB_CUDA(cudaStreamSynchronize(E.stream));
+    PLB_CUDA(cudaGetLastError());
+    if (E.h_work.p[0]) {
+        g_err = "sample index outside [0, n)";
+        return PLB_ERR_ARG;
+    }
+    return PLB_OK;
+}
+
 // What is wrong with the memory of a device-form task, or null.  Sized by n (n > 0): a, b and the weights, when given,
 // must be device (or managed) memory of `device` aligned to the dtype's `elem` bytes; sized by m (m > 0): models, scores
-// and counts, 8-byte aligned; the inliers the task writes must be device memory.
+// and counts, 8-byte aligned; the inliers the task writes must be device memory; sized by s (s > 0, generate tasks):
+// samples and n_models 4-byte, models, scores and counts 8-byte aligned.
 static const char *device_io_error(const Task &t, int device, size_t elem) {
     if (t.n > 0)
         for (const void *q : {(const void *)t.a, (const void *)t.b, t.weights}) {
@@ -2684,6 +2970,16 @@ static const char *device_io_error(const Task &t, int device, size_t elem) {
         }
     if (t.n > 0 && t.inliers && !device_memory(t.inliers, device))
         return "inliers must be NULL or device memory of the current device";
+    if (t.generate && t.s > 0) {
+        for (const void *q : {(const void *)t.samples, (const void *)t.n_models}) {
+            if (!device_memory(q, device)) return "samples / n_models must be device memory of the current device";
+            if ((uintptr_t)q % sizeof(int32_t)) return "samples / n_models are not 4-byte aligned";
+        }
+        for (const void *q : {(const void *)t.gen_models, (const void *)t.scores, (const void *)t.counts}) {
+            if (!device_memory(q, device)) return "models / scores / num_inliers must be device memory of the current device";
+            if ((uintptr_t)q % sizeof(double)) return "models / scores / num_inliers are not 8-byte aligned";
+        }
+    }
     return nullptr;
 }
 
@@ -2691,7 +2987,7 @@ static const char *device_io_error(const Task &t, int device, size_t elem) {
 // PLB_ERR_ARG, writing nothing; then each failure writes its code into every status and nothing else:
 //   an unknown dtype (device forms); prepare() of each problem in order, the first failure's code; n_gpus < min_gpus;
 //   no device (PLB_ERR_CUDA); n_gpus above the device count; resident correspondences on a device the call does not
-//   use; device forms: device_io_error of each task.
+//   use; device forms: device_io_error of each task, then the sample indices of the generate tasks on the device.
 // Then the caller's stream gets the event the groups wait on (device forms), the tasks' writes are committed, the tasks
 // run, every status gets the result, and on success every task gets its post-step.
 // n_gpus: -1 the calling thread's device, 0 every device of the process, k the first k.  dtype: PLB_DTYPE_* of a device
@@ -2748,6 +3044,7 @@ static int run_batch(P *problems, size_t count, Prepare prepare, int n_gpus, int
             t.f32 = dtype == PLB_DTYPE_F32;
             t.ready = E->ev_in;
         }
+        if (int rc = check_device_samples(tasks, *E)) return fail_all(rc, g_err);
     }
     for (Task &t : tasks) commit_task(t);
     const int rc = run_tasks(tasks, dev_of, devs.data(), (int)devs.size(), streams);
@@ -2795,6 +3092,16 @@ int plb_score_batch(plb_score_problem *problems, size_t count, int n_gpus, int s
 // engine's input buffer, k_score reads the caller's models and writes the caller's records and masks.
 int plb_score_batch_device(plb_score_problem *problems, size_t count, int dtype, void *stream, int streams) {
     return run_batch(problems, count, score_prepare, -1, -1, streams, dtype, stream);
+}
+
+int plb_generate_batch(plb_generate_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, generate_host_prepare, n_gpus, -1, streams_per_gpu);
+}
+// The same on the calling thread's device with everything sized by n or s in its memory: the indices are range-checked
+// by one kernel before anything gathers with them, k_take_samples copies them into the round's table and k_put_hyps
+// writes the records into the caller's rows.
+int plb_generate_batch_device(plb_generate_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    return run_batch(problems, count, generate_device_prepare, -1, -1, streams, dtype, stream);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {

@@ -1711,6 +1711,67 @@ void launch_hypotheses(int kind, const RoundDesc &R, const HypOut &out, int mode
     cudaMemsetAsync(out.prob_count, 0, sizeof(int) * R.n_active, stream);
     with_kind(kind, [&](auto K) { launch_hyp_t<K>(R, out, mode, max_n_pad, fctx, stream, ev_between); });
 }
+
+// ---- caller-drawn samples (plb_generate_batch): the round's sample table in, its records out ------------------------
+// One problem per blockIdx.y (strided: a check covers every problem of a call), blockIdx.x strides over its indices.
+// CHECK writes nothing but the flag, so an index outside [0, n) is found before any kernel gathers with it.
+template <bool CHECK>
+__global__ void __launch_bounds__(256) k_take_samples(const TakeDesc *__restrict__ descs, int n_desc, int *bad) {
+    for (int d = blockIdx.y; d < n_desc; d += gridDim.y) {
+        const TakeDesc D = descs[d];
+        for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < D.count; i += (long long)gridDim.x * 256) {
+            const int32_t v = D.src[i];
+            if (CHECK) {
+                if (v < 0 || v >= D.n) *bad = 1;
+            } else {
+                D.dst[i] = (uint32_t)v;
+            }
+        }
+    }
+}
+void launch_take_samples(const TakeDesc *descs_dev, int n_desc, long long max_count, int *bad, cudaStream_t stream) {
+    if (n_desc <= 0 || max_count <= 0) return;
+    const dim3 grid((unsigned)std::min<long long>((max_count + 255) / 256, 512), (unsigned)std::min(n_desc, 65535), 1);
+    if (bad)
+        k_take_samples<true><<<grid, 256, 0, stream>>>(descs_dev, n_desc, bad);
+    else
+        k_take_samples<false><<<grid, 256, 0, stream>>>(descs_dev, n_desc, nullptr);
+}
+// One thread per sample g of the round: its n_models[g] models of slots [first_slot[g], first_slot[g] + n_models[g]) with
+// their exact records, into row j = g - g_off[a] of active problem a's descriptor (direct), or packed: problem a's used
+// segment prefix moves to cbase[a] (the models of the problems before it), slot order kept.
+__global__ void __launch_bounds__(256) k_put_hyps(const RoundDesc R, const HypOut out, const PutDesc *__restrict__ descs,
+                                                  int msz, int maxm, int packed) {
+    extern __shared__ int cbase[]; // packed: n_active entries
+    if (packed && threadIdx.x == 0)
+        for (int a = 0, c = 0; a < R.n_active; ++a) {
+            cbase[a] = c;
+            c += seg_models(out, a);
+        }
+    __syncthreads();
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= R.n_total) return;
+    const int a = sample_problem_slot(R, g);
+    const int j = g - __ldg(R.g_off + a);
+    const PutDesc &D = descs[a];
+    const int nm = out.n_models[g], fs = out.first_slot[g];
+    const long long o = packed ? (long long)cbase[a] + fs - __ldg(out.seg_base + a) : (long long)j * maxm;
+    D.n_models[j] = nm;
+    if (packed) D.offsets[j] = (int)o;
+    double *models = D.models + o * msz, *scores = D.scores + o;
+    long long *counts = D.counts + o;
+    for (int m = 0; m < nm; ++m) {
+        for (int k = 0; k < msz; ++k) models[m * msz + k] = out.models[(size_t)(fs + m) * msz + k];
+        scores[m] = out.scores[fs + m];
+        counts[m] = out.counts[fs + m];
+    }
+}
+void launch_put_hyps(const RoundDesc &R, const HypOut &out, const PutDesc *descs_dev, int msz, int maxm, bool packed,
+                     cudaStream_t stream) {
+    if (R.n_total <= 0) return;
+    const size_t smem = packed ? sizeof(int) * (size_t)R.n_active : 0;
+    k_put_hyps<<<(R.n_total + 255) / 256, 256, smem, stream>>>(R, out, descs_dev, msz, maxm, packed ? 1 : 0);
+}
 void launch_confirm(int kind, const ProblemDev *probs, const SelectArgs &A, const double *models, cudaStream_t stream) {
     if (A.na <= 0) return;
     int gx = (8 * sm_count() + A.na - 1) / A.na;

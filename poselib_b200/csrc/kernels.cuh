@@ -254,6 +254,27 @@ struct ScoreDesc {
     uint32_t *counts32; // when counts is null: the counts as uint32 (the round's record layout)
 };
 
+// Caller-drawn sample indices of one problem (plb_generate_batch_device): `count` int32 indices at src, copied to the
+// round's sample table at dst, or (the argument check) tested against [0, n).
+struct TakeDesc {
+    const int32_t *src;
+    uint32_t *dst;
+    long long count;
+    int n;
+    int reserved;
+};
+// Where the records of one active problem of a generate chunk go.  Direct (the device form): row j of the caller's arrays
+// holds sample j's n_models[j] models, maxm slots per row.  Packed (the host form): every problem of the chunk shares
+// one staging buffer, models packed problem after problem; n_models[j] and offsets[j] give sample j's count and first
+// packed slot.
+struct PutDesc {
+    int *n_models;
+    int *offsets;     // packed only
+    double *models;
+    double *scores;
+    long long *counts;
+};
+
 // ---- launchers (all asynchronous on `stream`) --------------------------------------------------------------
 // normalize_points for n_desc problems (descriptors in device memory), one CTA each.
 void launch_normalize(const NormDesc *descs_dev, int n_desc, cudaStream_t stream);
@@ -327,6 +348,13 @@ void launch_pack_mask(const char *mask, uint32_t *bits, size_t n_bytes, cudaStre
 void launch_ingest(const IngestDesc *descs_dev, int n_desc, size_t max_vals, cudaStream_t stream);
 // Final masks straight into the callers' device buffers for n_desc problems; max_n: the largest n of the descriptors.
 void launch_scatter_masks(const char *mask, const ScatterDesc *descs_dev, int n_desc, int max_n, cudaStream_t stream);
+// Caller-drawn samples for n_desc problems (descriptors in device memory); max_count: the largest count.  bad null: copy
+// them into the round's sample table; bad non-null: copy nothing and set *bad to 1 when some index is outside [0, n).
+void launch_take_samples(const TakeDesc *descs_dev, int n_desc, long long max_count, int *bad, cudaStream_t stream);
+// The records of the round's samples (after launch_hypotheses in mode 0) into the layout of descs_dev[a] for active
+// problem a: direct rows of maxm slots, or packed (see PutDesc).
+void launch_put_hyps(const RoundDesc &R, const HypOut &out, const PutDesc *descs_dev, int msz, int maxm, bool packed,
+                     cudaStream_t stream);
 // Batched direct solver calls (solvers/*.h surface): one thread per instance.  kind KIND_RELPOSE also needs the s5_*
 // phase buffers of s5 for `count` instances (the other fields are unused).  Returns the number of kernels launched.
 int launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out, int *n_out,
