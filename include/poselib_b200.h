@@ -296,7 +296,8 @@ int plb_refine_homography_weighted(const double *x1_xy, const double *x2_xy, siz
 
 /* ---- batch of independent problems (BASELINE config 5); sharded by the caller across GPUs ---------- */
 /* Every batch call below (plb_ransac_batch[_multi], plb_estimate_batch[_device], plb_refine_batch[_device],
- * plb_score_batch[_device], plb_generate_batch[_device]) checks its arguments in one order, before any copy or launch:
+ * plb_score_batch[_device], plb_generate_batch[_device], plb_camera_batch[_device]) checks its arguments in one order,
+ * before any copy or launch:
  *   1. count 0 -> PLB_OK, nothing written;
  *   2. problems NULL -> PLB_ERR_ARG, nothing written;
  *   3. device forms: a dtype other than PLB_DTYPE_F64 / PLB_DTYPE_F32 -> PLB_ERR_ARG;
@@ -537,6 +538,45 @@ int plb_generate_batch(plb_generate_problem *problems, size_t count, int n_gpus,
  * complete.  A pointer that is not device memory of the current device or is misaligned -> PLB_ERR_ARG (step 8); the
  * sample indices are range-checked on the device (step 9). */
 int plb_generate_batch_device(plb_generate_problem *problems, size_t count, int dtype, void *stream, int streams);
+
+/* The Camera functions of misc/camera_models.h over many points of many cameras, for callers who undistort keypoints,
+ * need normalised image coordinates or reprojections, or Jacobians for their own optimisers.  Per point:
+ *   op                    jac and jac_params NULL                  either given
+ *   PLB_CAMOP_PROJECT     Camera::project (camera_models.cc:149-161)  Camera::project_with_jac (:162-175)
+ *   PLB_CAMOP_UNPROJECT   Camera::unproject to a bearing (:176-188)  Camera::unproject_with_jac (:190-203)
+ *   PLB_CAMOP_UNPROJECT_2D the 2D unproject wrapper, hnormalized (camera_models.h:98-102)   (not allowed)
+ * `out` receives the point the function of the row writes (the point of a *_with_jac call is not claimed to equal the
+ * plain call's).  jac_params without jac is the reference's call with jac = nullptr.  Matrices are column-major, as
+ * Eigen stores them: jac 2x3 (PROJECT) or 3x2 (UNPROJECT) per point, jac_params 2 x P or 3 x P, P the model's parameter
+ * count (the NULL camera has P = 0 and writes no parameter Jacobian).  The 2D project wrapper, which normalises through
+ * Eigen's unpinned summation order, is not offered.  None of the outputs depends on the rest of the batch, n_gpus,
+ * streams, the mode or the form of the call. */
+enum { PLB_CAMOP_PROJECT = 0, PLB_CAMOP_UNPROJECT = 1, PLB_CAMOP_UNPROJECT_2D = 2 };
+typedef struct plb_camera_problem {
+    int32_t op;               /* PLB_CAMOP_* */
+    int32_t reserved;
+    uint64_t n;
+    plb_camera camera;
+    const double *in;         /* PROJECT: n x 3 camera-frame points; UNPROJECT[_2D]: n x 2 pixels; row-major */
+    double *out;              /* out: PROJECT n x 2 pixels; UNPROJECT n x 3 bearings; UNPROJECT_2D n x 2 */
+    double *jac;              /* out: NULL, or n Jacobians w.r.t. the point, 2x3 (PROJECT) / 3x2 (UNPROJECT) */
+    double *jac_params;       /* out: NULL, or n Jacobians w.r.t. the parameters, 2 x P / 3 x P */
+    int32_t status;           /* out */
+    int32_t reserved2;
+} plb_camera_problem;
+/* n_gpus: 0 = every device of the process, k > 0 = the first k, -1 = the calling thread's device (plb_set_device);
+ * streams_per_gpu groups of problems are in flight on each device.  Every pointer is host memory.
+ * Each problem is checked: an unknown op, in / out NULL with n > 0, jac or jac_params with PLB_CAMOP_UNPROJECT_2D, or
+ * n x (the widest of its rows) doubles overflowing size_t bytes -> PLB_ERR_ARG; a camera outside the ten models ->
+ * PLB_ERR_NYI (the reference's "NYI", camera_models.cc:157-158).  n = 0 writes nothing. */
+int plb_camera_batch(plb_camera_problem *problems, size_t count, int n_gpus, int streams_per_gpu);
+/* plb_camera_batch(problems, count, -1, streams) with in, out, jac and jac_params in device (or managed) memory of the
+ * calling thread's device: `in` a contiguous array of `dtype` aligned to it (PLB_DTYPE_F32: `const float *` cast into
+ * the `const double *` field; widened exactly, so a float call gives the double call's results on the widened values),
+ * out / jac / jac_params fp64, 8-byte aligned.  Nothing sized by n crosses PCIe.  Inputs are read after the work queued
+ * on `stream` ahead of the call; when the call returns, every device write it made is complete.  A pointer that is not
+ * device memory of the current device or is misaligned -> PLB_ERR_ARG (step 8). */
+int plb_camera_batch_device(plb_camera_problem *problems, size_t count, int dtype, void *stream, int streams);
 
 /* Correspondences kept resident in HBM across calls (measurement of the device-resident throughput, and callers
  * that run several estimations on the same matches).  kind: PLB_KIND_*; returns a handle > 0 or an error < 0. */

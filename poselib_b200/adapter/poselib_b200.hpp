@@ -642,4 +642,91 @@ ScoreResult score_homographies(const std::vector<P2> &x1, const std::vector<P2> 
     return detail::score_models(q, detail::matrix_rows(H), want_inliers);
 }
 
+// ---- Camera::project / unproject over many cameras (plb_camera_batch) ------------------------------------------------
+// The vector forms of Camera::project, project_with_jac (misc/camera_models.cc:205-251), unproject and unproject_with_jac
+// (:253-300) for many cameras in one call: camera i's points x[i] -> (*out)[i], with (*jac)[i] and (*jac_params)[i] when
+// those are given.  P2 / P3 are dense 2- / 3-vectors of doubles, J a dense column-major 2x3 (project) or 3x2
+// (unproject) matrix of doubles (Eigen::Matrix<double, 2, 3> / <3, 2>), JP a matrix with resize(rows, cols) and a
+// column-major data() (Eigen::Matrix<double, 2 | 3, Eigen::Dynamic>).  These are separate names on purpose: the drop-in
+// does not redefine Camera's members, which PoseLib's own CPU code calls one point at a time.
+namespace detail {
+struct Mat6 { // the type of an absent point Jacobian argument
+    double d[6];
+};
+struct DynMat { // the type of an absent parameter Jacobian argument
+    std::vector<double> v;
+    void resize(int r, int c) { v.resize((size_t)r * c); }
+    double *data() { return v.data(); }
+};
+inline int camera_num_params(int model_id) {
+    switch (model_id) {
+    case PLB_CAMERA_SIMPLE_PINHOLE: return 3;
+    case PLB_CAMERA_PINHOLE: case PLB_CAMERA_SIMPLE_RADIAL: case PLB_CAMERA_SIMPLE_RADIAL_FISHEYE:
+    case PLB_CAMERA_SIMPLE_DIVISION: return 4;
+    case PLB_CAMERA_RADIAL: case PLB_CAMERA_RADIAL_FISHEYE: case PLB_CAMERA_DIVISION: return 5;
+    case PLB_CAMERA_OPENCV: return 8;
+    default: return 0;
+    }
+}
+template <typename Camera, typename In, typename Out, typename J, typename JP>
+void camera_points(int op, const std::vector<Camera> &cameras, const std::vector<std::vector<In>> &x,
+                   std::vector<std::vector<Out>> *out, std::vector<std::vector<J>> *jac,
+                   std::vector<std::vector<JP>> *jac_params) {
+    const int in_w = op == PLB_CAMOP_PROJECT ? 3 : 2, out_w = op == PLB_CAMOP_PROJECT ? 2 : 3, rows = out_w;
+    static_assert(sizeof(J) == 6 * sizeof(double), "dense 2x3 / 3x2 Jacobians of doubles required");
+    if (sizeof(In) != in_w * sizeof(double) || sizeof(Out) != out_w * sizeof(double))
+        throw std::invalid_argument("poselib_b200: dense point layout required");
+    if (x.size() != cameras.size()) throw std::invalid_argument("poselib_b200: one point list per camera required");
+    const size_t count = cameras.size();
+    std::vector<plb_camera_problem> P(count);
+    std::vector<std::vector<double>> jp(count);
+    out->resize(count);
+    if (jac) jac->resize(count);
+    if (jac_params) jac_params->resize(count);
+    for (size_t i = 0; i < count; ++i) {
+        plb_camera_problem &q = P[i] = plb_camera_problem();
+        const size_t n = x[i].size();
+        q.op = op;
+        q.n = n;
+        q.camera = camera_to_c(cameras[i]);
+        q.in = raw(x[i]);
+        (*out)[i].resize(n);
+        q.out = n ? reinterpret_cast<double *>((*out)[i].data()) : nullptr;
+        if (jac) {
+            (*jac)[i].resize(n);
+            q.jac = n ? reinterpret_cast<double *>((*jac)[i].data()) : nullptr;
+        }
+        if (jac_params) {
+            jp[i].assign(n * rows * camera_num_params(q.camera.model_id) + 1, 0.0);
+            q.jac_params = jp[i].data();
+        }
+    }
+    check(plb_camera_batch(P.data(), count, -1, 1));
+    if (!jac_params) return;
+    for (size_t i = 0; i < count; ++i) {
+        const int np = camera_num_params(P[i].camera.model_id);
+        std::vector<JP> &dst = (*jac_params)[i];
+        dst.resize(x[i].size());
+        for (size_t k = 0; k < dst.size(); ++k) {
+            dst[k].resize(rows, np);
+            for (int e = 0; e < rows * np; ++e) dst[k].data()[e] = jp[i][k * rows * np + e];
+        }
+    }
+}
+} // namespace detail
+// Camera::project (jac and jac_params null) or project_with_jac of each camera's points x[i] -> xp[i]
+template <typename Camera, typename P3, typename P2, typename J = detail::Mat6, typename JP = detail::DynMat>
+void project_points(const std::vector<Camera> &cameras, const std::vector<std::vector<P3>> &x,
+                    std::vector<std::vector<P2>> *xp, std::vector<std::vector<J>> *jac = nullptr,
+                    std::vector<std::vector<JP>> *jac_params = nullptr) {
+    detail::camera_points(PLB_CAMOP_PROJECT, cameras, x, xp, jac, jac_params);
+}
+// Camera::unproject to bearings (jac and jac_params null) or unproject_with_jac of each camera's pixels xp[i] -> x[i]
+template <typename Camera, typename P2, typename P3, typename J = detail::Mat6, typename JP = detail::DynMat>
+void unproject_points(const std::vector<Camera> &cameras, const std::vector<std::vector<P2>> &xp,
+                      std::vector<std::vector<P3>> *x, std::vector<std::vector<J>> *jac = nullptr,
+                      std::vector<std::vector<JP>> *jac_params = nullptr) {
+    detail::camera_points(PLB_CAMOP_UNPROJECT, cameras, xp, x, jac, jac_params);
+}
+
 } // namespace poselib_b200

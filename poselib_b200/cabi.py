@@ -106,6 +106,7 @@ EXPORTS = [
     "plb_refine_relpose_cameras_weighted", "plb_refine_relpose_pair_weighted", "plb_refine_fundamental_weighted",
     "plb_refine_homography_weighted", "plb_estimate_batch_device", "plb_refine_batch", "plb_refine_batch_device",
     "plb_score_batch", "plb_score_batch_device", "plb_generate_batch", "plb_generate_batch_device",
+    "plb_camera_batch", "plb_camera_batch_device",
 ]
 DTYPE_F64, DTYPE_F32 = 0, 1
 
@@ -144,6 +145,16 @@ class GenerateProblem(C.Structure):
                 ("sq_threshold", C.c_double), ("n_models", C.POINTER(C.c_int32)), ("models", C.POINTER(C.c_double)),
                 ("scores", C.POINTER(C.c_double)), ("num_inliers", C.POINTER(C.c_int64)), ("status", C.c_int32),
                 ("reserved2", C.c_int32)]
+
+
+class CameraProblem(C.Structure):
+    _fields_ = [("op", C.c_int32), ("reserved", C.c_int32), ("n", C.c_uint64), ("camera", Camera),
+                ("in_", C.POINTER(C.c_double)), ("out", C.POINTER(C.c_double)), ("jac", C.POINTER(C.c_double)),
+                ("jac_params", C.POINTER(C.c_double)), ("status", C.c_int32), ("reserved2", C.c_int32)]
+
+
+# plb_camera_problem::op
+CAMOP = {"project": 0, "unproject": 1, "unproject_2d": 2}
 
 
 # plb_generate_problem: indices per sample (k) and model slots per sample (M) of each kind
@@ -984,6 +995,103 @@ def generate_batch_device(problems, stream=None, streams=8):
                         "scores": scores[i].view(ss[i], Ms[i]), "num_inliers": counts[i].view(ss[i], Ms[i])})
     _check(_lib.plb_generate_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
                                           int(streams)))
+    for r, q in zip(out, arr):
+        r["status"] = q.status
+    return out
+
+
+# ---- the camera functions over many points (plb_camera_batch) ----------------------------------------------------
+def _camera_shapes(op, cam):
+    """Row widths of one camera problem: input, output, and the Jacobians' (rows, columns) as the C-ABI stores them
+    column-major per point."""
+    P = CAMERA_NUM_PARAMS.get(int(cam.model_id), 0)
+    if op == "project":
+        return 3, 2, (2, 3), (2, P)
+    return 2, 3 if op == "unproject" else 2, (3, 2), (3, P)
+
+
+def _camera_mats(m, n, rc):
+    """n column-major rows x cols matrices -> [n, rows, cols] [r,c] (a view)."""
+    return m.reshape(n, rc[1], rc[0]).swapaxes(-1, -2)
+
+
+def camera_batch(problems, n_gpus=-1, streams=8):
+    """PoseLib's Camera functions over many points of many cameras (plb_camera_batch).  problems: list of dict(op [a
+    CAMOP key], cam [Camera], x [n,3] camera-frame points (project) or [n,2] pixels (unproject, unproject_2d), jac=False,
+    jac_params=False).  project / unproject with jac or jac_params are project_with_jac / unproject_with_jac.
+    n_gpus: -1 current device, 0 all devices, k the first k.  Returns list of dict(out [n,2] / [n,3], jac [n,2,3] /
+    [n,3,2] or None, jac_params [n,2,P] / [n,3,P] or None, all [r,c], status)."""
+    count = len(problems)
+    arr = (CameraProblem * count)()
+    out = []
+    keep = []
+    for i, p in enumerate(problems):
+        q = arr[i]
+        op, cam = p["op"], p["cam"]
+        iw, ow, jrc, prc = _camera_shapes(op, cam)
+        xa = np.ascontiguousarray(np.asarray(p["x"], dtype=np.float64).reshape(-1, iw))
+        n = len(xa)
+        r = {"out": np.zeros((n, ow)),
+             "jac": np.zeros(n * 6) if p.get("jac") else None,
+             "jac_params": np.zeros(n * prc[0] * prc[1]) if p.get("jac_params") else None}
+        keep.append(xa)
+        out.append(r)
+        q.op, q.n, q.camera = CAMOP.get(op, -1) if isinstance(op, str) else int(op), n, cam
+        q.in_, q.out = xa.ctypes.data_as(_P), r["out"].ctypes.data_as(_P)
+        q.jac = r["jac"].ctypes.data_as(_P) if r["jac"] is not None else None
+        q.jac_params = r["jac_params"].ctypes.data_as(_P) if r["jac_params"] is not None else None
+    _check(_lib.plb_camera_batch(arr, C.c_size_t(count), int(n_gpus), int(streams)))
+    for p, r, q in zip(problems, out, arr):
+        _, _, jrc, prc = _camera_shapes(p["op"], p["cam"])
+        n = len(r["out"])
+        if r["jac"] is not None:
+            r["jac"] = _camera_mats(r["jac"], n, jrc)
+        if r["jac_params"] is not None:
+            r["jac_params"] = _camera_mats(r["jac_params"], n, prc)
+        r["status"] = q.status
+    return out
+
+
+def camera_batch_device(problems, stream=None, streams=8):
+    """camera_batch (n_gpus=-1) with everything on the GPU (plb_camera_batch_device).  problems: the dicts camera_batch
+    takes, with x a CUDA torch tensor, all of one device and one dtype, float32 or float64.  The call runs on that device
+    and reads the inputs after the work queued on `stream` (a torch.cuda.Stream or a cudaStream_t handle; default: the
+    device's current stream).  Returns the dicts of camera_batch with CUDA float64 tensors (the outputs of one call are
+    views of one allocation per field)."""
+    import torch
+    form = _device_form("camera_batch_device", "x", [p["x"] for p in problems], stream=stream)
+    if form is None:
+        return []
+    dev, dtype, stream = form
+    count = len(problems)
+    arr = (CameraProblem * count)()
+    keep = []
+    out = []
+    ptr = lambda t: C.cast(C.c_void_p(t.data_ptr() if t is not None and t.numel() else None), _P)
+    with torch.cuda.stream(stream):  # the copies and outputs below are ordered before the call's reads and writes
+        shapes = [_camera_shapes(p["op"], p["cam"]) for p in problems]
+        xs = [p["x"].reshape(-1, sh[0]).contiguous() for p, sh in zip(problems, shapes)]
+        ns = [len(x) for x in xs]
+        outs = torch.zeros(sum(n * sh[1] for n, sh in zip(ns, shapes)), dtype=torch.float64, device=dev).split(
+            [n * sh[1] for n, sh in zip(ns, shapes)])
+        jsz = [n * 6 if p.get("jac") else 0 for n, p in zip(ns, problems)]
+        psz = [n * sh[3][0] * sh[3][1] if p.get("jac_params") else 0 for n, sh, p in zip(ns, shapes, problems)]
+        jacs = torch.zeros(sum(jsz), dtype=torch.float64, device=dev).split(jsz)
+        jps = torch.zeros(sum(psz), dtype=torch.float64, device=dev).split(psz)
+        for i, p in enumerate(problems):
+            q = arr[i]
+            op, n, (iw, ow, jrc, prc) = p["op"], ns[i], shapes[i]
+            keep.append(xs[i])
+            q.op, q.n, q.camera = CAMOP.get(op, -1) if isinstance(op, str) else int(op), n, p["cam"]
+            q.in_, q.out = ptr(xs[i]), ptr(outs[i])
+            # a requested Jacobian with P = 0 (the NULL camera) still passes a pointer, as the host form does
+            q.jac = ptr(jacs[i]) if p.get("jac") else None
+            q.jac_params = C.cast(C.c_void_p(jps[i].data_ptr() or None), _P) if p.get("jac_params") else None
+            out.append({"out": outs[i].view(n, ow),
+                        "jac": _camera_mats(jacs[i], n, jrc) if p.get("jac") else None,
+                        "jac_params": _camera_mats(jps[i], n, prc) if p.get("jac_params") else None})
+    _check(_lib.plb_camera_batch_device(arr, C.c_size_t(count), dtype, C.c_void_p(stream.cuda_stream or None),
+                                        int(streams)))
     for r, q in zip(out, arr):
         r["status"] = q.status
     return out

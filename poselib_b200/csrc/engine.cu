@@ -251,6 +251,11 @@ struct Engine {
     DevBuf<double> gen_stage;
     PinBuf<double> h_gen_stage;
     MapBuf<int> h_gen;
+    // camera functions (plb_camera_batch): the descriptors and the host form's outputs (inputs go up through in / h_in)
+    DevBuf<CamOpDesc> cdesc;
+    PinBuf<CamOpDesc> h_cdesc;
+    DevBuf<double> cam_res;
+    PinBuf<double> h_cam_res;
     DevBuf<LmJob> jobs;
     PinBuf<double> h_in, h_lm_in;
     PinBuf<int> h_act, h_work;
@@ -608,6 +613,11 @@ struct Task {
     const int32_t *samples = nullptr;
     int32_t *n_models = nullptr;
     double *gen_models = nullptr;
+    // Camera functions instead of LO-RANSAC (run_camera_group): op (CAMOP_*) of camera cam_a over the n points at `a`,
+    // outputs to cam_out, and the Jacobians to cam_jac / cam_jac_params when they are given.
+    bool camop = false;
+    int cam_op = 0;
+    double *cam_out = nullptr, *cam_jac = nullptr, *cam_jac_params = nullptr;
     // doubles per correspondence the group uploads: the caller layout, then the weight
     size_t in_per_point(int in_arr) const { return (size_t)in_arr + (weights ? 1 : 0); }
 };
@@ -1231,6 +1241,92 @@ struct Group {
                 for (int k = 0; k < S.n; ++k) dst[k] = (char)((w[k >> 5] >> (k & 31)) & 1u);
             }
             maskoff += t.m * (size_t)S.n_pad;
+        }
+        return PLB_OK;
+    }
+    // ---- camera functions (plb_camera_batch): one k_camera launch over the group's (problem, tile) list, one wait -----
+    // Host tasks: every input goes up in one copy from a pinned staging buffer, and every output (per task its points,
+    // then the Jacobians it asks for) comes back in one copy that the host spreads over the callers' arrays.  Device
+    // tasks: after the caller's stream event, k_camera reads and writes the callers' arrays directly.
+    int camera() {
+        const Task &t0 = *PS[0].t; // a group's tasks share the op, the form and whether they want Jacobians
+        const bool host = !t0.dev_io;
+        const int op = t0.cam_op, in_w = op == CAMOP_PROJECT ? 3 : 2, out_w = op == CAMOP_UNPROJECT ? 3 : 2;
+        const size_t jp_rows = op == CAMOP_PROJECT ? 2 : 3;
+        auto res_w = [&](const Task &t) { // doubles per point of the task's outputs
+            return (size_t)out_w + (t.cam_jac ? 6 : 0) + (t.cam_jac_params ? jp_rows * cam_num_params(t.cam_a.model) : 0);
+        };
+        std::vector<int> order;
+        size_t in_total = 0, res_total = 0;
+        for (int i = 0; i < NP; ++i)
+            if (PS[i].t->n > 0) {
+                order.push_back(i);
+                in_total += PS[i].t->n * in_w;
+                res_total += PS[i].t->n * res_w(*PS[i].t);
+            }
+        const int nd = (int)order.size();
+        if (!nd) return PLB_OK;
+        int rc;
+        if ((rc = E.cdesc.ensure(nd)) || (rc = E.h_cdesc.ensure(nd))) return rc;
+        if (host && ((rc = E.in.ensure(in_total)) || (rc = E.h_in.ensure(in_total)) || (rc = E.cam_res.ensure(res_total)) ||
+                     (rc = E.h_cam_res.ensure(res_total))))
+            return rc;
+        size_t in_off = 0, res_off = 0;
+        long long tiles = 0;
+        for (int j = 0; j < nd; ++j) {
+            const Task &t = *PS[order[j]].t;
+            CamOpDesc &D = E.h_cdesc.p[j];
+            D.cam = t.cam_a;
+            D.n = (long long)t.n;
+            D.tile0 = tiles;
+            tiles += (D.n + CAM_TILE - 1) / CAM_TILE;
+            if (host) {
+                std::memcpy(E.h_in.p + in_off, t.a, sizeof(double) * t.n * in_w);
+                D.in = E.in.p + in_off;
+                double *r = E.cam_res.p + res_off;
+                D.out = r;
+                r += t.n * out_w;
+                D.jac = t.cam_jac ? r : nullptr;
+                r += t.cam_jac ? t.n * 6 : 0;
+                D.jac_params = t.cam_jac_params ? r : nullptr;
+                in_off += t.n * in_w;
+                res_off += t.n * res_w(t);
+            } else {
+                D.in = t.a;
+                D.out = t.cam_out;
+                D.jac = t.cam_jac;
+                D.jac_params = t.cam_jac_params;
+            }
+        }
+        if (host) {
+            PLB_CUDA(cudaMemcpyAsync(E.in.p, E.h_in.p, sizeof(double) * in_total, cudaMemcpyHostToDevice, st));
+            h2d += sizeof(double) * in_total;
+        } else {
+            PLB_CUDA(cudaStreamWaitEvent(st, t0.ready, 0));
+        }
+        PLB_CUDA(cudaMemcpyAsync(E.cdesc.p, E.h_cdesc.p, sizeof(CamOpDesc) * nd, cudaMemcpyHostToDevice, st));
+        h2d += sizeof(CamOpDesc) * nd;
+        launch_camera(op, t0.cam_jac || t0.cam_jac_params, t0.f32, E.cdesc.p, nd, tiles, st);
+        E.launches++;
+        if (host) {
+            PLB_CUDA(cudaMemcpyAsync(E.h_cam_res.p, E.cam_res.p, sizeof(double) * res_total, cudaMemcpyDeviceToHost, st));
+            d2h += sizeof(double) * res_total;
+        }
+        if ((rc = sync())) return rc;
+        PLB_CUDA(cudaGetLastError());
+        if (!host) return PLB_OK;
+        res_off = 0;
+        for (int i : order) {
+            const Task &t = *PS[i].t;
+            const double *r = E.h_cam_res.p + res_off;
+            std::copy(r, r + t.n * out_w, t.cam_out);
+            r += t.n * out_w;
+            if (t.cam_jac) {
+                std::copy(r, r + t.n * 6, t.cam_jac);
+                r += t.n * 6;
+            }
+            if (t.cam_jac_params) std::copy(r, r + t.n * jp_rows * cam_num_params(t.cam_a.model), t.cam_jac_params);
+            res_off += t.n * res_w(t);
         }
         return PLB_OK;
     }
@@ -2013,6 +2109,15 @@ static int run_generate_group(int kind, std::vector<Task *> &tasks) {
     return PLB_OK;
 }
 
+// Runs a group of camera tasks of one op (Task::camop), all with or all without Jacobians: one k_camera launch
+// (Group::camera).  The group's kind is unused.
+static int run_camera_group(std::vector<Task *> &tasks) {
+    Group G(KIND_PNP, tasks);
+    int rc;
+    if ((rc = G.init()) || (rc = G.camera())) return rc;
+    return PLB_OK;
+}
+
 // plb_camera -> CamDev; models outside the ten on the path (cam_layout) are rejected like Camera::unproject's "NYI"
 // (misc/camera_models.cc:176-188)
 static int camera_dev(const plb_camera *c, CamDev *out) {
@@ -2654,6 +2759,7 @@ static double task_cost(const Task &t) {
     if (t.refine) return (double)std::max<size_t>(t.n, 1) * (double)std::max<uint64_t>(t.polish.bundle.max_iterations, 1);
     if (t.score) return (double)std::max<size_t>(t.n, 1) * (double)std::max<size_t>(t.m, 1);
     if (t.generate) return (double)std::max<size_t>(t.n, 1) * (double)std::max<size_t>(t.s, 1) * kind_max_models(t.kind);
+    if (t.camop) return (double)std::max<size_t>(t.n, 1);
     static const double its[5] = {4.0 * 1000, 0.5 * 14000, 2.0 * 30000, 1.0 * 1000, 0.5 * 14000}; // models x iterations, typical
     const double cap = (double)std::max<uint64_t>(t.opt.max_iterations, 1) * 4.0;
     return (double)std::max<size_t>(t.n, 1) * std::min(its[t.kind], cap);
@@ -2687,7 +2793,11 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
             }
         }
     }
-    // groups per device: tasks of the same engine kind run in lock-step (refiner tasks: in one LM phase)
+    // groups per device: tasks of the same engine kind run in lock-step (refiner tasks: in one LM phase); camera tasks
+    // form groups of one op, with or without Jacobians (one kernel instantiation each)
+    auto group_key = [](const Task &t) {
+        return t.camop ? KIND_RELPOSE_TS + 1 + 2 * t.cam_op + (t.cam_jac || t.cam_jac_params ? 1 : 0) : t.kind;
+    };
     const int nthreads_req = std::max(1, streams);
     struct Job {
         int device;
@@ -2696,10 +2806,10 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
     std::vector<Job> jobs; // one per (device, worker)
     for (int d = 0; d < n_dev; ++d) {
         std::vector<std::vector<Task *>> groups;
-        for (int kind = 0; kind <= KIND_RELPOSE_TS; ++kind) {
+        for (int key = 0; key <= KIND_RELPOSE_TS + 2 * CAMOP_UNPROJECT_2D + 2; ++key) {
             std::vector<Task *> of_kind;
             for (size_t i = 0; i < count; ++i)
-                if (tasks[i].kind == kind && dev_of[i] == devices[d] && !tasks[i].skip) of_kind.push_back(&tasks[i]);
+                if (group_key(tasks[i]) == key && dev_of[i] == devices[d] && !tasks[i].skip) of_kind.push_back(&tasks[i]);
             if (of_kind.empty()) continue;
             const size_t gsz = std::min<size_t>(256, std::max<size_t>(1, (of_kind.size() + nthreads_req - 1) / nthreads_req));
             for (size_t o = 0; o < of_kind.size(); o += gsz)
@@ -2730,6 +2840,7 @@ static int run_tasks(std::vector<Task> &tasks, std::vector<int> &dev_of, const i
             const int rc = grp[0]->refine     ? run_refine_group(grp[0]->kind, grp)
                            : grp[0]->score    ? run_score_group(grp[0]->kind, grp)
                            : grp[0]->generate ? run_generate_group(grp[0]->kind, grp)
+                           : grp[0]->camop    ? run_camera_group(grp)
                                               : run_group(grp[0]->kind, grp);
             if (rc != PLB_OK) {
                 int exp = PLB_OK;
@@ -2921,6 +3032,41 @@ static int generate_host_prepare(plb_generate_problem &p, Task &t) {
 }
 static int generate_device_prepare(plb_generate_problem &p, Task &t) { return generate_prepare(p, t); }
 
+// ---- the camera functions over many points (plb_camera_batch) -----------------------------------------------------
+// One problem checked and turned into the Task of run_camera_group: the argument errors first, then the camera (NYI).
+// Nothing is written here.
+static int camera_prepare(plb_camera_problem &p, Task &t) {
+    if (p.op < PLB_CAMOP_PROJECT || p.op > PLB_CAMOP_UNPROJECT_2D) {
+        g_err = "unknown camera op";
+        return PLB_ERR_ARG;
+    }
+    if (p.n > 0 && (!p.in || !p.out)) {
+        g_err = "null argument";
+        return PLB_ERR_ARG;
+    }
+    if (p.op == PLB_CAMOP_UNPROJECT_2D && (p.jac || p.jac_params)) {
+        g_err = "the 2D unproject has no Jacobians";
+        return PLB_ERR_ARG;
+    }
+    const uint64_t rows = p.op == PLB_CAMOP_PROJECT ? 2 : 3;
+    uint64_t widest = p.op == PLB_CAMOP_UNPROJECT_2D ? 2 : 3, bytes = 0; // in and out
+    if (p.jac) widest = std::max<uint64_t>(widest, 6);
+    if (p.jac_params) widest = std::max<uint64_t>(widest, rows * cam_num_params(p.camera.model_id));
+    if (__builtin_mul_overflow(p.n, widest * sizeof(double), &bytes) || bytes > SIZE_MAX) {
+        g_err = "too many points";
+        return PLB_ERR_ARG;
+    }
+    if (int r = camera_dev(&p.camera, &t.cam_a)) return r;
+    t.camop = true;
+    t.cam_op = p.op == PLB_CAMOP_PROJECT ? CAMOP_PROJECT : p.op == PLB_CAMOP_UNPROJECT ? CAMOP_UNPROJECT : CAMOP_UNPROJECT_2D;
+    t.a = p.in;
+    t.n = (size_t)p.n;
+    t.cam_out = p.out;
+    t.cam_jac = p.jac;
+    t.cam_jac_params = p.jac_params;
+    return PLB_OK;
+}
+
 // Step 9 of the device forms: every sample index of the generate tasks in [0, n), by one reduction kernel over all of
 // them, after the work queued on the caller's stream (E.ev_in), and one synchronisation.  The kernels that gather with
 // the indices run only after this has passed.
@@ -2954,8 +3100,20 @@ static int check_device_samples(const std::vector<Task> &tasks, Engine &E) {
 // What is wrong with the memory of a device-form task, or null.  Sized by n (n > 0): a, b and the weights, when given,
 // must be device (or managed) memory of `device` aligned to the dtype's `elem` bytes; sized by m (m > 0): models, scores
 // and counts, 8-byte aligned; the inliers the task writes must be device memory; sized by s (s > 0, generate tasks):
-// samples and n_models 4-byte, models, scores and counts 8-byte aligned.
+// samples and n_models 4-byte, models, scores and counts 8-byte aligned.  Camera tasks (n > 0): in aligned to the dtype,
+// out and the Jacobians given 8-byte aligned.
 static const char *device_io_error(const Task &t, int device, size_t elem) {
+    if (t.camop) {
+        if (t.n == 0) return nullptr;
+        if (!device_memory(t.a, device)) return "in must be device memory of the current device";
+        if ((uintptr_t)t.a % elem) return "in is not aligned to the dtype";
+        for (const void *q : {(const void *)t.cam_out, (const void *)t.cam_jac, (const void *)t.cam_jac_params}) {
+            if (!q) continue; // only the Jacobians may be null
+            if (!device_memory(q, device)) return "out / jac / jac_params must be device memory of the current device";
+            if ((uintptr_t)q % sizeof(double)) return "out / jac / jac_params are not 8-byte aligned";
+        }
+        return nullptr;
+    }
     if (t.n > 0)
         for (const void *q : {(const void *)t.a, (const void *)t.b, t.weights}) {
             if (!q) continue; // only the weights may be null
@@ -3102,6 +3260,14 @@ int plb_generate_batch(plb_generate_problem *problems, size_t count, int n_gpus,
 // writes the records into the caller's rows.
 int plb_generate_batch_device(plb_generate_problem *problems, size_t count, int dtype, void *stream, int streams) {
     return run_batch(problems, count, generate_device_prepare, -1, -1, streams, dtype, stream);
+}
+
+int plb_camera_batch(plb_camera_problem *problems, size_t count, int n_gpus, int streams_per_gpu) {
+    return run_batch(problems, count, camera_prepare, n_gpus, -1, streams_per_gpu);
+}
+// The same on the calling thread's device with in, out and the Jacobians in its memory: k_camera reads and writes them.
+int plb_camera_batch_device(plb_camera_problem *problems, size_t count, int dtype, void *stream, int streams) {
+    return run_batch(problems, count, camera_prepare, -1, -1, streams, dtype, stream);
 }
 
 int plb_resident_create(int kind, const double *a, const double *b, size_t n_pts) {

@@ -274,6 +274,19 @@ struct PutDesc {
     double *scores;
     long long *counts;
 };
+// One camera problem of plb_camera_batch: n points of `cam` at `in` (T of the launch: 3 per point to project, 2 to
+// unproject), outputs row-major at out, column-major matrices at jac / jac_params (either may be null).  It owns the
+// tiles [tile0, tile0 + ceil(n / CAM_TILE)) of the launch, tile j its points j * CAM_TILE ..; descriptors are ordered by
+// tile0.
+struct CamOpDesc {
+    CamDev cam;
+    const void *in;
+    double *out, *jac, *jac_params;
+    long long n;
+    long long tile0;
+};
+constexpr int CAM_TILE = 256;
+enum { CAMOP_PROJECT = 0, CAMOP_UNPROJECT = 1, CAMOP_UNPROJECT_2D = 2 };
 
 // ---- launchers (all asynchronous on `stream`) --------------------------------------------------------------
 // normalize_points for n_desc problems (descriptors in device memory), one CTA each.
@@ -355,6 +368,10 @@ void launch_take_samples(const TakeDesc *descs_dev, int n_desc, long long max_co
 // problem a: direct rows of maxm slots, or packed (see PutDesc).
 void launch_put_hyps(const RoundDesc &R, const HypOut &out, const PutDesc *descs_dev, int msz, int maxm, bool packed,
                      cudaStream_t stream);
+// The camera functions of `op` over the tiles of n_desc descriptors (device memory): jac: some descriptor has a jac or
+// jac_params; f32: the inputs are float.
+void launch_camera(int op, bool jac, bool f32, const CamOpDesc *descs_dev, int n_desc, long long n_tiles,
+                   cudaStream_t stream);
 // Batched direct solver calls (solvers/*.h surface): one thread per instance.  kind KIND_RELPOSE also needs the s5_*
 // phase buffers of s5 for `count` instances (the other fields are unused).  Returns the number of kernels launched.
 int launch_solver_batch(int kind, int variant, size_t count, const double *a, const double *b, double *out, int *n_out,

@@ -13,10 +13,17 @@ import numpy as np
 
 from . import cabi
 
-__all__ = ["CameraPose", "Image", "estimate_absolute_pose", "estimate_relative_pose", "estimate_fundamental",
+__all__ = ["Camera", "CameraPose", "Image", "estimate_absolute_pose", "estimate_relative_pose", "estimate_fundamental",
            "estimate_homography", "p3p", "p3p_lambdatwist", "relpose_5pt", "essential_matrix_5pt", "relpose_7pt", "homography_4pt"]
 
 _CAMERA_IDS = dict(cabi.CAMERA)
+# the reference's other models (camera_models.h): a Camera can hold them, its functions raise NYI on them
+_OTHER_CAMERA_IDS = {"OPENCV_FISHEYE": 5, "FULL_OPENCV": 6, "FOV": 7, "THIN_PRISM_FISHEYE": 10,
+                     "RAD_TAN_THIN_PRISM_FISHEYE": 11, "RADIAL_1D": 99, "SPHERICAL": 100}
+_CAMERA_NAMES = {v: k for k, v in {**_CAMERA_IDS, **_OTHER_CAMERA_IDS}.items()}
+# focal lengths and principal-point coordinates at the front of each model's parameters (camera.cuh cam_layout)
+_CAMERA_FOCALS = {-1: (0, 0), 0: (1, 2), 1: (2, 2), 2: (1, 2), 3: (1, 2), 4: (2, 2), 8: (1, 2), 9: (1, 2), 101: (2, 2),
+                  102: (1, 2)}
 
 
 class CameraPose:
@@ -41,6 +48,76 @@ class CameraPose:
         return f"CameraPose(q={self.q.tolist()}, t={self.t.tolist()})"
 
 
+class Camera:
+    """poselib.Camera (pybind/bindings/types.cc:64-113): Camera(), Camera(model_name, params, width, height) or
+    Camera(dict), with model_id, width, height, params, model_name(), todict() and the vector forms of project,
+    project_with_jac and unproject, evaluated on the device (cabi.camera_batch)."""
+
+    def __init__(self, *args):
+        if len(args) == 1 and isinstance(args[0], dict):  # camera_from_dict (helpers.h:255-264): params as given
+            d = args[0]
+            self.model_id = Camera._id(str(d["model"]))
+            self.width, self.height = int(d.get("width", 0)), int(d.get("height", 0))
+            self.params = [float(v) for v in d["params"]]
+            return
+        if len(args) == 0:
+            args = ("NULL", [], 0, 0)
+        if len(args) != 4:
+            raise TypeError("Camera(), Camera(model_name, params, width, height) or Camera(dict)")
+        self.model_id = Camera._id(str(args[0]))
+        self.params = [float(v) for v in args[1]]
+        self.width, self.height = int(args[2]), int(args[3])
+        self._init_params()
+
+    @staticmethod
+    def _id(name):
+        """Camera::id_from_string (camera_models.cc:123-133): an unknown name is the NULL camera's id, -1."""
+        return {**_CAMERA_IDS, **_OTHER_CAMERA_IDS}.get(name, -1)
+
+    def _init_params(self):
+        """Camera::init_params (camera_models.cc:75-93) for the ten models on the path."""
+        if self.model_id not in _CAMERA_FOCALS:
+            return
+        fresh = not self.params
+        npar = cabi.CAMERA_NUM_PARAMS[self.model_id]
+        self.params = (self.params + [0.0] * npar)[:npar]
+        nf, npp = _CAMERA_FOCALS[self.model_id]
+        if fresh and npar:
+            big = self.width > 0 and self.height > 0
+            f = max(self.width, self.height) * 1.2 if big else 1.0
+            self.params[:nf] = [f] * nf
+            self.params[nf:nf + npp] = [self.width / 2.0, self.height / 2.0] if big else [0.0, 0.0]
+
+    def model_name(self):
+        return _CAMERA_NAMES.get(self.model_id, "INVALID_MODEL")
+
+    def todict(self):
+        return {"model": self.model_name(), "width": self.width, "height": self.height, "params": list(self.params)}
+
+    def _cabi(self):
+        return cabi.Camera(self.model_id, tuple(self.params), self.width, self.height)
+
+    def _run(self, op, x, dim, jac=False):
+        x = np.asarray(x, dtype=np.float64).reshape(-1, dim)
+        return cabi.camera_batch([dict(op=op, cam=self._cabi(), x=x, jac=jac)])[0]
+
+    def project(self, x):
+        """Camera::project of a list of 3D points -> list of 2-vectors."""
+        return list(self._run("project", x, 3)["out"])
+
+    def project_with_jac(self, x):
+        """Camera::project_with_jac -> (list of 2-vectors, list of 2x3 Jacobians)."""
+        r = self._run("project", x, 3, jac=True)
+        return list(r["out"]), list(r["jac"].copy())
+
+    def unproject(self, xp):
+        """Camera::unproject of a list of pixels -> list of unit bearings (3-vectors)."""
+        return list(self._run("unproject", xp, 2)["out"])
+
+    def __repr__(self):
+        return f"Camera({self.model_name()!r}, {self.params}, {self.width}, {self.height})"
+
+
 class Image:
     """camera_pose.h `Image`: pose + camera (what estimate_absolute_pose returns)."""
 
@@ -50,9 +127,12 @@ class Image:
 
 
 def _camera(cam):
-    """camera_from_dict (helpers.h:255-264): {"model", "width", "height", "params"}; a cabi.Camera passes through."""
+    """camera_from_dict (helpers.h:255-264): {"model", "width", "height", "params"}; a cabi.Camera passes through, a
+    Camera is converted."""
     if isinstance(cam, cabi.Camera):
         return cam
+    if isinstance(cam, Camera):
+        return cam._cabi()
     if cam is None:
         return cabi.Camera("NULL", ())
     name = str(cam["model"]).upper()
